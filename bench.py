@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- the driver's benchmark contract for carla_ppo_b200.
 
-    python bench.py --gpus N --steps K --warmup W            (this build: sm_100a CUDA behind the C ABI)
+    python bench.py --gpus N --steps K --warmup W            (this build: sm_90a CUDA behind the C ABI)
+    python bench.py ... --dump-outputs DIR                   (also writes the last timed step's outputs as DIR/<name>.npy)
     python bench.py --impl reference --steps K --warmup W    (the reference's CPU path on the host cores)
     python bench.py --config 5 [--gpus N]                    (BASELINE configs[4]: 100 k frames -> encode -> PPO loop)
 
@@ -48,30 +49,6 @@ MAC = {"conv1": 4_732_416, "conv2": 22_413_312, "conv3": 18_874_368, "conv4": 12
        "deconv3": 35_020_800, "deconv4": 4_732_416}
 
 
-def kernel_source_hash():
-    """sha256 over the CUDA sources: the committed ncu traffic table is only valid for the sources it was captured from."""
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "carla_ppo_b200", "csrc")
-    for fn in sorted(os.listdir(d)):
-        if fn.endswith((".cu", ".cuh")):
-            with open(os.path.join(d, fn), "rb") as f:
-                h.update(fn.encode()); h.update(f.read())
-    return h.hexdigest()[:16]
-
-
-def load_ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of each labelled kernel group, extracted from the committed
-    `ncu --set full` capture by scripts/ncu_traffic.py into profiles/r2_ncu_traffic.json together with the hash of the
-    sources it was captured from -- so a kernel change that is not re-profiled shows up as `traffic_stale`."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    if not os.path.isfile(path):
-        return {}, None
-    with open(path) as f:
-        t = json.load(f)
-    return t.get("bytes_per_launch", {}), t.get("source_hash")
-
-
 def load_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(path):
@@ -79,7 +56,8 @@ def load_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p["hbm_gbs"], bf16_burst=p["bf16_tflops"], bf16_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card; dense BF16): a ceiling for the fractions below, not a measured rate
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="H100 SXM data sheet, not measured")
 
 
 def measure_fp32_peaks(seconds=0.6):
@@ -338,7 +316,7 @@ def run_ours(args):
     tmp = tempfile.mkdtemp()
     vae = make_vae(tmp, data_parallel=world > 1)
     g = torch.Generator(device="cuda"); g.manual_seed(1234 + rank)
-    x = torch.rand(B, 80, 160, 3, generator=g, device="cuda")            # 629 MB at B=4096: larger than the 126 MB L2
+    x = torch.rand(B, 80, 160, 3, generator=g, device="cuda")            # 629 MB at B=4096: larger than the 50 MB L2
     eps = torch.randn(B, Z_DIM, generator=g, device="cuda")
 
     def barrier():
@@ -357,9 +335,12 @@ def run_ours(args):
     barrier()
     e0.record()
     for _ in range(args.steps):
-        vae.train_step_device(x, x, eps)
+        losses = vae.train_step_device(x, x, eps)
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        # what the last timed step hands its caller: [recon, kl] and the updated parameters, plus the gradient it applied
+        dump_outputs(args.dump_outputs, {"losses": losses, "params": vae.params, "grads": vae.grads})
     launches = int(lib.cpb_launch_count())
     elapsed = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -447,7 +428,6 @@ def run_ours(args):
     if rank == 0:
         peaks = load_peaks()
         fp32_peaks = measure_fp32_peaks()
-        traffic_tab, traffic_hash = load_ncu_traffic()
         roof = None
         if groups:
             # dominant = the labelled conv/deconv kernel group with the largest share of the step
@@ -465,11 +445,8 @@ def run_ours(args):
             tc_flop = sum(flops(k) for k in conv_like if k.split(".")[0] not in ("conv1", "deconv4"))
             roof = {"bound": "tensor", "kernel": dom, "achieved": ach, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
                     "frac": ach / peaks["bf16_sustained"],
-                    "traffic": traffic_tab.get(dom) if world == 1 else None,
-                    "traffic_source": "profiles/r2_ncu_traffic.json (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum per launch at B=4096)",
-                    "traffic_stale": (traffic_hash != kernel_source_hash()) if traffic_hash else None,
                     "share_of_step": conv_like[dom]["ms_per_step"] / total_ms,
-                    "math_mode": "tcgen05 kind::tf32, 3xTF32 split (fp32-accurate)" if mode == 1 else "fp32 SIMT FMA",
+                    "math_mode": "wgmma tf32, 3xTF32 split (fp32-accurate)" if mode == 1 else "fp32 SIMT FMA",
                     "measured_peaks": {"tf32_tflops": fp32_peaks["tf32_tflops"], "fp32_fma_tflops": fp32_peaks["fp32_fma_tflops"], "how": fp32_peaks["how"],
                                        "bf16_tflops_sustained": peaks["bf16_sustained"], "hbm_gbs": peaks["hbm_gbs"], "source": peaks["source"]},
                     "frac_of_tf32_peak": ach / fp32_peaks["tf32_tflops"],
@@ -492,7 +469,7 @@ def run_ours(args):
                                       "(BASELINE configs[1]%s)" % ("" if world == 1 else "; configs[3]: sharded %d/GPU, one NCCL all-reduce of the flat gradient" % B),
                           "global_batch": GLOBAL_BATCH, "per_gpu_batch": B, "z_dim": Z_DIM, "loss": "mse", "lr": 1e-4,
                           "weights": "glorot-uniform random init (reference architecture)",
-                          "l2": "inputs (629 MB/step at N=1) and activations (GBs) exceed the 126 MB L2; no explicit flush"},
+                          "l2": "inputs (629 MB/step at N=1) and activations (GBs) exceed the 50 MB L2; no explicit flush"},
                "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d * world, "d2h_bytes_per_step": d2h * world,
                        "ms_per_step": float(e2e_ms.item()), "steps": e2e_steps,
                        "path": "ConvVAE.train_step_async(host frames): pinned fp32 frames H2D on a copy stream (2 staging slots, "
@@ -517,6 +494,22 @@ def run_ours(args):
         os.dup2(2, 1)
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy in float32.  If together they exceed 64 MB, every array is replaced by the
+    same fixed, seeded sample of its flat elements (indices sorted), sized to fit."""
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: v.detach().float().cpu().numpy().ravel() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    for name, a in host.items():
+        if total > DUMP_LIMIT_BYTES:
+            keep = max(1, int(a.size * DUMP_LIMIT_BYTES // total))
+            a = a[np.sort(np.random.RandomState(0).choice(a.size, keep, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 # ============================================================================================= reference arm
 def run_reference(args):
     """The reference's own CPU implementation of the path: torch-CPU fp32 restatement of the TF-1.13 graph
@@ -534,7 +527,7 @@ def run_reference(args):
     pick_cpu_threads(lambda: tr.step(x[:64], x[:64], eps[:64]))
     for _ in range(max(1, min(args.warmup, 2))):
         tr.step(x, x, eps, micro_batch=micro)
-    steps = max(1, min(args.steps, 20))
+    steps = args.steps
     t0 = time.perf_counter()
     for _ in range(steps):
         tr.step(x, x, eps, micro_batch=micro)
@@ -556,14 +549,27 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 10)")
+    ap.add_argument("--warmup", type=int, default=None, help="untimed steps before them (default 3)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (losses, parameters, gradient) as DIR/<name>.npy")
     ap.add_argument("--config", type=int, default=2, choices=[2, 5],
                     help="2 (default): the BASELINE metric, ConvVAE train step at batch 4096; 5: BASELINE configs[4], the offline "
                          "100k-frame encode -> PPO update pipeline (scripts/config5.py; frames sharded over the ranks)")
     args = ap.parse_args()
+    if args.config == 5:
+        # the offline pipeline is a fixed workload: it has no step count and no single step whose outputs could be dumped
+        for flag, value in (("--steps", args.steps), ("--warmup", args.warmup), ("--dump-outputs", args.dump_outputs)):
+            if value is not None:
+                ap.error("%s does not apply to --config 5" % flag)
+    elif args.impl == "reference" and args.dump_outputs is not None:
+        ap.error("--dump-outputs applies to the CUDA implementation only")
+    args.steps = 10 if args.steps is None else args.steps
+    args.warmup = 3 if args.warmup is None else args.warmup
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.config == 5:
         import runpy
         sys.argv = [os.path.join(ROOT, "scripts", "config5.py")]

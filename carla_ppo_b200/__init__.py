@@ -1,4 +1,4 @@
-"""carla_ppo_b200 -- B200-native (sm_100a) implementation of the neural hot path of bitsauce/Carla-ppo:
+"""carla_ppo_b200 -- H100-native (sm_90a) implementation of the neural hot path of bitsauce/Carla-ppo:
 the ConvVAE training step and the PPO update that consumes its latents.
 
 Layout (only what the path needs):

@@ -142,5 +142,5 @@ def current_stream_handle(device=None) -> int:
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise CpbError("no CUDA device: carla_ppo_b200 runs on B200 (sm_100a) only and has no CPU fallback")
+        raise CpbError("no CUDA device: carla_ppo_b200 runs on H100 (sm_90a) only and has no CPU fallback")
     return torch

@@ -1,4 +1,4 @@
-// Shared helpers for libcarla_ppo_b200 (sm_100a only).
+// Shared helpers for libcarla_ppo_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -244,7 +244,7 @@ int32_t launch_edge_gather(const float* big4, int cb, const float* w, const floa
 
 int edge_wgrad_ctas(int batch) {
     const long long nrows = (long long)batch * SH;
-    long long ctas = 148 * 2;
+    long long ctas = 132 * 2;                     // two CTAs per SM of an H100 SXM
     if (ctas > nrows) ctas = nrows;
     return (int)(ctas < 1 ? 1 : ctas);
 }

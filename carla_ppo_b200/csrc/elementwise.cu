@@ -270,7 +270,7 @@ __global__ void finalize_losses_kernel(const float* __restrict__ frame_loss, con
 // ------------------------------------------------------------------------------------------
 // column sums (bias gradients): pass 1 -> partial[blocks][pitch]
 // ------------------------------------------------------------------------------------------
-constexpr int kColsumMaxBlocks = 148 * 8;
+constexpr int kColsumMaxBlocks = 132 * 8;   // 8 blocks per SM of an H100 SXM
 // number of row-chunk blocks; block b sums the row tiles b, b + nblocks, b + 2 nblocks, ... (a tile = the rows one
 // pass of the block covers), so that at any moment the resident blocks read one contiguous stretch of memory.
 // (Giving each block ONE contiguous range made the ~1200 concurrent streams start 1.3 MB apart and ran the
@@ -338,25 +338,6 @@ __global__ void colsum_final_kernel(const float* __restrict__ partial, int nbloc
     float s = 0.f;
     for (int b = lane; b < nblocks; b += 32) s += partial[(long long)b * pitch + c];
     s = warp_sum(s);
-    if (lane == 0) out[c] = s;
-}
-
-// Column sums produced by a tap-GEMM epilogue (TapGemmParams::colsum): out[c] = sum over the `rows` (CTA, quarter) rows and
-// the N / cb parity classes of partial[row][class * cb + c].  One warp per channel, fixed order.
-__global__ void colsum_fold_kernel(const float* __restrict__ partial, int rows, int N, int cb, float* __restrict__ out) {
-    const int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (c >= cb) return;
-    // rows % 128 == 0 (kTc2ColsumRows): 4 independent accumulators keep 4+ loads in flight per lane
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    for (int r = lane; r + 96 < rows; r += 128)
-        for (int k = c; k < N; k += cb) {
-            s0 += partial[(long long)r * N + k];
-            s1 += partial[(long long)(r + 32) * N + k];
-            s2 += partial[(long long)(r + 64) * N + k];
-            s3 += partial[(long long)(r + 96) * N + k];
-        }
-    float s = warp_sum((s0 + s1) + (s2 + s3));
     if (lane == 0) out[c] = s;
 }
 
@@ -542,14 +523,6 @@ int32_t launch_finalize_losses(const float* frame_loss, const float* kl_rows, in
 
 long long colsum_scratch_floats(long long rows, int pitch) {
     return colsum_blocks(rows, pitch) * pitch;
-}
-
-int32_t launch_colsum_fold(const float* partial, int rows, int N, int cb, float* out, cudaStream_t stream) {
-    CPB_REQUIRE(cb > 0 && N % cb == 0 && rows % 128 == 0, "colsum_fold: N must be a multiple of the channel count, rows of 128");
-    ProfScope prof("bias_grad.colsum", stream);
-    colsum_fold_kernel<<<cdiv(cb, 8), 256, 0, stream>>>(partial, rows, N, cb, out);
-    CPB_LAUNCHED();
-    return CPB_OK;
 }
 
 int32_t launch_colsum(const float* g, long long rows, int pitch, int c_real, float* out, float* scratch,

@@ -53,8 +53,6 @@ int32_t launch_finalize_losses(const float* frame_loss, const float* kl_rows, in
 
 // out[c] = sum_r g[r*pitch + c]  for c < c_real   (deterministic two-pass; scratch >= colsum_scratch_floats)
 long long colsum_scratch_floats(long long rows, int pitch);
-// folds the (CTA, quarter) rows a tap-GEMM epilogue accumulated (TapGemmParams::colsum) into out[0:cb]
-int32_t launch_colsum_fold(const float* partial, int rows, int N, int cb, float* out, cudaStream_t stream);
 int32_t launch_colsum(const float* g, long long rows, int pitch, int c_real, float* out, float* scratch,
                       cudaStream_t stream);
 

@@ -630,8 +630,8 @@ int32_t run_loss_grad(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan
 // ---------------------------------------------------------------------------------------------
 // The driver's whole update block as ONE persistent cooperative kernel (train.py:171-207 after GAE / theta_old):
 // num_epochs x ceil(T / batch) minibatch steps, each = forward (2 trunks x 2 layers) -> head + loss -> backward ->
-// TF-Adam, with grid-wide barriers between the dependent phases instead of ~9 kernel launches per minibatch (round 1:
-// ~330 launches of 5-30 us kernels, 5.3 ms per learn()).  One CTA per SM, 2 independent groups of 128 threads per CTA;
+// TF-Adam, with grid-wide barriers between the dependent phases instead of ~9 kernel launches per minibatch (~330
+// launches of 5-30 us kernels per learn() otherwise).  One CTA per SM, 2 independent groups of 128 threads per CTA;
 // a phase's 32x32 output tiles are dealt round-robin to the 4 x gridDim groups; the arithmetic per tile is the
 // stand-alone small_gemm_kernel's (same gemm_tile), so the results are those of the launch-per-kernel path up to the
 // order in which the per-CTA loss partials are summed.
@@ -784,10 +784,9 @@ int32_t learn_persistent_init() {
     CPB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
     CPB_CUDA(cudaFuncSetAttribute(ppo_learn_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLearnSmem));
     CPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ppo_learn_persistent_kernel, kLearnThreads, kLearnSmem));
-    // Opt-in (CPB_PPO_PERSISTENT=1).  Measured on B200 at BASELINE configs[2]: 7.1 ms per learn() against 5.5 ms for the
-    // launch-per-kernel path -- the 32x32 / 64-thread gemm_tile is latency-bound (8 dependent global round trips per K = 500
-    // tile) and one CTA per SM leaves 8 warps to hide them, where the stand-alone kernels run ~16 CTAs per SM; the barriers are
-    // not the cost.  Kept because it is parity-green (tests run both paths) and is the skeleton for a tile routine that
+    // Opt-in (CPB_PPO_PERSISTENT=1): slower than the launch-per-kernel path -- the 32x32 / 64-thread gemm_tile is latency-bound
+    // (8 dependent global round trips per K = 500 tile) and one CTA per SM leaves 8 warps to hide them, where the stand-alone
+    // kernels run ~16 CTAs per SM; the barriers are not the cost.  Kept because it is parity-green (tests run both paths) and is the skeleton for a tile routine that
     // stages a whole K strip per barrier phase.
     const char* e = getenv("CPB_PPO_PERSISTENT");
     const bool want = e != nullptr && atoi(e) != 0;

@@ -69,10 +69,7 @@ struct TapGemmParams {
     int quad_cb;
     int quad_lcb;         // log2(quad_cb), set by the launcher
     int cluster;          // tensor-core path: CTAs per cluster (set by the launcher)
-    float* colsum;        // tc2 path only: if set, the epilogue adds the column sums of what it stores (= the bias gradient of the layer
-                          // whose pre-activation gradient dst is) into colsum[(cta * 4 + lane quarter) * N + column]; the caller
-                          // zeroes the kTc2ColsumRows x N buffer before and folds it with launch_colsum_fold afterwards
-    int debug;            // tensor-core path: timing decomposition (CPB_TC_DEBUG): 1 no MMA, 2 no A copies, 4 A copies zero-fill only, 8 no weight copies, 16 cycle accounting
+    int debug;            // tensor-core path: timing decomposition (CPB_TC_DEBUG): 2 no A copies, 4 A copies zero-fill only, 8 no weight copies
     TapClass cls[4];
 };
 
@@ -84,7 +81,7 @@ int tapgemm_pick_ksplit(int rows, int N, int ybatch, int K);
 // One-time opt-in for >48 KB dynamic shared memory (called from the API layer).
 int32_t tapgemm_init();
 
-// ---- tcgen05 (3xTF32) variant of the same contraction -------------------------------------------------
+// ---- tensor-core (wgmma, 3xTF32) variant of the same contraction -------------------------------------------------
 struct TcWeightJob {
     long long src_off;          // float offset of the TF kernel [k,k,Cb,Cs] in the parameter buffer
     long long dst_hi, dst_lo;   // float offset of the operand (2 * taps * N * C floats, hi and lo interleaved by block) / unused
@@ -93,13 +90,10 @@ struct TcWeightJob {
     int k, cb, cs;
     int N, C;                   // logical rows / reduction length per tap
     long long count;
-    int raw;                    // 1 (tc2 kernels): blocks ordered (n-tile y, tap, k-block): block index (y * ntaps + tap) * (C/32) + kc,
-                                // each block = [hi image | lo image] = 2*BN*32 floats (one bulk copy per k-block);
-                                // 2 (tc2, CTA-pair MMAs): same block order, block = [hi rows 0:h | lo rows 0:h | hi rows h:2h | lo rows h:2h], h = BN/2
-    int ntaps;                  // taps of the operand (raw layout only)
 };
-// rows of the N axis handled per CTA tile (also fixes the block size of the stored operand)
-__host__ __device__ constexpr int tc_bn(int N) { return N % 128 == 0 ? 128 : (N % 64 == 0 ? 64 : 32); }
+// rows of the N axis handled per CTA tile (also fixes the block size of the stored operand); at most 64, because each
+// consumer thread holds 1.5 x BN fp32 accumulators in registers
+__host__ __device__ constexpr int tc_bn(int N) { return N % 64 == 0 ? 64 : 32; }
 constexpr int kMaxTcWeightJobs = 12;
 struct TcWeightTable {
     int njobs;

@@ -1,29 +1,27 @@
-// Tensor-core tap-GEMM for sm_100a: the same contraction as tapgemm.cu, computed with tcgen05.mma
-// (kind::tf32, fp32 accumulators in TMEM) using the error-compensated 3xTF32 split
+// Tensor-core tap-GEMM for sm_90a: the same contraction as tapgemm.cu, computed with wgmma.mma_async
+// (kind tf32, fp32 accumulators in registers) using the error-compensated 3xTF32 split
 //
 //     a*b  ~=  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo ,   x_hi = x with the 13 low mantissa bits cleared,  x_lo = x - x_hi
 //
 // so that results stay fp32-accurate (relative error ~1e-6; a single TF32 pass gives ~3e-4 and would break the
 // 1e-5 parity bar).  The tensor core itself ignores the 13 low mantissa bits of a TF32 operand, so the raw fp32
 // tensor IS x_hi; x_lo is a second fp32 plane (written by the producing kernel's epilogue, or by lo_plane_kernel).
-// Operands are staged in shared memory in the UMMA canonical K-major SWIZZLE_128B layout (rows of 32 floats =
-// 128 B, 8-row groups of 1024 B, 16-byte chunk index XOR row%8):
+// Operands are staged in shared memory in the wgmma canonical K-major SWIZZLE_128B layout (rows of 32 floats =
+// 128 B, 8-row groups of 1024 B, 16-byte chunk index XOR row%8) -- the only layout wgmma accepts for TF32 operands:
 //   * A (activations, gathered rows) : cp.async 16 B per thread and row from the raw tensor (hi) and its lo plane,
 //                                      zero-filled outside the image, completion counted on the stage's mbarrier;
 //   * B (weights)                    : stored by tc_weights_kernel as ready-made swizzled tile images [hi | lo]; one
-//                                      cp.async.bulk per k-block (optionally multicast to the CTAs of a cluster).
-// Persistent, warp-specialised kernel (see tc_tapgemm_kernel): loader warps, one weight-producer lane, one MMA-issuer
-// lane (8 MMAs per 32-wide k-block: [main | cross] += a_hi x [b_hi | b_lo] with N = 2*BN, cross += a_lo x b_hi),
-// eight drain / epilogue warps.
+//                                      cp.async.bulk per k-block (multicast to the CTAs of a cluster).
+// Persistent, warp-specialised kernel (see tc_tapgemm_kernel): two consumer warpgroups (64 tile rows each, 8 wgmma per
+// 32-wide k-block: [main | cross] (+)= a_hi x [b_hi | b_lo] with N = 2*BN, cross += a_lo x b_hi) and four A-loader warps,
+// the first lane of which also issues the weight-tile copies.
 //
-// Accumulation.  The tensor core adds into its fp32 accumulator with round-toward-zero, which shrinks a long
-// running sum systematically (measured on B200: relative bias -6.5e-9 x K, i.e. -7e-6 at K=1024, -2.6e-5 at
-// K=4096; scripts/diag_tc.py).  Two measures bring this back to fp32-FMA level:
-//   * the cross terms (2^-11 of the main term) accumulate in their OWN TMEM columns, so they do not re-truncate the
+// Accumulation.  The tensor core adds into its fp32 accumulator with truncation, which shrinks a long running sum
+// systematically (relative bias growing linearly with K).  Two measures bring this back to fp32-FMA level:
+//   * the cross terms (2^-11 of the main term) accumulate in their OWN registers, so they do not re-truncate the
 //     large accumulator;
-//   * accumulation inside TMEM only runs over chunks of 128 k (4 k-blocks) into two ping-pong (main | cross)
-//     buffers; each finished chunk is drained with tcgen05.ld and added to per-thread fp32 REGISTER accumulators
-//     (round-to-nearest) by the drain warps while the tensor core works on the next chunk.
+//   * wgmma accumulation only runs over chunks of 128 k (4 k-blocks); each finished chunk is added to per-thread fp32
+//     register accumulators (round-to-nearest).
 // The register accumulators feed the bias / ReLU / ReLU-mask epilogue directly; the epilogue also writes the lo plane
 // of its output when the consumer is another tensor-core layer.
 #include "tapgemm.cuh"
@@ -39,22 +37,19 @@ template <int BN>
 struct TcCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : ((STAGE_BYTES * 3 <= 200 * 1024) ? 3 : 2);
+    static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : 3;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // +1024: manual 1 KB alignment
-    static constexpr int TMEM_COLS = 4 * BN;                         // 2 chunk buffers x (main | cross): 512 / 256 / 128
 };
-constexpr int CHUNK_KB = 4;   // k-blocks accumulated inside TMEM before draining to registers (must be >= STAGES)
+constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 register accumulators
 
-constexpr int kDrainWarps = 8;                        // warps 0-7: accumulator drain (TMEM -> registers) + epilogue
+constexpr int kConsumerWarps = 8;                     // warps 0-7: two wgmma warpgroups + epilogue
 constexpr int kLoaderWarp0 = 8;                       // warps 8-11: A loaders (cp.async)
 constexpr int kLoaderWarps = 4;
 constexpr int kLoaderThreads = kLoaderWarps * 32;
-constexpr int kIssuerWarp = 12;                       // warp 12: MMA issuer (one elected lane)
-constexpr int kWeightWarp = 13;                       // warp 13: weight-tile producer (bulk copies, one elected lane)
-constexpr int kTcThreads = 448;                       // 14 warps; registers are granted as for 16 (128 per thread)
+constexpr int kTcThreads = 384;                       // a multiple of 4 warps: registers are granted per 4 warps
 
 int g_tc_cluster = 1;         // CTAs per cluster = multicast width of the weight tiles (CPB_TC_CLUSTER, 1/2/4/8)
-int g_tc_clusters[3] = {0, 0, 0};   // co-resident clusters of the persistent grid, per BN instantiation (32/64/128)
+int g_tc_clusters[2] = {0, 0};   // co-resident clusters of the persistent grid, per BN instantiation (32/64)
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
@@ -76,46 +71,28 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(dst), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask, bool multicast) {
-    if (multicast)
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                     ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-    else
-        umma_commit(bar);
-}
-
-// PROF: per-phase clock64 accounting, printed by CTA 0 (CPB_TC_DEBUG & 16; instrumented instantiation)
-#define TC_PROF(slot) do { if constexpr (PROF) { const long long now_ = clock64(); prof[slot] += now_ - tlast; tlast = now_; } } while (0)
 
 // PERSISTENT, CLUSTERED kernel.  A cluster of CS CTAs works on super-tiles (class z, n-tile y, group of CS m-tiles):
 // CTA r of the cluster owns m-tile CS*xs + r, and all CS CTAs need the SAME weight tiles in the same order.  Each
 // k-block's weight tile (pre-split hi | lo, stored in global memory as the ready-made swizzled shared-memory image,
 // tc_weights_kernel) is therefore fetched ONCE per cluster: CTA r bulk-copies slice r of it and the copy engine
-// multicasts the slice into every CTA's stage.  Without this, every SM pulls the same 2*BN*128 bytes per k-block
-// through L2 -- twice the activation traffic, all SMs on the same few L2 slices at the same time -- and the kernel
-// is L2-bound at a third of the tensor-core rate.
-// The k-blocks of all super-tiles of a cluster form one stream through the stage ring and the two TMEM accumulator
-// buffers; a chunk never spans two tiles.  Chunk c is drained (one chunk late) while the tensor core already runs
-// chunk c+1 -- also across a tile boundary, so the bias / ReLU / mask epilogue of tile t and the first loads of
-// tile t+1 overlap the MMAs.
-template <int BN, bool PROF>
-__global__ void __launch_bounds__(kTcThreads, 1)
+// multicasts the slice into every CTA's stage, so a stage is free again only when the consumers of EVERY CTA of the
+// cluster are done with it (each consumer warp arrives on the stage's empty barrier in all CTAs).
+// The k-blocks of all super-tiles of a cluster form one stream through the stage ring; a chunk never spans two tiles.
+template <int BN>
+__global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
 tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, const int total_st) {
     using Cfg = TcCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int B_TILE_BYTES = Cfg::B_TILE_BYTES;
     constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
-    static_assert(STAGES <= CHUNK_KB, "late drain relies on the stage ring being no deeper than a chunk");
 
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES];     // A loader threads (cp.async completion) + weight bytes -> issuer
-    __shared__ uint64_t empty_bar[STAGES];    // tensor cores of ALL CTAs of the cluster -> producers: stage is free everywhere
-    __shared__ uint64_t chunk_bar[2];         // tensor core -> loaders: accumulator buffer b holds a finished chunk
-    __shared__ uint64_t drained_bar[2];       // drain warps -> issuer: buffer b was added to the register accumulators
-    __shared__ uint32_t tmem_slot;
+    __shared__ uint64_t full_bar[STAGES];     // A loader threads (cp.async completion) + weight bytes -> consumers
+    __shared__ uint64_t empty_bar[STAGES];    // consumer warps of ALL CTAs of the cluster -> producers: stage is free everywhere
 
     const int tid = threadIdx.x;
-    const int warp = tid >> 5, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform for the compiler
     const int ntn = p.N / BN;
     const int CS = (int)p.cluster;
     const int rank = CS > 1 ? (int)cluster_ctarank() : 0;
@@ -128,17 +105,11 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 
     if (tid == 0) {
 #pragma unroll
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], kLoaderThreads + 1); mbar_init(&empty_bar[s], (uint32_t)CS); }
-        mbar_init(&chunk_bar[0], 1); mbar_init(&chunk_bar[1], 1);
-        mbar_init(&drained_bar[0], kDrainWarps); mbar_init(&drained_bar[1], kDrainWarps);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], kLoaderThreads + 1); mbar_init(&empty_bar[s], (uint32_t)(kConsumerWarps * CS)); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) tmem_alloc<Cfg::TMEM_COLS>(&tmem_slot);
-    tc_fence_before();
     __syncthreads();
     if (CS > 1) cluster_sync_all();             // peers' barriers are initialised before anything is sent to them
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_slot;
 
     // super-tile st -> (class z, m-group xs, n-tile y), n fastest: clusters running side by side share the A rows through L2
     auto st_z = [&](int st) { return st / (ntn * mgroups); };
@@ -146,95 +117,14 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     auto st_m0 = [&](int st) { return (long long)(((st / ntn) % mgroups) * CS + rank) * TBM; };
     const int kb_per_tap = p.C / TBK;
 
-    if (warp == kIssuerWarp) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-            int g = 0, gc = 0;                  // k-blocks / chunks issued so far (all tiles)
-            long long prof[4] = {0, 0, 0, 0}, tlast = 0;
-            if constexpr (PROF) tlast = clock64();
-            const long long tstart = tlast;
-            for (int st = cl_id; st < total_st; st += cl_n) {
-                const int nkb = p.cls[st_z(st)].ntaps * kb_per_tap;
-                for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % STAGES;
-                    const uint32_t stage = smem_base + s * STAGE_BYTES;
-                    const int b = gc & 1;
-                    TC_PROF(3);
-                    mbar_wait(&full_bar[s], (uint32_t)((g / STAGES) & 1));
-                    TC_PROF(0);
-                    if (kb % CHUNK_KB == 0 && gc >= 2)      // buffer b must have been drained of chunk gc - 2
-                        mbar_wait(&drained_bar[b], (uint32_t)(((gc >> 1) - 1) & 1));
-                    TC_PROF(1);
-                    fence_async_smem();     // the A rows were written by cp.async (generic proxy); the MMA reads through the async proxy
-                    tc_fence_after();
-                    const uint64_t a_hi = make_desc(stage);
-                    const uint64_t a_lo = make_desc(stage + A_TILE_BYTES);
-                    const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
-                    // per 8-wide k-step:  [main | cross] (+)= a_hi x [b_hi | b_lo]   (ONE N = 2*BN MMA: the b_hi and b_lo
-                    //                                                  images are adjacent in the stage)
-                    //                      cross           += a_lo x b_hi
-                    // -- 20 KB of operand reads instead of 24 KB for three N = BN MMAs (the SS-mode MMA is bound by its
-                    // shared-memory operand reads), and 8 instead of 12 instructions per k-block
-                    const uint32_t d_main = tmem_base + (uint32_t)(b * 2 * BN);
-                    const uint32_t d_cross = d_main + (uint32_t)BN;
-                    if (!(p.debug & 1))
-#pragma unroll
-                    for (int ks = 0; ks < TBK / 8; ++ks) {
-                        const uint64_t adv = (uint64_t)(ks * 2);      // 32 bytes per k-step, in 16-byte units
-                        umma_tf32(d_main, a_hi + adv, b_hi + adv, idesc2, ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u);
-                        umma_tf32(d_cross, a_lo + adv, b_hi + adv, idesc, 1u);
-                    }
-                    umma_commit_mc(&empty_bar[s], cl_mask, CS > 1);
-                    if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) { umma_commit(&chunk_bar[b]); ++gc; }
-                    TC_PROF(2);
-                }
-            }
-            if constexpr (PROF) {
-                if (blockIdx.x == 0)
-                    printf("tcprof BN=%d N=%d C=%d quad=%d supertiles=%d cluster=%d kb/cta=%d | issuer total %lld: wait_full %lld wait_drained %lld issue %lld other %lld\n",
-                           BN, p.N, p.C, p.quad, total_st, CS, g, clock64() - tstart, prof[0], prof[1], prof[2], prof[3]);
-            }
-        }
-        __syncwarp();
-    } else if (warp == kWeightWarp) {
-        // ================================ weight-tile producer ================================
-        // global layout (tc_weights_kernel): per tap 2*N*C floats; inside, block (n-tile y, k-block kc) holds the
-        // swizzled shared-memory image [hi: BN rows x 128 B | lo: BN rows x 128 B]
-        if (lane == 0) {
-            const uint32_t slice = (uint32_t)(2 * B_TILE_BYTES / CS);
-            int g = 0;
-            for (int st = cl_id; st < total_st; st += cl_n) {
-                const TapClass& cls = p.cls[st_z(st)];
-                const int y = st_y(st);
-                for (int tap = 0; tap < cls.ntaps; ++tap) {
-                    const float* wt = p.wk_hi + 2 * cls.taps[tap].w_off + (long long)y * kb_per_tap * (2 * BN * TBK);
-                    for (int kc = 0; kc < kb_per_tap; ++kc, ++g) {
-                        const int s = g % STAGES;
-                        if (g >= STAGES) mbar_wait(&empty_bar[s], (uint32_t)((g / STAGES - 1) & 1));
-                        if (!(p.debug & 8)) {
-                            mbar_expect_tx(&full_bar[s], (uint32_t)(2 * B_TILE_BYTES));
-                            const uint32_t dst = smem_base + s * STAGE_BYTES + 2 * A_TILE_BYTES + (uint32_t)rank * slice;
-                            const char* src = reinterpret_cast<const char*>(wt + (long long)kc * (2 * BN * TBK)) + (size_t)rank * slice;
-                            bulk_g2s(dst, src, slice, &full_bar[s], cl_mask, CS > 1);
-                        } else {
-                            mbar_arrive(&full_bar[s]);      // timing decomposition: no weight copy
-                        }
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp >= kLoaderWarp0 && warp < kLoaderWarp0 + kLoaderWarps) {
+    if (warp >= kLoaderWarp0) {
         // ================================ A loaders ================================
-        // The tensor core ignores the 13 low mantissa bits of a TF32 operand (scripts/diag_trunc.py: bit-identical
-        // results), so the raw fp32 activations ARE the "hi" operand; the "lo" operand (x - trunc(x)) comes from a
+        // The tensor core reads only the TF32 bits of an fp32 operand (the 13 low mantissa bits are ignored; the parity
+        // tests against float64 hold with the raw tensor as "hi"), so the raw fp32 activations ARE the "hi" operand; the "lo" operand (x - trunc(x)) comes from a
         // plane written by lo_plane_kernel before this launch.  A tile rows are therefore copied global -> swizzled
         // shared memory with cp.async (16 B per thread and row, zero-filled outside the image), completion is
         // counted on the stage's mbarrier (cp.async.mbarrier.arrive.noinc) -- no registers, no split, no stores,
-        // no wait in the loader.  The loader warps are INSTRUCTION bound otherwise (8 warps feed a 768-cycle MMA
-        // block per k-block), which is why the per-k-block code is kept this small.
+        // no wait in the loader, which keeps the per-k-block instruction count of the loader warps small.
         const int tl = tid - kLoaderWarp0 * 32;      // 0..127
         const int a_chunk = tl & 7;
         // row r = tl/8 + 16*i lives at (r/8)*1024 + (r%8)*128 + ((chunk ^ r%8) * 16): i only moves the 1 KB group (2 per i)
@@ -307,163 +197,164 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             }
         };
 
+        // weight tile of the cursor's k-block.  Global layout (tc_weights_kernel): per tap 2*N*C floats; inside, block
+        // (n-tile y, k-block kc) holds the swizzled shared-memory image [hi: BN rows x 128 B | lo: BN rows x 128 B];
+        // this CTA copies slice `rank` of it, multicast to every CTA of the cluster
+        const uint32_t slice = (uint32_t)(2 * B_TILE_BYTES / CS);
+        auto issue_b = [&](uint32_t stage, uint64_t* full) {
+            if (p.debug & 8) { mbar_arrive(full); return; }      // timing decomposition: no weight copy
+            mbar_expect_tx(full, (uint32_t)(2 * B_TILE_BYTES));
+            const float* wt = p.wk_hi + 2 * clsA->taps[tapA].w_off + ((long long)st_y(stA) * kb_per_tap + cA / TBK) * (2 * BN * TBK);
+            bulk_g2s(stage + 2 * A_TILE_BYTES + (uint32_t)rank * slice, reinterpret_cast<const char*>(wt) + (size_t)rank * slice,
+                     slice, full, cl_mask, CS > 1);
+        };
+
         // ---- copy stream: the loaders run ahead of the tensor core by as many k-blocks as there are free stages
         int sS = 0;                                 // stage of the next k-block and the parity its empty barrier
         uint32_t phS = 1;                           // shows once free (fresh barrier: parity 1 counts as complete)
         while (stA < total_st) {
             mbar_wait(&empty_bar[sS], phS);
+            if (tl == 0) issue_b(smem_base + sS * STAGE_BYTES, &full_bar[sS]);
             issue_a(smem_base + sS * STAGE_BYTES, &full_bar[sS]);
             if (++sS == STAGES) { sS = 0; phS ^= 1u; }
         }
-    } else if (warp < kDrainWarps) {
-        // ================================ accumulator drain + epilogue ================================
-        // ---- register accumulators: this thread owns row (q*32 + lane) x columns [half*BN/2, +BN/2) of the tile
-        //      being drained (stD)
-        constexpr int HALF_COLS = BN / 2;
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access
-        const int half = warp >> 2;                  // column half handled by this warp
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HALF_COLS);
-        float acc[HALF_COLS];
+    } else {
+        // ================================ wgmma consumers + epilogue ================================
+        // warpgroup wg owns tile rows [64*wg, 64*wg + 64); thread layout of the accumulators: see wgmma_tf32
+        constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
+        const int wg = warp >> 2;
+        float acc[HALF];                             // fp32 register accumulators of the tile (main + cross)
+        float dm[HALF], dc[HALF];                    // chunk accumulators of the main and the cross terms
 #pragma unroll
-        for (int i = 0; i < HALF_COLS; ++i) acc[i] = 0.f;
+        for (int i = 0; i < HALF; ++i) { acc[i] = 0.f; dm[i] = 0.f; dc[i] = 0.f; }
 
         auto epilogue = [&](int st) {                // bias / ReLU / mask -> global, from the register accumulators
             const TapClass& cls = p.cls[st_z(st)];
             const int Wo = cls.Wo, HoWo = cls.Ho * Wo;
-            const long long m = st_m0(st) + q * 32 + lane;
-            if (m >= (long long)p.batch * HoWo) return;
-            const int n = (int)(m / HoWo);
-            const int rem = (int)(m - (long long)n * HoWo);
-            const int oy = rem / Wo;
-            const int ox = rem - oy * Wo;
-            const int col0 = st_y(st) * BN + half * HALF_COLS;
-            // destination float offsets fit 32 bits (checked at launch)
-            const uint32_t img = (uint32_t)n * (uint32_t)p.dst_img;
-            const uint32_t off_plain = img + (uint32_t)(((oy * p.dstride + cls.py) * p.Wd + (ox * p.dstride + cls.px)) * p.dst_pitch);
+            const int col0 = st_y(st) * BN + 2 * (lane & 3);
             const int lcb = p.quad_lcb;              // log2(quad_cb)
-            // groups of 4 columns, handled 4 at a time so that the ReLU-mask loads of a batch are all in flight
-            // together (one at a time they serialise 16 global round trips per thread)
-            constexpr int NG = HALF_COLS / 4;
-            constexpr int GB = NG < 4 ? NG : 4;
 #pragma unroll
-            for (int g0 = 0; g0 < NG; g0 += GB) {
-                uint32_t offs[GB];
-                int chs[GB];
-                bool oks[GB];
-                float4 mks[GB];
+            for (int h = 0; h < 2; ++h) {
+                const long long m = st_m0(st) + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+                if (m >= (long long)p.batch * HoWo) continue;
+                const int n = (int)(m / HoWo);
+                const int rem = (int)(m - (long long)n * HoWo);
+                const int oy = rem / Wo;
+                const int ox = rem - oy * Wo;
+                // destination float offsets fit 32 bits (checked at launch)
+                const uint32_t img = (uint32_t)n * (uint32_t)p.dst_img;
+                const uint32_t off_plain = img + (uint32_t)(((oy * p.dstride + cls.py) * p.Wd + (ox * p.dstride + cls.px)) * p.dst_pitch);
+                // groups of 4 column pairs, so that the ReLU-mask loads of a group are in flight together
+                constexpr int NG = BN / 8;
+                constexpr int GB = NG < 4 ? NG : 4;
 #pragma unroll
-                for (int u = 0; u < GB; ++u) {
-                    const int col = col0 + (g0 + u) * 4;
-                    oks[u] = true;
-                    if (p.quad) {
-                        const int c = col >> lcb;
-                        chs[u] = col & (p.quad_cb - 1);
-                        const int y = oy * 2 + (c >> 1), x = ox * 2 + (c & 1);
-                        oks[u] = y < p.Hd && x < p.Wd;
-                        offs[u] = img + (uint32_t)((y * p.Wd + x) * p.dst_pitch + chs[u]);
-                    } else {
-                        chs[u] = col;
-                        offs[u] = off_plain + (uint32_t)col;
+                for (int j0 = 0; j0 < NG; j0 += GB) {
+                    uint32_t offs[GB];
+                    int chs[GB];
+                    bool oks[GB];
+                    float2 mks[GB];
+#pragma unroll
+                    for (int u = 0; u < GB; ++u) {
+                        const int col = col0 + (j0 + u) * 8;
+                        oks[u] = true;
+                        if (p.quad) {
+                            const int c = col >> lcb;
+                            chs[u] = col & (p.quad_cb - 1);
+                            const int y = oy * 2 + (c >> 1), x = ox * 2 + (c & 1);
+                            oks[u] = y < p.Hd && x < p.Wd;
+                            offs[u] = img + (uint32_t)((y * p.Wd + x) * p.dst_pitch + chs[u]);
+                        } else {
+                            chs[u] = col;
+                            offs[u] = off_plain + (uint32_t)col;
+                        }
                     }
-                }
-                if (p.mask) {
-#pragma unroll
-                    for (int u = 0; u < GB; ++u)
-                        mks[u] = oks[u] ? __ldg(reinterpret_cast<const float4*>(p.mask + offs[u])) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int u = 0; u < GB; ++u) {
-                    if (!oks[u]) continue;
-                    const int g = g0 + u;
-                    float4 o = make_float4(acc[g * 4 + 0], acc[g * 4 + 1], acc[g * 4 + 2], acc[g * 4 + 3]);
-                    if (p.bias) {
-                        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + chs[u]));
-                        o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w;
-                    }
-                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
                     if (p.mask) {
-                        o.x = mks[u].x > 0.f ? o.x : 0.f; o.y = mks[u].y > 0.f ? o.y : 0.f;
-                        o.z = mks[u].z > 0.f ? o.z : 0.f; o.w = mks[u].w > 0.f ? o.w : 0.f;
+#pragma unroll
+                        for (int u = 0; u < GB; ++u)
+                            mks[u] = oks[u] ? __ldg(reinterpret_cast<const float2*>(p.mask + offs[u])) : make_float2(0.f, 0.f);
                     }
-                    *reinterpret_cast<float4*>(p.dst + offs[u]) = o;
-                    if (p.dst_lo != nullptr) {           // second TF32 operand of the consumer layer
-                        float4 h, l;
-                        split_tf32(o.x, h.x, l.x); split_tf32(o.y, h.y, l.y); split_tf32(o.z, h.z, l.z); split_tf32(o.w, h.w, l.w);
-                        *reinterpret_cast<float4*>(p.dst_lo + offs[u]) = l;
+#pragma unroll
+                    for (int u = 0; u < GB; ++u) {
+                        if (!oks[u]) continue;
+                        const int r = 4 * (j0 + u) + 2 * h;
+                        float2 o = make_float2(acc[r], acc[r + 1]);
+                        if (p.bias) {
+                            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + chs[u]));
+                            o.x += b.x; o.y += b.y;
+                        }
+                        if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                        if (p.mask) { o.x = mks[u].x > 0.f ? o.x : 0.f; o.y = mks[u].y > 0.f ? o.y : 0.f; }
+                        *reinterpret_cast<float2*>(p.dst + offs[u]) = o;
+                        if (p.dst_lo != nullptr) {           // second TF32 operand of the consumer layer
+                            float2 hi, lo;
+                            split_tf32(o.x, hi.x, lo.x); split_tf32(o.y, hi.y, lo.y);
+                            *reinterpret_cast<float2*>(p.dst_lo + offs[u]) = lo;
+                        }
                     }
                 }
             }
         };
 
-        // ---- drain cursor: chunk `drained` belongs to super-tile stD, which has chunksD chunks left
-        auto st_chunks = [&](int st) { return (p.cls[st_z(st)].ntaps * kb_per_tap + CHUNK_KB - 1) / CHUNK_KB; };
-        int drained = 0;
-        // acc += 32 lanes x BN/2 columns of TMEM; two tcgen05.ld in flight per wait (a single one per round trip
-        // costs ~200 cycles each while the MMAs are running)
-        auto drain_cols = [&](uint32_t taddr) {
+        // stage s is free in this CTA's consumers: lane r < CS arrives on the stage's empty barrier of cluster CTA r
+        auto release = [&](int s) {
+            if (lane < CS) {
+                if (CS > 1) mbar_arrive_cluster(&empty_bar[s], (uint32_t)lane);
+                else mbar_arrive(&empty_bar[s]);
+            }
+        };
+
+        int g = 0;                                   // k-blocks consumed so far (all tiles)
+        for (int st = cl_id; st < total_st; st += cl_n) {
+            const int nkb = p.cls[st_z(st)].ntaps * kb_per_tap;
+            int prev = -1;                           // stage whose wgmma group may still be in flight
+            for (int kb = 0; kb < nkb; ++kb, ++g) {
+                const int s = g % STAGES;
+                const uint32_t stage = smem_base + s * STAGE_BYTES;
+                mbar_wait(&full_bar[s], (uint32_t)((g / STAGES) & 1));
+                // the A rows were written by cp.async (generic proxy); wgmma reads through the async proxy
+                fence_async_smem();
+                const uint64_t a_hi = make_desc(stage + wg * (A_TILE_BYTES / 2));
+                const uint64_t a_lo = make_desc(stage + A_TILE_BYTES + wg * (A_TILE_BYTES / 2));
+                const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
+                const uint64_t b_lo = make_desc(stage + 2 * A_TILE_BYTES + B_TILE_BYTES);
+                // per 8-wide k-step:  main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi
+                // (two disjoint accumulator arrays: wgmma groups writing overlapping register ranges are serialised)
+                wgmma_fence();
 #pragma unroll
-            for (int cc = 0; cc < HALF_COLS; cc += 32) {
-                if constexpr (HALF_COLS >= 32) {
-                    float v[16], w[16];
-                    tmem_ld16_issue(taddr + (uint32_t)cc, v);
-                    tmem_ld16_issue(taddr + (uint32_t)(cc + 16), w);
-                    tmem_ld_wait();
+                for (int ks = 0; ks < TBK / 8; ++ks) {
+                    const uint64_t adv = (uint64_t)(ks * 2);      // 32 bytes per k-step, in 16-byte units
+                    const uint32_t keep = ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u;
+                    wgmma_tf32<BN>(dm, a_hi + adv, b_hi + adv, keep);
+                    wgmma_tf32<BN>(dc, a_hi + adv, b_lo + adv, keep);
+                    wgmma_tf32<BN>(dc, a_lo + adv, b_hi + adv, 1u);
+                }
+                wgmma_commit();
+                if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
+                    wgmma_wait<0>();
+                    fence_regs<HALF>(dm);
+                    fence_regs<HALF>(dc);
+                    if (prev >= 0) release(prev);
+                    release(s);
+                    prev = -1;
 #pragma unroll
-                    for (int i = 0; i < 16; ++i) { acc[cc + i] += v[i]; acc[cc + 16 + i] += w[i]; }
+                    for (int i = 0; i < HALF; ++i) { acc[i] += dm[i]; acc[i] += dc[i]; }
                 } else {
-                    float v[16];
-                    tmem_ld16(taddr + (uint32_t)cc, v);
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[cc + i] += v[i];
+                    if (prev >= 0) { wgmma_wait<1>(); release(prev); }
+                    prev = s;
                 }
             }
-        };
-        int stD = cl_id;
-        int chunksD = stD < total_st ? st_chunks(stD) : 0;
-        long long prof[4] = {0, 0, 0, 0}, tlast = 0;
-        if constexpr (PROF) tlast = clock64();
-        const long long tstart = tlast;
-        auto drain_one = [&]() {
-            const int b = drained & 1;
-            TC_PROF(3);
-            mbar_wait(&chunk_bar[b], (uint32_t)((drained >> 1) & 1));
-            TC_PROF(0);
-            tc_fence_after();
-            drain_cols(tmem_lane + (uint32_t)(b * 2 * BN));            // main term of the chunk
-            drain_cols(tmem_lane + (uint32_t)(b * 2 * BN + BN));       // its cross terms
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&drained_bar[b]);
-            ++drained;
-            TC_PROF(1);
-            if (--chunksD == 0) {
-                epilogue(stD);
-                TC_PROF(2);
+            epilogue(st);
 #pragma unroll
-                for (int i = 0; i < HALF_COLS; ++i) acc[i] = 0.f;
-                stD += cl_n;
-                chunksD = stD < total_st ? st_chunks(stD) : 0;
-            }
-        };
-
-        // chunks are drained as soon as the tensor core finishes them; the issuer may run two chunks ahead (two
-        // accumulator buffers), which hides the epilogue of a tile behind the MMAs of the next one
-        while (stD < total_st) drain_one();
-        if constexpr (PROF) {
-            if (blockIdx.x == 0 && lane == 0 && (warp == 0 || warp == 5))
-                printf("tcprof   drain warp %d total %lld: wait_chunk %lld drain %lld epilogue %lld other %lld (chunks %d)\n",
-                       warp, clock64() - tstart, prof[0], prof[1], prof[2], prof[3], drained);
+            for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
         }
     }
-    tc_fence_before();
     __syncthreads();
     if (CS > 1) cluster_sync_all();             // nobody leaves while a peer may still multicast to / arrive on it
-    if (warp == 0) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
-constexpr int tc_bn_slot(int BN) { return BN == 128 ? 2 : (BN == 64 ? 1 : 0); }
+constexpr int tc_bn_slot(int BN) { return BN == 64 ? 1 : 0; }
 
-template <int BN, bool PROF>
+template <int BN>
 int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_st, unsigned grid, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -475,7 +366,7 @@ int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_st, unsigned 
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = (unsigned)p.cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
-    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN, PROF>, p, mgroups, total_st));
+    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN>, p, mgroups, total_st));
     CPB_LAUNCHED();
     return CPB_OK;
 }
@@ -504,15 +395,14 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
         while ((1 << p.quad_lcb) < p.quad_cb) ++p.quad_lcb;
     }
     const unsigned grid = (unsigned)((total_st < resident ? total_st : resident) * p.cluster);
-    if (p.debug & 16) return tc_launch_t<BN, true>(p, (int)mgroups, (int)total_st, grid, stream);
-    return tc_launch_t<BN, false>(p, (int)mgroups, (int)total_st, grid, stream);
+    return tc_launch_t<BN>(p, (int)mgroups, (int)total_st, grid, stream);
 }
 
 template <int BN>
 int32_t tc_init_one() {
     using Cfg = TcCfg<BN>;
-    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     // how many clusters of this kernel are co-resident (GPC boundaries can strand SMs for cluster sizes > 1)
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -524,7 +414,7 @@ int32_t tc_init_one() {
     attr.val.clusterDim.x = (unsigned)g_tc_cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
     int n = 0;
-    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN, false>, &cfg));
+    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN>, &cfg));
     CPB_REQUIRE(n > 0, "tc_tapgemm: no resident cluster of %d CTAs possible", g_tc_cluster);
     g_tc_clusters[tc_bn_slot(BN)] = n;
     return CPB_OK;
@@ -581,21 +471,6 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
     }
     const int BN = tc_bn(job.N);
     const int nn = n % BN, cc = c % TBK;
-    if (job.raw) {      // tc2 block order (n-tile, tap, k-block); each block = [hi image | lo image]
-        const long long block = ((long long)(n / BN) * job.ntaps + tap) * (job.C / TBK) + c / TBK;
-        const float hi2 = __uint_as_float(__float_as_uint(x) & 0xffffe000u);
-        if (job.raw == 2) {     // CTA-pair order: CTA r of the pair copies [hi rows r*h .. | lo rows r*h ..], h = BN/2
-            const int h = BN / 2, r = nn / h, nl = nn - r * h;
-            const long long at3 = job.dst_hi + block * (2 * BN * TBK) + (long long)r * (2 * h * TBK) + (nl >> 3) * 256 + (nl & 7) * 32 + ((((cc >> 2) ^ (nl & 7))) << 2) + (cc & 3);
-            dst[at3] = hi2;
-            dst[at3 + h * TBK] = x - hi2;
-            return;
-        }
-        const long long at2 = job.dst_hi + block * (2 * BN * TBK) + (nn >> 3) * 256 + (nn & 7) * 32 + ((((cc >> 2) ^ (nn & 7))) << 2) + (cc & 3);
-        dst[at2] = hi2;
-        dst[at2 + BN * TBK] = x - hi2;
-        return;
-    }
     const long long block = ((long long)tap * (job.N / BN) + n / BN) * (job.C / TBK) + c / TBK;
     const long long at = job.dst_hi + block * (2 * BN * TBK) + (nn >> 3) * 256 + (nn & 7) * 32 + ((((cc >> 2) ^ (nn & 7))) << 2) + (cc & 3);
     const float hi = __uint_as_float(__float_as_uint(x) & 0xffffe000u);
@@ -606,16 +481,11 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
 }  // namespace
 
 int32_t tc_tapgemm_init() {
-    int dev = 0, sms = 0;
-    CPB_CUDA(cudaGetDevice(&dev));
-    CPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    (void)sms;
     const char* e = getenv("CPB_TC_CLUSTER");
     g_tc_cluster = e ? atoi(e) : 2;
     CPB_REQUIRE(g_tc_cluster == 1 || g_tc_cluster == 2 || g_tc_cluster == 4 || g_tc_cluster == 8, "CPB_TC_CLUSTER must be 1, 2, 4 or 8");
     CPB_TRY(tc_init_one<32>());
     CPB_TRY(tc_init_one<64>());
-    CPB_TRY(tc_init_one<128>());
     return CPB_OK;
 }
 
@@ -627,7 +497,6 @@ bool tc_tapgemm_supported(const TapGemmParams& p) {
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
     CPB_REQUIRE(tc_tapgemm_supported(p), "tc_tapgemm: unsupported problem (C=%d, N=%d)", p.C, p.N);
     switch (tc_bn(p.N)) {
-        case 128: return tc_launch<128>(p, stream);
         case 64: return tc_launch<64>(p, stream);
         default: return tc_launch<32>(p, stream);
     }
@@ -638,7 +507,7 @@ int32_t launch_lo_plane(const float* x, float* lo, long long count, cudaStream_t
     if (count == 0) return CPB_OK;
     const long long n4 = count / 4;
     const long long want = (n4 + 255) / 256;
-    lo_plane_kernel<<<(unsigned)(want < 148 * 16 ? want : 148 * 16), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(lo), n4);
+    lo_plane_kernel<<<(unsigned)(want < 132 * 16 ? want : 132 * 16), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(lo), n4);
     CPB_LAUNCHED();
     return CPB_OK;
 }

@@ -1,20 +1,20 @@
-// Tensor-core weight gradient for sm_100a (tf Conv2DBackpropFilter for conv and transposed-conv layers):
+// Tensor-core weight gradient for sm_90a (tf Conv2DBackpropFilter for conv and transposed-conv layers):
 //
 //   gw[i, j] = sum_{m}  big[row(m) + tap_off[i / run] + i % run] * small[m * J + j]        (same contract as wgrad.cu)
 //
 // as D[128 x BN] += A^T B with the REDUCTION index m on the MMA K axis.  In NHWC memory the channel index -- not m --
-// is contiguous, while the tensor core wants K-major tiles (for 32-bit operands the MN-major alternative is the
-// special SWIZZLE_128B_BASE32B layout), so unlike tc_tapgemm.cu this kernel keeps a register path: a loader thread
+// is contiguous, while wgmma takes TF32 operands only K-major, so this kernel stages through registers: a loader thread
 // reads the float4 of 4 channels at 4 consecutive reduction positions (4 x LDG.128), regroups them into 4 vectors
 // "one channel x 4 positions" (4x4 register transpose), splits them into TF32 hi / lo parts and writes each as ONE
 // 16-byte chunk of the K-major SWIZZLE_128B tile (8 STS.128).  A quarter-warp covers 8 consecutive channel groups of
 // ONE position (a contiguous 128-byte line per LDG.128); the tile rows are permuted (channel 4*cg + c lives in row
 // 32*c + cg) so that the swizzled stores stay conflict-free, and the accumulator rows / columns are un-permuted
-// when the partial is stored.  Warps 0-7 load A (and drain the accumulator chunks), warps 8-11 load B, warp 12
-// issues the MMAs; two k-blocks are in flight per loader thread; the position cursor advances without divisions.
-// 3xTF32 products, the separate cross-term tile and the chunked drain into fp32 register accumulators are those of
-// tc_tapgemm.cu.  Each (i-tile, j-tile, split) CTA of the single split-K wave writes its partial [128 x BN] block;
-// reduce_partials() sums the splits in a fixed order (deterministic).
+// when the partial is stored.  Warps 0-7 load A and, as two warpgroups of 64 tile rows, issue the wgmma of the stage
+// they just filled while the next k-block's loads are in flight; warps 8-11 load B; two k-blocks are in flight per
+// loader thread; the position cursor advances without divisions.
+// 3xTF32 products, the separate cross-term registers and the chunked accumulation into fp32 register accumulators are
+// those of tc_tapgemm.cu.  Each (i-tile, j-tile, split) CTA of the single split-K wave writes its partial [128 x BN]
+// block; reduce_partials() sums the splits in a fixed order (deterministic).
 #include "tc_common.cuh"
 #include "wgrad.cuh"
 
@@ -32,40 +32,26 @@ struct TcWgCfg {
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
     static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : 3;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
-    // MERGED (BN <= 64): [main | cross] (+)= a_hi x [b_hi | b_lo] as ONE N = 2*BN MMA + cross += a_lo x b_hi, i.e. 8 instead of 12
-    // instructions per k-block (every M = 128 tcgen05.mma costs ~95 clk however narrow N is); the cross terms then reset per
-    // chunk with the main ones and are drained with them.  Measured: deconv3.wgrad 3.27 -> 2.94 ms, conv2.wgrad 1.85 -> 1.70 ms.
-    // At BN = 128 the doubled per-chunk drain (done by the A-loader warps, which are the LSU-bound part of this kernel) costs
-    // more than the saved instruction: 0.96 -> 2.30 ms -- so BN = 128 keeps three N = 128 MMAs and ONE cross accumulator that
-    // lives for the whole reduction.
-    static constexpr bool MERGED = BN <= 64;
-    static constexpr int TMEM_COLS = MERGED ? 4 * BN : (BN == 128 ? 512 : (BN == 64 ? 256 : 128));
 };
 
-constexpr int kWgLoaderWarps = 8;                         // warps 0-7: A (big) loaders, accumulator drain, partial store
+constexpr int kWgLoaderWarps = 8;                         // warps 0-7: A (big) loaders, wgmma, partial store
 constexpr int kWgBWarps = 4;                              // warps 8-11: B (small) loaders
-constexpr int kWgIssuerWarp = kWgLoaderWarps + kWgBWarps; // warp 12: MMA issuer (one elected lane)
-constexpr int kWgThreads = (kWgIssuerWarp + 1) * 32;
+constexpr int kWgThreads = (kWgLoaderWarps + kWgBWarps) * 32;
 
 template <int BN>
-__global__ void __launch_bounds__(kWgThreads, 1)
+__global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
 tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
     using Cfg = TcWgCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int B_TILE_BYTES = Cfg::B_TILE_BYTES;
     constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
-    static_assert(STAGES <= CHUNK_KB, "late drain relies on the stage ring being no deeper than a chunk");
 
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t full_bar[STAGES];     // loader warps -> issuer (one arrival per warp)
-    __shared__ uint64_t empty_bar[STAGES];    // tensor core -> loaders
-    __shared__ uint64_t chunk_bar[2];         // tensor core -> loaders: main tile b holds a finished chunk
-    __shared__ uint64_t drained_bar[2];       // loader warps -> issuer: main tile b was added to the registers
-    __shared__ uint64_t done_bar;
-    __shared__ uint32_t tmem_slot;
+    __shared__ uint64_t full_bar[STAGES];     // loader warps -> wgmma (one arrival per warp)
+    __shared__ uint64_t empty_bar[STAGES];    // wgmma warps -> loaders (one arrival per warp once its wgmma are done)
 
     const int tid = threadIdx.x;
-    const int warp = tid >> 5, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform for the compiler
     const int i0 = blockIdx.x * TBM;
     const int j0 = blockIdx.y * BN;
     const int HoWo = p.Ho * p.Wo;
@@ -78,23 +64,12 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     if (tid == 0) {
 #pragma unroll
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], kWgLoaderWarps + kWgBWarps); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&chunk_bar[0], 1);
-        mbar_init(&chunk_bar[1], 1);
-        mbar_init(&drained_bar[0], kWgLoaderWarps);
-        mbar_init(&drained_bar[1], kWgLoaderWarps);
-        mbar_init(&done_bar, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], kWgLoaderWarps + kWgBWarps); mbar_init(&empty_bar[s], kWgLoaderWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) tmem_alloc<Cfg::TMEM_COLS>(&tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_slot;
-    const int nchunks = (nkb + CHUNK_KB - 1) / CHUNK_KB;
     constexpr int BQ = BN / 4;                       // channel groups of the B tile
     const int len = (int)(m_end - m_begin);          // reduction positions of this split
-
     // 4x4 register transpose + split + store: x[j] = 4 channels at position j  ->  one chunk per channel
     auto store_t = [&](uint32_t tile_hi, uint32_t tile_lo, const float4* x, const uint32_t* so) {
         const float xs[4][4] = {{x[0].x, x[1].x, x[2].x, x[3].x}, {x[0].y, x[1].y, x[2].y, x[3].y},
@@ -109,92 +84,40 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         }
     };
 
-    if (warp == kWgIssuerWarp) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t stage = smem_base + s * STAGE_BYTES;
-                const int chunk = kb / CHUNK_KB;
-                mbar_wait(&full_bar[s], (uint32_t)((kb / STAGES) & 1));
-                if (kb % CHUNK_KB == 0 && chunk >= 2)
-                    mbar_wait(&drained_bar[chunk & 1], (uint32_t)(((chunk >> 1) - 1) & 1));
-                tc_fence_after();
-                const uint64_t a_hi = make_desc(stage);
-                const uint64_t a_lo = make_desc(stage + A_TILE_BYTES);
-                const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
-                if constexpr (Cfg::MERGED) {
-                    const uint32_t d_main = tmem_base + (uint32_t)((chunk & 1) * 2 * BN);
-                    const uint32_t d_cross = d_main + (uint32_t)BN;
-#pragma unroll
-                    for (int ks = 0; ks < TBK / 8; ++ks) {
-                        const uint64_t adv = (uint64_t)(ks * 2);          // 32 bytes per k-step (K-major)
-                        umma_tf32(d_main, a_hi + adv, b_hi + adv, idesc2, ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u);
-                        umma_tf32(d_cross, a_lo + adv, b_hi + adv, idesc, 1u);
-                    }
-                } else {
-                    const uint64_t b_lo = make_desc(stage + 2 * A_TILE_BYTES + B_TILE_BYTES);
-                    const uint32_t d_main = tmem_base + (uint32_t)((chunk & 1) * BN);
-                    const uint32_t d_cross = tmem_base + (uint32_t)(2 * BN);
-#pragma unroll
-                    for (int ks = 0; ks < TBK / 8; ++ks) {
-                        const uint64_t adv = (uint64_t)(ks * 2);
-                        umma_tf32(d_main, a_hi + adv, b_hi + adv, idesc, ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u);
-                        umma_tf32(d_cross, a_lo + adv, b_hi + adv, idesc, (kb | ks) != 0 ? 1u : 0u);
-                        umma_tf32(d_cross, a_hi + adv, b_lo + adv, idesc, 1u);
-                    }
-                }
-                umma_commit(&empty_bar[s]);
-                if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) umma_commit(&chunk_bar[chunk & 1]);
-                if (!Cfg::MERGED && kb == nkb - 1) umma_commit(&done_bar);
-            }
-        }
-        __syncwarp();
-    } else if (warp >= kWgLoaderWarps) {
+    if (warp >= kWgLoaderWarps) {
         // ================================ B (small) loaders ================================
         // 128 threads = (channel group of 4 output channels) x (position block of 4 reduction positions), a
-        // quarter-warp again covering 128 contiguous bytes; BN = 128 needs two position blocks per thread, BN = 32
-        // leaves half of the threads idle.  Same 4x4 transpose + split + swizzled store as the A side.
+        // quarter-warp again covering 128 contiguous bytes; BN = 32 leaves half of the threads idle.  Same 4x4
+        // transpose + split + swizzled store as the A side.
         constexpr int NCGH = BQ >= 8 ? BQ / 8 : 1;
-        constexpr int REPS = BN == 128 ? 2 : 1;
         const int r = (tid - kWgLoaderWarps * 32) >> 3;           // 0..15
         const int cgb = (r % NCGH) * 8 + (lane & 7);
-        const int mb0 = r / NCGH;                                  // BN 32: 0..15 (>= 8 idle), 64: 0..7, 128: 0..3 (+4)
+        const int mb0 = r / NCGH;                                  // BN 32: 0..15 (>= 8 idle), 64: 0..7
         const bool active = mb0 < 8;
-        uint32_t soffb[REPS][4];
+        uint32_t soffb[4];
 #pragma unroll
-        for (int rp = 0; rp < REPS; ++rp)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int mbb = mb0 + 4 * rp;
-                const int rb = BQ * c + cgb;
-                soffb[rp][c] = (uint32_t)((rb >> 3) * 1024 + (rb & 7) * 128 + ((mbb ^ (rb & 7)) << 4));
-            }
+        for (int c = 0; c < 4; ++c) {
+            const int rb = BQ * c + cgb;
+            soffb[c] = (uint32_t)((rb >> 3) * 1024 + (rb & 7) * 128 + ((mb0 ^ (rb & 7)) << 4));
+        }
         int relB = mb0 * 4;
         const float* bptr = p.small + (m_begin + relB) * p.J + j0 + cgb * 4;
-        auto load_b = [&](float4 (*xb)[4]) {
+        auto load_b = [&](float4* xb) {
 #pragma unroll
-            for (int rp = 0; rp < REPS; ++rp)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    xb[rp][j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (active && relB + 16 * rp + j < len) xb[rp][j] = __ldg(reinterpret_cast<const float4*>(bptr + (16 * rp + j) * p.J));
-                }
+            for (int j = 0; j < 4; ++j) {
+                xb[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (active && relB + j < len) xb[j] = __ldg(reinterpret_cast<const float4*>(bptr + j * p.J));
+            }
             relB += TBK;
             bptr += TBK * p.J;
         };
-        float4 xb0[REPS][4], xb1[REPS][4];
+        float4 xb0[4], xb1[4];
         int sS = 0;
         uint32_t phS = 1;
-        auto step_b = [&](int kb, float4 (*xb)[4]) {
+        auto step_b = [&](int kb, float4* xb) {
             const uint32_t stage = smem_base + sS * STAGE_BYTES + 2 * A_TILE_BYTES;
             mbar_wait(&empty_bar[sS], phS);
-            if (active) {
-#pragma unroll
-                for (int rp = 0; rp < REPS; ++rp) store_t(stage, stage + B_TILE_BYTES, xb[rp], soffb[rp]);
-            }
+            if (active) store_t(stage, stage + B_TILE_BYTES, xb, soffb);
             fence_async_smem();
             __syncwarp();
             if (lane == 0) mbar_arrive(&full_bar[sS]);
@@ -208,7 +131,7 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             if (kb + 1 < nkb) step_b(kb + 1, xb1);
         }
     } else {
-        // ================================ A loaders / drain / partial store ================================
+        // ================================ A loaders / wgmma / partial store ================================
         // thread = (channel group cg of 4 channels, position block mb of 4 reduction positions).
         // A quarter-warp = 8 consecutive channel groups of ONE position: its LDG.128 is one contiguous 128-byte line
         // (the L1 data pipe charges a wavefront per 32-byte sector when a quarter-warp straddles lines).
@@ -260,65 +183,62 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             while (remL >= HoWo) { remL -= HoWo; ++nL; }
         };
 
-        constexpr int HALF_COLS = BN / 2;
-        const int q = warp & 3;
-        const int half = warp >> 2;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * HALF_COLS);
-        float acc[HALF_COLS];
+        constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
+        const int wg = warp >> 2;                    // warpgroup: tile rows [64*wg, 64*wg + 64)
+        float acc[HALF];                             // fp32 register accumulators (main + cross)
+        float d[BN];                                 // chunk accumulators: [main (HALF) | cross (HALF)]
 #pragma unroll
-        for (int i = 0; i < HALF_COLS; ++i) acc[i] = 0.f;
-        int drained = 0;
-        // acc += 32 lanes x BN/2 columns of TMEM, two tcgen05.ld in flight per wait
-        auto drain_cols = [&](uint32_t taddr) {
+        for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
 #pragma unroll
-            for (int cc = 0; cc < HALF_COLS; cc += 32) {
-                if constexpr (HALF_COLS >= 32) {
-                    float v[16], w[16];
-                    tmem_ld16_issue(taddr + (uint32_t)cc, v);
-                    tmem_ld16_issue(taddr + (uint32_t)(cc + 16), w);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) { acc[cc + i] += v[i]; acc[cc + 16 + i] += w[i]; }
-                } else {
-                    float v[16];
-                    tmem_ld16(taddr + (uint32_t)cc, v);
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[cc + i] += v[i];
-                }
-            }
-        };
-        auto drain_one = [&]() {
-            const int b = drained & 1;
-            mbar_wait(&chunk_bar[b], (uint32_t)((drained >> 1) & 1));
-            tc_fence_after();
-            if constexpr (Cfg::MERGED) {
-                drain_cols(tmem_lane + (uint32_t)(b * 2 * BN));            // main term of the chunk
-                drain_cols(tmem_lane + (uint32_t)(b * 2 * BN + BN));       // its cross terms
-            } else {
-                drain_cols(tmem_lane + (uint32_t)(b * BN));
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&drained_bar[b]);
-            ++drained;
-        };
+        for (int i = 0; i < BN; ++i) d[i] = 0.f;
 
         // two k-blocks of operand rows are in flight per thread (register double buffer): with one, every
         // k-block costs a full L2 round trip per warp
         float4 xa0[4], xa1[4];
         int sS = 0;                                 // stage of the k-block being stored and the parity its empty
         uint32_t phS = 1;                           // barrier shows once free (fresh barrier: parity 1 counts as complete)
+        int prev = -1;                              // stage whose wgmma group may still be in flight
         auto step = [&](int kb, float4* xa) {
-            const uint32_t stage = smem_base + sS * STAGE_BYTES;
-            mbar_wait(&empty_bar[sS], phS);
-            if ((kb & (CHUNK_KB - 1)) == 0) {
-                while (drained < kb / CHUNK_KB - 1) drain_one();
-            }
+            const int s = sS;
+            const uint32_t stage = smem_base + s * STAGE_BYTES;
+            mbar_wait(&empty_bar[s], phS);
             store_t(stage, stage + A_TILE_BYTES, xa, soff);
             fence_async_smem();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&full_bar[sS]);
+            if (lane == 0) mbar_arrive(&full_bar[s]);
             if (kb + 2 < nkb) load_regs(xa);
+            mbar_wait(&full_bar[s], (uint32_t)((kb / STAGES) & 1));
+            const uint64_t a_hi = make_desc(stage + wg * (A_TILE_BYTES / 2));
+            const uint64_t a_lo = make_desc(stage + A_TILE_BYTES + wg * (A_TILE_BYTES / 2));
+            const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
+            // [main | cross] (+)= a_hi x [b_hi | b_lo] as ONE N = 2*BN wgmma (the images are adjacent), cross += a_lo x b_hi.
+            // ptxas serialises the wgmma of this kernel whichever way the products are split (C7518); the merged form issues
+            // two instead of three per k-step and measures faster than three disjoint N = BN products.
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < TBK / 8; ++ks) {
+                const uint64_t adv = (uint64_t)(ks * 2);          // 32 bytes per k-step (K-major)
+                wgmma_tf32<2 * BN>(d, a_hi + adv, b_hi + adv, ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u);
+                wgmma_tf32<BN>(d + HALF, a_lo + adv, b_hi + adv, 1u);
+            }
+            wgmma_commit();
+            if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
+                wgmma_wait<0>();
+                fence_regs<BN>(d);
+                if (lane == 0) {
+                    if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+                    mbar_arrive(&empty_bar[s]);
+                }
+                prev = -1;
+#pragma unroll
+                for (int i = 0; i < HALF; ++i) { acc[i] += d[i]; acc[i] += d[HALF + i]; }
+            } else {
+                if (prev >= 0) {
+                    wgmma_wait<1>();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = s;
+            }
             if (++sS == STAGES) { sS = 0; phS ^= 1u; }
         };
         if (nkb > 0) load_regs(xa0);
@@ -328,28 +248,24 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             if (kb + 1 < nkb) step(kb + 1, xa1);
         }
 
-        while (drained < nchunks) drain_one();
-        if (!Cfg::MERGED && nkb > 0) {
-            mbar_wait(&done_bar, 0);
-            tc_fence_after();
-            drain_cols(tmem_lane + (uint32_t)(2 * BN));            // the cross accumulator of the whole reduction
-        }
-        // ---- partial[split][i][j]: TMEM lane rho = q*32 + lane holds channel i = 4*lane + q; accumulator column
-        //      rho_b = half*BN/2 + a holds j = 4*(rho_b % BQ) + rho_b / BQ, i.e. this thread has the column pairs
-        //      (4*cgb + 2*half, +1) for every cgb
-        const int i = i0 + 4 * lane + q;
-        if (i < p.I) {
-            float* out = p.partial + ((long long)blockIdx.z * p.I + i) * p.J + j0 + 2 * half;
+        // ---- partial[split][i][j]: tile row rho holds channel i = 4*(rho % 32) + rho / 32; accumulator column rb holds
+        //      j = 4*(rb % BQ) + rb / BQ
 #pragma unroll
-            for (int cgb = 0; cgb < BQ; ++cgb)
-                *reinterpret_cast<float2*>(out + 4 * cgb) = make_float2(acc[cgb], acc[BQ + cgb]);
+        for (int h = 0; h < 2; ++h) {
+            const int rho = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            const int i = i0 + 4 * (rho & 31) + (rho >> 5);
+            if (i >= p.I) continue;
+            float* out = p.partial + ((long long)blockIdx.z * p.I + i) * p.J + j0;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int rb = 8 * j + 2 * (lane & 3) + c;
+                    out[4 * (rb % BQ) + rb / BQ] = acc[4 * j + 2 * h + c];
+                }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
-
 template <int BN>
 int32_t tc_wg_launch(const WgradParams& p, cudaStream_t stream) {
     dim3 grid((unsigned)cdiv(p.I, TBM), (unsigned)(p.J / BN), (unsigned)p.splits);
@@ -364,14 +280,13 @@ int32_t tc_wg_init_one() {
     return CPB_OK;
 }
 
-int tc_wg_bn(int J) { return J % 128 == 0 ? 128 : (J % 64 == 0 ? 64 : 32); }
+int tc_wg_bn(int J) { return J % 64 == 0 ? 64 : 32; }   // at most 64: see tc_bn
 
 }  // namespace
 
 int32_t tc_wgrad_init() {
     CPB_TRY(tc_wg_init_one<32>());
     CPB_TRY(tc_wg_init_one<64>());
-    CPB_TRY(tc_wg_init_one<128>());
     return CPB_OK;
 }
 
@@ -379,7 +294,7 @@ bool tc_wgrad_supported(int I, int J, int run) { return run % 4 == 0 && J % 32 =
 
 int tc_wgrad_pick_splits(int I, int J, long long M) {
     const long long tiles = (long long)cdiv(I, TBM) * (J / tc_wg_bn(J));
-    long long splits = 148 / tiles;                         // ONE wave: one CTA per SM (192 KB of shared memory each)
+    long long splits = kTcWaveCtas / tiles;                 // ONE wave: one CTA per SM (193 KB of shared memory each)
     const long long max_splits = (M + 1023) / 1024;         // keep >= 1024 reduction positions per split
     if (splits > max_splits) splits = max_splits;
     if (splits < 1) splits = 1;
@@ -392,7 +307,6 @@ int32_t launch_tc_wgrad(const WgradParams& p, cudaStream_t stream) {
     CPB_REQUIRE((long long)p.batch * p.big_img < (1ll << 31) && p.m_per_split < (1ll << 30) && p.Wo < 65536 && p.Ho * p.Wo < 65536,
                 "tc_wgrad: tensor too large for 32-bit offsets");
     switch (tc_wg_bn(p.J)) {
-        case 128: return tc_wg_launch<128>(p, stream);
         case 64: return tc_wg_launch<64>(p, stream);
         default: return tc_wg_launch<32>(p, stream);
     }

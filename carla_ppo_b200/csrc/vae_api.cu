@@ -7,7 +7,6 @@
 
 #include "elementwise.cuh"
 #include "tapgemm.cuh"
-#include "tc2.cuh"
 #include "wgrad.cuh"
 
 namespace cpb {
@@ -44,7 +43,7 @@ void profile_end(cudaStream_t s) {
     g_open = -1;
 }
 
-int g_math_mode = 1;   // 0: fp32 SIMT everywhere; 1: 3xTF32 tcgen05 for the dense conv/deconv layers
+int g_math_mode = 1;   // 0: fp32 SIMT everywhere; 1: 3xTF32 wgmma for the dense conv/deconv layers
 // Per-device one-time setup (cudaFuncSetAttribute for > 48 KB dynamic shared memory and the co-resident cluster counts
 // of the persistent kernels are PER DEVICE): keyed by cudaGetDevice() so that a process driving several GPUs works.
 constexpr int kMaxDevices = 64;
@@ -61,9 +60,6 @@ int32_t ensure_init() {
         if (st == CPB_OK) st = wgrad_init();
         if (st == CPB_OK) st = tc_tapgemm_init();
         if (st == CPB_OK) st = tc_wgrad_init();
-        if (st == CPB_OK) st = tc2_tapgemm_init();
-        if (st == CPB_OK) st = tc2_wgrad_init();
-        if (st == CPB_OK) st = tc3_wgrad_init();
         g_init_status[dev] = st;
         g_init_done[dev] = st == CPB_OK ? 1 : 2;
     }
@@ -179,15 +175,12 @@ static Relayout make_relayout(int z) {
     return r;
 }
 
-constexpr long long kColsumPartialFloats = (long long)kTc2ColsumRows * 512;      // column-sum rows of the widest layer (N = 512)
-
 struct VaePlan {
     int B, ct, z, mode;
     Relayout rl;
     float *relayout, *xp, *yp, *a1, *a2, *a3, *a4, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss;
     float *d1, *b1, *b2, *b3, *logits_p;
     float *gA, *gB, *gz, *gheads, *partial, *colsum;
-    float* cs_partial;  // (CTA, quarter) x N column sums written by the tc2 tap-GEMM epilogues (bias gradients)
     float* cs_edge;     // per-CTA column sums of deconv4's data gradient (edge_gather), [edge_gather_blocks(B)][32]
     float* frame_dsum;  // per-frame channel sums of d loss / d logits, [B][4]
     float* lo;          // lo plane scratch for tensor-core sources whose producer does not write one (small tensors)
@@ -210,9 +203,8 @@ static int64_t max_partial_floats(int B, int z) {
         {z, FEAT, (long long)B},                    // dense1
     };
     int64_t best = (int64_t)edge_wgrad_ctas(B) * 48 * C1;
-    // the tensor-core weight gradients run ONE wave of (i-tile, j-tile, split) CTAs with 128 x BN <= 128 tiles:
-    // splits * I * J <= 148 * 128 * 128 floats whatever the split rule (tc_wgrad.cu, tc2_wgrad.cu)
-    if (best < 148LL * 128 * 128) best = 148LL * 128 * 128;
+    // the tensor-core weight gradient runs ONE wave of (i-tile, j-tile, split) CTAs with 128 x BN <= 128 x 64 tiles
+    if (best < (int64_t)kTcWaveCtas * 128 * 64) best = (int64_t)kTcWaveCtas * 128 * 64;
     for (const P& p : ps) {
         int64_t n = (int64_t)wgrad_pick_splits(p.I, p.J, p.M) * p.I * p.J;
         if (n > best) best = n;
@@ -239,14 +231,10 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     p.heads = a.take<float>(2 * b * z);
     p.lo = a.take<float>(b * FEAT);
     p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * z);
-    // lo planes (x - trunc_tf32(x)) exist only for the round-1 tensor-core kernels (CPB_TC2=0): the tc2 kernels derive them in
-    // shared memory.  (A size query made before the library initialised on a device still counts them: conservative.)
-    const bool need_lo = !tc2_enabled();
-    if (need_lo) {
-        p.a1_lo = a.take<float>(b * H1 * W1 * C1);
-        p.a2_lo = a.take<float>(b * H2 * W2 * C2);
-        p.a3_lo = a.take<float>(b * H3 * W3 * C3);
-    }
+    // lo planes (x - trunc_tf32(x)): the second TF32 operand of every tensor-core source, written by its producer
+    p.a1_lo = a.take<float>(b * H1 * W1 * C1);
+    p.a2_lo = a.take<float>(b * H2 * W2 * C2);
+    p.a3_lo = a.take<float>(b * H3 * W3 * C3);
     if (mode >= CPB_WS_FORWARD) {
         p.yp = a.take<float>(b * NPIX * 4);
         p.zbuf = a.take<float>(b * z);
@@ -255,10 +243,8 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
         p.frame_loss = a.take<float>(b);
         p.d1 = a.take<float>(b * FEAT);
         p.b1 = a.take<float>(b * H3 * W3 * C3);
-        if (need_lo) {
-            p.b1_lo = a.take<float>(b * H3 * W3 * C3);
-            p.b2_lo = a.take<float>(b * H2 * W2 * C2);
-        }
+        p.b1_lo = a.take<float>(b * H3 * W3 * C3);
+        p.b2_lo = a.take<float>(b * H2 * W2 * C2);
         p.b2 = a.take<float>(b * H2 * W2 * C2);
         p.b3 = a.take<float>(b * H1 * W1 * C1);
         p.logits_p = a.take<float>(b * NPIX * 4);
@@ -266,16 +252,13 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     if (mode >= CPB_WS_TRAIN) {
         p.gA = a.take<float>(b * H1 * W1 * C1);
         p.gB = a.take<float>(b * H1 * W1 * C1);
-        if (need_lo) {
-            p.gA_lo = a.take<float>(b * H1 * W1 * C1);
-            p.gB_lo = a.take<float>(b * H1 * W1 * C1);
-        }
+        p.gA_lo = a.take<float>(b * H1 * W1 * C1);
+        p.gB_lo = a.take<float>(b * H1 * W1 * C1);
         p.gz = a.take<float>(b * z);
         p.gheads = a.take<float>(2 * b * z);
         p.partial = a.take<float>(max_partial_floats(B, z));
         p.colsum = a.take<float>(colsum_scratch_floats(b * NPIX, 4) + colsum_scratch_floats(b * H1 * W1, C1) +
                                  colsum_scratch_floats(b, FEAT));
-        p.cs_partial = a.take<float>(kColsumPartialFloats);
         p.cs_edge = a.take<float>(edge_gather_blocks(B) * C1);
         p.frame_dsum = a.take<float>(b * 4);
     }
@@ -391,38 +374,12 @@ static thread_local float* tl_lo_scratch = nullptr;   // lo plane of the current
 
 // src_lo / dst_lo: lo planes (x - trunc_tf32(x)) of the source (written by its producer; nullptr: computed here into the
 // scratch plane) and of the destination (written by the epilogue for the consuming layer; nullptr: not needed)
-// bias_out / cs_partial: when given and the layer runs on the tc2 kernel, the epilogue also produces the column sums of dst
-// (the bias gradient of the layer whose pre-activation gradient dst is) and *bias_done is set; otherwise the caller runs
-// launch_colsum on dst afterwards.
 static int32_t tg(const char* label, const TapGemmParams& p, cudaStream_t s, int scatter_k = 0,
-                  const float* src_lo = nullptr, float* dst_lo = nullptr, float* bias_out = nullptr, float* cs_partial = nullptr,
-                  bool* bias_done = nullptr) {
-    if (bias_done != nullptr) *bias_done = false;
-    if (g_math_mode == 1 && p.wk_hi != nullptr && tl_lo_scratch != nullptr) {
-        TapGemmParams q = scatter_k > 0 ? quad_from_scatter(p, scatter_k) : p;
-        q.debug = tc_debug_flags();
-        if (tc2_tapgemm_supported(q, scatter_k)) {                                               // TMA tensor maps, no lo planes
-            const bool fold = bias_out != nullptr && cs_partial != nullptr && (long long)q.N * kTc2ColsumRows <= kColsumPartialFloats;
-            if (fold) {
-                CPB_CUDA(cudaMemsetAsync(cs_partial, 0, sizeof(float) * (size_t)q.N * kTc2ColsumRows, s));
-                q.colsum = cs_partial;
-            }
-            { ProfScope prof(label, s);
-              CPB_TRY(launch_tc2_tapgemm(q, scatter_k, s)); }
-            if (fold) {
-                CPB_TRY(launch_colsum_fold(cs_partial, kTc2ColsumRows, q.N, q.quad ? q.quad_cb : q.N, bias_out, s));
-                *bias_done = true;
-            }
-            return CPB_OK;
-        }
-    }
+                  const float* src_lo = nullptr, float* dst_lo = nullptr) {
     ProfScope prof(label, s);
     if (g_math_mode == 1 && p.wk_hi != nullptr && tl_lo_scratch != nullptr) {
         TapGemmParams q = scatter_k > 0 ? quad_from_scatter(p, scatter_k) : p;
         q.debug = tc_debug_flags();
-        // with tc2 enabled the weight images are in the tc2 block order and the SIMT transposes are not written: a layer the
-        // tc2 kernel cannot take must not silently run on stale operands (cannot happen with the fixed 80x160 geometry)
-        CPB_REQUIRE(!tc2_enabled(), "layer %s is not supported by the tc2 tap-GEMM (C=%d, N=%d)", label, q.C, q.N);
         q.src_lo = src_lo != nullptr ? src_lo : tl_lo_scratch;
         q.dst_lo = dst_lo;
         if (tc_tapgemm_supported(q)) {
@@ -445,28 +402,9 @@ static int32_t run_wgrad(const char* label, const float* big, int Wb, int pitch,
     for (int kh = 0; kh < k; ++kh) w.tap_off[kh] = (long long)kh * Wb * pitch;
     w.I = k * k * pitch; w.J = J;
     const long long M = (long long)B * Ho * Wo;
-    // tc2_wgrad (MN-major operands by TMA) is parity-green but, like every SS-mode 3xTF32 kernel here, bound by the 128 B/clk
-    // of shared-memory bandwidth: its staging (copy-engine write + splitter read + write) costs 3 passes over each operand
-    // byte against 2 for the register path of tc_wgrad.cu, and measures 10-40 % slower (profiles/r2_cycle_accounting.md).
-    // Opt in with CPB_TC2_WGRAD=1; the unit tests exercise it through cpb_debug_tc_wgrad either way.
-    static const bool tc2_wg = [] { const char* e = getenv("CPB_TC2_WGRAD"); return e != nullptr && atoi(e) != 0; }();
-    if (g_math_mode == 1 && tc3_wgrad_supported(w) && !(tc_debug_flags() & 32)) {
-        // J <= 64 (conv2, deconv3): A operand in tensor memory, see tc3_wgrad.cu
-        const long long tiles = (long long)cdiv(w.I, 128), boxes = tc3_wgrad_boxes(w);
-        long long sp = 148 / tiles;
-        if (sp > boxes) sp = boxes;
-        w.splits = (int)(sp < 1 ? 1 : sp);
-        w.tc_variant = tc_debug_flags();
-        CPB_TRY(launch_tc3_wgrad(w, s));
-    } else if (g_math_mode == 1 && tc2_wg && tc2_wgrad_supported(w) && !(tc_debug_flags() & 32)) {
-        int bw, bh, bn; long long nboxes;
-        tc2_wgrad_plan(w, bw, bh, bn, nboxes);
-        w.splits = tc2_wgrad_pick_splits(w.I, w.J, nboxes);
-        CPB_TRY(launch_tc2_wgrad(w, s));
-    } else if (g_math_mode == 1 && tc_wgrad_supported(w.I, w.J, w.run)) {
+    if (g_math_mode == 1 && tc_wgrad_supported(w.I, w.J, w.run)) {
         w.splits = tc_wgrad_pick_splits(w.I, w.J, M);
         w.m_per_split = align_up((M + w.splits - 1) / w.splits, 32);
-        w.tc_variant = tc_debug_flags();
         CPB_TRY(launch_tc_wgrad(w, s));
     } else {
         w.splits = wgrad_pick_splits(w.I, w.J, M);
@@ -516,15 +454,12 @@ static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const flo
         j.count = mode == 0 ? (long long)taps * rows * cols : (long long)taps * rows_pad * cols;
         t.total += j.count;
     };
-    // the transposed conv / deconv kernels feed the SIMT scatter-form tap-GEMM only: with the tensor-core path active
-    // (math mode 1, tc2) nothing reads them, and at a 512-frame shard this launch is 1 % of the step
-    const bool simt_scatter = !(g_math_mode == 1 && tc2_enabled());
-    if (decoder && simt_scatter) {
+    if (decoder) {
         add(L.off[T_DECONV1_K], pl.rl.deconv1T, 16, C3, C4, 0, 0);
         add(L.off[T_DECONV2_K], pl.rl.deconv2T, 16, C2, C3, 0, 0);
         add(L.off[T_DECONV3_K], pl.rl.deconv3T, 25, C1, C2, 0, 0);
     }
-    if (backward && simt_scatter) {
+    if (backward) {
         add(L.off[T_CONV2_K], pl.rl.conv2T, 16, C1, C2, 0, 0);
         add(L.off[T_CONV3_K], pl.rl.conv3T, 16, C2, C3, 0, 0);
         add(L.off[T_CONV4_K], pl.rl.conv4T, 16, C3, C4, 0, 0);
@@ -544,14 +479,12 @@ static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const flo
             TcWeightJob& j = w.jobs[w.njobs++];
             j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].f_hi; j.dst_lo = pl.rl.tc[slot].f_lo;
             j.mode = 1; j.k = k; j.cb = cb; j.cs = cs; j.N = cs; j.C = k * cb; j.count = n; w.total += n;
-            j.raw = tc2_enabled() ? tc2_weight_layout() : 0; j.ntaps = k;
         }
         if (scatter) {
             TcWeightJob& j = w.jobs[w.njobs++];
             j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].t_hi; j.dst_lo = pl.rl.tc[slot].t_lo;
             const int win = (k + 1) / 2;
             j.mode = 2; j.k = k; j.cb = cb; j.cs = cs; j.N = 4 * cb; j.C = cs; j.count = (long long)win * win * 4 * cb * cs; w.total += j.count;
-            j.raw = tc2_enabled() ? tc2_weight_layout() : 0; j.ntaps = win * win;
         }
     };
     // conv layers run gather-form forward / scatter-form dgrad; deconv layers the other way round
@@ -576,7 +509,7 @@ static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_
       CPB_TRY(launch_prep_frames(source, cfg->source_dtype, sscale, 3, (long long)B * NPIX, pl.xp, flags, 1, s)); }
     { ProfScope prof("conv1.fwd", s);
       CPB_TRY(launch_edge_gather(pl.xp, 3, params + L.off[T_CONV1_K], params + L.off[T_CONV1_B], nullptr, pl.a1,
-                                 g_math_mode == 1 && !tc2_enabled() ? pl.a1_lo : nullptr, B, s)); }
+                                 g_math_mode == 1 ? pl.a1_lo : nullptr, B, s)); }
     TapGemmParams p;
     p = gather_problem(pl.a1, B, H1, W1, C1, 4, params + L.off[T_CONV2_K], C2, params + L.off[T_CONV2_B], nullptr, pl.a2, 1,
                        pl.relayout + pl.rl.tc[TC_CONV2].f_hi, pl.relayout + pl.rl.tc[TC_CONV2].f_lo);
@@ -666,7 +599,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.frame_dsum, B, 4, pl.ct, grads + L.off[T_DECONV4_B], cs, s));
     { ProfScope prof("deconv4.dgrad", s);
       CPB_TRY(launch_edge_gather(dlog, pl.ct, params + L.off[T_DECONV4_K], nullptr, pl.b3, pl.gA,
-                                 g_math_mode == 1 && !tc2_enabled() ? pl.gA_lo : nullptr, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
+                                 g_math_mode == 1 ? pl.gA_lo : nullptr, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
     TapGemmParams p;
     // ---- deconv3
     CPB_TRY(run_wgrad("deconv3.wgrad", pl.gA, W1, C1, (long long)H1 * W1 * C1, 5, pl.b2, B, H2, W2, C2, 5 * 5 * C1, 5 * 5 * C1,
@@ -674,19 +607,18 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.cs_edge, edge_gather_blocks(B), C1, C1, grads + L.off[T_DECONV3_B], cs, s));
     p = gather_problem(pl.gA, B, H1, W1, C1, 5, params + L.off[T_DECONV3_K], C2, nullptr, pl.b2, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV3].f_hi, pl.relayout + pl.rl.tc[TC_DECONV3].f_lo);
-    bool bias_done = false;
-    CPB_TRY(tg("deconv3.dgrad", p, s, 0, pl.gA_lo, pl.gB_lo, grads + L.off[T_DECONV2_B], pl.cs_partial, &bias_done));   // gB = g(b2)
+    CPB_TRY(tg("deconv3.dgrad", p, s, 0, pl.gA_lo, pl.gB_lo));   // gB = g(b2)
     // ---- deconv2
     CPB_TRY(run_wgrad("deconv2.wgrad", pl.gB, W2, C2, (long long)H2 * W2 * C2, 4, pl.b1, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_DECONV2_K], s));
-    if (!bias_done) CPB_TRY(launch_colsum(pl.gB, (long long)B * H2 * W2, C2, C2, grads + L.off[T_DECONV2_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gB, (long long)B * H2 * W2, C2, C2, grads + L.off[T_DECONV2_B], cs, s));
     p = gather_problem(pl.gB, B, H2, W2, C2, 4, params + L.off[T_DECONV2_K], C3, nullptr, pl.b1, pl.gA, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV2].f_hi, pl.relayout + pl.rl.tc[TC_DECONV2].f_lo);
-    CPB_TRY(tg("deconv2.dgrad", p, s, 0, pl.gB_lo, pl.gA_lo, grads + L.off[T_DECONV1_B], pl.cs_partial, &bias_done));   // gA = g(b1)
+    CPB_TRY(tg("deconv2.dgrad", p, s, 0, pl.gB_lo, pl.gA_lo));   // gA = g(b1)
     // ---- deconv1
     CPB_TRY(run_wgrad("deconv1.wgrad", pl.gA, W3, C3, (long long)H3 * W3 * C3, 4, pl.d1, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
                       grads + L.off[T_DECONV1_K], s));
-    if (!bias_done) CPB_TRY(launch_colsum(pl.gA, (long long)B * H3 * W3, C3, C3, grads + L.off[T_DECONV1_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gA, (long long)B * H3 * W3, C3, C3, grads + L.off[T_DECONV1_B], cs, s));
     p = gather_problem(pl.gA, B, H3, W3, C3, 4, params + L.off[T_DECONV1_K], C4, nullptr, nullptr, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV1].f_hi, pl.relayout + pl.rl.tc[TC_DECONV1].f_lo);
     CPB_TRY(tg("deconv1.dgrad", p, s, 0, pl.gA_lo, nullptr));                                   // gB = g(d1) [B, 6144]
@@ -719,26 +651,26 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.gA, (long long)B * H4 * W4, C4, C4, grads + L.off[T_CONV4_B], cs, s));
     p = scatter_problem(pl.gA, B, H4, W4, C4, 4, pl.relayout + pl.rl.conv4T, C3, nullptr, pl.a3, pl.gB, H3, W3, 0,
                         pl.relayout + pl.rl.tc[TC_CONV4].t_hi, pl.relayout + pl.rl.tc[TC_CONV4].t_lo);
-    CPB_TRY(tg("conv4.dgrad", p, s, 4, nullptr, pl.gB_lo, grads + L.off[T_CONV3_B], pl.cs_partial, &bias_done));   // gB = g(a3)
+    CPB_TRY(tg("conv4.dgrad", p, s, 4, nullptr, pl.gB_lo));   // gB = g(a3)
     // ---- conv3
     CPB_TRY(run_wgrad("conv3.wgrad", pl.a2, W2, C2, (long long)H2 * W2 * C2, 4, pl.gB, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_CONV3_K], s));
-    if (!bias_done) CPB_TRY(launch_colsum(pl.gB, (long long)B * H3 * W3, C3, C3, grads + L.off[T_CONV3_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gB, (long long)B * H3 * W3, C3, C3, grads + L.off[T_CONV3_B], cs, s));
     p = scatter_problem(pl.gB, B, H3, W3, C3, 4, pl.relayout + pl.rl.conv3T, C2, nullptr, pl.a2, pl.gA, H2, W2, 0,
                         pl.relayout + pl.rl.tc[TC_CONV3].t_hi, pl.relayout + pl.rl.tc[TC_CONV3].t_lo);
-    CPB_TRY(tg("conv3.dgrad", p, s, 4, pl.gB_lo, pl.gA_lo, grads + L.off[T_CONV2_B], pl.cs_partial, &bias_done));   // gA = g(a2)
+    CPB_TRY(tg("conv3.dgrad", p, s, 4, pl.gB_lo, pl.gA_lo));   // gA = g(a2)
     // ---- conv2
     CPB_TRY(run_wgrad("conv2.wgrad", pl.a1, W1, C1, (long long)H1 * W1 * C1, 4, pl.gA, B, H2, W2, C2, 16 * C1, 16 * C1, pl.partial,
                       grads + L.off[T_CONV2_K], s));
-    if (!bias_done) CPB_TRY(launch_colsum(pl.gA, (long long)B * H2 * W2, C2, C2, grads + L.off[T_CONV2_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gA, (long long)B * H2 * W2, C2, C2, grads + L.off[T_CONV2_B], cs, s));
     p = scatter_problem(pl.gA, B, H2, W2, C2, 4, pl.relayout + pl.rl.conv2T, C1, nullptr, pl.a1, pl.gB, H1, W1, 0,
                         pl.relayout + pl.rl.tc[TC_CONV2].t_hi, pl.relayout + pl.rl.tc[TC_CONV2].t_lo);
-    CPB_TRY(tg("conv2.dgrad", p, s, 4, pl.gA_lo, nullptr, grads + L.off[T_CONV1_B], pl.cs_partial, &bias_done));   // gB = g(a1)
+    CPB_TRY(tg("conv2.dgrad", p, s, 4, pl.gA_lo, nullptr));   // gB = g(a1)
     // ---- conv1 (its input gradient is never used: the reference computes and discards it)
     { ProfScope prof("conv1.wgrad", s);
       CPB_TRY(launch_edge_wgrad(pl.xp, 3, pl.gB, B, pl.partial, s));
       CPB_TRY(launch_reduce_partials(pl.partial, edge_wgrad_ctas(B), 48, C1, 48, 48, grads + L.off[T_CONV1_K], s)); }
-    if (!bias_done) CPB_TRY(launch_colsum(pl.gB, (long long)B * H1 * W1, C1, C1, grads + L.off[T_CONV1_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gB, (long long)B * H1 * W1, C1, C1, grads + L.off[T_CONV1_B], cs, s));
     return CPB_OK;
 }
 
@@ -939,7 +871,7 @@ using namespace cpb;
 extern "C" {
 
 const char* cpb_last_error(void) { return cpb::g_err; }
-const char* cpb_build_info(void) { return "carla_ppo_b200 0.2 (sm_100a; tcgen05 3xTF32 + fp32 SIMT tap-GEMM)"; }
+const char* cpb_build_info(void) { return "carla_ppo_b200 0.3 (sm_90a; wgmma 3xTF32 + fp32 SIMT tap-GEMM)"; }
 int64_t cpb_launch_count(void) { return cpb::g_launches; }
 void cpb_reset_launch_count(void) { cpb::g_launches = 0; }
 
@@ -965,10 +897,7 @@ int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, 
     TapGemmParams p = dense_problem(a, m, k, nullptr, n, nullptr, nullptr, d, 0);
     p.wk_hi = scratch; p.wk_lo = scratch + (long long)n * k;
     p.debug = tc_debug_flags();
-    const bool use_tc2 = tc2_tapgemm_supported(p, 0);
-    w.jobs[0].raw = use_tc2 ? tc2_weight_layout() : 0; w.jobs[0].ntaps = 1;
     CPB_TRY(launch_tc_weights(bt, scratch, w, s));
-    if (use_tc2) return launch_tc2_tapgemm(p, 0, s);
     float* lo = scratch + 2LL * n * k;
     p.src_lo = lo;
     CPB_TRY(launch_lo_plane(a, lo, (long long)m * k, s));
@@ -987,20 +916,12 @@ int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int
     w.ntaps = 1; w.run = i; w.tap_off[0] = 0; w.I = i; w.J = j; w.tc_variant = variant;
     w.splits = 2;
     w.m_per_split = align_up(((long long)m + 1) / 2, 32);
-    if ((variant & 128) && tc3_wgrad_available(w)) {             // variant & 128: J <= 64 kernel with the A operand in tensor memory
-        CPB_TRY(launch_tc3_wgrad(w, s));
-        return launch_reduce_partials(partial, w.splits, i, j, i, i, out, s);
-    }
-    if (tc2_wgrad_supported(w) && !(variant & 32)) {       // variant & 1: descriptor probe (LBO / SBO swapped); & 32: round-1 kernel
-        CPB_TRY(launch_tc2_wgrad(w, s));
-        return launch_reduce_partials(partial, w.splits, i, j, i, i, out, s);
-    }
     CPB_TRY(launch_tc_wgrad(w, s));
     return launch_reduce_partials(partial, w.splits, i, j, i, i, out, s);
 }
 
 int32_t cpb_set_math_mode(int32_t mode) {
-    CPB_REQUIRE(mode == 0 || mode == 1, "math mode must be 0 (fp32 SIMT) or 1 (3xTF32 tcgen05)");
+    CPB_REQUIRE(mode == 0 || mode == 1, "math mode must be 0 (fp32 SIMT) or 1 (3xTF32 wgmma)");
     cpb::g_math_mode = mode;
     return CPB_OK;
 }
@@ -1050,21 +971,11 @@ int32_t cpb_vae_layout(int32_t ct, int32_t z, int64_t* offsets, int64_t* sizes, 
     return CPB_OK;
 }
 
-// The plan depends on which kernel family this device will run (the tc2 kernels need no lo planes): initialise first when a
-// device is usable, so that the size handed out is the size the calls will use.  Without a device (symbol / layout checks
-// on a CPU-only host) the query stays conservative.
-static void init_if_device_present() {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) == cudaSuccess && n > 0) (void)cpb::ensure_init();
-    else (void)cudaGetLastError();
-}
-
 int64_t cpb_vae_workspace_bytes(int32_t batch, int32_t ct, int32_t z, int32_t mode) {
     if (batch < 1 || (ct != 1 && ct != 3) || z < 64 || z % 64 != 0 || mode < 0 || mode > 2) {
         cpb::set_error("cpb_vae_workspace_bytes: bad arguments");
         return CPB_ERR_INVALID_ARGUMENT;
     }
-    init_if_device_present();
     return make_plan(nullptr, 0, batch, ct, z, mode).bytes;
 }
 

@@ -212,7 +212,7 @@ int wgrad_pick_splits(int I, int J, long long M) {
     int bi, bj;
     tile_dims(pick_tile(I, J), bi, bj);
     const long long tiles = (long long)cdiv(I, bi) * (J / bj);
-    long long target = 148 * 4;                   // ~2 waves at 2 CTAs/SM
+    long long target = 132 * 4;                   // ~2 waves at 2 CTAs/SM (132 SMs)
     long long splits = (target + tiles - 1) / tiles;
     const long long max_splits = (M + 255) / 256;  // keep >= 256 reduction positions per split
     if (splits > max_splits) splits = max_splits;

@@ -35,7 +35,8 @@ int wgrad_pick_splits(int I, int J, long long M);
 int32_t launch_wgrad(const WgradParams& p, cudaStream_t stream);
 int32_t wgrad_init();
 
-// tensor-core (tcgen05, 3xTF32) variant -- tc_wgrad.cu.  Same WgradParams; m_per_split must be a multiple of 32.
+// tensor-core (wgmma, 3xTF32) variant -- tc_wgrad.cu.  Same WgradParams; m_per_split must be a multiple of 32.
+constexpr int kTcWaveCtas = 132;   // CTAs of the single split-K wave: one per SM of an H100 SXM
 int32_t tc_wgrad_init();
 bool tc_wgrad_supported(int I, int J, int run);
 int tc_wgrad_pick_splits(int I, int J, long long M);

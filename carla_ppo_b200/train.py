@@ -1,6 +1,6 @@
 """Drop-in for the reference's ``train.py`` (train.py:23-216 ``train(params, start_carla, restart)`` and the CLI :218-276) over
 the offline replay environment (SURVEY.md section 8f-3): the same episode / horizon / update structure, the same
-hyper-parameter flags and TensorBoard tags, with the neural work on the B200 library:
+hyper-parameter flags and TensorBoard tags, with the neural work on the H100 library:
 
   * every environment step:  FusedActor = VAE encode + PPO predict in one C call (cpb_encode_predict) instead of two
     TensorFlow session runs                                                              (train.py:143 + vae_common.py:45-61)

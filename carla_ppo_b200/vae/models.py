@@ -1,5 +1,5 @@
 """Drop-in for the reference's ``vae/models.py``: same class names, constructor arguments, methods,
-attributes and NumPy-in / NumPy-out conventions, backed by libcarla_ppo_b200.so (hand-written sm_100a
+attributes and NumPy-in / NumPy-out conventions, backed by libcarla_ppo_b200.so (hand-written sm_90a
 CUDA behind a C ABI) instead of a TensorFlow session.
 
 Reference surface mirrored here (paths relative to the reference repo root):

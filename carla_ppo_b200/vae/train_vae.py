@@ -1,6 +1,6 @@
 """VAE training CLI with the reference's command line (reference vae/train_vae.py:47-161): same flags, same
 model-directory naming, same 90/10 split, same early stopping (patience 10 on the validation reconstruction
-loss, checkpoint on improvement) -- driving the B200 ConvVAE instead of a TensorFlow session.
+loss, checkpoint on improvement) -- driving the H100 ConvVAE instead of a TensorFlow session.
 
 What is different on purpose: frames stay uint8 end to end.  The PNGs are decoded once, uploaded once and kept
 resident in HBM (38.4 KB/frame); the `/255` (rgb) and `/12` (segmentation class ids, train_vae.py:26-29) scalings

@@ -1,5 +1,5 @@
 /*
- * carla_ppo_b200.h -- C ABI of libcarla_ppo_b200.so: the B200 (sm_100a) implementation of the
+ * carla_ppo_b200.h -- C ABI of libcarla_ppo_b200.so: the H100 (sm_90a) implementation of the
  * neural hot path of bitsauce/Carla-ppo (ConvVAE train step + PPO update).
  *
  * The reference has no FFI: its boundary is the Python class surface of vae/models.py, ppo.py and
@@ -46,7 +46,7 @@ enum { CPB_FRAME_F32 = 0, CPB_FRAME_U8 = 1 };
 enum { CPB_WS_ENCODE = 0, CPB_WS_FORWARD = 1, CPB_WS_TRAIN = 2 };
 
 const char* cpb_last_error(void);
-/* "sm_100a" build tag + version, for diagnostics */
+/* "sm_90a" build tag + version, for diagnostics */
 const char* cpb_build_info(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -249,7 +249,7 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
 /* Arithmetic used for the dense conv / transposed-conv contractions of the VAE (both are fp32-accurate):
- *   1 (default) tcgen05.mma kind::tf32 with the error-compensated 3xTF32 split, fp32 accumulators in TMEM;
+ *   1 (default) wgmma tf32 with the error-compensated 3xTF32 split, fp32 accumulators in registers;
  *   0           fp32 FMA (SIMT) tap-GEMM -- also used in mode 1 for the layers the tensor-core kernel does
  *               not cover (3-channel edge layers, dense heads, weight gradients). */
 int32_t cpb_set_math_mode(int32_t mode);

@@ -43,7 +43,7 @@ else:
     for _ in range(2):
         vae.train_step_device(xd, xd, ed)
     got = vae.get_weights()
-    print("B %d pair %s" % (B, os.environ.get("CPB_TC_PAIR", "default")))
+    print("B %d" % B)
     for k in w0:
         d = np.abs(got[k].astype(np.float64) - r["p64/" + k])
         print("  %-26s params gpu %.2e cpu32 %.2e | first grad gpu %.2e | max|dp| %.2e (lr=1e-4) n=%d" % (

@@ -27,7 +27,7 @@ p64 = {k: v.astype(np.float64) for k, v in w.items()}
 ref = vo.loss_and_grads(p64, x, x, eps)
 g32 = torch_ref.vae_loss_and_grads(w, x, x, eps, dtype=torch.float32)["grads"]
 got = vae.get_grads()
-print("seed %d B %d pair %s" % (seed, B, os.environ.get("CPB_TC_PAIR", "default")))
+print("seed %d B %d" % (seed, B))
 for k in p64:
     d = np.abs(got[k].astype(np.float64) - ref["grads"][k])
     print("  %-26s gpu %.2e  cpu32 %.2e   max|d| %.2e at %s (|g| there %.2e, max|g| %.2e)" % (

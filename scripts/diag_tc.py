@@ -1,4 +1,4 @@
-"""GPU diagnostics for the tcgen05 3xTF32 kernel: dense GEMM error vs fp64 as a function of K and data
+"""GPU diagnostics for the wgmma 3xTF32 kernel: dense GEMM error vs fp64 as a function of K and data
 statistics, and per-buffer differences between math mode 0 (SIMT) and 1 (tensor core) after a VAE forward."""
 import os, sys, ctypes as C, tempfile
 import numpy as np, torch

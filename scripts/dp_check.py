@@ -43,7 +43,7 @@ if rank == 0:
     # same three steps that differ only in summation order -> parameters and losses within 1e-5 (the path's tolerance), replicas
     # bit-identical.  The distance of BOTH runs to the float64 oracle (and the float32 CPU restatement's own distance) is
     # REPORTED next to it, not gated: parameters after the first Adam steps from zero slots move by ~lr * sign(g), so a tensor's
-    # distance to float64 is decided by the handful of elements whose gradient is ~0 (profiles/r2_parity_conditioning.md);
+    # distance to float64 is decided by the handful of elements whose gradient is ~0;
     # the oracle parity of the single-GPU step is what tests/test_vae_gpu.py and tests/test_vae_large_gpu.py gate.
     # (oracle/ is test infrastructure: this script is a test, not the product.)
     from oracle import vae_oracle as vo

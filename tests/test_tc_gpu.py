@@ -1,6 +1,6 @@
-"""Unit parity of the two tensor-core kernels through their C-ABI debug entries (cpb_debug_tc_gemm / cpb_debug_tc_wgrad)
-against float64 NumPy, at shapes that exercise every tile width, ragged row counts, one / many k-blocks and
-multi-tile persistence; plus bit-identity of the tap-GEMM across cluster (weight-multicast) sizes.
+"""Unit parity of the two tensor-core (wgmma) kernels through their C-ABI debug entries (cpb_debug_tc_gemm /
+cpb_debug_tc_wgrad) against float64 NumPy, at shapes that exercise every tile width, ragged row counts, one / many
+k-blocks and multi-tile persistence; plus bit-identity of the tap-GEMM across cluster (weight-multicast) sizes.
 
 Tolerance: 3xTF32 with chunked accumulation measures 6e-7 .. 9e-7 norm-wise (scripts/diag_tc.py); the bar here is
 2e-6, five times inside the 1e-5 the layer-level tests use."""
@@ -46,7 +46,8 @@ def test_tc_gemm_matches_float64(m, n, k):
 
 
 def test_tc_gemm_positive_data_has_no_accumulation_bias():
-    """all-positive operands at K=4096: a plain TMEM accumulation (round-toward-zero) is off by -2.6e-5 here"""
+    """all-positive operands at K=4096: accumulating the whole reduction in the tensor core's truncating fp32 accumulator
+    would bias every output low; the chunked accumulation into fp32 registers must not"""
     rs = np.random.RandomState(7)
     a = rs.rand(256, 4096).astype(np.float32)
     bt = rs.rand(128, 4096).astype(np.float32)
@@ -56,12 +57,13 @@ def test_tc_gemm_positive_data_has_no_accumulation_bias():
     assert abs(np.mean((got - ref) / ref)) < 2e-6
 
 
-@pytest.mark.parametrize("variant", [32, 0, 128], ids=["register_path", "tc2_mn_major_tma", "tc3_a_in_tmem"])
-@pytest.mark.parametrize("m,i,j", [(4096, 128, 128), (5000, 256, 64), (4100, 128, 32), (1031, 384, 256)])
-def test_tc_wgrad_matches_float64(m, i, j, variant):
-    """All three weight-gradient kernels through cpb_debug_tc_wgrad: 32 = tc_wgrad.cu (register transposes, the default in the
-    VAE step), 0 = tc2_wgrad.cu (both operands MN-major by TMA tensor maps), 128 = tc3_wgrad.cu (A operand in tensor memory,
-    J <= 64 only; other shapes fall through to tc2)."""
+@pytest.mark.parametrize("m,i,j", [(4096, 128, 128), (5000, 256, 64), (4100, 128, 32), (1031, 384, 256),
+                                   (32, 128, 32), (33, 128, 64), (95, 256, 32), (127, 200, 64), (2048, 640, 32),
+                                   (3001, 1024, 64), (16384, 128, 64), (777, 136, 96)])
+def test_tc_wgrad_matches_float64(m, i, j):
+    """The weight-gradient kernel (tc_wgrad.cu) through cpb_debug_tc_wgrad: one / few / many k-blocks per split, ragged
+    reduction lengths, I not a multiple of the 128-row tile, and J = 32 / 64 / 96 / 128 / 256 (one or more 32- or 64-wide
+    column tiles)."""
     import torch
     from carla_ppo_b200 import _lib
     lib = _lib.load()
@@ -71,7 +73,7 @@ def test_tc_wgrad_matches_float64(m, i, j, variant):
     tb, ts = torch.tensor(big, device="cuda"), torch.tensor(small, device="cuda")
     out = torch.full((i, j), float("nan"), device="cuda")
     part = torch.zeros(2 * i * j, device="cuda")          # the debug entry uses 2 splits
-    _lib.check(lib.cpb_debug_tc_wgrad(tb.data_ptr(), ts.data_ptr(), out.data_ptr(), m, i, j, variant, part.data_ptr(),
+    _lib.check(lib.cpb_debug_tc_wgrad(tb.data_ptr(), ts.data_ptr(), out.data_ptr(), m, i, j, 0, part.data_ptr(),
                                       _lib.current_stream_handle()))
     torch.cuda.synchronize()
     ref = big.astype(np.float64).T @ small.astype(np.float64)
@@ -97,15 +99,13 @@ print("ERR", float(np.linalg.norm(d.cpu().numpy() - ref) / np.linalg.norm(ref)))
 
 
 def test_tc_gemm_is_bit_identical_across_cluster_sizes():
-    """With 1-CTA MMAs (CPB_TC_PAIR=0) CPB_TC_CLUSTER only changes who copies which slice of a weight tile (multicast), never
-    the arithmetic.  The CTA-pair kernel (cta_group::2, the default at cluster size 2) sums the third 3xTF32 product into a
-    different accumulator column for half of the outputs, so it is compared against float64 instead of bitwise."""
+    """CPB_TC_CLUSTER only changes who copies which slice of a weight tile (multicast), never the arithmetic."""
     hashes, errs = {}, {}
-    for cs, pair in (("1", "0"), ("2", "0"), ("4", "0"), ("2", "1")):
-        env = dict(os.environ, CPB_TC_CLUSTER=cs, CPB_TC_PAIR=pair)
+    for cs in ("1", "2", "4"):
+        env = dict(os.environ, CPB_TC_CLUSTER=cs)
         res = subprocess.run([sys.executable, "-c", _SNIPPET % ROOT], env=env, capture_output=True, text=True, timeout=300)
         assert res.returncode == 0, res.stderr[-2000:]
-        hashes[cs, pair] = [ln for ln in res.stdout.splitlines() if ln.startswith("HASH")][0]
-        errs[cs, pair] = float([ln for ln in res.stdout.splitlines() if ln.startswith("ERR")][0].split()[1])
-    assert hashes["1", "0"] == hashes["2", "0"] == hashes["4", "0"]
-    assert errs["2", "1"] < 2e-6 and errs["1", "0"] < 2e-6, errs
+        hashes[cs] = [ln for ln in res.stdout.splitlines() if ln.startswith("HASH")][0]
+        errs[cs] = float([ln for ln in res.stdout.splitlines() if ln.startswith("ERR")][0].split()[1])
+    assert hashes["1"] == hashes["2"] == hashes["4"]
+    assert errs["1"] < 2e-6, errs
