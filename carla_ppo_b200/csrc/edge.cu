@@ -28,7 +28,7 @@ constexpr int EH = 80, EW = 160, SH = 39, SW = 79, SC = 32;   // big image (pixe
 template <int CB, int EPI>   // EPI 0: bias + ReLU, 1: multiply by (mask > 0)
 __global__ void __launch_bounds__(128)
 edge_gather_kernel(const float4* __restrict__ big4, const float* __restrict__ w, const float* __restrict__ bias,
-                   const float* __restrict__ mask, float* __restrict__ small, float* __restrict__ small_lo, long long nwork,
+                   const float* __restrict__ mask, float* __restrict__ small, long long nwork,
                    float* __restrict__ cs_partial) {
     __shared__ __align__(16) float ws[16 * CB * SC];
     for (int i = threadIdx.x; i < 16 * CB * SC; i += blockDim.x) ws[i] = w[i];
@@ -104,12 +104,6 @@ edge_gather_kernel(const float4* __restrict__ big4, const float* __restrict__ w,
             }
             *reinterpret_cast<float4*>(small + o + j4 * 8) = v;
             if (EPI == 1) { csum[j4 * 4] += v.x; csum[j4 * 4 + 1] += v.y; csum[j4 * 4 + 2] += v.z; csum[j4 * 4 + 3] += v.w; }
-            if (small_lo != nullptr) {               // second TF32 operand of the tensor-core layer that consumes `small`
-                float4 l;
-                l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u); l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
-                l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u); l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
-                *reinterpret_cast<float4*>(small_lo + o + j4 * 8) = l;
-            }
         }
     }
     }   // t < nwork
@@ -224,7 +218,7 @@ edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ smal
 long long edge_gather_blocks(int batch) { return cdiv(2LL * batch * SH * ((SW + 3) / 4), 128); }
 
 int32_t launch_edge_gather(const float* big4, int cb, const float* w, const float* bias, const float* mask,
-                           float* small, float* small_lo, int batch, cudaStream_t stream, float* cs_partial) {
+                           float* small, int batch, cudaStream_t stream, float* cs_partial) {
     CPB_REQUIRE(cb == 1 || cb == 3, "edge_gather: channels must be 1 or 3");
     CPB_REQUIRE(cs_partial == nullptr || mask != nullptr, "edge_gather: column sums exist for the mask form only");
     const long long npairs = 2LL * batch * SH * ((SW + 3) / 4);      // (4-pixel group, channel half) work items
@@ -232,11 +226,11 @@ int32_t launch_edge_gather(const float* big4, int cb, const float* w, const floa
     const unsigned blocks = (unsigned)cdiv(npairs, 128);
     const float4* b4 = reinterpret_cast<const float4*>(big4);
     if (mask == nullptr) {
-        if (cb == 3) edge_gather_kernel<3, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, small_lo, npairs, nullptr);
-        else edge_gather_kernel<1, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, small_lo, npairs, nullptr);
+        if (cb == 3) edge_gather_kernel<3, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, npairs, nullptr);
+        else edge_gather_kernel<1, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, npairs, nullptr);
     } else {
-        if (cb == 3) edge_gather_kernel<3, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, small_lo, npairs, cs_partial);
-        else edge_gather_kernel<1, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, small_lo, npairs, cs_partial);
+        if (cb == 3) edge_gather_kernel<3, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, npairs, cs_partial);
+        else edge_gather_kernel<1, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, npairs, cs_partial);
     }
     CPB_LAUNCHED();
     return CPB_OK;

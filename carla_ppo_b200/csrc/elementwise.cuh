@@ -17,10 +17,9 @@ int32_t launch_deconv4_fwd(const float* small, const float* w /*[4,4,Ct,32]*/, c
 
 // 3-channel edge layers (edge.cu): big4 = float4-per-pixel padded image [B,80,160,4], small [B,39,79,32], w = TF kernel [4,4,cb,32]
 // gather: conv1 forward (mask == nullptr: bias + ReLU) / deconv4 data-gradient (mask != nullptr: ReLU mask, no bias)
-// small_lo (nullable): also write small - trunc_tf32(small), the second TF32 operand of the tensor-core consumer
 // cs_partial (optional, mask form only): [edge_gather_blocks(batch)][32] per-CTA column sums of `small` (bias gradient)
 int32_t launch_edge_gather(const float* big4, int cb, const float* w, const float* bias, const float* mask,
-                           float* small, float* small_lo, int batch, cudaStream_t stream, float* cs_partial = nullptr);
+                           float* small, int batch, cudaStream_t stream, float* cs_partial = nullptr);
 long long edge_gather_blocks(int batch);
 // weight gradient: partial[edge_wgrad_ctas(batch)][16*cb][32]; reduce with launch_reduce_partials
 int edge_wgrad_ctas(int batch);

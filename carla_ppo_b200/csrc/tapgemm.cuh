@@ -60,8 +60,6 @@ struct TapGemmParams {
     // tensor-core path only: K-major per-tap [N][C] weight blocks, pre-split into hi / lo (tc_tapgemm.cu)
     const float* wk_hi;
     const float* wk_lo;
-    const float* src_lo;  // tensor-core path only: lo plane of src (x - trunc_tf32(x)), same indexing as src
-    float* dst_lo;        // tensor-core path only: if set, the epilogue also writes the lo plane of dst (for the next layer)
     // tensor-core path only: quad-fused scatter form.  One GEMM row = one 2x2 output quad (qy, qx); the N axis is
     // (parity class, cb) = 4*quad_cb columns; cls[0] holds the union window taps (2x2 for k=4, 3x3 for k=5) and the
     // weight blocks carry zeros where a class does not use a tap.  The A tile is loaded once for all four classes.
@@ -92,7 +90,7 @@ struct TcWeightJob {
     long long count;
 };
 // rows of the N axis handled per CTA tile (also fixes the block size of the stored operand); at most 64, because each
-// consumer thread holds 1.5 x BN fp32 accumulators in registers
+// consumer thread holds 1.5 x BN fp32 accumulators plus a k-block's 32 hi / lo A-fragment registers
 __host__ __device__ constexpr int tc_bn(int N) { return N % 64 == 0 ? 64 : 32; }
 constexpr int kMaxTcWeightJobs = 12;
 struct TcWeightTable {
@@ -103,8 +101,6 @@ struct TcWeightTable {
 int32_t tc_tapgemm_init();
 bool tc_tapgemm_supported(const TapGemmParams& p);
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream);
-// lo[i] = x[i] - (x[i] with the 13 low mantissa bits cleared), count floats (multiple of 4)
-int32_t launch_lo_plane(const float* x, float* lo, long long count, cudaStream_t stream);
 int32_t launch_tc_weights(const float* params, float* dst, const TcWeightTable& table, cudaStream_t stream);
 
 }  // namespace cpb

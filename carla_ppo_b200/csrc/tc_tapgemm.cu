@@ -4,17 +4,18 @@
 //     a*b  ~=  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo ,   x_hi = x with the 13 low mantissa bits cleared,  x_lo = x - x_hi
 //
 // so that results stay fp32-accurate (relative error ~1e-6; a single TF32 pass gives ~3e-4 and would break the
-// 1e-5 parity bar).  The tensor core itself ignores the 13 low mantissa bits of a TF32 operand, so the raw fp32
-// tensor IS x_hi; x_lo is a second fp32 plane (written by the producing kernel's epilogue, or by lo_plane_kernel).
-// Operands are staged in shared memory in the wgmma canonical K-major SWIZZLE_128B layout (rows of 32 floats =
-// 128 B, 8-row groups of 1024 B, 16-byte chunk index XOR row%8) -- the only layout wgmma accepts for TF32 operands:
-//   * A (activations, gathered rows) : cp.async 16 B per thread and row from the raw tensor (hi) and its lo plane,
-//                                      zero-filled outside the image, completion counted on the stage's mbarrier;
+// 1e-5 parity bar).  Operands are staged in shared memory in the wgmma canonical K-major SWIZZLE_128B layout (rows of
+// 32 floats = 128 B, 8-row groups of 1024 B, 16-byte chunk index XOR row%8):
+//   * A (activations, gathered rows) : cp.async 16 B per thread and row of the raw fp32 tensor, zero-filled outside the
+//                                      image, completion counted on the stage's mbarrier.  Each consumer thread reads
+//                                      its register fragment of the k-block with ld.shared and splits it into hi / lo
+//                                      itself; both feed wgmma from registers (RS form), so no lo plane of an
+//                                      activation tensor ever exists in global memory;
 //   * B (weights)                    : stored by tc_weights_kernel as ready-made swizzled tile images [hi | lo]; one
 //                                      cp.async.bulk per k-block (multicast to the CTAs of a cluster).
-// Persistent, warp-specialised kernel (see tc_tapgemm_kernel): two consumer warpgroups (64 tile rows each, 8 wgmma per
-// 32-wide k-block: [main | cross] (+)= a_hi x [b_hi | b_lo] with N = 2*BN, cross += a_lo x b_hi) and four A-loader warps,
-// the first lane of which also issues the weight-tile copies.
+// Persistent, warp-specialised kernel (see tc_tapgemm_kernel): two consumer warpgroups (64 tile rows each, 12 wgmma per
+// 32-wide k-block in one commit group: main (+)= a_hi x b_hi, cross (+)= a_hi x b_lo, cross += a_lo x b_hi) and four
+// A-loader warps, the first lane of which also issues the weight-tile copies.
 //
 // Accumulation.  The tensor core adds into its fp32 accumulator with truncation, which shrinks a long running sum
 // systematically (relative bias growing linearly with K).  Two measures bring this back to fp32-FMA level:
@@ -22,8 +23,7 @@
 //     large accumulator;
 //   * wgmma accumulation only runs over chunks of 128 k (4 k-blocks); each finished chunk is added to per-thread fp32
 //     register accumulators (round-to-nearest).
-// The register accumulators feed the bias / ReLU / ReLU-mask epilogue directly; the epilogue also writes the lo plane
-// of its output when the consumer is another tensor-core layer.
+// The register accumulators feed the bias / ReLU / ReLU-mask epilogue directly.
 #include "tapgemm.cuh"
 #include "tc_common.cuh"
 
@@ -36,8 +36,8 @@ using namespace tc;
 template <int BN>
 struct TcCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
-    static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : 3;
+    static constexpr int STAGE_BYTES = A_TILE_BYTES + 2 * B_TILE_BYTES;    // raw A rows | weight image [hi | lo]
+    static constexpr int STAGES = 200 * 1024 / STAGE_BYTES;                 // BN 64: 6, BN 32: 8
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // +1024: manual 1 KB alignment
 };
 constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 register accumulators
@@ -119,12 +119,10 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 
     if (warp >= kLoaderWarp0) {
         // ================================ A loaders ================================
-        // The tensor core reads only the TF32 bits of an fp32 operand (the 13 low mantissa bits are ignored; the parity
-        // tests against float64 hold with the raw tensor as "hi"), so the raw fp32 activations ARE the "hi" operand; the "lo" operand (x - trunc(x)) comes from a
-        // plane written by lo_plane_kernel before this launch.  A tile rows are therefore copied global -> swizzled
-        // shared memory with cp.async (16 B per thread and row, zero-filled outside the image), completion is
-        // counted on the stage's mbarrier (cp.async.mbarrier.arrive.noinc) -- no registers, no split, no stores,
-        // no wait in the loader, which keeps the per-k-block instruction count of the loader warps small.
+        // The raw fp32 activation rows are copied global -> swizzled shared memory with cp.async (16 B per thread and
+        // row, zero-filled outside the image); the consumers split them into TF32 hi / lo in registers.  Completion is
+        // counted on the stage's mbarrier (cp.async.mbarrier.arrive.noinc) -- no registers, no stores, no wait in the
+        // loader, which keeps the per-k-block instruction count of the loader warps small.
         const int tl = tid - kLoaderWarp0 * 32;      // 0..127
         const int a_chunk = tl & 7;
         // row r = tl/8 + 16*i lives at (r/8)*1024 + (r%8)*128 + ((chunk ^ r%8) * 16): i only moves the 1 KB group (2 per i)
@@ -170,7 +168,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             tapbitA = 1u;
         };
         if (stA < total_st) setup_rows();
-        // copies the cursor's k-block into stage `stage` (hi = raw rows, lo = lo-plane rows) and advances the cursor
+        // copies the cursor's k-block into stage `stage` and advances the cursor
         auto issue_a = [&](uint32_t stage, uint64_t* full) {
             const uint32_t dst = stage + a_soff0;
 #pragma unroll
@@ -180,7 +178,6 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                 const uint32_t bytes = (v && !(p.debug & 4)) ? 16u : 0u;   // 0: the 16 destination bytes are zero-filled
                 if (p.debug & 2) continue;
                 asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + i * 2048), "l"(p.src + off), "r"(bytes) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + A_TILE_BYTES + i * 2048), "l"(p.src_lo + off), "r"(bytes) : "memory");
             }
             asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(full)) : "memory");
             cA += TBK; offA += TBK;
@@ -205,7 +202,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             if (p.debug & 8) { mbar_arrive(full); return; }      // timing decomposition: no weight copy
             mbar_expect_tx(full, (uint32_t)(2 * B_TILE_BYTES));
             const float* wt = p.wk_hi + 2 * clsA->taps[tapA].w_off + ((long long)st_y(stA) * kb_per_tap + cA / TBK) * (2 * BN * TBK);
-            bulk_g2s(stage + 2 * A_TILE_BYTES + (uint32_t)rank * slice, reinterpret_cast<const char*>(wt) + (size_t)rank * slice,
+            bulk_g2s(stage + A_TILE_BYTES + (uint32_t)rank * slice, reinterpret_cast<const char*>(wt) + (size_t)rank * slice,
                      slice, full, cl_mask, CS > 1);
         };
 
@@ -285,11 +282,6 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                         if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
                         if (p.mask) { o.x = mks[u].x > 0.f ? o.x : 0.f; o.y = mks[u].y > 0.f ? o.y : 0.f; }
                         *reinterpret_cast<float2*>(p.dst + offs[u]) = o;
-                        if (p.dst_lo != nullptr) {           // second TF32 operand of the consumer layer
-                            float2 hi, lo;
-                            split_tf32(o.x, hi.x, lo.x); split_tf32(o.y, hi.y, lo.y);
-                            *reinterpret_cast<float2*>(p.dst_lo + offs[u]) = lo;
-                        }
                     }
                 }
             }
@@ -303,44 +295,64 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             }
         };
 
+        // A fragment of this thread (wgmma_tf32_rs): tile rows r0 = 64*wg + 16*(warp%4) + lane/4 and r0 + 8 (the next
+        // 1 KB row group), k = lane%4 (+4) of each 8-wide k-step, i.e. 16-byte chunk 2*ks (+1) XOR r0%8 of the row.  The
+        // 8 rows a warp reads at once sit in 8 different chunks, so the 32-bit shared loads are bank-conflict free.
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const uint32_t a_row = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + (lane & 3) * 4);
+        const uint32_t a_swz = (uint32_t)((r0 & 7) << 4);
+
         int g = 0;                                   // k-blocks consumed so far (all tiles)
         for (int st = cl_id; st < total_st; st += cl_n) {
             const int nkb = p.cls[st_z(st)].ntaps * kb_per_tap;
-            int prev = -1;                           // stage whose wgmma group may still be in flight
             for (int kb = 0; kb < nkb; ++kb, ++g) {
                 const int s = g % STAGES;
                 const uint32_t stage = smem_base + s * STAGE_BYTES;
                 mbar_wait(&full_bar[s], (uint32_t)((g / STAGES) & 1));
-                // the A rows were written by cp.async (generic proxy); wgmma reads through the async proxy
-                fence_async_smem();
-                const uint64_t a_hi = make_desc(stage + wg * (A_TILE_BYTES / 2));
-                const uint64_t a_lo = make_desc(stage + A_TILE_BYTES + wg * (A_TILE_BYTES / 2));
-                const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
-                const uint64_t b_lo = make_desc(stage + 2 * A_TILE_BYTES + B_TILE_BYTES);
-                // per 8-wide k-step:  main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi
-                // (two disjoint accumulator arrays: wgmma groups writing overlapping register ranges are serialised)
+                // the k-block's A fragment, split into TF32 hi / lo: ahi[ks][2*h + v], alo[ks][2*h + v]
+                uint32_t ahi[TBK / 8][4], alo[TBK / 8][4];
+#pragma unroll
+                for (int ks = 0; ks < TBK / 8; ++ks)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int v = 0; v < 2; ++v) {
+                            float x, hi, lo;
+                            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
+                                         : "r"(stage + a_row + v * 1024 + ((uint32_t)((2 * ks + h) << 4) ^ a_swz)));
+                            split_tf32(x, hi, lo);
+                            ahi[ks][2 * h + v] = __float_as_uint(hi);
+                            alo[ks][2 * h + v] = __float_as_uint(lo);
+                        }
+                // the split stays before the fence: ptxas serialises a wgmma stream in which a non-wgmma instruction
+                // defines an A register while a group is in flight (C7513)
+#pragma unroll
+                for (int ks = 0; ks < TBK / 8; ++ks)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ahi[ks][i]), "+r"(alo[ks][i]));
+                const uint64_t b_hi = make_desc(stage + A_TILE_BYTES);
+                const uint64_t b_lo = make_desc(stage + A_TILE_BYTES + B_TILE_BYTES);
+                // per 8-wide k-step:  main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi, the whole
+                // k-block as one commit group.  Two disjoint accumulator arrays: a wgmma into a register range that only
+                // partly overlaps one in flight is serialised.  The group is retired before the next k-block's split
+                // (see above); the other consumer warpgroup's group keeps the tensor pipe busy meanwhile.
                 wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < TBK / 8; ++ks) {
                     const uint64_t adv = (uint64_t)(ks * 2);      // 32 bytes per k-step, in 16-byte units
                     const uint32_t keep = ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u;
-                    wgmma_tf32<BN>(dm, a_hi + adv, b_hi + adv, keep);
-                    wgmma_tf32<BN>(dc, a_hi + adv, b_lo + adv, keep);
-                    wgmma_tf32<BN>(dc, a_lo + adv, b_hi + adv, 1u);
+                    wgmma_tf32_rs<BN>(dm, ahi[ks], b_hi + adv, keep);
+                    wgmma_tf32_rs<BN>(dc, ahi[ks], b_lo + adv, keep);
+                    wgmma_tf32_rs<BN>(dc, alo[ks], b_hi + adv, 1u);
                 }
                 wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs<HALF>(dm);
+                fence_regs<HALF>(dc);
+                release(s);
                 if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
-                    wgmma_wait<0>();
-                    fence_regs<HALF>(dm);
-                    fence_regs<HALF>(dc);
-                    if (prev >= 0) release(prev);
-                    release(s);
-                    prev = -1;
 #pragma unroll
                     for (int i = 0; i < HALF; ++i) { acc[i] += dm[i]; acc[i] += dc[i]; }
-                } else {
-                    if (prev >= 0) { wgmma_wait<1>(); release(prev); }
-                    prev = s;
                 }
             }
             epilogue(st);
@@ -420,16 +432,6 @@ int32_t tc_init_one() {
     return CPB_OK;
 }
 
-// lo[i] = x[i] - trunc_tf32(x[i]): the second TF32 operand of an activation tensor (the first is x itself)
-__global__ void lo_plane_kernel(const float4* __restrict__ x, float4* __restrict__ lo, long long n4) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-        const float4 v = __ldg(x + i);
-        float4 h, l;
-        split_tf32(v.x, h.x, l.x); split_tf32(v.y, h.y, l.y); split_tf32(v.z, h.z, l.z); split_tf32(v.w, h.w, l.w);
-        lo[i] = l;
-    }
-}
-
 // weight preparation.  Logical operand: per tap a K-major [N][C] matrix.  Stored per tap as 2*N*C floats: for each
 // (n-tile y of BN rows, k-block kc of 32 floats) one block [hi image | lo image], each image the BN x 128-byte
 // SWIZZLE_128B shared-memory tile exactly as the tensor core reads it -- so a k-block's operand is ONE contiguous
@@ -491,7 +493,7 @@ int32_t tc_tapgemm_init() {
 
 bool tc_tapgemm_supported(const TapGemmParams& p) {
     if (p.quad && (p.N != 4 * p.quad_cb || p.nclass != 1)) return false;
-    return p.ybatch == 1 && p.C % TBK == 0 && (p.N == 32 || p.N % 64 == 0) && p.wk_hi != nullptr && p.wk_lo != nullptr && p.src_lo != nullptr;
+    return p.ybatch == 1 && p.C % TBK == 0 && (p.N == 32 || p.N % 64 == 0) && p.wk_hi != nullptr && p.wk_lo != nullptr;
 }
 
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
@@ -500,16 +502,6 @@ int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
         case 64: return tc_launch<64>(p, stream);
         default: return tc_launch<32>(p, stream);
     }
-}
-
-int32_t launch_lo_plane(const float* x, float* lo, long long count, cudaStream_t stream) {
-    CPB_REQUIRE(count % 4 == 0, "lo_plane: count must be a multiple of 4");
-    if (count == 0) return CPB_OK;
-    const long long n4 = count / 4;
-    const long long want = (n4 + 255) / 256;
-    lo_plane_kernel<<<(unsigned)(want < 132 * 16 ? want : 132 * 16), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(lo), n4);
-    CPB_LAUNCHED();
-    return CPB_OK;
 }
 
 int32_t launch_tc_weights(const float* params, float* dst, const TcWeightTable& table, cudaStream_t stream) {

@@ -59,7 +59,11 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
     const long long m_begin = (long long)blockIdx.z * p.m_per_split;
     long long m_end = m_begin + p.m_per_split;
     if (m_end > M) m_end = M;
-    const int nkb = m_end > m_begin ? (int)((m_end - m_begin + TBK - 1) / TBK) : 0;
+    // k-blocks of this split, rounded up to an even count: the loops below take two k-blocks per iteration (one per
+    // register buffer) with no branch around the second, which ptxas would otherwise treat as divergent and answer by
+    // serialising every wgmma (C7518).  The padding k-block loads nothing (positions >= len are zero-filled), and
+    // adding zero products leaves the accumulators bit-for-bit unchanged.
+    const int nkb = m_end > m_begin ? 2 * (int)((m_end - m_begin + 2 * TBK - 1) / (2 * TBK)) : 0;
 
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     if (tid == 0) {
@@ -128,7 +132,7 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         if (nkb > 1) load_b(xb1);
         for (int kb = 0; kb < nkb; kb += 2) {
             step_b(kb, xb0);
-            if (kb + 1 < nkb) step_b(kb + 1, xb1);
+            step_b(kb + 1, xb1);
         }
     } else {
         // ================================ A loaders / wgmma / partial store ================================
@@ -211,14 +215,17 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             const uint64_t a_hi = make_desc(stage + wg * (A_TILE_BYTES / 2));
             const uint64_t a_lo = make_desc(stage + A_TILE_BYTES + wg * (A_TILE_BYTES / 2));
             const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
-            // [main | cross] (+)= a_hi x [b_hi | b_lo] as ONE N = 2*BN wgmma (the images are adjacent), cross += a_lo x b_hi.
-            // ptxas serialises the wgmma of this kernel whichever way the products are split (C7518); the merged form issues
-            // two instead of three per k-step and measures faster than three disjoint N = BN products.
+            const uint64_t b_lo = make_desc(stage + 2 * A_TILE_BYTES + B_TILE_BYTES);
+            // main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi.  Each product writes exactly one of
+            // the two disjoint accumulator arrays: a wgmma into a register range that only partly overlaps an earlier
+            // one in flight (e.g. one N = 2*BN product over [main | cross]) makes ptxas serialise the stream (C7511).
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < TBK / 8; ++ks) {
                 const uint64_t adv = (uint64_t)(ks * 2);          // 32 bytes per k-step (K-major)
-                wgmma_tf32<2 * BN>(d, a_hi + adv, b_hi + adv, ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u);
+                const uint32_t keep = ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u;
+                wgmma_tf32<BN>(d, a_hi + adv, b_hi + adv, keep);
+                wgmma_tf32<BN>(d + HALF, a_hi + adv, b_lo + adv, keep);
                 wgmma_tf32<BN>(d + HALF, a_lo + adv, b_hi + adv, 1u);
             }
             wgmma_commit();
@@ -245,8 +252,9 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         if (nkb > 1) load_regs(xa1);
         for (int kb = 0; kb < nkb; kb += 2) {
             step(kb, xa0);
-            if (kb + 1 < nkb) step(kb + 1, xa1);
+            step(kb + 1, xa1);
         }
+        wgmma_wait<0>();     // a no-op (the last k-block ends a chunk); without it ptxas injects one before the stores
 
         // ---- partial[split][i][j]: tile row rho holds channel i = 4*(rho % 32) + rho / 32; accumulator column rb holds
         //      j = 4*(rb % BQ) + rb / BQ

@@ -183,8 +183,6 @@ struct VaePlan {
     float *gA, *gB, *gz, *gheads, *partial, *colsum;
     float* cs_edge;     // per-CTA column sums of deconv4's data gradient (edge_gather), [edge_gather_blocks(B)][32]
     float* frame_dsum;  // per-frame channel sums of d loss / d logits, [B][4]
-    float* lo;          // lo plane scratch for tensor-core sources whose producer does not write one (small tensors)
-    float *a1_lo, *a2_lo, *a3_lo, *b1_lo, *b2_lo, *gA_lo, *gB_lo;   // lo planes written by the producing kernels
     float* ksplit;      // partial results of the k-split dense layers: kMaxKSplit x [2, B, z]
     int64_t bytes;
     bool ok;
@@ -229,12 +227,7 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     p.a3 = a.take<float>(b * H3 * W3 * C3);
     p.a4 = a.take<float>(b * FEAT);
     p.heads = a.take<float>(2 * b * z);
-    p.lo = a.take<float>(b * FEAT);
     p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * z);
-    // lo planes (x - trunc_tf32(x)): the second TF32 operand of every tensor-core source, written by its producer
-    p.a1_lo = a.take<float>(b * H1 * W1 * C1);
-    p.a2_lo = a.take<float>(b * H2 * W2 * C2);
-    p.a3_lo = a.take<float>(b * H3 * W3 * C3);
     if (mode >= CPB_WS_FORWARD) {
         p.yp = a.take<float>(b * NPIX * 4);
         p.zbuf = a.take<float>(b * z);
@@ -243,8 +236,6 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
         p.frame_loss = a.take<float>(b);
         p.d1 = a.take<float>(b * FEAT);
         p.b1 = a.take<float>(b * H3 * W3 * C3);
-        p.b1_lo = a.take<float>(b * H3 * W3 * C3);
-        p.b2_lo = a.take<float>(b * H2 * W2 * C2);
         p.b2 = a.take<float>(b * H2 * W2 * C2);
         p.b3 = a.take<float>(b * H1 * W1 * C1);
         p.logits_p = a.take<float>(b * NPIX * 4);
@@ -252,8 +243,6 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     if (mode >= CPB_WS_TRAIN) {
         p.gA = a.take<float>(b * H1 * W1 * C1);
         p.gB = a.take<float>(b * H1 * W1 * C1);
-        p.gA_lo = a.take<float>(b * H1 * W1 * C1);
-        p.gB_lo = a.take<float>(b * H1 * W1 * C1);
         p.gz = a.take<float>(b * z);
         p.gheads = a.take<float>(2 * b * z);
         p.partial = a.take<float>(max_partial_floats(B, z));
@@ -370,22 +359,12 @@ static int tc_debug_flags() {
     return v;
 }
 
-static thread_local float* tl_lo_scratch = nullptr;   // lo plane of the current tensor-core source (VaePlan::lo)
-
-// src_lo / dst_lo: lo planes (x - trunc_tf32(x)) of the source (written by its producer; nullptr: computed here into the
-// scratch plane) and of the destination (written by the epilogue for the consuming layer; nullptr: not needed)
-static int32_t tg(const char* label, const TapGemmParams& p, cudaStream_t s, int scatter_k = 0,
-                  const float* src_lo = nullptr, float* dst_lo = nullptr) {
+static int32_t tg(const char* label, const TapGemmParams& p, cudaStream_t s, int scatter_k = 0) {
     ProfScope prof(label, s);
-    if (g_math_mode == 1 && p.wk_hi != nullptr && tl_lo_scratch != nullptr) {
+    if (g_math_mode == 1 && p.wk_hi != nullptr) {
         TapGemmParams q = scatter_k > 0 ? quad_from_scatter(p, scatter_k) : p;
         q.debug = tc_debug_flags();
-        q.src_lo = src_lo != nullptr ? src_lo : tl_lo_scratch;
-        q.dst_lo = dst_lo;
-        if (tc_tapgemm_supported(q)) {
-            if (src_lo == nullptr) CPB_TRY(launch_lo_plane(q.src, tl_lo_scratch, (long long)q.batch * q.src_img, s));
-            return launch_tc_tapgemm(q, s);
-        }
+        if (tc_tapgemm_supported(q)) return launch_tc_tapgemm(q, s);
     }
     return launch_tapgemm(p, s);
 }
@@ -501,25 +480,23 @@ static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const flo
 
 static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_config* cfg, const float* params,
                            const void* source, int32_t* flags, cudaStream_t s) {
-    tl_lo_scratch = pl.lo;
     using namespace geo;
     const int B = pl.B;
     const float sscale = cfg->source_dtype == CPB_FRAME_U8 ? 1.f / 255.f : 1.f;
     { ProfScope prof("prep_frames", s);
       CPB_TRY(launch_prep_frames(source, cfg->source_dtype, sscale, 3, (long long)B * NPIX, pl.xp, flags, 1, s)); }
     { ProfScope prof("conv1.fwd", s);
-      CPB_TRY(launch_edge_gather(pl.xp, 3, params + L.off[T_CONV1_K], params + L.off[T_CONV1_B], nullptr, pl.a1,
-                                 g_math_mode == 1 ? pl.a1_lo : nullptr, B, s)); }
+      CPB_TRY(launch_edge_gather(pl.xp, 3, params + L.off[T_CONV1_K], params + L.off[T_CONV1_B], nullptr, pl.a1, B, s)); }
     TapGemmParams p;
     p = gather_problem(pl.a1, B, H1, W1, C1, 4, params + L.off[T_CONV2_K], C2, params + L.off[T_CONV2_B], nullptr, pl.a2, 1,
                        pl.relayout + pl.rl.tc[TC_CONV2].f_hi, pl.relayout + pl.rl.tc[TC_CONV2].f_lo);
-    CPB_TRY(tg("conv2.fwd", p, s, 0, pl.a1_lo, pl.a2_lo));
+    CPB_TRY(tg("conv2.fwd", p, s, 0));
     p = gather_problem(pl.a2, B, H2, W2, C2, 4, params + L.off[T_CONV3_K], C3, params + L.off[T_CONV3_B], nullptr, pl.a3, 1,
                        pl.relayout + pl.rl.tc[TC_CONV3].f_hi, pl.relayout + pl.rl.tc[TC_CONV3].f_lo);
-    CPB_TRY(tg("conv3.fwd", p, s, 0, pl.a2_lo, pl.a3_lo));
+    CPB_TRY(tg("conv3.fwd", p, s, 0));
     p = gather_problem(pl.a3, B, H3, W3, C3, 4, params + L.off[T_CONV4_K], C4, params + L.off[T_CONV4_B], nullptr, pl.a4, 1,
                        pl.relayout + pl.rl.tc[TC_CONV4].f_hi, pl.relayout + pl.rl.tc[TC_CONV4].f_lo);
-    CPB_TRY(tg("conv4.fwd", p, s, 0, pl.a3_lo, nullptr));
+    CPB_TRY(tg("conv4.fwd", p, s, 0));
     // both heads as one y-batched dense problem: heads[0] = mean, heads[1] = logstd_sq
     p = dense_problem(pl.a4, B, FEAT, params + L.off[T_MEAN_K], pl.z, params + L.off[T_MEAN_B], nullptr, pl.heads, 0);
     p.ybatch = 2;
@@ -536,7 +513,6 @@ static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_
 // zbuf -> d1 -> b1 -> b2 -> b3 -> (logits_p and/or sigmoid)
 static int32_t run_decoder(const VaePlan& pl, const VaeLayout& L, const float* params, const float* zsrc,
                            float* logits_p, float* sigm, cudaStream_t s) {
-    tl_lo_scratch = pl.lo;
     using namespace geo;
     const int B = pl.B;
     TapGemmParams p = dense_problem(zsrc, B, pl.z, params + L.off[T_DENSE1_K], FEAT, params + L.off[T_DENSE1_B],
@@ -544,13 +520,13 @@ static int32_t run_decoder(const VaePlan& pl, const VaeLayout& L, const float* p
     CPB_TRY(tg("dense1.fwd", p, s));
     p = scatter_problem(pl.d1, B, H4, W4, C4, 4, pl.relayout + pl.rl.deconv1T, C3, params + L.off[T_DECONV1_B],
                         nullptr, pl.b1, H3, W3, 1, pl.relayout + pl.rl.tc[TC_DECONV1].t_hi, pl.relayout + pl.rl.tc[TC_DECONV1].t_lo);
-    CPB_TRY(tg("deconv1.fwd", p, s, 4, nullptr, pl.b1_lo));
+    CPB_TRY(tg("deconv1.fwd", p, s, 4));
     p = scatter_problem(pl.b1, B, H3, W3, C3, 4, pl.relayout + pl.rl.deconv2T, C2, params + L.off[T_DECONV2_B],
                         nullptr, pl.b2, H2, W2, 1, pl.relayout + pl.rl.tc[TC_DECONV2].t_hi, pl.relayout + pl.rl.tc[TC_DECONV2].t_lo);
-    CPB_TRY(tg("deconv2.fwd", p, s, 4, pl.b1_lo, pl.b2_lo));
+    CPB_TRY(tg("deconv2.fwd", p, s, 4));
     p = scatter_problem(pl.b2, B, H2, W2, C2, 5, pl.relayout + pl.rl.deconv3T, C1, params + L.off[T_DECONV3_B],
                         nullptr, pl.b3, H1, W1, 1, pl.relayout + pl.rl.tc[TC_DECONV3].t_hi, pl.relayout + pl.rl.tc[TC_DECONV3].t_lo);
-    CPB_TRY(tg("deconv3.fwd", p, s, 5, pl.b2_lo, nullptr));
+    CPB_TRY(tg("deconv3.fwd", p, s, 5));
     ProfScope prof("deconv4.fwd", s);
     return launch_deconv4_fwd(pl.b3, params + L.off[T_DECONV4_K], params + L.off[T_DECONV4_B], B, pl.ct, logits_p,
                               sigm, s);
@@ -582,7 +558,6 @@ static int32_t run_forward_loss(const VaePlan& pl, const VaeLayout& L, const cpb
 
 static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae_config* cfg, const float* params,
                             const float* eps, float* grads, cudaStream_t s) {
-    tl_lo_scratch = pl.lo;
     using namespace geo;
     const int B = pl.B;
     const int z = pl.z;
@@ -598,8 +573,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     // (recon_loss: per-frame channel sums; edge_gather: per-CTA column sums) instead of separate passes over 0.8 + 1.6 GB
     CPB_TRY(launch_colsum(pl.frame_dsum, B, 4, pl.ct, grads + L.off[T_DECONV4_B], cs, s));
     { ProfScope prof("deconv4.dgrad", s);
-      CPB_TRY(launch_edge_gather(dlog, pl.ct, params + L.off[T_DECONV4_K], nullptr, pl.b3, pl.gA,
-                                 g_math_mode == 1 ? pl.gA_lo : nullptr, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
+      CPB_TRY(launch_edge_gather(dlog, pl.ct, params + L.off[T_DECONV4_K], nullptr, pl.b3, pl.gA, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
     TapGemmParams p;
     // ---- deconv3
     CPB_TRY(run_wgrad("deconv3.wgrad", pl.gA, W1, C1, (long long)H1 * W1 * C1, 5, pl.b2, B, H2, W2, C2, 5 * 5 * C1, 5 * 5 * C1,
@@ -607,21 +581,21 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.cs_edge, edge_gather_blocks(B), C1, C1, grads + L.off[T_DECONV3_B], cs, s));
     p = gather_problem(pl.gA, B, H1, W1, C1, 5, params + L.off[T_DECONV3_K], C2, nullptr, pl.b2, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV3].f_hi, pl.relayout + pl.rl.tc[TC_DECONV3].f_lo);
-    CPB_TRY(tg("deconv3.dgrad", p, s, 0, pl.gA_lo, pl.gB_lo));   // gB = g(b2)
+    CPB_TRY(tg("deconv3.dgrad", p, s, 0));   // gB = g(b2)
     // ---- deconv2
     CPB_TRY(run_wgrad("deconv2.wgrad", pl.gB, W2, C2, (long long)H2 * W2 * C2, 4, pl.b1, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_DECONV2_K], s));
     CPB_TRY(launch_colsum(pl.gB, (long long)B * H2 * W2, C2, C2, grads + L.off[T_DECONV2_B], cs, s));
     p = gather_problem(pl.gB, B, H2, W2, C2, 4, params + L.off[T_DECONV2_K], C3, nullptr, pl.b1, pl.gA, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV2].f_hi, pl.relayout + pl.rl.tc[TC_DECONV2].f_lo);
-    CPB_TRY(tg("deconv2.dgrad", p, s, 0, pl.gB_lo, pl.gA_lo));   // gA = g(b1)
+    CPB_TRY(tg("deconv2.dgrad", p, s, 0));   // gA = g(b1)
     // ---- deconv1
     CPB_TRY(run_wgrad("deconv1.wgrad", pl.gA, W3, C3, (long long)H3 * W3 * C3, 4, pl.d1, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
                       grads + L.off[T_DECONV1_K], s));
     CPB_TRY(launch_colsum(pl.gA, (long long)B * H3 * W3, C3, C3, grads + L.off[T_DECONV1_B], cs, s));
     p = gather_problem(pl.gA, B, H3, W3, C3, 4, params + L.off[T_DECONV1_K], C4, nullptr, nullptr, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV1].f_hi, pl.relayout + pl.rl.tc[TC_DECONV1].f_lo);
-    CPB_TRY(tg("deconv1.dgrad", p, s, 0, pl.gA_lo, nullptr));                                   // gB = g(d1) [B, 6144]
+    CPB_TRY(tg("deconv1.dgrad", p, s, 0));                                   // gB = g(d1) [B, 6144]
     // ---- dense1
     CPB_TRY(run_dense_wgrad("dense1.wgrad", pl.zbuf, z, pl.gB, B, FEAT, pl.partial, grads + L.off[T_DENSE1_K], s));
     CPB_TRY(launch_colsum(pl.gB, B, FEAT, FEAT, grads + L.off[T_DENSE1_B], cs, s));
@@ -651,21 +625,21 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.gA, (long long)B * H4 * W4, C4, C4, grads + L.off[T_CONV4_B], cs, s));
     p = scatter_problem(pl.gA, B, H4, W4, C4, 4, pl.relayout + pl.rl.conv4T, C3, nullptr, pl.a3, pl.gB, H3, W3, 0,
                         pl.relayout + pl.rl.tc[TC_CONV4].t_hi, pl.relayout + pl.rl.tc[TC_CONV4].t_lo);
-    CPB_TRY(tg("conv4.dgrad", p, s, 4, nullptr, pl.gB_lo));   // gB = g(a3)
+    CPB_TRY(tg("conv4.dgrad", p, s, 4));   // gB = g(a3)
     // ---- conv3
     CPB_TRY(run_wgrad("conv3.wgrad", pl.a2, W2, C2, (long long)H2 * W2 * C2, 4, pl.gB, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_CONV3_K], s));
     CPB_TRY(launch_colsum(pl.gB, (long long)B * H3 * W3, C3, C3, grads + L.off[T_CONV3_B], cs, s));
     p = scatter_problem(pl.gB, B, H3, W3, C3, 4, pl.relayout + pl.rl.conv3T, C2, nullptr, pl.a2, pl.gA, H2, W2, 0,
                         pl.relayout + pl.rl.tc[TC_CONV3].t_hi, pl.relayout + pl.rl.tc[TC_CONV3].t_lo);
-    CPB_TRY(tg("conv3.dgrad", p, s, 4, pl.gB_lo, pl.gA_lo));   // gA = g(a2)
+    CPB_TRY(tg("conv3.dgrad", p, s, 4));   // gA = g(a2)
     // ---- conv2
     CPB_TRY(run_wgrad("conv2.wgrad", pl.a1, W1, C1, (long long)H1 * W1 * C1, 4, pl.gA, B, H2, W2, C2, 16 * C1, 16 * C1, pl.partial,
                       grads + L.off[T_CONV2_K], s));
     CPB_TRY(launch_colsum(pl.gA, (long long)B * H2 * W2, C2, C2, grads + L.off[T_CONV2_B], cs, s));
     p = scatter_problem(pl.gA, B, H2, W2, C2, 4, pl.relayout + pl.rl.conv2T, C1, nullptr, pl.a1, pl.gB, H1, W1, 0,
                         pl.relayout + pl.rl.tc[TC_CONV2].t_hi, pl.relayout + pl.rl.tc[TC_CONV2].t_lo);
-    CPB_TRY(tg("conv2.dgrad", p, s, 4, pl.gA_lo, nullptr));   // gB = g(a1)
+    CPB_TRY(tg("conv2.dgrad", p, s, 4));   // gB = g(a1)
     // ---- conv1 (its input gradient is never used: the reference computes and discards it)
     { ProfScope prof("conv1.wgrad", s);
       CPB_TRY(launch_edge_wgrad(pl.xp, 3, pl.gB, B, pl.partial, s));
@@ -886,7 +860,8 @@ int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t ct, int32_t z, int32
     return n;
 }
 
-/* debug: D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core tap-GEMM (dense, one tap).  scratch: 2*N*K + M*K floats. */
+/* debug: D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core tap-GEMM (dense, one tap).  scratch: at least 2*N*K floats
+   (the weight image); callers sized for an older layout pass 2*N*K + M*K, of which the rest goes unused. */
 int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, int32_t n, int32_t k, float* scratch, void* stream) {
     CPB_TRY(ensure_init());
     cudaStream_t s = (cudaStream_t)stream;
@@ -898,9 +873,6 @@ int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, 
     p.wk_hi = scratch; p.wk_lo = scratch + (long long)n * k;
     p.debug = tc_debug_flags();
     CPB_TRY(launch_tc_weights(bt, scratch, w, s));
-    float* lo = scratch + 2LL * n * k;
-    p.src_lo = lo;
-    CPB_TRY(launch_lo_plane(a, lo, (long long)m * k, s));
     return launch_tc_tapgemm(p, s);
 }
 

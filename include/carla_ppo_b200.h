@@ -255,7 +255,7 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
 int32_t cpb_set_math_mode(int32_t mode);
 /* Debug / test hooks (not part of the reference-facing surface): workspace buffer offsets in bytes for
  * [xp,a1,a2,a3,a4,heads,z,d1,b1,b2,b3,logits_p,gA,gB,frame_loss,kl_rows] (-1 = absent in that mode), and a dense
- * D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: 2*N*K + M*K floats). */
+ * D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
 int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t target_channels, int32_t z_dim, int32_t mode,
                                      int64_t* offsets, int32_t capacity);
 int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int32_t m, int32_t i, int32_t j,
