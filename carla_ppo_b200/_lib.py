@@ -15,6 +15,8 @@ LIB_PATH = os.path.join(_HERE, "libcarla_ppo_b200.so")
 LOSS_MSE, LOSS_BCE, LOSS_BCE_V2 = 0, 1, 2
 FRAME_F32, FRAME_U8 = 0, 1
 WS_ENCODE, WS_FORWARD, WS_TRAIN = 0, 1, 2
+# cpb_set_math_mode: fp32 SIMT, 3xTF32 wgmma (default, fp32-accurate), one TF32 wgmma pass (not fp32-accurate)
+MATH_SIMT, MATH_3XTF32, MATH_TF32 = 0, 1, 2
 
 
 class CpbError(RuntimeError):

@@ -68,6 +68,7 @@ struct TapGemmParams {
     int quad_lcb;         // log2(quad_cb), set by the launcher
     int cluster;          // tensor-core path: CTAs per cluster (set by the launcher)
     int debug;            // tensor-core path: timing decomposition (CPB_TC_DEBUG): 2 no A copies, 4 A copies zero-fill only, 8 no weight copies
+    int passes;           // tensor-core path: 3 (3xTF32) or 1 (one TF32 pass; weights from jobs with round_nearest set)
     TapClass cls[4];
 };
 
@@ -79,7 +80,7 @@ int tapgemm_pick_ksplit(int rows, int N, int ybatch, int K);
 // One-time opt-in for >48 KB dynamic shared memory (called from the API layer).
 int32_t tapgemm_init();
 
-// ---- tensor-core (wgmma, 3xTF32) variant of the same contraction -------------------------------------------------
+// ---- tensor-core (wgmma, 3xTF32 or a single TF32 pass) variant of the same contraction -----------------------------
 struct TcWeightJob {
     long long src_off;          // float offset of the TF kernel [k,k,Cb,Cs] in the parameter buffer
     long long dst_hi, dst_lo;   // float offset of the operand (2 * taps * N * C floats, hi and lo interleaved by block) / unused
@@ -88,6 +89,7 @@ struct TcWeightJob {
     int k, cb, cs;
     int N, C;                   // logical rows / reduction length per tap
     long long count;
+    int round_nearest;          // 0: hi = x truncated to TF32 (3xTF32 split); 1: hi = x rounded to nearest (single pass)
 };
 // rows of the N axis handled per CTA tile (also fixes the block size of the stored operand); at most 64, because each
 // consumer thread holds 1.5 x BN fp32 accumulators plus a k-block's 32 hi / lo A-fragment registers

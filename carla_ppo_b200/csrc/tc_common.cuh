@@ -119,5 +119,13 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     lo = x - hi;
 }
 
+// x rounded to the nearest TF32 value (ties away from zero) -- the single-pass operand.  The tensor core itself only
+// reads the top 19 bits of an fp32 operand, i.e. truncates, which would make every product slightly too small.
+__device__ __forceinline__ uint32_t round_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+
 }  // namespace tc
 }  // namespace cpb

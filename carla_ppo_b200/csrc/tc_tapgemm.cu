@@ -24,6 +24,11 @@
 //   * wgmma accumulation only runs over chunks of 128 k (4 k-blocks); each finished chunk is added to per-thread fp32
 //     register accumulators (round-to-nearest).
 // The register accumulators feed the bias / ReLU / ReLU-mask epilogue directly.
+//
+// Single-pass variant (PASSES = 1, math mode 2): a*b ~= rna(a) * rna(b), both operands rounded to the nearest TF32
+// value (the A fragment in registers, the weights by tc_weights_kernel), ONE wgmma per 8-wide k-step into the chunk
+// accumulator, no cross terms; a stage holds A + the hi weight image only.  Relative error ~3e-4 per product, unbiased;
+// the chunked accumulation into fp32 registers is the same as above.
 #include "tapgemm.cuh"
 #include "tc_common.cuh"
 
@@ -33,11 +38,12 @@ namespace {
 
 using namespace tc;
 
-template <int BN>
+template <int BN, int PASSES>
 struct TcCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
-    static constexpr int STAGE_BYTES = A_TILE_BYTES + 2 * B_TILE_BYTES;    // raw A rows | weight image [hi | lo]
-    static constexpr int STAGES = 200 * 1024 / STAGE_BYTES;                 // BN 64: 6, BN 32: 8
+    static constexpr int B_IMAGES = PASSES == 3 ? 2 : 1;                    // weight images per k-block: [hi | lo] or [hi]
+    static constexpr int STAGE_BYTES = A_TILE_BYTES + B_IMAGES * B_TILE_BYTES;   // raw A rows | weight image(s)
+    static constexpr int STAGES = 200 * 1024 / STAGE_BYTES;                 // 3 passes: BN 64: 6, BN 32: 8; 1 pass: 8, 10
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // +1024: manual 1 KB alignment
 };
 constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 register accumulators
@@ -49,7 +55,7 @@ constexpr int kLoaderThreads = kLoaderWarps * 32;
 constexpr int kTcThreads = 384;                       // a multiple of 4 warps: registers are granted per 4 warps
 
 int g_tc_cluster = 1;         // CTAs per cluster = multicast width of the weight tiles (CPB_TC_CLUSTER, 1/2/4/8)
-int g_tc_clusters[2] = {0, 0};   // co-resident clusters of the persistent grid, per BN instantiation (32/64)
+int g_tc_clusters[2][2] = {{0, 0}, {0, 0}};   // co-resident clusters of the persistent grid, per instantiation [passes 3/1][BN 32/64]
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
@@ -79,10 +85,11 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 // multicasts the slice into every CTA's stage, so a stage is free again only when the consumers of EVERY CTA of the
 // cluster are done with it (each consumer warp arrives on the stage's empty barrier in all CTAs).
 // The k-blocks of all super-tiles of a cluster form one stream through the stage ring; a chunk never spans two tiles.
-template <int BN>
+template <int BN, int PASSES>
 __global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
 tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, const int total_st) {
-    using Cfg = TcCfg<BN>;
+    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or a single TF32 pass");
+    using Cfg = TcCfg<BN, PASSES>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int B_TILE_BYTES = Cfg::B_TILE_BYTES;
     constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -195,12 +202,14 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         };
 
         // weight tile of the cursor's k-block.  Global layout (tc_weights_kernel): per tap 2*N*C floats; inside, block
-        // (n-tile y, k-block kc) holds the swizzled shared-memory image [hi: BN rows x 128 B | lo: BN rows x 128 B];
-        // this CTA copies slice `rank` of it, multicast to every CTA of the cluster
-        const uint32_t slice = (uint32_t)(2 * B_TILE_BYTES / CS);
+        // (n-tile y, k-block kc) holds the swizzled shared-memory image [hi: BN rows x 128 B | lo: BN rows x 128 B]
+        // (the single pass copies the hi image only); this CTA copies slice `rank` of it, multicast to every CTA of
+        // the cluster
+        constexpr int B_BYTES = Cfg::B_IMAGES * B_TILE_BYTES;
+        const uint32_t slice = (uint32_t)(B_BYTES / CS);
         auto issue_b = [&](uint32_t stage, uint64_t* full) {
             if (p.debug & 8) { mbar_arrive(full); return; }      // timing decomposition: no weight copy
-            mbar_expect_tx(full, (uint32_t)(2 * B_TILE_BYTES));
+            mbar_expect_tx(full, (uint32_t)B_BYTES);
             const float* wt = p.wk_hi + 2 * clsA->taps[tapA].w_off + ((long long)st_y(stA) * kb_per_tap + cA / TBK) * (2 * BN * TBK);
             bulk_g2s(stage + A_TILE_BYTES + (uint32_t)rank * slice, reinterpret_cast<const char*>(wt) + (size_t)rank * slice,
                      slice, full, cl_mask, CS > 1);
@@ -221,7 +230,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
         const int wg = warp >> 2;
         float acc[HALF];                             // fp32 register accumulators of the tile (main + cross)
-        float dm[HALF], dc[HALF];                    // chunk accumulators of the main and the cross terms
+        float dm[HALF], dc[HALF];                    // chunk accumulators of the main and the cross terms (3 passes)
 #pragma unroll
         for (int i = 0; i < HALF; ++i) { acc[i] = 0.f; dm[i] = 0.f; dc[i] = 0.f; }
 
@@ -310,6 +319,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                 const uint32_t stage = smem_base + s * STAGE_BYTES;
                 mbar_wait(&full_bar[s], (uint32_t)((g / STAGES) & 1));
                 // the k-block's A fragment, split into TF32 hi / lo: ahi[ks][2*h + v], alo[ks][2*h + v]
+                // (single pass: ahi = the fragment rounded to nearest TF32, no alo)
                 uint32_t ahi[TBK / 8][4], alo[TBK / 8][4];
 #pragma unroll
                 for (int ks = 0; ks < TBK / 8; ++ks)
@@ -317,42 +327,56 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                     for (int h = 0; h < 2; ++h)
 #pragma unroll
                         for (int v = 0; v < 2; ++v) {
-                            float x, hi, lo;
+                            float x;
                             asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
                                          : "r"(stage + a_row + v * 1024 + ((uint32_t)((2 * ks + h) << 4) ^ a_swz)));
-                            split_tf32(x, hi, lo);
-                            ahi[ks][2 * h + v] = __float_as_uint(hi);
-                            alo[ks][2 * h + v] = __float_as_uint(lo);
+                            if constexpr (PASSES == 3) {
+                                float hi, lo;
+                                split_tf32(x, hi, lo);
+                                ahi[ks][2 * h + v] = __float_as_uint(hi);
+                                alo[ks][2 * h + v] = __float_as_uint(lo);
+                            } else {
+                                ahi[ks][2 * h + v] = round_tf32(x);
+                            }
                         }
                 // the split stays before the fence: ptxas serialises a wgmma stream in which a non-wgmma instruction
                 // defines an A register while a group is in flight (C7513)
 #pragma unroll
                 for (int ks = 0; ks < TBK / 8; ++ks)
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ahi[ks][i]), "+r"(alo[ks][i]));
+                    for (int i = 0; i < 4; ++i) {
+                        if constexpr (PASSES == 3) asm volatile("" : "+r"(ahi[ks][i]), "+r"(alo[ks][i]));
+                        else asm volatile("" : "+r"(ahi[ks][i]));
+                    }
                 const uint64_t b_hi = make_desc(stage + A_TILE_BYTES);
                 const uint64_t b_lo = make_desc(stage + A_TILE_BYTES + B_TILE_BYTES);
                 // per 8-wide k-step:  main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi, the whole
-                // k-block as one commit group.  Two disjoint accumulator arrays: a wgmma into a register range that only
-                // partly overlaps one in flight is serialised.  The group is retired before the next k-block's split
-                // (see above); the other consumer warpgroup's group keeps the tensor pipe busy meanwhile.
+                // k-block as one commit group (single pass: main (+)= a x b only).  Two disjoint accumulator arrays: a
+                // wgmma into a register range that only partly overlaps one in flight is serialised.  The group is
+                // retired before the next k-block's split (see above); the other consumer warpgroup's group keeps the
+                // tensor pipe busy meanwhile.
                 wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < TBK / 8; ++ks) {
                     const uint64_t adv = (uint64_t)(ks * 2);      // 32 bytes per k-step, in 16-byte units
                     const uint32_t keep = ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u;
                     wgmma_tf32_rs<BN>(dm, ahi[ks], b_hi + adv, keep);
-                    wgmma_tf32_rs<BN>(dc, ahi[ks], b_lo + adv, keep);
-                    wgmma_tf32_rs<BN>(dc, alo[ks], b_hi + adv, 1u);
+                    if constexpr (PASSES == 3) {
+                        wgmma_tf32_rs<BN>(dc, ahi[ks], b_lo + adv, keep);
+                        wgmma_tf32_rs<BN>(dc, alo[ks], b_hi + adv, 1u);
+                    }
                 }
                 wgmma_commit();
                 wgmma_wait<0>();
                 fence_regs<HALF>(dm);
-                fence_regs<HALF>(dc);
+                if constexpr (PASSES == 3) fence_regs<HALF>(dc);
                 release(s);
                 if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
 #pragma unroll
-                    for (int i = 0; i < HALF; ++i) { acc[i] += dm[i]; acc[i] += dc[i]; }
+                    for (int i = 0; i < HALF; ++i) {
+                        acc[i] += dm[i];
+                        if constexpr (PASSES == 3) acc[i] += dc[i];
+                    }
                 }
             }
             epilogue(st);
@@ -365,25 +389,26 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 }
 
 constexpr int tc_bn_slot(int BN) { return BN == 64 ? 1 : 0; }
+constexpr int tc_passes_slot(int PASSES) { return PASSES == 1 ? 1 : 0; }
 
-template <int BN>
+template <int BN, int PASSES>
 int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_st, unsigned grid, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = TcCfg<BN>::SMEM_BYTES;
+    cfg.dynamicSmemBytes = TcCfg<BN, PASSES>::SMEM_BYTES;
     cfg.stream = stream;
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = (unsigned)p.cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
-    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN>, p, mgroups, total_st));
+    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN, PASSES>, p, mgroups, total_st));
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
-template <int BN>
+template <int BN, int PASSES>
 int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     long long max_m = 0;
     for (int c = 0; c < p0.nclass; ++c) {
@@ -396,7 +421,7 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     const long long mtiles = (max_m + TBM - 1) / TBM;
     const long long mgroups = (mtiles + p.cluster - 1) / p.cluster;
     const long long total_st = mgroups * (p.N / BN) * p.nclass;
-    const int resident = g_tc_clusters[tc_bn_slot(BN)];
+    const int resident = g_tc_clusters[tc_passes_slot(PASSES)][tc_bn_slot(BN)];
     CPB_REQUIRE(total_st < (1ll << 30) && resident > 0, "tc_tapgemm: bad tile count");
     CPB_REQUIRE((long long)p.batch * p.src_img < (1ll << 31) && (long long)p.batch * p.dst_img < (1ll << 31),
                 "tc_tapgemm: tensors too large for 32-bit row offsets");
@@ -407,14 +432,14 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
         while ((1 << p.quad_lcb) < p.quad_cb) ++p.quad_lcb;
     }
     const unsigned grid = (unsigned)((total_st < resident ? total_st : resident) * p.cluster);
-    return tc_launch_t<BN>(p, (int)mgroups, (int)total_st, grid, stream);
+    return tc_launch_t<BN, PASSES>(p, (int)mgroups, (int)total_st, grid, stream);
 }
 
-template <int BN>
+template <int BN, int PASSES>
 int32_t tc_init_one() {
-    using Cfg = TcCfg<BN>;
-    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    using Cfg = TcCfg<BN, PASSES>;
+    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     // how many clusters of this kernel are co-resident (GPC boundaries can strand SMs for cluster sizes > 1)
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -426,16 +451,17 @@ int32_t tc_init_one() {
     attr.val.clusterDim.x = (unsigned)g_tc_cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
     int n = 0;
-    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN>, &cfg));
+    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN, PASSES>, &cfg));
     CPB_REQUIRE(n > 0, "tc_tapgemm: no resident cluster of %d CTAs possible", g_tc_cluster);
-    g_tc_clusters[tc_bn_slot(BN)] = n;
+    g_tc_clusters[tc_passes_slot(PASSES)][tc_bn_slot(BN)] = n;
     return CPB_OK;
 }
 
 // weight preparation.  Logical operand: per tap a K-major [N][C] matrix.  Stored per tap as 2*N*C floats: for each
 // (n-tile y of BN rows, k-block kc of 32 floats) one block [hi image | lo image], each image the BN x 128-byte
 // SWIZZLE_128B shared-memory tile exactly as the tensor core reads it -- so a k-block's operand is ONE contiguous
-// 2*BN*128-byte bulk copy (tc_tapgemm_kernel, weight-tile producer).
+// 2*BN*128-byte bulk copy (tc_tapgemm_kernel, weight-tile producer).  job.round_nearest: hi = x rounded to the nearest
+// TF32 value (the single-pass operand; lo = x - hi is written but not read) instead of x truncated.
 __global__ void tc_weights_kernel(const float* __restrict__ params, float* __restrict__ dst, const __grid_constant__ TcWeightTable t) {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= t.total) return;
@@ -475,7 +501,7 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
     const int nn = n % BN, cc = c % TBK;
     const long long block = ((long long)tap * (job.N / BN) + n / BN) * (job.C / TBK) + c / TBK;
     const long long at = job.dst_hi + block * (2 * BN * TBK) + (nn >> 3) * 256 + (nn & 7) * 32 + ((((cc >> 2) ^ (nn & 7))) << 2) + (cc & 3);
-    const float hi = __uint_as_float(__float_as_uint(x) & 0xffffe000u);
+    const float hi = job.round_nearest ? __uint_as_float(round_tf32(x)) : __uint_as_float(__float_as_uint(x) & 0xffffe000u);
     dst[at] = hi;
     dst[at + BN * TBK] = x - hi;
 }
@@ -486,8 +512,10 @@ int32_t tc_tapgemm_init() {
     const char* e = getenv("CPB_TC_CLUSTER");
     g_tc_cluster = e ? atoi(e) : 2;
     CPB_REQUIRE(g_tc_cluster == 1 || g_tc_cluster == 2 || g_tc_cluster == 4 || g_tc_cluster == 8, "CPB_TC_CLUSTER must be 1, 2, 4 or 8");
-    CPB_TRY(tc_init_one<32>());
-    CPB_TRY(tc_init_one<64>());
+    CPB_TRY((tc_init_one<32, 3>()));
+    CPB_TRY((tc_init_one<64, 3>()));
+    CPB_TRY((tc_init_one<32, 1>()));
+    CPB_TRY((tc_init_one<64, 1>()));
     return CPB_OK;
 }
 
@@ -498,10 +526,9 @@ bool tc_tapgemm_supported(const TapGemmParams& p) {
 
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
     CPB_REQUIRE(tc_tapgemm_supported(p), "tc_tapgemm: unsupported problem (C=%d, N=%d)", p.C, p.N);
-    switch (tc_bn(p.N)) {
-        case 64: return tc_launch<64>(p, stream);
-        default: return tc_launch<32>(p, stream);
-    }
+    CPB_REQUIRE(p.passes == 3 || p.passes == 1, "tc_tapgemm: passes must be 3 or 1, got %d", p.passes);
+    if (p.passes == 1) return tc_bn(p.N) == 64 ? tc_launch<64, 1>(p, stream) : tc_launch<32, 1>(p, stream);
+    return tc_bn(p.N) == 64 ? tc_launch<64, 3>(p, stream) : tc_launch<32, 3>(p, stream);
 }
 
 int32_t launch_tc_weights(const float* params, float* dst, const TcWeightTable& table, cudaStream_t stream) {

@@ -15,6 +15,8 @@
 // 3xTF32 products, the separate cross-term registers and the chunked accumulation into fp32 register accumulators are
 // those of tc_tapgemm.cu.  Each (i-tile, j-tile, split) CTA of the single split-K wave writes its partial [128 x BN]
 // block; reduce_partials() sums the splits in a fixed order (deterministic).
+// Single-pass variant (PASSES = 1, math mode 2): the loaders round both operands to the nearest TF32 value and store
+// the hi tiles only (a stage is A + B), one wgmma per 8-wide k-step into the chunk accumulator, no cross terms.
 #include "tc_common.cuh"
 #include "wgrad.cuh"
 
@@ -26,10 +28,12 @@ using namespace tc;
 
 constexpr int CHUNK_KB = 4;
 
-template <int BN>
+template <int BN, int PASSES>
 struct TcWgCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
-    static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+    static constexpr int PARTS = PASSES == 3 ? 2 : 1;                // tiles per operand: [hi | lo] or [hi]
+    static constexpr int B_OFF = PARTS * A_TILE_BYTES;               // stage layout: A tile(s) | B tile(s)
+    static constexpr int STAGE_BYTES = PARTS * A_TILE_BYTES + PARTS * B_TILE_BYTES;
     static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : 3;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
 };
@@ -38,12 +42,14 @@ constexpr int kWgLoaderWarps = 8;                         // warps 0-7: A (big) 
 constexpr int kWgBWarps = 4;                              // warps 8-11: B (small) loaders
 constexpr int kWgThreads = (kWgLoaderWarps + kWgBWarps) * 32;
 
-template <int BN>
+template <int BN, int PASSES>
 __global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
 tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
-    using Cfg = TcWgCfg<BN>;
+    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or a single TF32 pass");
+    using Cfg = TcWgCfg<BN, PASSES>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int B_TILE_BYTES = Cfg::B_TILE_BYTES;
+    constexpr int B_OFF = Cfg::B_OFF;
     constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
 
     extern __shared__ uint8_t smem_raw[];
@@ -75,16 +81,22 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
     constexpr int BQ = BN / 4;                       // channel groups of the B tile
     const int len = (int)(m_end - m_begin);          // reduction positions of this split
     // 4x4 register transpose + split + store: x[j] = 4 channels at position j  ->  one chunk per channel
+    // (single pass: rounded to nearest TF32, hi tile only)
     auto store_t = [&](uint32_t tile_hi, uint32_t tile_lo, const float4* x, const uint32_t* so) {
         const float xs[4][4] = {{x[0].x, x[1].x, x[2].x, x[3].x}, {x[0].y, x[1].y, x[2].y, x[3].y},
                                 {x[0].z, x[1].z, x[2].z, x[3].z}, {x[0].w, x[1].w, x[2].w, x[3].w}};
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
-            float4 hi, lo;
-            split_tf32(xs[c][0], hi.x, lo.x); split_tf32(xs[c][1], hi.y, lo.y);
-            split_tf32(xs[c][2], hi.z, lo.z); split_tf32(xs[c][3], hi.w, lo.w);
-            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(tile_hi + so[c]), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
-            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(tile_lo + so[c]), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
+            if constexpr (PASSES == 3) {
+                float4 hi, lo;
+                split_tf32(xs[c][0], hi.x, lo.x); split_tf32(xs[c][1], hi.y, lo.y);
+                split_tf32(xs[c][2], hi.z, lo.z); split_tf32(xs[c][3], hi.w, lo.w);
+                asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(tile_hi + so[c]), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
+                asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(tile_lo + so[c]), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
+            } else {
+                asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(tile_hi + so[c]), "r"(round_tf32(xs[c][0])),
+                             "r"(round_tf32(xs[c][1])), "r"(round_tf32(xs[c][2])), "r"(round_tf32(xs[c][3])) : "memory");
+            }
         }
     };
 
@@ -119,7 +131,7 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         int sS = 0;
         uint32_t phS = 1;
         auto step_b = [&](int kb, float4* xb) {
-            const uint32_t stage = smem_base + sS * STAGE_BYTES + 2 * A_TILE_BYTES;
+            const uint32_t stage = smem_base + sS * STAGE_BYTES + B_OFF;
             mbar_wait(&empty_bar[sS], phS);
             if (active) store_t(stage, stage + B_TILE_BYTES, xb, soffb);
             fence_async_smem();
@@ -189,12 +201,13 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
 
         constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
         const int wg = warp >> 2;                    // warpgroup: tile rows [64*wg, 64*wg + 64)
+        constexpr int DN = PASSES == 3 ? BN : HALF;
         float acc[HALF];                             // fp32 register accumulators (main + cross)
-        float d[BN];                                 // chunk accumulators: [main (HALF) | cross (HALF)]
+        float d[DN];                                 // chunk accumulators: [main (HALF) | cross (HALF, 3 passes only)]
 #pragma unroll
         for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
 #pragma unroll
-        for (int i = 0; i < BN; ++i) d[i] = 0.f;
+        for (int i = 0; i < DN; ++i) d[i] = 0.f;
 
         // two k-blocks of operand rows are in flight per thread (register double buffer): with one, every
         // k-block costs a full L2 round trip per warp
@@ -214,31 +227,37 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             mbar_wait(&full_bar[s], (uint32_t)((kb / STAGES) & 1));
             const uint64_t a_hi = make_desc(stage + wg * (A_TILE_BYTES / 2));
             const uint64_t a_lo = make_desc(stage + A_TILE_BYTES + wg * (A_TILE_BYTES / 2));
-            const uint64_t b_hi = make_desc(stage + 2 * A_TILE_BYTES);
-            const uint64_t b_lo = make_desc(stage + 2 * A_TILE_BYTES + B_TILE_BYTES);
-            // main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi.  Each product writes exactly one of
-            // the two disjoint accumulator arrays: a wgmma into a register range that only partly overlaps an earlier
-            // one in flight (e.g. one N = 2*BN product over [main | cross]) makes ptxas serialise the stream (C7511).
+            const uint64_t b_hi = make_desc(stage + B_OFF);
+            const uint64_t b_lo = make_desc(stage + B_OFF + B_TILE_BYTES);
+            // main (+)= a_hi x b_hi,  cross (+)= a_hi x b_lo,  cross += a_lo x b_hi (single pass: main (+)= a x b only).
+            // Each product writes exactly one of the two disjoint accumulator arrays: a wgmma into a register range
+            // that only partly overlaps an earlier one in flight (e.g. one N = 2*BN product over [main | cross]) makes
+            // ptxas serialise the stream (C7511).
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < TBK / 8; ++ks) {
                 const uint64_t adv = (uint64_t)(ks * 2);          // 32 bytes per k-step (K-major)
                 const uint32_t keep = ((kb % CHUNK_KB) | ks) != 0 ? 1u : 0u;
                 wgmma_tf32<BN>(d, a_hi + adv, b_hi + adv, keep);
-                wgmma_tf32<BN>(d + HALF, a_hi + adv, b_lo + adv, keep);
-                wgmma_tf32<BN>(d + HALF, a_lo + adv, b_hi + adv, 1u);
+                if constexpr (PASSES == 3) {
+                    wgmma_tf32<BN>(d + HALF, a_hi + adv, b_lo + adv, keep);
+                    wgmma_tf32<BN>(d + HALF, a_lo + adv, b_hi + adv, 1u);
+                }
             }
             wgmma_commit();
             if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
                 wgmma_wait<0>();
-                fence_regs<BN>(d);
+                fence_regs<DN>(d);
                 if (lane == 0) {
                     if (prev >= 0) mbar_arrive(&empty_bar[prev]);
                     mbar_arrive(&empty_bar[s]);
                 }
                 prev = -1;
 #pragma unroll
-                for (int i = 0; i < HALF; ++i) { acc[i] += d[i]; acc[i] += d[HALF + i]; }
+                for (int i = 0; i < HALF; ++i) {
+                    acc[i] += d[i];
+                    if constexpr (PASSES == 3) acc[i] += d[HALF + i];
+                }
             } else {
                 if (prev >= 0) {
                     wgmma_wait<1>();
@@ -274,17 +293,17 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         }
     }
 }
-template <int BN>
+template <int BN, int PASSES>
 int32_t tc_wg_launch(const WgradParams& p, cudaStream_t stream) {
     dim3 grid((unsigned)cdiv(p.I, TBM), (unsigned)(p.J / BN), (unsigned)p.splits);
-    tc_wgrad_kernel<BN><<<grid, kWgThreads, TcWgCfg<BN>::SMEM_BYTES, stream>>>(p);
+    tc_wgrad_kernel<BN, PASSES><<<grid, kWgThreads, TcWgCfg<BN, PASSES>::SMEM_BYTES, stream>>>(p);
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
-template <int BN>
+template <int BN, int PASSES>
 int32_t tc_wg_init_one() {
-    CPB_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcWgCfg<BN>::SMEM_BYTES));
+    CPB_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<BN, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcWgCfg<BN, PASSES>::SMEM_BYTES));
     return CPB_OK;
 }
 
@@ -293,8 +312,10 @@ int tc_wg_bn(int J) { return J % 64 == 0 ? 64 : 32; }   // at most 64: see tc_bn
 }  // namespace
 
 int32_t tc_wgrad_init() {
-    CPB_TRY(tc_wg_init_one<32>());
-    CPB_TRY(tc_wg_init_one<64>());
+    CPB_TRY((tc_wg_init_one<32, 3>()));
+    CPB_TRY((tc_wg_init_one<64, 3>()));
+    CPB_TRY((tc_wg_init_one<32, 1>()));
+    CPB_TRY((tc_wg_init_one<64, 1>()));
     return CPB_OK;
 }
 
@@ -314,10 +335,9 @@ int32_t launch_tc_wgrad(const WgradParams& p, cudaStream_t stream) {
     CPB_REQUIRE(p.m_per_split % TBK == 0 && p.splits >= 1, "tc_wgrad: bad split");
     CPB_REQUIRE((long long)p.batch * p.big_img < (1ll << 31) && p.m_per_split < (1ll << 30) && p.Wo < 65536 && p.Ho * p.Wo < 65536,
                 "tc_wgrad: tensor too large for 32-bit offsets");
-    switch (tc_wg_bn(p.J)) {
-        case 64: return tc_wg_launch<64>(p, stream);
-        default: return tc_wg_launch<32>(p, stream);
-    }
+    CPB_REQUIRE(p.passes == 3 || p.passes == 1, "tc_wgrad: passes must be 3 or 1, got %d", p.passes);
+    if (p.passes == 1) return tc_wg_bn(p.J) == 64 ? tc_wg_launch<64, 1>(p, stream) : tc_wg_launch<32, 1>(p, stream);
+    return tc_wg_bn(p.J) == 64 ? tc_wg_launch<64, 3>(p, stream) : tc_wg_launch<32, 3>(p, stream);
 }
 
 }  // namespace cpb

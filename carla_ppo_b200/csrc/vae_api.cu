@@ -43,7 +43,10 @@ void profile_end(cudaStream_t s) {
     g_open = -1;
 }
 
-int g_math_mode = 1;   // 0: fp32 SIMT everywhere; 1: 3xTF32 wgmma for the dense conv/deconv layers
+// 0: fp32 SIMT everywhere; 1: 3xTF32 wgmma for the dense conv/deconv layers; 2: the same layers as ONE TF32 wgmma
+// pass with operands rounded to nearest (not fp32-accurate: up to 2^-10 relative error per product)
+int g_math_mode = 1;
+static int tc_passes() { return g_math_mode == 2 ? 1 : 3; }
 // Per-device one-time setup (cudaFuncSetAttribute for > 48 KB dynamic shared memory and the co-resident cluster counts
 // of the persistent kernels are PER DEVICE): keyed by cudaGetDevice() so that a process driving several GPUs works.
 constexpr int kMaxDevices = 64;
@@ -361,9 +364,10 @@ static int tc_debug_flags() {
 
 static int32_t tg(const char* label, const TapGemmParams& p, cudaStream_t s, int scatter_k = 0) {
     ProfScope prof(label, s);
-    if (g_math_mode == 1 && p.wk_hi != nullptr) {
+    if (g_math_mode >= 1 && p.wk_hi != nullptr) {
         TapGemmParams q = scatter_k > 0 ? quad_from_scatter(p, scatter_k) : p;
         q.debug = tc_debug_flags();
+        q.passes = tc_passes();
         if (tc_tapgemm_supported(q)) return launch_tc_tapgemm(q, s);
     }
     return launch_tapgemm(p, s);
@@ -381,7 +385,8 @@ static int32_t run_wgrad(const char* label, const float* big, int Wb, int pitch,
     for (int kh = 0; kh < k; ++kh) w.tap_off[kh] = (long long)kh * Wb * pitch;
     w.I = k * k * pitch; w.J = J;
     const long long M = (long long)B * Ho * Wo;
-    if (g_math_mode == 1 && tc_wgrad_supported(w.I, w.J, w.run)) {
+    if (g_math_mode >= 1 && tc_wgrad_supported(w.I, w.J, w.run)) {
+        w.passes = tc_passes();
         w.splits = tc_wgrad_pick_splits(w.I, w.J, M);
         w.m_per_split = align_up((M + w.splits - 1) / w.splits, 32);
         CPB_TRY(launch_tc_wgrad(w, s));
@@ -449,19 +454,22 @@ static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const flo
     }
     ProfScope prof("relayout_weights", s);
     CPB_TRY(launch_relayout(params, pl.relayout, t, s));
-    if (g_math_mode != 1) return CPB_OK;
+    if (g_math_mode == 0) return CPB_OK;
     TcWeightTable w;
     memset(&w, 0, sizeof(w));
+    const int round_nearest = tc_passes() == 1 ? 1 : 0;
     auto addw = [&](int tensor, int slot, int k, int cb, int cs, bool gather, bool scatter) {
         const long long n = (long long)k * k * cb * cs;
         if (gather) {
             TcWeightJob& j = w.jobs[w.njobs++];
             j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].f_hi; j.dst_lo = pl.rl.tc[slot].f_lo;
+            j.round_nearest = round_nearest;
             j.mode = 1; j.k = k; j.cb = cb; j.cs = cs; j.N = cs; j.C = k * cb; j.count = n; w.total += n;
         }
         if (scatter) {
             TcWeightJob& j = w.jobs[w.njobs++];
             j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].t_hi; j.dst_lo = pl.rl.tc[slot].t_lo;
+            j.round_nearest = round_nearest;
             const int win = (k + 1) / 2;
             j.mode = 2; j.k = k; j.cb = cb; j.cs = cs; j.N = 4 * cb; j.C = cs; j.count = (long long)win * win * 4 * cb * cs; w.total += j.count;
         }
@@ -860,8 +868,9 @@ int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t ct, int32_t z, int32
     return n;
 }
 
-/* debug: D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core tap-GEMM (dense, one tap).  scratch: at least 2*N*K floats
-   (the weight image); callers sized for an older layout pass 2*N*K + M*K, of which the rest goes unused. */
+/* debug: D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core tap-GEMM (dense, one tap); the single-pass kernel in math
+   mode 2, 3xTF32 otherwise.  scratch: at least 2*N*K floats (the weight image); callers sized for an older layout pass
+   2*N*K + M*K, of which the rest goes unused. */
 int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, int32_t n, int32_t k, float* scratch, void* stream) {
     CPB_TRY(ensure_init());
     cudaStream_t s = (cudaStream_t)stream;
@@ -869,14 +878,17 @@ int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, 
     memset(&w, 0, sizeof(w));
     w.njobs = 1; w.total = (long long)n * k;
     w.jobs[0].src_off = 0; w.jobs[0].dst_hi = 0; w.jobs[0].dst_lo = (long long)n * k; w.jobs[0].mode = 0; w.jobs[0].N = n; w.jobs[0].C = k; w.jobs[0].count = w.total;
+    w.jobs[0].round_nearest = tc_passes() == 1 ? 1 : 0;
     TapGemmParams p = dense_problem(a, m, k, nullptr, n, nullptr, nullptr, d, 0);
     p.wk_hi = scratch; p.wk_lo = scratch + (long long)n * k;
     p.debug = tc_debug_flags();
+    p.passes = tc_passes();
     CPB_TRY(launch_tc_weights(bt, scratch, w, s));
     return launch_tc_tapgemm(p, s);
 }
 
-/* debug: out[I,J] = big[M,I]^T small[M,J] through the tensor-core wgrad kernel (1x1 "image", one tap). */
+/* debug: out[I,J] = big[M,I]^T small[M,J] through the tensor-core wgrad kernel (1x1 "image", one tap); the single-pass
+   kernel in math mode 2, 3xTF32 otherwise. */
 int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int32_t m, int32_t i, int32_t j,
                            int32_t variant, float* partial, void* stream) {
     CPB_TRY(ensure_init());
@@ -886,6 +898,7 @@ int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int
     w.big = big; w.small = small; w.partial = partial;
     w.batch = m; w.Wb = 1; w.big_pitch = i; w.big_img = i; w.Ho = w.Wo = 1; w.sstride = 1;
     w.ntaps = 1; w.run = i; w.tap_off[0] = 0; w.I = i; w.J = j; w.tc_variant = variant;
+    w.passes = tc_passes();
     w.splits = 2;
     w.m_per_split = align_up(((long long)m + 1) / 2, 32);
     CPB_TRY(launch_tc_wgrad(w, s));
@@ -893,7 +906,7 @@ int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int
 }
 
 int32_t cpb_set_math_mode(int32_t mode) {
-    CPB_REQUIRE(mode == 0 || mode == 1, "math mode must be 0 (fp32 SIMT) or 1 (3xTF32 wgmma)");
+    CPB_REQUIRE(mode >= 0 && mode <= 2, "math mode must be 0 (fp32 SIMT), 1 (3xTF32 wgmma) or 2 (single-pass TF32 wgmma), got %d", mode);
     cpb::g_math_mode = mode;
     return CPB_OK;
 }

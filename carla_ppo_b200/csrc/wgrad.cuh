@@ -28,6 +28,7 @@ struct WgradParams {
     int splits;
     long long m_per_split; // multiple of 16
     int tc_variant;        // unused (kept for the cpb_debug_tc_wgrad signature)
+    int passes;            // tensor-core path: 3 (3xTF32) or 1 (one TF32 pass, operands rounded to nearest)
 };
 
 // how many splits launch_wgrad will use for this problem (caller sizes `partial` with it)
@@ -35,7 +36,8 @@ int wgrad_pick_splits(int I, int J, long long M);
 int32_t launch_wgrad(const WgradParams& p, cudaStream_t stream);
 int32_t wgrad_init();
 
-// tensor-core (wgmma, 3xTF32) variant -- tc_wgrad.cu.  Same WgradParams; m_per_split must be a multiple of 32.
+// tensor-core (wgmma, 3xTF32 or one TF32 pass) variant -- tc_wgrad.cu.  Same WgradParams; m_per_split must be a
+// multiple of 32.
 constexpr int kTcWaveCtas = 132;   // CTAs of the single split-K wave: one per SM of an H100 SXM
 int32_t tc_wgrad_init();
 bool tc_wgrad_supported(int I, int J, int run);

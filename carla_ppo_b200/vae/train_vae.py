@@ -16,6 +16,8 @@ import shutil
 
 import numpy as np
 
+from .. import _lib
+
 
 def read_png_dir(directory: str, channels: int) -> np.ndarray:
     """All ``*.png`` of a directory (os.listdir order, like the reference) as one uint8 array [N,80,160,channels]."""
@@ -37,6 +39,9 @@ def split_validation(frames: np.ndarray, val_portion: float = 0.1):
     return frames[cut:], frames[:cut]
 
 
+MATH_MODES = {"simt": _lib.MATH_SIMT, "3xtf32": _lib.MATH_3XTF32, "tf32": _lib.MATH_TF32}
+
+
 def build_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(description="Trains a VAE with RGB images as source and RGB or segmentation images as target")
     p.add_argument("--model_name", type=str, default=None)
@@ -53,6 +58,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("-restart", action="store_true")
     p.add_argument("--max_epochs", type=int, default=0, help="(addition) stop after this many epochs; 0 = early stopping only")
     p.add_argument("--models_root", type=str, default="models", help="(addition) parent directory of the model directories")
+    p.add_argument("--math_mode", choices=sorted(MATH_MODES), default="3xtf32",
+                   help="(addition) arithmetic of the ConvVAE's conv2-4 / deconv1-3 layers: 3xtf32 (fp32-accurate), "
+                        "tf32 (one TF32 tensor-core pass, not fp32-accurate) or simt (fp32 FMA)")
     return p
 
 
@@ -109,6 +117,7 @@ def main(argv=None):
     vae.init_session()
     if not restart:
         vae.load_latest_checkpoint()
+    _lib.check(_lib.load().cpb_set_math_mode(MATH_MODES[args.math_mode]), "cpb_set_math_mode")
 
     print("Training")
     best, stale = float("inf"), 0

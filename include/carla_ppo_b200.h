@@ -248,10 +248,19 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
                            void* vae_workspace, int64_t vae_workspace_bytes,
                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
-/* Arithmetic used for the dense conv / transposed-conv contractions of the VAE (both are fp32-accurate):
+/* Arithmetic used for the dense conv / transposed-conv contractions of the VAE (modes 1 and 0 are fp32-accurate):
  *   1 (default) wgmma tf32 with the error-compensated 3xTF32 split, fp32 accumulators in registers;
- *   0           fp32 FMA (SIMT) tap-GEMM -- also used in mode 1 for the layers the tensor-core kernel does
- *               not cover (3-channel edge layers, dense heads, weight gradients). */
+ *   0           fp32 FMA (SIMT) tap-GEMM -- also used in modes 1 and 2 for the layers the tensor-core kernel does
+ *               not cover (3-channel edge layers, dense heads, weight gradients);
+ *   2           ONE wgmma tf32 pass, NOT fp32-accurate: both operands are rounded to the nearest TF32 value (10-bit
+ *               mantissa, ties away from zero), so each product carries a relative error of up to 2^-10 with no
+ *               systematic sign; accumulation stays fp32 (chunks of 128 k added into fp32 registers).
+ *               The comparable setting of cuDNN / TensorFlow on this hardware is their TF32 default.
+ * Modes 1 and 2 cover the same layers of the ConvVAE: forward, data gradient and weight gradient of conv2-4 and
+ * deconv1-3, in every entry point that runs them (encode, decode, forward, loss_grad, train_step(_host),
+ * cpb_encode_predict).  conv1, deconv4, the heads, dense1, the dense weight gradients, the MlpVAE and PPO use the
+ * fp32 kernels in every mode.  The mode is process-global and read when a call is enqueued; other values are
+ * rejected (CPB_ERR_INVALID_ARGUMENT). */
 int32_t cpb_set_math_mode(int32_t mode);
 /* Debug / test hooks (not part of the reference-facing surface): workspace buffer offsets in bytes for
  * [xp,a1,a2,a3,a4,heads,z,d1,b1,b2,b3,logits_p,gA,gB,frame_loss,kl_rows] (-1 = absent in that mode), and a dense
