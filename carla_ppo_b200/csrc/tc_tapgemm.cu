@@ -510,7 +510,9 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
 
 int32_t tc_tapgemm_init() {
     const char* e = getenv("CPB_TC_CLUSTER");
-    g_tc_cluster = e ? atoi(e) : 2;
+    // default: no cluster.  Multicasting the weight tiles halves their L2 reads, but ties every stage of the CTAs of
+    // a cluster to the slowest of their consumers, which costs more than the reads (measurements: DESIGN.md section 3)
+    g_tc_cluster = e ? atoi(e) : 1;
     CPB_REQUIRE(g_tc_cluster == 1 || g_tc_cluster == 2 || g_tc_cluster == 4 || g_tc_cluster == 8, "CPB_TC_CLUSTER must be 1, 2, 4 or 8");
     CPB_TRY((tc_init_one<32, 3>()));
     CPB_TRY((tc_init_one<64, 3>()));
