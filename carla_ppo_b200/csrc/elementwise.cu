@@ -138,20 +138,21 @@ deconv4_fwd_kernel(const float* __restrict__ small, const float* __restrict__ w,
 // sampling + KL: one warp per row
 // ------------------------------------------------------------------------------------------
 __global__ void reparam_kernel(const float* __restrict__ heads, const float* __restrict__ eps, int batch,
-                               int zdim, float kl_floor, int use_floor, float* __restrict__ zout,
+                               int zdim, int pitch, float kl_floor, int use_floor, float* __restrict__ zout,
                                float* __restrict__ kl_rows, float* __restrict__ kl_active) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= batch) return;
-    const float* mu = heads + (long long)row * zdim;
-    const float* lv = heads + (long long)batch * zdim + (long long)row * zdim;
+    const float* mu = heads + (long long)row * pitch;
+    const float* lv = heads + (long long)batch * pitch + (long long)row * pitch;
     float s = 0.f;
     for (int j = lane; j < zdim; j += 32) {
         const float m = mu[j], l = lv[j];
         const float z = eps != nullptr ? fmaf(eps[(long long)row * zdim + j], expf(0.5f * l), m) : m;
-        zout[(long long)row * zdim + j] = z;
+        zout[(long long)row * pitch + j] = z;
         s += 1.f + l - m * m - expf(l);
     }
+    for (int j = zdim + lane; j < pitch; j += 32) zout[(long long)row * pitch + j] = 0.f;
     s = warp_sum(s);
     if (lane == 0) {
         float kl = -0.5f * s;
@@ -167,17 +168,33 @@ __global__ void reparam_kernel(const float* __restrict__ heads, const float* __r
 
 __global__ void reparam_bwd_kernel(const float* __restrict__ heads, const float* __restrict__ eps,
                                    const float* __restrict__ gz, const float* __restrict__ kl_active,
-                                   int batch, int zdim, float coef, float* __restrict__ gheads) {
+                                   int batch, int zdim, int pitch, float coef, float* __restrict__ gheads) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long n = (long long)batch * zdim;
+    const long long n = (long long)batch * pitch;
     if (idx >= n) return;
-    const int row = (int)(idx / zdim);
+    const int row = (int)(idx / pitch);
+    const int col = (int)(idx - (long long)row * pitch);
+    if (col >= zdim) {
+        gheads[idx] = 0.f;
+        gheads[n + idx] = 0.f;
+        return;
+    }
     const float m = heads[idx], l = heads[n + idx];
     const float g = gz[idx];
     const float a = kl_active[row] * coef;
-    const float e = eps != nullptr ? eps[idx] : 0.f;
+    const float e = eps != nullptr ? eps[(long long)row * zdim + col] : 0.f;
     gheads[idx] = fmaf(a, m, g);
     gheads[n + idx] = g * (0.5f * e * expf(0.5f * l)) + a * 0.5f * (expf(l) - 1.f);
+}
+
+// dst[r, c] = c < src_pitch ? src[r, c] : 0   for c < dst_pitch (both pitches multiples of 4)
+__global__ void pitch_copy_kernel(const float4* __restrict__ src, int src_p4, float4* __restrict__ dst, int dst_p4,
+                                  long long n4) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const long long r = i / dst_p4;
+    const int c = (int)(i - r * dst_p4);
+    dst[i] = c < src_p4 ? src[r * src_p4 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -351,21 +368,21 @@ __global__ void relayout_kernel(const float* __restrict__ params, float* __restr
     int j = 0;
     while (j < t.njobs - 1 && idx >= t.jobs[j].count) { idx -= t.jobs[j].count; ++j; }
     const RelayoutJob& job = t.jobs[j];
+    int r, c, tap;
     if (job.mode == 0) {
-        // dst [taps][cols][rows]
-        const int r = (int)(idx % job.rows);
-        const long long rest = idx / job.rows;
-        const int c = (int)(rest % job.cols);
-        const int tap = (int)(rest / job.cols);
-        dst[job.dst_off + idx] = params[job.src_off + ((long long)tap * job.rows + r) * job.cols + c];
+        // dst [taps][cols_pad][rows_pad]
+        r = (int)(idx % job.rows_pad);
+        const long long rest = idx / job.rows_pad;
+        c = (int)(rest % job.cols_pad);
+        tap = (int)(rest / job.cols_pad);
     } else {
-        // dst [taps][rows_pad][cols]
-        const int c = (int)(idx % job.cols);
-        const long long rest = idx / job.cols;
-        const int r = (int)(rest % job.rows_pad);
-        const int tap = (int)(rest / job.rows_pad);
-        dst[job.dst_off + idx] = r < job.rows ? params[job.src_off + ((long long)tap * job.rows + r) * job.cols + c] : 0.f;
+        // dst [taps][rows_pad][cols_pad]
+        c = (int)(idx % job.cols_pad);
+        const long long rest = idx / job.cols_pad;
+        r = (int)(rest % job.rows_pad);
+        tap = (int)(rest / job.rows_pad);
     }
+    dst[job.dst_off + idx] = r < job.rows && c < job.cols ? params[job.src_off + ((long long)tap * job.rows + r) * job.cols + c] : 0.f;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -436,21 +453,30 @@ int32_t launch_deconv4_fwd(const float* small, const float* w, const float* bias
     return CPB_OK;
 }
 
-int32_t launch_reparam(const float* heads, const float* eps, int batch, int zdim, float kl_tolerance,
+int32_t launch_reparam(const float* heads, const float* eps, int batch, int zdim, int pitch, float kl_tolerance,
                        float* zout, float* kl_rows, float* kl_active, cudaStream_t stream) {
     if (batch == 0) return CPB_OK;
     const int warps = 8;
-    reparam_kernel<<<cdiv(batch, warps), warps * 32, 0, stream>>>(heads, eps, batch, zdim, kl_tolerance * zdim,
+    reparam_kernel<<<cdiv(batch, warps), warps * 32, 0, stream>>>(heads, eps, batch, zdim, pitch, kl_tolerance * zdim,
                                                                    kl_tolerance > 0.f ? 1 : 0, zout, kl_rows, kl_active);
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
 int32_t launch_reparam_bwd(const float* heads, const float* eps, const float* gz, const float* kl_active,
-                           int batch, int zdim, float coef, float* gheads, cudaStream_t stream) {
-    const long long n = (long long)batch * zdim;
+                           int batch, int zdim, int pitch, float coef, float* gheads, cudaStream_t stream) {
+    const long long n = (long long)batch * pitch;
     if (n == 0) return CPB_OK;
-    reparam_bwd_kernel<<<cdiv(n, 256), 256, 0, stream>>>(heads, eps, gz, kl_active, batch, zdim, coef, gheads);
+    reparam_bwd_kernel<<<cdiv(n, 256), 256, 0, stream>>>(heads, eps, gz, kl_active, batch, zdim, pitch, coef, gheads);
+    CPB_LAUNCHED();
+    return CPB_OK;
+}
+
+int32_t launch_pitch_copy(const float* src, int src_pitch, float* dst, int dst_pitch, int rows, cudaStream_t stream) {
+    CPB_REQUIRE(src_pitch % 4 == 0 && dst_pitch % 4 == 0, "pitch_copy: pitches must be multiples of 4");
+    const long long n4 = (long long)rows * (dst_pitch / 4);
+    if (n4 == 0) return CPB_OK;
+    pitch_copy_kernel<<<cdiv(n4, 256), 256, 0, stream>>>((const float4*)src, src_pitch / 4, (float4*)dst, dst_pitch / 4, n4);
     CPB_LAUNCHED();
     return CPB_OK;
 }

@@ -25,14 +25,19 @@ long long edge_gather_blocks(int batch);
 int edge_wgrad_ctas(int batch);
 int32_t launch_edge_wgrad(const float* big4, int cb, const float* small, int batch, float* partial, cudaStream_t stream);
 
-// heads [2][B][z] (mean block, logvar block), eps [B,z] or nullptr -> zout [B,z], kl_rows [B],
-// kl_active [B] (1 when the KL term of that row has a gradient, i.e. above the tolerance floor).
-int32_t launch_reparam(const float* heads, const float* eps, int batch, int zdim, float kl_tolerance,
+// heads [2][B][pitch] (mean block, logvar block), eps [B,zdim] or nullptr -> zout [B,pitch], kl_rows [B],
+// kl_active [B] (1 when the KL term of that row has a gradient, i.e. above the tolerance floor).  The KL sums the
+// zdim real columns; zout's columns zdim..pitch-1 are written as 0.
+int32_t launch_reparam(const float* heads, const float* eps, int batch, int zdim, int pitch, float kl_tolerance,
                        float* zout, float* kl_rows, float* kl_active, cudaStream_t stream);
 
-// gz [B,z] -> gheads [2][B][z];  coef = beta * loss_scale / B
+// gz [B,pitch] -> gheads [2][B][pitch] (columns zdim..pitch-1 written as 0);  coef = beta * loss_scale / B
 int32_t launch_reparam_bwd(const float* heads, const float* eps, const float* gz, const float* kl_active,
-                           int batch, int zdim, float coef, float* gheads, cudaStream_t stream);
+                           int batch, int zdim, int pitch, float coef, float* gheads, cudaStream_t stream);
+
+// [rows, src_pitch] -> [rows, dst_pitch]: copies min(src_pitch, dst_pitch) columns, zero-fills the rest of each row
+// (the latent boundary: callers' [B, z] rows <-> the library's [B, z_pad] rows).  Pitches are multiples of 4.
+int32_t launch_pitch_copy(const float* src, int src_pitch, float* dst, int dst_pitch, int rows, cudaStream_t stream);
 
 // logits_p, target_p [B,12800,4] -> frame_loss [B]; dlogits_p [B,12800,4] (nullable) = gscale * dl/dx
 // frame_dsum (optional): [batch][4] per-frame channel sums of the gradient image (column-summed later = last layer's bias gradient)
@@ -59,12 +64,12 @@ int32_t launch_colsum(const float* g, long long rows, int pitch, int c_real, flo
 struct RelayoutJob {
     long long src_off, dst_off;   // float offsets into the params buffer / the relayout buffer
     int taps, rows, cols;         // source is [taps][rows][cols]
-    int mode;                     // 0: transpose each tap -> [taps][cols][rows]
-                                  // 1: pad rows -> [taps][rows_pad=4][cols]
-    int rows_pad;
+    int mode;                     // 0: transpose each tap -> [taps][cols_pad][rows_pad]
+                                  // 1: copy each tap -> [taps][rows_pad][cols_pad]
+    int rows_pad, cols_pad;       // >= rows, cols; the padding is zero-filled
     long long count;              // destination elements
 };
-constexpr int kMaxRelayoutJobs = 12;   // (MlpVAE uses 6)
+constexpr int kMaxRelayoutJobs = 16;   // (the ConvVAE step uses up to 12)
 struct RelayoutTable {
     int njobs;
     long long total;

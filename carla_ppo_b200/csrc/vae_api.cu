@@ -149,12 +149,20 @@ struct TcW { int64_t f_hi, f_lo, t_hi, t_lo; };   // gather-form / quad-scatter-
 struct Relayout {
     int64_t conv2T, conv3T, conv4T, deconv1T, deconv2T, deconv3T, dense1T, headsT, conv1P, deconv4P;
     TcW tc[6];          // conv2, conv3, conv4, deconv1, deconv2, deconv3
+    // z < z_pad only (empty otherwise): zero-padded copies of the z-sized weights, [2][6144][z_pad], [2][z_pad], [z_pad][6144]
+    int64_t headsP, headsBP, dense1P;
     int64_t total;
 };
 enum { TC_CONV2, TC_CONV3, TC_CONV4, TC_DECONV1, TC_DECONV2, TC_DECONV3 };
 
+// Inside the library the latent has z_pad = 64 * ceil(z / 64) columns: the heads and dense1 then run the shapes of a
+// multiple-of-64 model (the k-split tap-GEMM needs N % 64 == 0).  The padded columns hold zeros.
+static int z_pad(int z) { return (int)align_up(z, 64); }
+
 static Relayout make_relayout(int z) {
     using namespace geo;
+    const int zp = z_pad(z);
+    const bool padded = zp != z;
     Relayout r;
     int64_t o = 0;
     auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
@@ -164,8 +172,8 @@ static Relayout make_relayout(int z) {
     r.deconv1T = take(16LL * C3 * C4);
     r.deconv2T = take(16LL * C2 * C3);
     r.deconv3T = take(25LL * C1 * C2);
-    r.dense1T = take((int64_t)z * FEAT);
-    r.headsT = take(2LL * z * FEAT);
+    r.dense1T = take((int64_t)zp * FEAT);
+    r.headsT = take(2LL * zp * FEAT);
     r.conv1P = take(16LL * 4 * C1);
     r.deconv4P = take(16LL * 4 * C1);
     const int64_t sizes[6] = {16LL * C1 * C2, 16LL * C2 * C3, 16LL * C3 * C4, 16LL * C3 * C4, 16LL * C2 * C3, 25LL * C1 * C2};
@@ -174,24 +182,27 @@ static Relayout make_relayout(int z) {
         r.tc[i].f_hi = take(sizes[i]); r.tc[i].f_lo = take(sizes[i]);
         r.tc[i].t_hi = take(qsizes[i]); r.tc[i].t_lo = take(qsizes[i]);
     }
+    r.headsP = take(padded ? 2LL * FEAT * zp : 0);
+    r.headsBP = take(padded ? 2LL * zp : 0);
+    r.dense1P = take(padded ? (int64_t)zp * FEAT : 0);
     r.total = o;
     return r;
 }
 
 struct VaePlan {
-    int B, ct, z, mode;
+    int B, ct, z, zp, mode;     // zp = z_pad(z): row pitch of every latent buffer (heads, zbuf, gz, gheads, ksplit)
     Relayout rl;
     float *relayout, *xp, *yp, *a1, *a2, *a3, *a4, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss;
     float *d1, *b1, *b2, *b3, *logits_p;
     float *gA, *gB, *gz, *gheads, *partial, *colsum;
     float* cs_edge;     // per-CTA column sums of deconv4's data gradient (edge_gather), [edge_gather_blocks(B)][32]
     float* frame_dsum;  // per-frame channel sums of d loss / d logits, [B][4]
-    float* ksplit;      // partial results of the k-split dense layers: kMaxKSplit x [2, B, z]
+    float* ksplit;      // partial results of the k-split dense layers: kMaxKSplit x [2, B, z_pad]
     int64_t bytes;
     bool ok;
 };
 
-static int64_t max_partial_floats(int B, int z) {
+static int64_t max_partial_floats(int B, int zp) {
     using namespace geo;
     struct P { int I, J; long long M; };
     const P ps[] = {
@@ -200,8 +211,8 @@ static int64_t max_partial_floats(int B, int z) {
         {16 * C2, C3, (long long)B * H3 * W3},     // conv3 / deconv2
         {16 * C3, C4, (long long)B * H4 * W4},     // conv4 / deconv1
         {25 * C1, C2, (long long)B * H2 * W2},     // deconv3
-        {FEAT, z, (long long)B},                    // heads
-        {z, FEAT, (long long)B},                    // dense1
+        {FEAT, zp, (long long)B},                   // heads
+        {zp, FEAT, (long long)B},                   // dense1
     };
     int64_t best = (int64_t)edge_wgrad_ctas(B) * 48 * C1;
     // the tensor-core weight gradient runs ONE wave of (i-tile, j-tile, split) CTAs with 128 x BN <= 128 x 64 tiles
@@ -219,8 +230,9 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     using namespace geo;
     VaePlan p;
     memset(&p, 0, sizeof(p));
-    p.B = B; p.ct = ct; p.z = z; p.mode = mode;
+    p.B = B; p.ct = ct; p.z = z; p.zp = z_pad(z); p.mode = mode;
     p.rl = make_relayout(z);
+    const int64_t zp = p.zp;
     Arena a(ws, ws_bytes);
     const int64_t b = B;
     p.relayout = a.take<float>(p.rl.total);
@@ -229,11 +241,11 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     p.a2 = a.take<float>(b * H2 * W2 * C2);
     p.a3 = a.take<float>(b * H3 * W3 * C3);
     p.a4 = a.take<float>(b * FEAT);
-    p.heads = a.take<float>(2 * b * z);
-    p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * z);
+    p.heads = a.take<float>(2 * b * zp);
+    p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * zp);
     if (mode >= CPB_WS_FORWARD) {
         p.yp = a.take<float>(b * NPIX * 4);
-        p.zbuf = a.take<float>(b * z);
+        p.zbuf = a.take<float>(b * zp);
         p.kl_rows = a.take<float>(b);
         p.kl_active = a.take<float>(b);
         p.frame_loss = a.take<float>(b);
@@ -246,9 +258,9 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
     if (mode >= CPB_WS_TRAIN) {
         p.gA = a.take<float>(b * H1 * W1 * C1);
         p.gB = a.take<float>(b * H1 * W1 * C1);
-        p.gz = a.take<float>(b * z);
-        p.gheads = a.take<float>(2 * b * z);
-        p.partial = a.take<float>(max_partial_floats(B, z));
+        p.gz = a.take<float>(b * zp);
+        p.gheads = a.take<float>(2 * b * zp);
+        p.partial = a.take<float>(max_partial_floats(B, p.zp));
         p.colsum = a.take<float>(colsum_scratch_floats(b * NPIX, 4) + colsum_scratch_floats(b * H1 * W1, C1) +
                                  colsum_scratch_floats(b, FEAT));
         p.cs_edge = a.take<float>(edge_gather_blocks(B) * C1);
@@ -395,11 +407,12 @@ static int32_t run_wgrad(const char* label, const float* big, int Wb, int pitch,
         w.m_per_split = align_up((M + w.splits - 1) / w.splits, 16);
         CPB_TRY(launch_wgrad(w, s));
     }
-    return launch_reduce_partials(partial, w.splits, w.I, w.J, c_pad, c_real, out, s);
+    return launch_reduce_partials(partial, w.splits, w.I, w.J, c_pad, c_real, w.J, out, s);
 }
 
-static int32_t run_dense_wgrad(const char* label, const float* x, int K, const float* g, int B, int J, float* partial,
-                               float* out, cudaStream_t s) {
+// out[k_real][j_real] = x[B, K]^T g[B, J], dropping the padded rows k >= k_real and columns j >= j_real
+static int32_t run_dense_wgrad(const char* label, const float* x, int K, int k_real, const float* g, int B, int J, int j_real,
+                               float* partial, float* out, cudaStream_t s) {
     ProfScope prof(label, s);
     WgradParams w;
     memset(&w, 0, sizeof(w));
@@ -409,48 +422,65 @@ static int32_t run_dense_wgrad(const char* label, const float* x, int K, const f
     w.splits = wgrad_pick_splits(w.I, w.J, B);
     w.m_per_split = align_up(((long long)B + w.splits - 1) / w.splits, 16);
     CPB_TRY(launch_wgrad(w, s));
-    return launch_reduce_partials(partial, w.splits, w.I, w.J, K, K, out, s);
+    return launch_reduce_partials(partial, w.splits, w.I, w.J, K, k_real, j_real, out, s);
 }
 
 // ---------------------------------------------------------------------------------------------
 // passes
 // ---------------------------------------------------------------------------------------------
+// multiples of 4: every [B, z] row that crosses the ABI starts 16-byte aligned, so the pitch changes move float4
+static bool z_ok(int z) { return z >= 4 && z % 4 == 0 && z <= 1024; }
+#define CPB_Z_RULE "z_dim=%d must be a multiple of 4 in [4,1024]"
+
 static int32_t check_cfg(const cpb_vae_config* cfg) {
     CPB_REQUIRE(cfg != nullptr, "cfg is NULL");
     CPB_REQUIRE(cfg->batch >= 1 && cfg->batch <= (1 << 20), "batch=%d out of range", cfg->batch);
     CPB_REQUIRE(cfg->target_channels == 1 || cfg->target_channels == 3, "target_channels must be 1 or 3, got %d", cfg->target_channels);
-    CPB_REQUIRE(cfg->z_dim >= 64 && cfg->z_dim % 64 == 0 && cfg->z_dim <= 1024, "z_dim=%d must be a multiple of 64 in [64,1024]", cfg->z_dim);
+    CPB_REQUIRE(z_ok(cfg->z_dim), CPB_Z_RULE, cfg->z_dim);
     CPB_REQUIRE(cfg->loss_type >= 0 && cfg->loss_type <= 2, "unknown loss_type %d", cfg->loss_type);
     CPB_REQUIRE(cfg->source_dtype == CPB_FRAME_F32 || cfg->source_dtype == CPB_FRAME_U8, "bad source_dtype");
     CPB_REQUIRE(cfg->target_dtype == CPB_FRAME_F32 || cfg->target_dtype == CPB_FRAME_U8, "bad target_dtype");
     return CPB_OK;
 }
 
-static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const float* params, bool decoder,
+static void add_relayout(RelayoutTable& t, int64_t src, int64_t dst, int taps, int rows, int cols, int mode,
+                         int rows_pad, int cols_pad) {
+    RelayoutJob& j = t.jobs[t.njobs++];
+    j.src_off = src; j.dst_off = dst; j.taps = taps; j.rows = rows; j.cols = cols; j.mode = mode;
+    j.rows_pad = rows_pad; j.cols_pad = cols_pad;
+    j.count = (long long)taps * rows_pad * cols_pad;
+    t.total += j.count;
+}
+
+static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const float* params, bool encoder, bool decoder,
                                 bool backward, cudaStream_t s) {
     using namespace geo;
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols, int mode, int rows_pad) {
-        RelayoutJob& j = t.jobs[t.njobs++];
-        j.src_off = src; j.dst_off = dst; j.taps = taps; j.rows = rows; j.cols = cols; j.mode = mode;
-        j.rows_pad = rows_pad;
-        j.count = mode == 0 ? (long long)taps * rows * cols : (long long)taps * rows_pad * cols;
-        t.total += j.count;
+    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols, int mode, int rows_pad, int cols_pad) {
+        add_relayout(t, src, dst, taps, rows, cols, mode, rows_pad, cols_pad);
     };
     if (decoder) {
-        add(L.off[T_DECONV1_K], pl.rl.deconv1T, 16, C3, C4, 0, 0);
-        add(L.off[T_DECONV2_K], pl.rl.deconv2T, 16, C2, C3, 0, 0);
-        add(L.off[T_DECONV3_K], pl.rl.deconv3T, 25, C1, C2, 0, 0);
+        add(L.off[T_DECONV1_K], pl.rl.deconv1T, 16, C3, C4, 0, C3, C4);
+        add(L.off[T_DECONV2_K], pl.rl.deconv2T, 16, C2, C3, 0, C2, C3);
+        add(L.off[T_DECONV3_K], pl.rl.deconv3T, 25, C1, C2, 0, C1, C2);
     }
     if (backward) {
-        add(L.off[T_CONV2_K], pl.rl.conv2T, 16, C1, C2, 0, 0);
-        add(L.off[T_CONV3_K], pl.rl.conv3T, 16, C2, C3, 0, 0);
-        add(L.off[T_CONV4_K], pl.rl.conv4T, 16, C3, C4, 0, 0);
+        add(L.off[T_CONV2_K], pl.rl.conv2T, 16, C1, C2, 0, C1, C2);
+        add(L.off[T_CONV3_K], pl.rl.conv3T, 16, C2, C3, 0, C2, C3);
+        add(L.off[T_CONV4_K], pl.rl.conv4T, 16, C3, C4, 0, C3, C4);
     }
     if (backward) {
-        add(L.off[T_DENSE1_K], pl.rl.dense1T, 1, pl.z, FEAT, 0, 0);
-        add(L.off[T_MEAN_K], pl.rl.headsT, 2, FEAT, pl.z, 0, 0);   // mean and logvar kernels are adjacent
+        add(L.off[T_DENSE1_K], pl.rl.dense1T, 1, pl.z, FEAT, 0, pl.zp, FEAT);      // [6144][z_pad]
+        add(L.off[T_MEAN_K], pl.rl.headsT, 2, FEAT, pl.z, 0, FEAT, pl.zp);        // [2][z_pad][6144]: mean and logvar kernels are adjacent
+    }
+    if (pl.zp != pl.z) {
+        if (encoder) {
+            add(L.off[T_MEAN_K], pl.rl.headsP, 2, FEAT, pl.z, 1, FEAT, pl.zp);
+            add(L.off[T_MEAN_B], pl.rl.headsBP, 1, 1, pl.z, 1, 1, pl.zp);
+            add(L.off[T_LOGVAR_B], pl.rl.headsBP + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
+        }
+        if (decoder) add(L.off[T_DENSE1_K], pl.rl.dense1P, 1, pl.z, FEAT, 1, pl.zp, FEAT);
     }
     ProfScope prof("relayout_weights", s);
     CPB_TRY(launch_relayout(params, pl.relayout, t, s));
@@ -505,26 +535,27 @@ static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_
     p = gather_problem(pl.a3, B, H3, W3, C3, 4, params + L.off[T_CONV4_K], C4, params + L.off[T_CONV4_B], nullptr, pl.a4, 1,
                        pl.relayout + pl.rl.tc[TC_CONV4].f_hi, pl.relayout + pl.rl.tc[TC_CONV4].f_lo);
     CPB_TRY(tg("conv4.fwd", p, s, 0));
-    // both heads as one y-batched dense problem: heads[0] = mean, heads[1] = logstd_sq
-    p = dense_problem(pl.a4, B, FEAT, params + L.off[T_MEAN_K], pl.z, params + L.off[T_MEAN_B], nullptr, pl.heads, 0);
+    // both heads as one y-batched dense problem: heads[0] = mean, heads[1] = logstd_sq; z_pad columns (the weights
+    // are the parameters themselves when z == z_pad, their zero-padded copies otherwise)
+    const bool padded = pl.zp != pl.z;
+    p = dense_problem(pl.a4, B, FEAT, padded ? pl.relayout + pl.rl.headsP : params + L.off[T_MEAN_K], pl.zp,
+                      padded ? pl.relayout + pl.rl.headsBP : params + L.off[T_MEAN_B], nullptr, pl.heads, 0);
     p.ybatch = 2;
-    p.w_ystride = L.off[T_LOGVAR_K] - L.off[T_MEAN_K];
-    p.bias_ystride = L.off[T_LOGVAR_B] - L.off[T_MEAN_B];
-    p.dst_ystride = (long long)B * pl.z;
-    if (pl.z % 64 == 0) {
-        p.ksplit = tapgemm_pick_ksplit(B, pl.z, 2, FEAT);
-        p.kpartial = pl.ksplit; p.kpartial_stride = 2LL * B * pl.z;
-    }
+    p.w_ystride = padded ? (long long)FEAT * pl.zp : L.off[T_LOGVAR_K] - L.off[T_MEAN_K];
+    p.bias_ystride = padded ? pl.zp : L.off[T_LOGVAR_B] - L.off[T_MEAN_B];
+    p.dst_ystride = (long long)B * pl.zp;
+    p.ksplit = tapgemm_pick_ksplit(B, pl.zp, 2, FEAT);
+    p.kpartial = pl.ksplit; p.kpartial_stride = 2LL * B * pl.zp;
     return tg("heads.fwd", p, s);
 }
 
-// zbuf -> d1 -> b1 -> b2 -> b3 -> (logits_p and/or sigmoid)
+// zsrc [B, z_pad] -> d1 -> b1 -> b2 -> b3 -> (logits_p and/or sigmoid)
 static int32_t run_decoder(const VaePlan& pl, const VaeLayout& L, const float* params, const float* zsrc,
                            float* logits_p, float* sigm, cudaStream_t s) {
     using namespace geo;
     const int B = pl.B;
-    TapGemmParams p = dense_problem(zsrc, B, pl.z, params + L.off[T_DENSE1_K], FEAT, params + L.off[T_DENSE1_B],
-                                    nullptr, pl.d1, 0);
+    const float* w1 = pl.zp != pl.z ? pl.relayout + pl.rl.dense1P : params + L.off[T_DENSE1_K];
+    TapGemmParams p = dense_problem(zsrc, B, pl.zp, w1, FEAT, params + L.off[T_DENSE1_B], nullptr, pl.d1, 0);
     CPB_TRY(tg("dense1.fwd", p, s));
     p = scatter_problem(pl.d1, B, H4, W4, C4, 4, pl.relayout + pl.rl.deconv1T, C3, params + L.off[T_DECONV1_B],
                         nullptr, pl.b1, H3, W3, 1, pl.relayout + pl.rl.tc[TC_DECONV1].t_hi, pl.relayout + pl.rl.tc[TC_DECONV1].t_lo);
@@ -546,7 +577,7 @@ static int32_t run_forward_loss(const VaePlan& pl, const VaeLayout& L, const cpb
     using namespace geo;
     const int B = pl.B;
     CPB_TRY(run_encoder(pl, L, cfg, params, source, flags, s));
-    CPB_TRY(launch_reparam(pl.heads, eps, B, pl.z, cfg->kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
+    CPB_TRY(launch_reparam(pl.heads, eps, B, pl.z, pl.zp, cfg->kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
     CPB_TRY(run_decoder(pl, L, params, pl.zbuf, pl.logits_p, sigm, s));
     const float* yp = pl.yp;
     if (target == source && cfg->target_channels == 3 && cfg->target_dtype == cfg->source_dtype &&
@@ -568,14 +599,14 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
                             const float* eps, float* grads, cudaStream_t s) {
     using namespace geo;
     const int B = pl.B;
-    const int z = pl.z;
+    const int z = pl.z, zp = pl.zp;
     float* dlog = pl.logits_p;   // overwritten in place by the loss kernel
     float* cs = pl.colsum;
     CPB_TRY(launch_fill_zero(grads, L.total, s));
     // ---- deconv4 (padded to 4 channels on the big side)
     { ProfScope prof("deconv4.wgrad", s);
       CPB_TRY(launch_edge_wgrad(dlog, pl.ct, pl.b3, B, pl.partial, s));
-      CPB_TRY(launch_reduce_partials(pl.partial, edge_wgrad_ctas(B), 16 * pl.ct, C1, 16 * pl.ct, 16 * pl.ct,
+      CPB_TRY(launch_reduce_partials(pl.partial, edge_wgrad_ctas(B), 16 * pl.ct, C1, 16 * pl.ct, 16 * pl.ct, C1,
                                      grads + L.off[T_DECONV4_K], s)); }
     // the bias gradients of the two outermost layers come out of the kernels that write their pre-activation gradients
     // (recon_loss: per-frame channel sums; edge_gather: per-CTA column sums) instead of separate passes over 0.8 + 1.6 GB
@@ -605,27 +636,26 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
                        pl.relayout + pl.rl.tc[TC_DECONV1].f_hi, pl.relayout + pl.rl.tc[TC_DECONV1].f_lo);
     CPB_TRY(tg("deconv1.dgrad", p, s, 0));                                   // gB = g(d1) [B, 6144]
     // ---- dense1
-    CPB_TRY(run_dense_wgrad("dense1.wgrad", pl.zbuf, z, pl.gB, B, FEAT, pl.partial, grads + L.off[T_DENSE1_K], s));
+    CPB_TRY(run_dense_wgrad("dense1.wgrad", pl.zbuf, zp, z, pl.gB, B, FEAT, FEAT, pl.partial, grads + L.off[T_DENSE1_K], s));
     CPB_TRY(launch_colsum(pl.gB, B, FEAT, FEAT, grads + L.off[T_DENSE1_B], cs, s));
-    p = dense_problem(pl.gB, B, FEAT, pl.relayout + pl.rl.dense1T, z, nullptr, nullptr, pl.gz, 0);
-    if (z % 64 == 0) {
-        p.ksplit = tapgemm_pick_ksplit(B, z, 1, FEAT);
-        p.kpartial = pl.ksplit; p.kpartial_stride = (long long)B * z;
-    }
+    p = dense_problem(pl.gB, B, FEAT, pl.relayout + pl.rl.dense1T, zp, nullptr, nullptr, pl.gz, 0);
+    p.ksplit = tapgemm_pick_ksplit(B, zp, 1, FEAT);
+    p.kpartial = pl.ksplit; p.kpartial_stride = (long long)B * zp;
     CPB_TRY(tg("dense1.dgrad", p, s));
     // ---- sampling + KL
-    CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, cfg->beta * cfg->loss_scale / (float)B,
+    CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, cfg->beta * cfg->loss_scale / (float)B,
                                pl.gheads, s));
     // ---- heads
-    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, pl.gheads, B, z, pl.partial, grads + L.off[T_MEAN_K], s));
-    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, pl.gheads + (long long)B * z, B, z, pl.partial, grads + L.off[T_LOGVAR_K], s));
-    CPB_TRY(launch_colsum(pl.gheads, B, z, z, grads + L.off[T_MEAN_B], cs, s));
-    CPB_TRY(launch_colsum(pl.gheads + (long long)B * z, B, z, z, grads + L.off[T_LOGVAR_B], cs, s));
-    p = dense_problem(pl.gheads, B, z, pl.relayout + pl.rl.headsT, FEAT, nullptr, pl.a4, pl.gA, 0);
+    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, FEAT, pl.gheads, B, zp, z, pl.partial, grads + L.off[T_MEAN_K], s));
+    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, FEAT, pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
+                            grads + L.off[T_LOGVAR_K], s));
+    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[T_MEAN_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[T_LOGVAR_B], cs, s));
+    p = dense_problem(pl.gheads, B, zp, pl.relayout + pl.rl.headsT, FEAT, nullptr, pl.a4, pl.gA, 0);
     p.cls[0].ntaps = 2;                                              // g(a4) = gmean Wm^T + glogvar Wl^T
     p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
-    p.cls[0].taps[1].src_off = (long long)B * z;
-    p.cls[0].taps[1].w_off = (long long)z * FEAT;
+    p.cls[0].taps[1].src_off = (long long)B * zp;
+    p.cls[0].taps[1].w_off = (long long)zp * FEAT;
     CPB_TRY(tg("heads.dgrad", p, s));                                   // gA = g(a4 pre-activation)
     // ---- conv4
     CPB_TRY(run_wgrad("conv4.wgrad", pl.a3, W3, C3, (long long)H3 * W3 * C3, 4, pl.gA, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
@@ -651,7 +681,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     // ---- conv1 (its input gradient is never used: the reference computes and discards it)
     { ProfScope prof("conv1.wgrad", s);
       CPB_TRY(launch_edge_wgrad(pl.xp, 3, pl.gB, B, pl.partial, s));
-      CPB_TRY(launch_reduce_partials(pl.partial, edge_wgrad_ctas(B), 48, C1, 48, 48, grads + L.off[T_CONV1_K], s)); }
+      CPB_TRY(launch_reduce_partials(pl.partial, edge_wgrad_ctas(B), 48, C1, 48, 48, C1, grads + L.off[T_CONV1_K], s)); }
     CPB_TRY(launch_colsum(pl.gB, (long long)B * H1 * W1, C1, C1, grads + L.off[T_CONV1_B], cs, s));
     return CPB_OK;
 }
@@ -695,10 +725,12 @@ static MlpLayout make_mlp_layout(const cpb_mlpvae_config* c) {
 }
 
 struct MlpPlan {
-    int B, IN, OUT, z, e1, e2, d1, d2;
+    int B, IN, OUT, z, zp, e1, e2, d1, d2;     // zp = z_pad(z), the row pitch of the latent buffers (as in VaePlan)
     float *x, *y, *h1, *h2, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss, *g1, *g2, *logits;
     float *ga, *gb, *gz, *gheads, *partial, *colsum, *wT, *ksplit;
     int64_t tE2, tHeads, tD1, tD2, tD3;      // float offsets of the transposed kernels inside wT
+    float* wP;                               // z < z_pad only: zero-padded heads [2][enc2][z_pad], biases [2][z_pad], D1 [z_pad][dec1]
+    int64_t pHeads, pHeadsB, pD1;
     int64_t bytes;
     bool ok;
 };
@@ -708,16 +740,24 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config
     memset(&p, 0, sizeof(p));
     const int64_t b = c->base.batch;
     p.B = (int)b; p.IN = geo::NPIX * 3; p.OUT = geo::NPIX * c->base.target_channels; p.z = c->base.z_dim;
+    p.zp = z_pad(p.z);
     p.e1 = c->enc1; p.e2 = c->enc2; p.d1 = c->dec1; p.d2 = c->dec2;
+    const int64_t zp = p.zp;
     Arena a(ws, ws_bytes);
     p.x = a.take<float>(b * p.IN);
     p.h1 = a.take<float>(b * p.e1);
     p.h2 = a.take<float>(b * p.e2);
-    p.heads = a.take<float>(2 * b * p.z);
-    p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * p.z);
+    p.heads = a.take<float>(2 * b * zp);
+    p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * zp);
+    if (p.zp != p.z) {
+        int64_t o = 0;
+        auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
+        p.pHeads = take(2LL * p.e2 * zp); p.pHeadsB = take(2LL * zp); p.pD1 = take(zp * p.d1);
+        p.wP = a.take<float>(o);
+    }
     if (mode >= CPB_WS_FORWARD) {
         p.y = a.take<float>(b * p.OUT);
-        p.zbuf = a.take<float>(b * p.z);
+        p.zbuf = a.take<float>(b * zp);
         p.kl_rows = a.take<float>(b); p.kl_active = a.take<float>(b); p.frame_loss = a.take<float>(b);
         p.g1 = a.take<float>(b * p.d1);
         p.g2 = a.take<float>(b * p.d2);
@@ -727,15 +767,15 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config
         const int64_t widest = std::max<int64_t>(std::max(p.e1, p.e2), std::max(p.d1, p.d2));
         p.ga = a.take<float>(b * widest);
         p.gb = a.take<float>(b * widest);
-        p.gz = a.take<float>(b * p.z);
-        p.gheads = a.take<float>(2 * b * p.z);
+        p.gz = a.take<float>(b * zp);
+        p.gheads = a.take<float>(2 * b * zp);
         int64_t o = 0;
         auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
-        p.tE2 = take((int64_t)p.e1 * p.e2); p.tHeads = take(2LL * p.e2 * p.z); p.tD1 = take((int64_t)p.z * p.d1);
+        p.tE2 = take((int64_t)p.e1 * p.e2); p.tHeads = take(2LL * p.e2 * zp); p.tD1 = take(zp * p.d1);
         p.tD2 = take((int64_t)p.d1 * p.d2); p.tD3 = take((int64_t)p.d2 * p.OUT);
         p.wT = a.take<float>(o);
         struct P { int I, J; };
-        const P ps[] = {{p.IN, p.e1}, {p.e1, p.e2}, {p.e2, p.z}, {p.z, p.d1}, {p.d1, p.d2}, {p.d2, p.OUT}};
+        const P ps[] = {{p.IN, p.e1}, {p.e1, p.e2}, {p.e2, p.zp}, {p.zp, p.d1}, {p.d1, p.d2}, {p.d2, p.OUT}};
         int64_t best = 0;
         for (const P& q : ps) best = std::max<int64_t>(best, (int64_t)wgrad_pick_splits(q.I, q.J, b) * q.I * q.J);
         p.partial = a.take<float>(best);
@@ -746,6 +786,18 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config
     return p;
 }
 
+// z < z_pad: the zero-padded copies of the z-sized weights that the forward pass reads (one launch)
+static int32_t mlp_pad_weights(const MlpPlan& pl, const MlpLayout& L, const float* params, cudaStream_t s) {
+    if (pl.zp == pl.z) return CPB_OK;
+    RelayoutTable t;
+    memset(&t, 0, sizeof(t));
+    add_relayout(t, L.off[M_MEAN_K], pl.pHeads, 2, pl.e2, pl.z, 1, pl.e2, pl.zp);
+    add_relayout(t, L.off[M_MEAN_B], pl.pHeadsB, 1, 1, pl.z, 1, 1, pl.zp);
+    add_relayout(t, L.off[M_LOGVAR_B], pl.pHeadsB + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
+    add_relayout(t, L.off[M_D1_K], pl.pD1, 1, pl.z, pl.d1, 1, pl.zp, pl.d1);
+    return launch_relayout(params, pl.wP, t, s);
+}
+
 static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
                            int32_t* flags, cudaStream_t s) {
     const float sscale = c->base.source_dtype == CPB_FRAME_U8 ? 1.f / 255.f : 1.f;
@@ -754,16 +806,19 @@ static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpv
     CPB_TRY(launch_tapgemm(p, s));
     p = dense_problem(pl.h1, pl.B, pl.e1, params + L.off[M_E2_K], pl.e2, params + L.off[M_E2_B], nullptr, pl.h2, 1);
     CPB_TRY(launch_tapgemm(p, s));
-    p = dense_problem(pl.h2, pl.B, pl.e2, params + L.off[M_MEAN_K], pl.z, params + L.off[M_MEAN_B], nullptr, pl.heads, 0);
+    const bool padded = pl.zp != pl.z;
+    p = dense_problem(pl.h2, pl.B, pl.e2, padded ? pl.wP + pl.pHeads : params + L.off[M_MEAN_K], pl.zp,
+                      padded ? pl.wP + pl.pHeadsB : params + L.off[M_MEAN_B], nullptr, pl.heads, 0);
     p.ybatch = 2;
-    p.w_ystride = L.off[M_LOGVAR_K] - L.off[M_MEAN_K];
-    p.bias_ystride = L.off[M_LOGVAR_B] - L.off[M_MEAN_B];
-    p.dst_ystride = (long long)pl.B * pl.z;
+    p.w_ystride = padded ? (long long)pl.e2 * pl.zp : L.off[M_LOGVAR_K] - L.off[M_MEAN_K];
+    p.bias_ystride = padded ? pl.zp : L.off[M_LOGVAR_B] - L.off[M_MEAN_B];
+    p.dst_ystride = (long long)pl.B * pl.zp;
     return launch_tapgemm(p, s);
 }
 
 static int32_t mlp_decoder(const MlpPlan& pl, const MlpLayout& L, const float* params, const float* zsrc, float* logits, cudaStream_t s) {
-    TapGemmParams p = dense_problem(zsrc, pl.B, pl.z, params + L.off[M_D1_K], pl.d1, params + L.off[M_D1_B], nullptr, pl.g1, 1);
+    const float* w1 = pl.zp != pl.z ? pl.wP + pl.pD1 : params + L.off[M_D1_K];
+    TapGemmParams p = dense_problem(zsrc, pl.B, pl.zp, w1, pl.d1, params + L.off[M_D1_B], nullptr, pl.g1, 1);
     CPB_TRY(launch_tapgemm(p, s));
     p = dense_problem(pl.g1, pl.B, pl.d1, params + L.off[M_D2_K], pl.d2, params + L.off[M_D2_B], nullptr, pl.g2, 1);
     CPB_TRY(launch_tapgemm(p, s));
@@ -774,7 +829,7 @@ static int32_t mlp_decoder(const MlpPlan& pl, const MlpLayout& L, const float* p
 static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
                                 const void* target, const float* eps, bool want_dlogits, int32_t* flags, cudaStream_t s) {
     CPB_TRY(mlp_encoder(pl, L, c, params, source, flags, s));
-    CPB_TRY(launch_reparam(pl.heads, eps, pl.B, pl.z, c->base.kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
+    CPB_TRY(launch_reparam(pl.heads, eps, pl.B, pl.z, pl.zp, c->base.kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
     CPB_TRY(mlp_decoder(pl, L, params, pl.zbuf, pl.logits, s));
     const float* y = pl.y;
     if (target == source && c->base.target_channels == 3 && c->base.target_dtype == c->base.source_dtype &&
@@ -790,57 +845,65 @@ static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb
 
 static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const float* eps,
                             float* grads, cudaStream_t s) {
-    const int B = pl.B, z = pl.z;
+    const int B = pl.B, z = pl.z, zp = pl.zp;
     float* dlog = pl.logits;
     float* cs = pl.colsum;
     CPB_TRY(launch_fill_zero(grads, L.total, s));
     // transposed kernels for the data gradients ([in,out] -> [out,in]); the two head kernels are adjacent (2 "taps")
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols) {
-        RelayoutJob& j = t.jobs[t.njobs++];
-        j.src_off = src; j.dst_off = dst; j.taps = taps; j.rows = rows; j.cols = cols; j.mode = 0; j.rows_pad = 0;
-        j.count = (long long)taps * rows * cols; t.total += j.count;
+    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols, int rows_pad, int cols_pad) {
+        add_relayout(t, src, dst, taps, rows, cols, 0, rows_pad, cols_pad);
     };
-    add(L.off[M_E2_K], pl.tE2, 1, pl.e1, pl.e2);
-    add(L.off[M_MEAN_K], pl.tHeads, 2, pl.e2, z);
-    add(L.off[M_D1_K], pl.tD1, 1, z, pl.d1);
-    add(L.off[M_D2_K], pl.tD2, 1, pl.d1, pl.d2);
-    add(L.off[M_D3_K], pl.tD3, 1, pl.d2, pl.OUT);
+    add(L.off[M_E2_K], pl.tE2, 1, pl.e1, pl.e2, pl.e1, pl.e2);
+    add(L.off[M_MEAN_K], pl.tHeads, 2, pl.e2, z, pl.e2, zp);      // [2][z_pad][enc2]
+    add(L.off[M_D1_K], pl.tD1, 1, z, pl.d1, zp, pl.d1);           // [dec1][z_pad]
+    add(L.off[M_D2_K], pl.tD2, 1, pl.d1, pl.d2, pl.d1, pl.d2);
+    add(L.off[M_D3_K], pl.tD3, 1, pl.d2, pl.OUT, pl.d2, pl.OUT);
     CPB_TRY(launch_relayout(params, pl.wT, t, s));
     TapGemmParams p;
     // ---- decoder
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g2, pl.d2, dlog, B, pl.OUT, pl.partial, grads + L.off[M_D3_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g2, pl.d2, pl.d2, dlog, B, pl.OUT, pl.OUT, pl.partial, grads + L.off[M_D3_K], s));
     CPB_TRY(launch_colsum(dlog, B, pl.OUT, pl.OUT, grads + L.off[M_D3_B], cs, s));
     p = dense_problem(dlog, B, pl.OUT, pl.wT + pl.tD3, pl.d2, nullptr, pl.g2, pl.ga, 0);                       // ga = g(g2 pre-activation)
     CPB_TRY(launch_tapgemm(p, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g1, pl.d1, pl.ga, B, pl.d2, pl.partial, grads + L.off[M_D2_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g1, pl.d1, pl.d1, pl.ga, B, pl.d2, pl.d2, pl.partial, grads + L.off[M_D2_K], s));
     CPB_TRY(launch_colsum(pl.ga, B, pl.d2, pl.d2, grads + L.off[M_D2_B], cs, s));
     p = dense_problem(pl.ga, B, pl.d2, pl.wT + pl.tD2, pl.d1, nullptr, pl.g1, pl.gb, 0);                         // gb = g(g1 pre-activation)
     CPB_TRY(launch_tapgemm(p, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.zbuf, z, pl.gb, B, pl.d1, pl.partial, grads + L.off[M_D1_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.zbuf, zp, z, pl.gb, B, pl.d1, pl.d1, pl.partial, grads + L.off[M_D1_K], s));
     CPB_TRY(launch_colsum(pl.gb, B, pl.d1, pl.d1, grads + L.off[M_D1_B], cs, s));
-    p = dense_problem(pl.gb, B, pl.d1, pl.wT + pl.tD1, z, nullptr, nullptr, pl.gz, 0);
+    p = dense_problem(pl.gb, B, pl.d1, pl.wT + pl.tD1, zp, nullptr, nullptr, pl.gz, 0);
     CPB_TRY(launch_tapgemm(p, s));
     // ---- sampling + KL, heads
-    CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, c->base.beta * c->base.loss_scale / (float)B, pl.gheads, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.gheads, B, z, pl.partial, grads + L.off[M_MEAN_K], s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.gheads + (long long)B * z, B, z, pl.partial, grads + L.off[M_LOGVAR_K], s));
-    CPB_TRY(launch_colsum(pl.gheads, B, z, z, grads + L.off[M_MEAN_B], cs, s));
-    CPB_TRY(launch_colsum(pl.gheads + (long long)B * z, B, z, z, grads + L.off[M_LOGVAR_B], cs, s));
-    p = dense_problem(pl.gheads, B, z, pl.wT + pl.tHeads, pl.e2, nullptr, pl.h2, pl.ga, 0);
+    CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, c->base.beta * c->base.loss_scale / (float)B, pl.gheads, s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.e2, pl.gheads, B, zp, z, pl.partial, grads + L.off[M_MEAN_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.e2, pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
+                            grads + L.off[M_LOGVAR_K], s));
+    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[M_MEAN_B], cs, s));
+    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[M_LOGVAR_B], cs, s));
+    p = dense_problem(pl.gheads, B, zp, pl.wT + pl.tHeads, pl.e2, nullptr, pl.h2, pl.ga, 0);
     p.cls[0].ntaps = 2;
     p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
-    p.cls[0].taps[1].src_off = (long long)B * z;
-    p.cls[0].taps[1].w_off = (long long)z * pl.e2;
+    p.cls[0].taps[1].src_off = (long long)B * zp;
+    p.cls[0].taps[1].w_off = (long long)zp * pl.e2;
     CPB_TRY(launch_tapgemm(p, s));                                                                               // ga = g(h2 pre-activation)
     // ---- encoder
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h1, pl.e1, pl.ga, B, pl.e2, pl.partial, grads + L.off[M_E2_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h1, pl.e1, pl.e1, pl.ga, B, pl.e2, pl.e2, pl.partial, grads + L.off[M_E2_K], s));
     CPB_TRY(launch_colsum(pl.ga, B, pl.e2, pl.e2, grads + L.off[M_E2_B], cs, s));
     p = dense_problem(pl.ga, B, pl.e2, pl.wT + pl.tE2, pl.e1, nullptr, pl.h1, pl.gb, 0);                         // gb = g(h1 pre-activation)
     CPB_TRY(launch_tapgemm(p, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.x, pl.IN, pl.gb, B, pl.e1, pl.partial, grads + L.off[M_E1_K], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.x, pl.IN, pl.IN, pl.gb, B, pl.e1, pl.e1, pl.partial, grads + L.off[M_E1_K], s));
     return launch_colsum(pl.gb, B, pl.e1, pl.e1, grads + L.off[M_E1_B], cs, s);
+}
+
+// [B, z_pad] latent rows of the workspace -> the caller's [B, z] rows
+static int32_t copy_latent_out(const float* src, float* dst, int B, int z, int zp, cudaStream_t s) {
+    if (zp == z) {
+        CPB_CUDA(cudaMemcpyAsync(dst, src, (size_t)B * z * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        return CPB_OK;
+    }
+    return launch_pitch_copy(src, zp, dst, z, B, s);
 }
 
 }  // namespace cpb
@@ -902,7 +965,7 @@ int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int
     w.splits = 2;
     w.m_per_split = align_up(((long long)m + 1) / 2, 32);
     CPB_TRY(launch_tc_wgrad(w, s));
-    return launch_reduce_partials(partial, w.splits, i, j, i, i, out, s);
+    return launch_reduce_partials(partial, w.splits, i, j, i, i, j, out, s);
 }
 
 int32_t cpb_set_math_mode(int32_t mode) {
@@ -945,7 +1008,7 @@ const char* cpb_vae_tensor_name(int32_t i) { return (i >= 0 && i < T_COUNT) ? kV
 
 int32_t cpb_vae_layout(int32_t ct, int32_t z, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
     CPB_REQUIRE(ct == 1 || ct == 3, "target_channels must be 1 or 3, got %d", ct);
-    CPB_REQUIRE(z >= 64 && z % 64 == 0 && z <= 1024, "z_dim=%d must be a multiple of 64 in [64,1024]", z);
+    CPB_REQUIRE(z_ok(z), CPB_Z_RULE, z);
     VaeLayout L = make_layout(ct, z);
     for (int i = 0; i < T_COUNT; ++i) {
         if (offsets) offsets[i] = L.off[i];
@@ -957,7 +1020,11 @@ int32_t cpb_vae_layout(int32_t ct, int32_t z, int64_t* offsets, int64_t* sizes, 
 }
 
 int64_t cpb_vae_workspace_bytes(int32_t batch, int32_t ct, int32_t z, int32_t mode) {
-    if (batch < 1 || (ct != 1 && ct != 3) || z < 64 || z % 64 != 0 || mode < 0 || mode > 2) {
+    if (!z_ok(z)) {
+        cpb::set_error("cpb_vae_workspace_bytes: bad arguments: " CPB_Z_RULE, z);
+        return CPB_ERR_INVALID_ARGUMENT;
+    }
+    if (batch < 1 || (ct != 1 && ct != 3) || mode < 0 || mode > 2) {
         cpb::set_error("cpb_vae_workspace_bytes: bad arguments");
         return CPB_ERR_INVALID_ARGUMENT;
     }
@@ -981,11 +1048,10 @@ int32_t cpb_vae_encode(const cpb_vae_config* cfg, const float* params, const voi
                        float* logvar, int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_PLAN(CPB_WS_ENCODE);
     CPB_REQUIRE(params && source && mean, "encode: NULL pointer");
-    CPB_TRY(relayout_weights(pl, L, params, false, false, s));
+    CPB_TRY(relayout_weights(pl, L, params, true, false, false, s));
     CPB_TRY(run_encoder(pl, L, cfg, params, source, flags, s));
-    const size_t n = (size_t)pl.B * pl.z * sizeof(float);
-    CPB_CUDA(cudaMemcpyAsync(mean, pl.heads, n, cudaMemcpyDeviceToDevice, s));
-    if (logvar) CPB_CUDA(cudaMemcpyAsync(logvar, pl.heads + (long long)pl.B * pl.z, n, cudaMemcpyDeviceToDevice, s));
+    CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
+    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
     return CPB_OK;
 }
 
@@ -993,7 +1059,11 @@ int32_t cpb_vae_decode(const cpb_vae_config* cfg, const float* params, const flo
                        void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && z && reconstruction, "decode: NULL pointer");
-    CPB_TRY(relayout_weights(pl, L, params, true, false, s));
+    CPB_TRY(relayout_weights(pl, L, params, false, true, false, s));
+    if (pl.zp != pl.z) {
+        CPB_TRY(launch_pitch_copy(z, pl.z, pl.zbuf, pl.zp, pl.B, s));
+        z = pl.zbuf;
+    }
     return run_decoder(pl, L, params, z, nullptr, reconstruction, s);
 }
 
@@ -1003,13 +1073,12 @@ int32_t cpb_vae_forward(const cpb_vae_config* cfg, const float* params, const vo
                         void* stream) {
     CPB_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && source && target && losses, "forward: NULL pointer");
-    CPB_TRY(relayout_weights(pl, L, params, true, false, s));
+    CPB_TRY(relayout_weights(pl, L, params, true, true, false, s));
     CPB_TRY(run_forward_loss(pl, L, cfg, params, source, target, eps, false, reconstruction, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->loss_scale, losses, s));
-    const size_t n = (size_t)pl.B * pl.z * sizeof(float);
-    if (mean) CPB_CUDA(cudaMemcpyAsync(mean, pl.heads, n, cudaMemcpyDeviceToDevice, s));
-    if (logvar) CPB_CUDA(cudaMemcpyAsync(logvar, pl.heads + (long long)pl.B * pl.z, n, cudaMemcpyDeviceToDevice, s));
-    if (z) CPB_CUDA(cudaMemcpyAsync(z, pl.zbuf, n, cudaMemcpyDeviceToDevice, s));
+    if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
+    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
+    if (z) CPB_TRY(copy_latent_out(pl.zbuf, z, pl.B, pl.z, pl.zp, s));
     return CPB_OK;
 }
 
@@ -1018,7 +1087,7 @@ int32_t cpb_vae_loss_grad(const cpb_vae_config* cfg, const float* params, const 
                           int64_t workspace_bytes, void* stream) {
     CPB_PLAN(CPB_WS_TRAIN);
     CPB_REQUIRE(params && source && target && grads && losses, "loss_grad: NULL pointer");
-    CPB_TRY(relayout_weights(pl, L, params, true, true, s));
+    CPB_TRY(relayout_weights(pl, L, params, true, true, true, s));
     CPB_TRY(run_forward_loss(pl, L, cfg, params, source, target, eps, true, nullptr, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->loss_scale, losses, s));
     return run_backward(pl, L, cfg, params, eps, grads, s);
@@ -1159,10 +1228,10 @@ int32_t cpb_mlpvae_encode(const cpb_mlpvae_config* cfg, const float* params, con
                           int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_ENCODE);
     CPB_REQUIRE(params && source && mean, "mlp encode: NULL pointer");
+    CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_encoder(pl, L, cfg, params, source, flags, s));
-    const size_t n = (size_t)pl.B * pl.z * sizeof(float);
-    CPB_CUDA(cudaMemcpyAsync(mean, pl.heads, n, cudaMemcpyDeviceToDevice, s));
-    if (logvar) CPB_CUDA(cudaMemcpyAsync(logvar, pl.heads + (long long)pl.B * pl.z, n, cudaMemcpyDeviceToDevice, s));
+    CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
+    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
     return CPB_OK;
 }
 
@@ -1170,6 +1239,11 @@ int32_t cpb_mlpvae_decode(const cpb_mlpvae_config* cfg, const float* params, con
                           int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && z && reconstruction, "mlp decode: NULL pointer");
+    CPB_TRY(mlp_pad_weights(pl, L, params, s));
+    if (pl.zp != pl.z) {
+        CPB_TRY(launch_pitch_copy(z, pl.z, pl.zbuf, pl.zp, pl.B, s));
+        z = pl.zbuf;
+    }
     CPB_TRY(mlp_decoder(pl, L, params, z, pl.logits, s));
     return launch_sigmoid(pl.logits, reconstruction, (long long)pl.B * pl.OUT, s);
 }
@@ -1179,12 +1253,12 @@ int32_t cpb_mlpvae_forward(const cpb_mlpvae_config* cfg, const float* params, co
                            void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && source && target && losses, "mlp forward: NULL pointer");
+    CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, false, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
-    const size_t n = (size_t)pl.B * pl.z * sizeof(float);
-    if (mean) CPB_CUDA(cudaMemcpyAsync(mean, pl.heads, n, cudaMemcpyDeviceToDevice, s));
-    if (logvar) CPB_CUDA(cudaMemcpyAsync(logvar, pl.heads + (long long)pl.B * pl.z, n, cudaMemcpyDeviceToDevice, s));
-    if (z) CPB_CUDA(cudaMemcpyAsync(z, pl.zbuf, n, cudaMemcpyDeviceToDevice, s));
+    if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
+    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
+    if (z) CPB_TRY(copy_latent_out(pl.zbuf, z, pl.B, pl.z, pl.zp, s));
     if (reconstruction) CPB_TRY(launch_sigmoid(pl.logits, reconstruction, (long long)pl.B * pl.OUT, s));
     return CPB_OK;
 }
@@ -1193,6 +1267,7 @@ int32_t cpb_mlpvae_loss_grad(const cpb_mlpvae_config* cfg, const float* params, 
                              float* grads, float* losses, int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_TRAIN);
     CPB_REQUIRE(params && source && target && grads && losses, "mlp loss_grad: NULL pointer");
+    CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, true, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
     return mlp_backward(pl, L, cfg, params, eps, grads, s);

@@ -176,7 +176,7 @@ void tile_dims(int tile, int& bi, int& bj) {
 // combined in a fixed order (deterministic).
 __global__ void __launch_bounds__(256)
 reduce_partials_kernel(const float* __restrict__ partial, int splits, long long IJ, int J, int c_pad, int c_real,
-                       float* __restrict__ out) {
+                       int j_real, float* __restrict__ out) {
     __shared__ float red[8][33];
     const int o = threadIdx.x & 31;
     const int l = threadIdx.x >> 5;
@@ -194,8 +194,8 @@ reduce_partials_kernel(const float* __restrict__ partial, int splits, long long 
     const int i = (int)(idx / J);
     const int t = i / c_pad;
     const int c = i - t * c_pad;
-    if (c >= c_real) return;
-    out[((long long)t * c_real + c) * J + j] = tot;
+    if (c >= c_real || j >= j_real) return;
+    out[((long long)t * c_real + c) * j_real + j] = tot;
 }
 
 }  // namespace
@@ -232,10 +232,10 @@ int32_t launch_wgrad(const WgradParams& p, cudaStream_t stream) {
     }
 }
 
-int32_t launch_reduce_partials(const float* partial, int splits, int I, int J, int c_pad, int c_real,
+int32_t launch_reduce_partials(const float* partial, int splits, int I, int J, int c_pad, int c_real, int j_real,
                                float* out, cudaStream_t stream) {
     const long long IJ = (long long)I * J;
-    reduce_partials_kernel<<<cdiv(IJ, 32), 256, 0, stream>>>(partial, splits, IJ, J, c_pad, c_real, out);
+    reduce_partials_kernel<<<cdiv(IJ, 32), 256, 0, stream>>>(partial, splits, IJ, J, c_pad, c_real, j_real, out);
     CPB_LAUNCHED();
     return CPB_OK;
 }

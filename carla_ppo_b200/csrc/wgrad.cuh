@@ -44,8 +44,8 @@ bool tc_wgrad_supported(int I, int J, int run);
 int tc_wgrad_pick_splits(int I, int J, long long M);
 int32_t launch_tc_wgrad(const WgradParams& p, cudaStream_t stream);
 
-// out[(t*c_real + c)*J + j] = sum_s partial[s][(t*c_pad + c)][j]   for c < c_real
-int32_t launch_reduce_partials(const float* partial, int splits, int I, int J, int c_pad, int c_real,
+// out[(t*c_real + c)*j_real + j] = sum_s partial[s][(t*c_pad + c)][j]   for c < c_real, j < j_real
+int32_t launch_reduce_partials(const float* partial, int splits, int I, int J, int c_pad, int c_real, int j_real,
                                float* out, cudaStream_t stream);
 
 }  // namespace cpb

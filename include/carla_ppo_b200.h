@@ -18,7 +18,8 @@
  *   - every function returns 0 on success or a negative cpb_status; cpb_last_error() returns a
  *     message for the calling thread.  Bad arguments never launch anything.
  *   - geometry: source frames are [B,80,160,3] (vae_common.py:18-20), targets [B,80,160,Ct] with
- *     Ct in {3,1}; z_dim must be a multiple of 64.
+ *     Ct in {3,1}; z_dim must be a multiple of 4 in [4,1024] (ConvVAE and MlpVAE).  Every [B,z] latent
+ *     row (eps, mean, logvar, z, latent) is dense at pitch z_dim.
  */
 #ifndef CARLA_PPO_B200_H
 #define CARLA_PPO_B200_H
@@ -55,7 +56,7 @@ const char* cpb_build_info(void);
 typedef struct {
     int32_t batch;            /* frames in this call (per rank) */
     int32_t target_channels;  /* 3 = rgb target, 1 = segmentation target (vae_common.py:15) */
-    int32_t z_dim;            /* latent size (64 in every shipped model) */
+    int32_t z_dim;            /* latent size: a multiple of 4 in [4,1024] (64 in every shipped model) */
     int32_t loss_type;        /* CPB_LOSS_* */
     int32_t source_dtype;     /* CPB_FRAME_F32: values in [0,1]; CPB_FRAME_U8: raw 0..255, scaled by 1/255 */
     int32_t target_dtype;     /* CPB_FRAME_F32, or CPB_FRAME_U8 scaled by target_u8_scale */

@@ -5,8 +5,8 @@
 The library path is fixed (carla_ppo_b200/libcarla_ppo_b200.so), so each run copies its build there first; runs
 alternate a, b, a, b, ... so that drift of the shared machine hits both sides alike.  Each run is one
 `bench.py --gpus 1 --steps S --warmup 3 --no-cpu-baseline --dump-outputs` process.  Writes DIR/ab.json: the card
-(name, power limit, max SM clock), every run's ms_per_step, e2e and per-group profile, the median and spread per
-side, and the largest differences between the two sides' dumped outputs (losses, parameters, gradient).
+(name, power limit, max SM clock), every run's ms_per_step, e2e, kernel launch count and per-group profile, the
+median and spread per side, and the largest differences between the two sides' dumped outputs (losses, parameters, gradient).
 With --b omitted only --a is timed (a "before" measurement).  The library at the fixed path is restored at the end.
 """
 import argparse
@@ -39,6 +39,7 @@ def run_bench(lib, steps, dump):
     line = [l for l in r.stdout.splitlines() if l.startswith("{")][-1]
     out = json.loads(line)
     return {"ms_per_step": out["ms_per_step"], "e2e_ms_per_step": out["e2e"]["ms_per_step"], "clocks": out.get("clocks"),
+            "gpu_launches": out.get("gpu_launches"),
             "groups_ms_per_step": out.get("roofline", {}).get("groups_ms_per_step")}
 
 
@@ -61,6 +62,7 @@ def summary(runs):
         for k, v in (r["groups_ms_per_step"] or {}).items():
             groups.setdefault(k, []).append(v)
     return {"ms_per_step": ms, "median_ms": statistics.median(ms), "spread_ms": max(ms) - min(ms),
+            "gpu_launches": sorted(set(r["gpu_launches"] for r in runs)),
             "e2e_median_ms": statistics.median(e2e),
             "groups_median_ms": {k: round(statistics.median(v), 4) for k, v in sorted(groups.items(), key=lambda kv: -statistics.median(kv[1]))}}
 
