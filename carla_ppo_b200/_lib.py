@@ -84,6 +84,7 @@ PROTOTYPES = {
                              _i32, _i32, _P, _P, _P, _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
+    "cpb_debug_mlpvae_buffer_offsets": (_i32, [_MC, _i32, _P, _i32]),
     "cpb_debug_tc_wgrad": (_i32, [_P, _P, _P, _i32, _i32, _i32, _i32, _P, _P]),
     "cpb_debug_tc_gemm": (_i32, [_P, _P, _P, _i32, _i32, _i32, _P, _P]),
     "cpb_get_math_mode": (_i32, []),

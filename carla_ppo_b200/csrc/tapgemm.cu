@@ -222,10 +222,11 @@ int32_t init_cfg() {
     return CPB_OK;
 }
 
-// out[e] = epilogue( sum_s partial[s][e] ) for the k-split dense problems: e runs over [ybatch][rows][N]
+// out[e] = epilogue( sum_s partial[s][e] ) for the k-split dense problems: e runs over [ybatch][rows][N]; the mask
+// (ybatch == 1 only) has the shape of dst
 __global__ void ksplit_reduce_kernel(const float* __restrict__ partial, long long stride, int ksplit, long long total,
                                      int N, long long ystride, const float* __restrict__ bias, long long bias_ystride,
-                                     int relu, float* __restrict__ dst) {
+                                     int relu, const float* __restrict__ mask, float* __restrict__ dst) {
     const long long e4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e4 * 4 >= total) return;
     const long long e = e4 * 4;
@@ -241,6 +242,10 @@ __global__ void ksplit_reduce_kernel(const float* __restrict__ partial, long lon
         a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
     }
     if (relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
+    if (mask != nullptr) {
+        const float4 mk = *reinterpret_cast<const float4*>(mask + e);
+        a.x = mk.x > 0.f ? a.x : 0.f; a.y = mk.y > 0.f ? a.y : 0.f; a.z = mk.z > 0.f ? a.z : 0.f; a.w = mk.w > 0.f ? a.w : 0.f;
+    }
     *reinterpret_cast<float4*>(dst + e) = a;
 }
 
@@ -277,12 +282,7 @@ int32_t launch_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
         CPB_REQUIRE(p.nclass == 1 && p.cls[0].Ho == 1 && p.cls[0].Wo == 1 && p.mask == nullptr && p.kpartial != nullptr &&
                     p.dst_pitch == p.N && p.N % 64 == 0, "tapgemm: k-split only for dense layers");
         CPB_TRY((launch_cfg<CPB_TILE_D>(p, stream)));
-        const long long total = p.ybatch > 1 ? (long long)p.ybatch * p.dst_ystride : (long long)p.batch * p.N;
-        ksplit_reduce_kernel<<<cdiv(total / 4, 256), 256, 0, stream>>>(p.kpartial, p.kpartial_stride, p.ksplit, total, p.N,
-                                                                     p.ybatch > 1 ? p.dst_ystride : 0, p.bias, p.bias_ystride,
-                                                                     p.relu, p.dst);
-        CPB_LAUNCHED();
-        return CPB_OK;
+        return launch_ksplit_reduce(p, stream);
     }
     if (p.N % 128 == 0) return launch_cfg<CPB_TILE_A>(p, stream);
     if (p.N % 64 == 0) {
@@ -290,6 +290,16 @@ int32_t launch_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
         return launch_cfg<CPB_TILE_B>(p, stream);
     }
     return launch_cfg<CPB_TILE_C>(p, stream);
+}
+
+int32_t launch_ksplit_reduce(const TapGemmParams& p, cudaStream_t stream) {
+    CPB_REQUIRE(p.mask == nullptr || p.ybatch == 1, "ksplit_reduce: a ReLU mask needs ybatch == 1");
+    const long long total = p.ybatch > 1 ? (long long)p.ybatch * p.dst_ystride : (long long)p.batch * p.N;
+    ksplit_reduce_kernel<<<cdiv(total / 4, 256), 256, 0, stream>>>(p.kpartial, p.kpartial_stride, p.ksplit, total, p.N,
+                                                                 p.ybatch > 1 ? p.dst_ystride : 0, p.bias, p.bias_ystride,
+                                                                 p.relu, p.mask, p.dst);
+    CPB_LAUNCHED();
+    return CPB_OK;
 }
 
 int tapgemm_pick_ksplit(int rows, int N, int ybatch, int K) {

@@ -54,9 +54,9 @@ struct TapGemmParams {
     int nclass;           // 1 or 4
     int ybatch;           // independent problems sharing src (fused heads): 1 or 2
     long long w_ystride, bias_ystride, dst_ystride;
-    int ksplit;           // >= 1; > 1 (SIMT path, dense layers only): the reduction is split over gridDim.z into
-    float* kpartial;      // kpartial[ksplit][kpartial_stride] raw partial results, then reduced with the epilogue
-    long long kpartial_stride;
+    int ksplit;           // >= 1; > 1 (dense layers only): the reduction is split (SIMT: over gridDim.z; tensor core:
+    float* kpartial;      // over the persistent work items) into kpartial[ksplit][kpartial_stride] raw partial
+    long long kpartial_stride;   // results, then reduced with the epilogue (launch_ksplit_reduce)
     // tensor-core path only: K-major per-tap [N][C] weight blocks, pre-split into hi / lo (tc_tapgemm.cu)
     const float* wk_hi;
     const float* wk_lo;
@@ -77,6 +77,8 @@ int32_t launch_tapgemm(const TapGemmParams& p, cudaStream_t stream);
 constexpr int kMaxKSplit = 8;
 // k-split factor for a dense [rows x K] x [K x N] layer with N % 64 == 0 (1 = do not split)
 int tapgemm_pick_ksplit(int rows, int N, int ybatch, int K);
+// dst = epilogue(sum over the p.ksplit slices of p.kpartial, in slice order): bias, ReLU, ReLU mask of p
+int32_t launch_ksplit_reduce(const TapGemmParams& p, cudaStream_t stream);
 // One-time opt-in for >48 KB dynamic shared memory (called from the API layer).
 int32_t tapgemm_init();
 
@@ -85,7 +87,8 @@ struct TcWeightJob {
     long long src_off;          // float offset of the TF kernel [k,k,Cb,Cs] in the parameter buffer
     long long dst_hi, dst_lo;   // float offset of the operand (2 * taps * N * C floats, hi and lo interleaved by block) / unused
     int mode;                   // logical operand per tap [N][C]:  0: plain K-major matrix; 1: gather form [kh][cs][kw*Cb+cb];
-                                // 2: quad scatter form [j][i][class*Cb+cb][cs], window w = (k+1)/2, zero where unused
+                                // 2: quad scatter form [j][i][class*Cb+cb][cs], window w = (k+1)/2, zero where unused;
+                                // 3: dense kernel stored [C][N] (TF [in][out]), transposed to K-major [N][C]
     int k, cb, cs;
     int N, C;                   // logical rows / reduction length per tap
     long long count;
@@ -101,6 +104,9 @@ struct TcWeightTable {
     TcWeightJob jobs[kMaxTcWeightJobs];
 };
 int32_t tc_tapgemm_init();
+// k-split factor of the tensor-core path for a dense layer reducing over K: a function of the shape only, so that a
+// frame's result never depends on the batch it is in
+int tc_tapgemm_pick_ksplit(int K);
 bool tc_tapgemm_supported(const TapGemmParams& p);
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream);
 int32_t launch_tc_weights(const float* params, float* dst, const TcWeightTable& table, cudaStream_t stream);

@@ -85,9 +85,14 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 // multicasts the slice into every CTA's stage, so a stage is free again only when the consumers of EVERY CTA of the
 // cluster are done with it (each consumer warp arrives on the stage's empty barrier in all CTAs).
 // The k-blocks of all super-tiles of a cluster form one stream through the stage ring; a chunk never spans two tiles.
-template <int BN, int PASSES>
+// K-split (KSPLIT instantiations, p.ksplit > 1, dense problems): the work items are (super-tile, split) pairs, split
+// fastest; item (st, ks) covers k-blocks [nkb*ks/ksplit, nkb*(ks+1)/ksplit) of the tile and stores its raw sums at
+// p.dst + ks * p.kpartial_stride (the launcher points dst at the partial buffer and clears the epilogue).  Without
+// KSPLIT the work items are the super-tiles and the split bookkeeping compiles away: the per-k-block loop of the
+// unsplit kernels keeps its instructions and registers.
+template <int BN, int PASSES, bool KSPLIT>
 __global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
-tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, const int total_st) {
+tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, const int total_w) {
     static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or a single TF32 pass");
     using Cfg = TcCfg<BN, PASSES>;
     constexpr int STAGES = Cfg::STAGES;
@@ -123,6 +128,9 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     auto st_y = [&](int st) { return st % ntn; };
     auto st_m0 = [&](int st) { return (long long)(((st / ntn) % mgroups) * CS + rank) * TBM; };
     const int kb_per_tap = p.C / TBK;
+    const int ksplit = KSPLIT ? p.ksplit : 1;
+    // first k-block of split ks of a tile with nkb k-blocks
+    auto split_kb = [&](int nkb, int ks) { return (int)((long long)nkb * ks / ksplit); };
 
     if (warp >= kLoaderWarp0) {
         // ================================ A loaders ================================
@@ -137,7 +145,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         constexpr int RPT = TBM / (kLoaderThreads / 8);     // rows per thread: 8
 
         // ---- A cursor: 8 threads cover the 128 bytes of one row, 16 rows per pass, 8 passes
-        int stA = cl_id, tapA = 0, cA = 0;
+        int wA = cl_id, stA = 0, tapA = 0, cA = 0;   // work item, its super-tile, tap and k offset inside the tap
+        int kbLeftA = 0;                        // k-blocks of the work item not yet issued
         int ntapsA = 0;
         int offA = 0;                           // taps[tapA].src_off + cA: float offset added to the row bases
         uint32_t tapbitA = 1u;
@@ -145,6 +154,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         uint32_t a_base[RPT];                     // float offset of the row's first tap position (< 2^31, checked at launch)
         uint32_t a_taps[RPT];                     // bit t: tap t of this row is inside the source image (0: row beyond M)
         auto setup_rows = [&]() {
+            stA = KSPLIT ? wA / ksplit : wA;
+            const int ksA = wA - stA * ksplit;
             clsA = &p.cls[st_z(stA)];
             ntapsA = clsA->ntaps;
             const int Wo = clsA->Wo, HoWo = clsA->Ho * Wo;
@@ -171,10 +182,20 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                 m += 16; rem += 16;
                 while (rem >= HoWo) { rem -= HoWo; ++n; }
             }
-            offA = (int)clsA->taps[0].src_off;
-            tapbitA = 1u;
+            if constexpr (KSPLIT) {
+                const int nkb = ntapsA * kb_per_tap;
+                const int kb0 = split_kb(nkb, ksA);
+                kbLeftA = split_kb(nkb, ksA + 1) - kb0;
+                tapA = kb0 / kb_per_tap;
+                cA = (kb0 - tapA * kb_per_tap) * TBK;
+                offA = (int)clsA->taps[tapA].src_off + cA;
+                tapbitA = 1u << tapA;
+            } else {
+                offA = (int)clsA->taps[0].src_off;
+                tapbitA = 1u;
+            }
         };
-        if (stA < total_st) setup_rows();
+        if (wA < total_w) setup_rows();
         // copies the cursor's k-block into stage `stage` and advances the cursor
         auto issue_a = [&](uint32_t stage, uint64_t* full) {
             const uint32_t dst = stage + a_soff0;
@@ -188,12 +209,22 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             }
             asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(full)) : "memory");
             cA += TBK; offA += TBK;
-            if (cA == p.C) {
+            if constexpr (KSPLIT) {
+                if (--kbLeftA == 0) {
+                    wA += cl_n;
+                    if (wA < total_w) setup_rows();
+                } else if (cA == p.C) {
+                    cA = 0;
+                    ++tapA;
+                    offA = (int)clsA->taps[tapA].src_off;
+                    tapbitA <<= 1;
+                }
+            } else if (cA == p.C) {
                 cA = 0;
                 if (++tapA == ntapsA) {
                     tapA = 0;
-                    stA += cl_n;
-                    if (stA < total_st) setup_rows();
+                    wA += cl_n;
+                    if (wA < total_w) setup_rows();
                 } else {
                     offA = (int)clsA->taps[tapA].src_off;
                     tapbitA <<= 1;
@@ -218,7 +249,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         // ---- copy stream: the loaders run ahead of the tensor core by as many k-blocks as there are free stages
         int sS = 0;                                 // stage of the next k-block and the parity its empty barrier
         uint32_t phS = 1;                           // shows once free (fresh barrier: parity 1 counts as complete)
-        while (stA < total_st) {
+        while (wA < total_w) {
             mbar_wait(&empty_bar[sS], phS);
             if (tl == 0) issue_b(smem_base + sS * STAGE_BYTES, &full_bar[sS]);
             issue_a(smem_base + sS * STAGE_BYTES, &full_bar[sS]);
@@ -234,8 +265,9 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 #pragma unroll
         for (int i = 0; i < HALF; ++i) { acc[i] = 0.f; dm[i] = 0.f; dc[i] = 0.f; }
 
-        auto epilogue = [&](int st) {                // bias / ReLU / mask -> global, from the register accumulators
+        auto epilogue = [&](int st, int ks) {        // bias / ReLU / mask -> global, from the register accumulators
             const TapClass& cls = p.cls[st_z(st)];
+            float* const dst = KSPLIT ? p.dst + (long long)ks * p.kpartial_stride : p.dst;
             const int Wo = cls.Wo, HoWo = cls.Ho * Wo;
             const int col0 = st_y(st) * BN + 2 * (lane & 3);
             const int lcb = p.quad_lcb;              // log2(quad_cb)
@@ -290,7 +322,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                         }
                         if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
                         if (p.mask) { o.x = mks[u].x > 0.f ? o.x : 0.f; o.y = mks[u].y > 0.f ? o.y : 0.f; }
-                        *reinterpret_cast<float2*>(p.dst + offs[u]) = o;
+                        *reinterpret_cast<float2*>(dst + offs[u]) = o;
                     }
                 }
             }
@@ -312,8 +344,10 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         const uint32_t a_swz = (uint32_t)((r0 & 7) << 4);
 
         int g = 0;                                   // k-blocks consumed so far (all tiles)
-        for (int st = cl_id; st < total_st; st += cl_n) {
-            const int nkb = p.cls[st_z(st)].ntaps * kb_per_tap;
+        for (int w = cl_id; w < total_w; w += cl_n) {
+            const int st = KSPLIT ? w / ksplit : w, ks = KSPLIT ? w - st * ksplit : 0;
+            const int nkb_tile = p.cls[st_z(st)].ntaps * kb_per_tap;
+            const int nkb = KSPLIT ? split_kb(nkb_tile, ks + 1) - split_kb(nkb_tile, ks) : nkb_tile;
             for (int kb = 0; kb < nkb; ++kb, ++g) {
                 const int s = g % STAGES;
                 const uint32_t stage = smem_base + s * STAGE_BYTES;
@@ -379,7 +413,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                     }
                 }
             }
-            epilogue(st);
+            epilogue(st, ks);
 #pragma unroll
             for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
         }
@@ -391,8 +425,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 constexpr int tc_bn_slot(int BN) { return BN == 64 ? 1 : 0; }
 constexpr int tc_passes_slot(int PASSES) { return PASSES == 1 ? 1 : 0; }
 
-template <int BN, int PASSES>
-int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_st, unsigned grid, cudaStream_t stream) {
+template <int BN, int PASSES, bool KSPLIT>
+int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_w, unsigned grid, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
@@ -403,7 +437,7 @@ int32_t tc_launch_t(const TapGemmParams& p, int mgroups, int total_st, unsigned 
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = (unsigned)p.cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
-    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN, PASSES>, p, mgroups, total_st));
+    CPB_CUDA(cudaLaunchKernelEx(&cfg, tc_tapgemm_kernel<BN, PASSES, KSPLIT>, p, mgroups, total_w));
     CPB_LAUNCHED();
     return CPB_OK;
 }
@@ -420,9 +454,9 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     p.cluster = g_tc_cluster;
     const long long mtiles = (max_m + TBM - 1) / TBM;
     const long long mgroups = (mtiles + p.cluster - 1) / p.cluster;
-    const long long total_st = mgroups * (p.N / BN) * p.nclass;
+    const long long total_w = mgroups * (p.N / BN) * p.nclass * p.ksplit;
     const int resident = g_tc_clusters[tc_passes_slot(PASSES)][tc_bn_slot(BN)];
-    CPB_REQUIRE(total_st < (1ll << 30) && resident > 0, "tc_tapgemm: bad tile count");
+    CPB_REQUIRE(total_w < (1ll << 30) && resident > 0, "tc_tapgemm: bad tile count");
     CPB_REQUIRE((long long)p.batch * p.src_img < (1ll << 31) && (long long)p.batch * p.dst_img < (1ll << 31),
                 "tc_tapgemm: tensors too large for 32-bit row offsets");
     for (int c = 0; c < p.nclass; ++c) CPB_REQUIRE(p.cls[c].ntaps <= 32, "tc_tapgemm: more than 32 taps");
@@ -431,15 +465,29 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
         p.quad_lcb = 0;
         while ((1 << p.quad_lcb) < p.quad_cb) ++p.quad_lcb;
     }
-    const unsigned grid = (unsigned)((total_st < resident ? total_st : resident) * p.cluster);
-    return tc_launch_t<BN, PASSES>(p, (int)mgroups, (int)total_st, grid, stream);
+    const unsigned grid = (unsigned)((total_w < resident ? total_w : resident) * p.cluster);
+    if (p.ksplit == 1) return tc_launch_t<BN, PASSES, false>(p, (int)mgroups, (int)total_w, grid, stream);
+    if constexpr (PASSES == 1) {
+        // raw split sums into kpartial; the reduction adds them in split order and applies p's epilogue
+        TapGemmParams q = p;
+        q.dst = p.kpartial; q.bias = nullptr; q.mask = nullptr; q.relu = 0;
+        CPB_TRY((tc_launch_t<BN, PASSES, true>(q, (int)mgroups, (int)total_w, grid, stream)));
+        return launch_ksplit_reduce(p, stream);
+    } else {
+        CPB_REQUIRE(false, "tc_tapgemm: the k-split is built for the single TF32 pass only");
+        return CPB_ERR_UNSUPPORTED;
+    }
 }
 
 template <int BN, int PASSES>
 int32_t tc_init_one() {
     using Cfg = TcCfg<BN, PASSES>;
-    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    if constexpr (PASSES == 1) {   // the k-split variant: same threads and shared memory, so the same resident count
+        CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    }
     // how many clusters of this kernel are co-resident (GPC boundaries can strand SMs for cluster sizes > 1)
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -451,7 +499,7 @@ int32_t tc_init_one() {
     attr.val.clusterDim.x = (unsigned)g_tc_cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr; cfg.numAttrs = 1;
     int n = 0;
-    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN, PASSES>, &cfg));
+    CPB_CUDA(cudaOccupancyMaxActiveClusters(&n, tc_tapgemm_kernel<BN, PASSES, false>, &cfg));
     CPB_REQUIRE(n > 0, "tc_tapgemm: no resident cluster of %d CTAs possible", g_tc_cluster);
     g_tc_clusters[tc_passes_slot(PASSES)][tc_bn_slot(BN)] = n;
     return CPB_OK;
@@ -461,7 +509,7 @@ int32_t tc_init_one() {
 // (n-tile y of BN rows, k-block kc of 32 floats) one block [hi image | lo image], each image the BN x 128-byte
 // SWIZZLE_128B shared-memory tile exactly as the tensor core reads it -- so a k-block's operand is ONE contiguous
 // 2*BN*128-byte bulk copy (tc_tapgemm_kernel, weight-tile producer).  job.round_nearest: hi = x rounded to the nearest
-// TF32 value (the single-pass operand; lo = x - hi is written but not read) instead of x truncated.
+// TF32 value (the single-pass operand; the lo image is left unwritten) instead of x truncated.
 __global__ void tc_weights_kernel(const float* __restrict__ params, float* __restrict__ dst, const __grid_constant__ TcWeightTable t) {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= t.total) return;
@@ -474,6 +522,11 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
         // plain K-major matrix [N][C], one tap
         tap = 0; n = (int)(idx / job.C); c = (int)(idx % job.C);
         x = params[job.src_off + idx];
+    } else if (job.mode == 3) {
+        // dense kernel stored [C][N]: strided reads (neighbouring n of later threads hit the same lines in L2),
+        // coalesced image writes
+        tap = 0; n = (int)(idx / job.C); c = (int)(idx % job.C);
+        x = params[job.src_off + (long long)c * job.N + n];
     } else if (job.mode == 2) {
         // quad scatter form: logical [j][i][class*Cb + cb][cs]; class (py,px) uses kernel tap (py+2j, px+2i)
         const int w = (job.k + 1) / 2;
@@ -503,7 +556,7 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
     const long long at = job.dst_hi + block * (2 * BN * TBK) + (nn >> 3) * 256 + (nn & 7) * 32 + ((((cc >> 2) ^ (nn & 7))) << 2) + (cc & 3);
     const float hi = job.round_nearest ? __uint_as_float(round_tf32(x)) : __uint_as_float(__float_as_uint(x) & 0xffffe000u);
     dst[at] = hi;
-    dst[at + BN * TBK] = x - hi;
+    if (!job.round_nearest) dst[at + BN * TBK] = x - hi;    // the single pass never reads the lo image
 }
 
 }  // namespace
@@ -521,9 +574,21 @@ int32_t tc_tapgemm_init() {
     return CPB_OK;
 }
 
+int tc_tapgemm_pick_ksplit(int K) {
+    // splits of at most 320 k-blocks, at most 4 of them: the MlpVAE's 38 400-long reductions into 512 columns run as
+    // 4 splits of 300 k-blocks, which at B = 512 (32 output tiles) fills the 132 SMs of an H100 SXM in one wave
+    const int s = (int)cdiv(K / TBK, 320);
+    return s < 1 ? 1 : (s > 4 ? 4 : s);
+}
+
 bool tc_tapgemm_supported(const TapGemmParams& p) {
     if (p.quad && (p.N != 4 * p.quad_cb || p.nclass != 1)) return false;
-    return p.ybatch == 1 && p.C % TBK == 0 && (p.N == 32 || p.N % 64 == 0) && p.wk_hi != nullptr && p.wk_lo != nullptr;
+    if (p.ksplit < 1 || p.ksplit > kMaxKSplit) return false;
+    // k-split: dense problems only (one output row per image), with room for the raw sums
+    if (p.ksplit > 1 && (p.nclass != 1 || p.quad || p.cls[0].Ho != 1 || p.cls[0].Wo != 1 || p.dst_pitch != p.N ||
+                         p.kpartial == nullptr || p.cls[0].ntaps * (p.C / TBK) < p.ksplit))
+        return false;
+    return p.ybatch == 1 && p.C % TBK == 0 && p.N % 32 == 0 && p.N > 0 && p.wk_hi != nullptr && p.wk_lo != nullptr;
 }
 
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {

@@ -689,8 +689,12 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
 
 // =============================================================================================
 // MlpVAE (reference vae/models.py:271-299): flatten -> dense E1 relu -> dense E2 relu -> [mean | logstd_sq] -> sample ->
-// dense D1 relu -> dense D2 relu -> dense 12800*Ct -> logits.  Same loss / sampling / Adam kernels as the ConvVAE; all
-// seven layers run on the fp32 SIMT tap-GEMM (dense form) and the SIMT weight-gradient kernel.
+// dense D1 relu -> dense D2 relu -> dense 12800*Ct -> logits.  Same loss / sampling / Adam kernels as the ConvVAE; the
+// seven layers run on the fp32 SIMT tap-GEMM (dense form) and the SIMT weight-gradient kernel, except in math mode 2:
+// there the five frame-wide products -- encoder/dense forward and weight gradient, decoder/dense_2 forward, data
+// gradient and weight gradient, 99 % of the step's multiply-adds -- run as ONE TF32 wgmma pass with both operands
+// rounded to nearest (the forward passes and the data gradient on the tensor-core tap-GEMM, k-split where they reduce
+// over a frame, the weight gradients on tc_wgrad).
 // =============================================================================================
 enum MlpTensor { M_E1_K, M_E1_B, M_E2_K, M_E2_B, M_MEAN_K, M_MEAN_B, M_LOGVAR_K, M_LOGVAR_B, M_D1_K, M_D1_B, M_D2_K, M_D2_B, M_D3_K, M_D3_B, M_COUNT };
 static const char* kMlpNames[M_COUNT] = {
@@ -731,9 +735,30 @@ struct MlpPlan {
     int64_t tE2, tHeads, tD1, tD2, tD3;      // float offsets of the transposed kernels inside wT
     float* wP;                               // z < z_pad only: zero-padded heads [2][enc2][z_pad], biases [2][z_pad], D1 [z_pad][dec1]
     int64_t pHeads, pHeadsB, pD1;
+    // math mode 2 only (tc): TF32 weight images of the frame-wide layers inside wTc -- encoder/dense K-major [e1][IN]
+    // (every mode), decoder/dense_2 K-major [OUT][d2] (forward and train) and as stored [d2][OUT] (train, data
+    // gradient) -- and tcScratch for the k-split partials and the tensor-core weight-gradient partials
+    bool tc;
+    float *wTc, *tcScratch;
+    int64_t iE1, iD3f, iD3t;
     int64_t bytes;
     bool ok;
 };
+
+// The tensor-core kernels address a frame-wide operand with 32-bit offsets (B * 38 400 < 2^31, i.e. B <= 55 923):
+// a larger batch runs the five products on the fp32 SIMT kernels in every mode.
+static bool mlp_tc_batch_ok(int64_t b, int in) { return b * in < (1LL << 31); }
+
+static int64_t mlp_tc_scratch_floats(const MlpPlan& p, int mode) {
+    const int64_t b = p.B;
+    int64_t n = (int64_t)tc_tapgemm_pick_ksplit(p.IN) * b * p.e1;                              // encoder/dense fwd
+    if (mode >= CPB_WS_TRAIN) {
+        n = std::max<int64_t>(n, (int64_t)tc_tapgemm_pick_ksplit(p.OUT) * b * p.d2);         // decoder/dense_2 dgrad
+        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.IN, p.e1, b) * p.IN * p.e1);
+        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.OUT, p.d2, b) * p.OUT * p.d2);
+    }
+    return n;
+}
 
 static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config* c, int mode) {
     MlpPlan p;
@@ -781,6 +806,17 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config
         p.partial = a.take<float>(best);
         p.colsum = a.take<float>(colsum_scratch_floats(b, p.OUT) + colsum_scratch_floats(b, (int)widest));
     }
+    // last, so that modes 0 and 1 and every buffer above keep their sizes and offsets
+    p.tc = g_math_mode == 2 && mlp_tc_batch_ok(b, p.IN);
+    if (p.tc) {
+        int64_t o = 0;
+        auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
+        p.iE1 = take(2LL * p.e1 * p.IN);
+        if (mode >= CPB_WS_FORWARD) p.iD3f = take(2LL * p.OUT * p.d2);
+        if (mode >= CPB_WS_TRAIN) p.iD3t = take(2LL * p.d2 * p.OUT);
+        p.wTc = a.take<float>(o);
+        p.tcScratch = a.take<float>(mlp_tc_scratch_floats(p, mode));
+    }
     p.bytes = a.off;
     p.ok = ws == nullptr || !a.overflow;
     return p;
@@ -798,12 +834,58 @@ static int32_t mlp_pad_weights(const MlpPlan& pl, const MlpLayout& L, const floa
     return launch_relayout(params, pl.wP, t, s);
 }
 
+// math mode 2: the TF32 weight images (rounded to nearest) of the frame-wide products the call runs (one launch)
+static int32_t mlp_tc_weights(const MlpPlan& pl, const MlpLayout& L, const float* params, bool encoder, bool decoder,
+                              bool backward, cudaStream_t s) {
+    if (!pl.tc) return CPB_OK;
+    TcWeightTable w;
+    memset(&w, 0, sizeof(w));
+    auto add = [&](int tensor, int64_t dst, int mode, int N, int C) {
+        TcWeightJob& j = w.jobs[w.njobs++];
+        j.src_off = L.off[tensor]; j.dst_hi = j.dst_lo = dst; j.mode = mode; j.N = N; j.C = C; j.round_nearest = 1;
+        j.count = (long long)N * C; w.total += j.count;
+    };
+    if (encoder) add(M_E1_K, pl.iE1, 3, pl.e1, pl.IN);       // [e1][IN] from the kernel [IN][e1]
+    if (decoder) add(M_D3_K, pl.iD3f, 3, pl.OUT, pl.d2);     // [OUT][d2] from the kernel [d2][OUT]
+    if (backward) add(M_D3_K, pl.iD3t, 0, pl.d2, pl.OUT);    // the kernel as stored: the data gradient's [N = d2][K = OUT]
+    ProfScope prof("mlp.tc_weights", s);
+    return launch_tc_weights(params, pl.wTc, w, s);
+}
+
+// a dense layer: one TF32 pass on the tensor-core tap-GEMM when `image` (its weight image) is given, k-split over
+// tcScratch where the reduction is frame-wide; the fp32 SIMT tap-GEMM otherwise
+static int32_t mlp_dense(const char* label, const MlpPlan& pl, TapGemmParams p, const float* image, cudaStream_t s) {
+    ProfScope prof(label, s);
+    if (image == nullptr) return launch_tapgemm(p, s);
+    p.wk_hi = p.wk_lo = image;        // single pass: the hi image only (the lo slots of the interleaved image are unused)
+    p.passes = 1;
+    p.ksplit = tc_tapgemm_pick_ksplit(p.C);
+    if (p.ksplit > 1) { p.kpartial = pl.tcScratch; p.kpartial_stride = (long long)p.batch * p.N; }
+    return launch_tc_tapgemm(p, s);
+}
+
+// math mode 2: out = big[B, I]^T small[B, J] as one TF32 pass on tc_wgrad (I >= 128); transposed: out is [J][I]
+static int32_t run_tc_dense_wgrad(const char* label, const float* big, int I, const float* small, int J, int B, float* partial,
+                                  float* out, bool transposed, cudaStream_t s) {
+    ProfScope prof(label, s);
+    WgradParams w;
+    memset(&w, 0, sizeof(w));
+    w.big = big; w.small = small; w.partial = partial;
+    w.batch = B; w.Wb = 1; w.big_pitch = I; w.big_img = I; w.Ho = w.Wo = 1; w.sstride = 1;
+    w.ntaps = 1; w.run = I; w.tap_off[0] = 0; w.I = I; w.J = J; w.passes = 1;
+    w.splits = tc_wgrad_pick_splits(I, J, B);
+    w.m_per_split = align_up(((long long)B + w.splits - 1) / w.splits, 32);
+    CPB_TRY(launch_tc_wgrad(w, s));
+    if (transposed) return launch_reduce_partials_t(partial, w.splits, I, J, out, s);
+    return launch_reduce_partials(partial, w.splits, I, J, I, I, J, out, s);
+}
+
 static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
                            int32_t* flags, cudaStream_t s) {
     const float sscale = c->base.source_dtype == CPB_FRAME_U8 ? 1.f / 255.f : 1.f;
     CPB_TRY(launch_prep_flat(source, c->base.source_dtype, sscale, (long long)pl.B * pl.IN, pl.x, flags, 1, s));
     TapGemmParams p = dense_problem(pl.x, pl.B, pl.IN, params + L.off[M_E1_K], pl.e1, params + L.off[M_E1_B], nullptr, pl.h1, 1);
-    CPB_TRY(launch_tapgemm(p, s));
+    CPB_TRY(mlp_dense("mlp.enc.fwd", pl, p, pl.tc ? pl.wTc + pl.iE1 : nullptr, s));
     p = dense_problem(pl.h1, pl.B, pl.e1, params + L.off[M_E2_K], pl.e2, params + L.off[M_E2_B], nullptr, pl.h2, 1);
     CPB_TRY(launch_tapgemm(p, s));
     const bool padded = pl.zp != pl.z;
@@ -823,7 +905,7 @@ static int32_t mlp_decoder(const MlpPlan& pl, const MlpLayout& L, const float* p
     p = dense_problem(pl.g1, pl.B, pl.d1, params + L.off[M_D2_K], pl.d2, params + L.off[M_D2_B], nullptr, pl.g2, 1);
     CPB_TRY(launch_tapgemm(p, s));
     p = dense_problem(pl.g2, pl.B, pl.d2, params + L.off[M_D3_K], pl.OUT, params + L.off[M_D3_B], nullptr, logits, 0);
-    return launch_tapgemm(p, s);
+    return mlp_dense("mlp.dec2.fwd", pl, p, pl.tc ? pl.wTc + pl.iD3f : nullptr, s);
 }
 
 static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
@@ -859,14 +941,18 @@ static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlp
     add(L.off[M_MEAN_K], pl.tHeads, 2, pl.e2, z, pl.e2, zp);      // [2][z_pad][enc2]
     add(L.off[M_D1_K], pl.tD1, 1, z, pl.d1, zp, pl.d1);           // [dec1][z_pad]
     add(L.off[M_D2_K], pl.tD2, 1, pl.d1, pl.d2, pl.d1, pl.d2);
-    add(L.off[M_D3_K], pl.tD3, 1, pl.d2, pl.OUT, pl.d2, pl.OUT);
+    if (!pl.tc) add(L.off[M_D3_K], pl.tD3, 1, pl.d2, pl.OUT, pl.d2, pl.OUT);    // mode 2 reads the TF32 image iD3t instead
     CPB_TRY(launch_relayout(params, pl.wT, t, s));
     TapGemmParams p;
-    // ---- decoder
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g2, pl.d2, pl.d2, dlog, B, pl.OUT, pl.OUT, pl.partial, grads + L.off[M_D3_K], s));
+    // ---- decoder.  Mode 2: decoder/dense_2's weight gradient runs as its transpose dlog^T g2 (I = OUT >= 12 800 rows,
+    // J = dec2 columns: tc_wgrad needs I >= 128 and dec2 may be 32), transposed back in the split reduction.
+    if (pl.tc)
+        CPB_TRY(run_tc_dense_wgrad("mlp.dec2.wgrad", dlog, pl.OUT, pl.g2, pl.d2, B, pl.tcScratch, grads + L.off[M_D3_K], true, s));
+    else
+        CPB_TRY(run_dense_wgrad("mlp.dec2.wgrad", pl.g2, pl.d2, pl.d2, dlog, B, pl.OUT, pl.OUT, pl.partial, grads + L.off[M_D3_K], s));
     CPB_TRY(launch_colsum(dlog, B, pl.OUT, pl.OUT, grads + L.off[M_D3_B], cs, s));
     p = dense_problem(dlog, B, pl.OUT, pl.wT + pl.tD3, pl.d2, nullptr, pl.g2, pl.ga, 0);                       // ga = g(g2 pre-activation)
-    CPB_TRY(launch_tapgemm(p, s));
+    CPB_TRY(mlp_dense("mlp.dec2.dgrad", pl, p, pl.tc ? pl.wTc + pl.iD3t : nullptr, s));
     CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g1, pl.d1, pl.d1, pl.ga, B, pl.d2, pl.d2, pl.partial, grads + L.off[M_D2_K], s));
     CPB_TRY(launch_colsum(pl.ga, B, pl.d2, pl.d2, grads + L.off[M_D2_B], cs, s));
     p = dense_problem(pl.ga, B, pl.d2, pl.wT + pl.tD2, pl.d1, nullptr, pl.g1, pl.gb, 0);                         // gb = g(g1 pre-activation)
@@ -893,7 +979,10 @@ static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlp
     CPB_TRY(launch_colsum(pl.ga, B, pl.e2, pl.e2, grads + L.off[M_E2_B], cs, s));
     p = dense_problem(pl.ga, B, pl.e2, pl.wT + pl.tE2, pl.e1, nullptr, pl.h1, pl.gb, 0);                         // gb = g(h1 pre-activation)
     CPB_TRY(launch_tapgemm(p, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.x, pl.IN, pl.IN, pl.gb, B, pl.e1, pl.e1, pl.partial, grads + L.off[M_E1_K], s));
+    if (pl.tc)
+        CPB_TRY(run_tc_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, pl.gb, pl.e1, B, pl.tcScratch, grads + L.off[M_E1_K], false, s));
+    else
+        CPB_TRY(run_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, pl.IN, pl.gb, B, pl.e1, pl.e1, pl.partial, grads + L.off[M_E1_K], s));
     return launch_colsum(pl.gb, B, pl.e1, pl.e1, grads + L.off[M_E1_B], cs, s);
 }
 
@@ -1207,6 +1296,18 @@ int32_t cpb_mlpvae_layout(const cpb_mlpvae_config* cfg, int64_t* offsets, int64_
     return CPB_OK;
 }
 
+/* debug: byte offsets of the named MlpVAE workspace buffers for (cfg, mode) in the current math mode; returns the count */
+int32_t cpb_debug_mlpvae_buffer_offsets(const cpb_mlpvae_config* cfg, int32_t mode, int64_t* offsets, int32_t capacity) {
+    CPB_TRY(check_mlp_cfg(cfg));
+    CPB_REQUIRE(mode >= CPB_WS_ENCODE && mode <= CPB_WS_TRAIN, "bad workspace mode %d", mode);
+    char* base = (char*)4096;   // fake non-null base: only differences are used
+    MlpPlan pl = make_mlp_plan(base, (int64_t)1 << 60, cfg, mode);
+    const float* ptrs[] = {pl.x, pl.h1, pl.h2, pl.heads, pl.zbuf, pl.g1, pl.g2, pl.logits, pl.ga, pl.gb};
+    const int n = (int)(sizeof(ptrs) / sizeof(ptrs[0]));
+    for (int i = 0; i < n && i < capacity; ++i) offsets[i] = ptrs[i] ? (int64_t)((const char*)ptrs[i] - base) : -1;
+    return n;
+}
+
 int64_t cpb_mlpvae_workspace_bytes(const cpb_mlpvae_config* cfg, int32_t mode) {
     if (check_mlp_cfg(cfg) != CPB_OK || mode < 0 || mode > 2) return CPB_ERR_INVALID_ARGUMENT;
     return make_mlp_plan(nullptr, 0, cfg, mode).bytes;
@@ -1229,6 +1330,7 @@ int32_t cpb_mlpvae_encode(const cpb_mlpvae_config* cfg, const float* params, con
     CPB_MLP_PLAN(CPB_WS_ENCODE);
     CPB_REQUIRE(params && source && mean, "mlp encode: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
+    CPB_TRY(mlp_tc_weights(pl, L, params, true, false, false, s));
     CPB_TRY(mlp_encoder(pl, L, cfg, params, source, flags, s));
     CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
     if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
@@ -1240,6 +1342,7 @@ int32_t cpb_mlpvae_decode(const cpb_mlpvae_config* cfg, const float* params, con
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && z && reconstruction, "mlp decode: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
+    CPB_TRY(mlp_tc_weights(pl, L, params, false, true, false, s));
     if (pl.zp != pl.z) {
         CPB_TRY(launch_pitch_copy(z, pl.z, pl.zbuf, pl.zp, pl.B, s));
         z = pl.zbuf;
@@ -1254,6 +1357,7 @@ int32_t cpb_mlpvae_forward(const cpb_mlpvae_config* cfg, const float* params, co
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && source && target && losses, "mlp forward: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
+    CPB_TRY(mlp_tc_weights(pl, L, params, true, true, false, s));
     CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, false, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
     if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
@@ -1268,6 +1372,7 @@ int32_t cpb_mlpvae_loss_grad(const cpb_mlpvae_config* cfg, const float* params, 
     CPB_MLP_PLAN(CPB_WS_TRAIN);
     CPB_REQUIRE(params && source && target && grads && losses, "mlp loss_grad: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
+    CPB_TRY(mlp_tc_weights(pl, L, params, true, true, true, s));
     CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, true, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
     return mlp_backward(pl, L, cfg, params, eps, grads, s);

@@ -198,7 +198,33 @@ reduce_partials_kernel(const float* __restrict__ partial, int splits, long long 
     out[((long long)t * c_real + c) * j_real + j] = tot;
 }
 
+// out[j][i] = sum_s partial[s][i][j] (splits in order) through a 32 x 32 shared-memory tile: reads and writes coalesced
+__global__ void __launch_bounds__(256)
+reduce_partials_t_kernel(const float* __restrict__ partial, int splits, int I, int J, float* __restrict__ out) {
+    __shared__ float tile[32][33];
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int i0 = blockIdx.x * 32, j0 = blockIdx.y * 32;
+    const long long IJ = (long long)I * J;
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) {
+        const long long at = (long long)(i0 + r) * J + j0 + tx;
+        float s = 0.f;
+        for (int k = 0; k < splits; ++k) s += partial[(long long)k * IJ + at];
+        tile[r][tx] = s;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) out[(long long)(j0 + r) * I + i0 + tx] = tile[tx][r];
+}
+
 }  // namespace
+
+int32_t launch_reduce_partials_t(const float* partial, int splits, int I, int J, float* out, cudaStream_t stream) {
+    CPB_REQUIRE(I % 32 == 0 && J % 32 == 0 && splits >= 1, "reduce_partials_t: I=%d, J=%d must be multiples of 32", I, J);
+    reduce_partials_t_kernel<<<dim3((unsigned)(I / 32), (unsigned)(J / 32)), 256, 0, stream>>>(partial, splits, I, J, out);
+    CPB_LAUNCHED();
+    return CPB_OK;
+}
 
 int32_t wgrad_init() {
     CPB_TRY((init_cfg<CPB_WG_A>()));

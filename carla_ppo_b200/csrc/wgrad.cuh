@@ -47,5 +47,7 @@ int32_t launch_tc_wgrad(const WgradParams& p, cudaStream_t stream);
 // out[(t*c_real + c)*j_real + j] = sum_s partial[s][(t*c_pad + c)][j]   for c < c_real, j < j_real
 int32_t launch_reduce_partials(const float* partial, int splits, int I, int J, int c_pad, int c_real, int j_real,
                                float* out, cudaStream_t stream);
+// out[j][i] = sum_s partial[s][i][j]  (I, J multiples of 32): a weight gradient computed as its transpose
+int32_t launch_reduce_partials_t(const float* partial, int splits, int I, int J, float* out, cudaStream_t stream);
 
 }  // namespace cpb

@@ -767,7 +767,11 @@ class ConvVAE(VAE):
 class MlpVAE(VAE):
     """The reference's dense VAE (vae/models.py:271-299): flatten -> dense(encoder_sizes, relu) -> mean / logstd_sqare ->
     sample -> dense(decoder_sizes, relu) -> dense(prod(target_shape)) = logits.  Same surface as ConvVAE; the seven
-    dense layers run on the fp32 SIMT kernels of the library (cpb_mlpvae_* entry points)."""
+    dense layers run on the fp32 SIMT kernels of the library (cpb_mlpvae_* entry points) in math modes 0 and 1.  In
+    math mode 2 (cpb_set_math_mode(2), ``train_vae.py --math_mode tf32``) the five frame-wide products --
+    encoder/dense forward and weight gradient, decoder/dense_2 forward, data gradient and weight gradient -- run as one
+    TF32 tensor-core pass with both operands rounded to nearest (not fp32-accurate); the rest runs as in mode 1.  The
+    workspace is re-sized on every call, so switching the mode between calls is safe."""
 
     _API = {"num_tensors": "cpb_mlpvae_num_tensors", "tensor_name": "cpb_mlpvae_tensor_name", "encode": "cpb_mlpvae_encode",
             "decode": "cpb_mlpvae_decode", "forward": "cpb_mlpvae_forward", "loss_grad": "cpb_mlpvae_loss_grad"}

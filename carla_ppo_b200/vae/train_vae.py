@@ -60,7 +60,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--models_root", type=str, default="models", help="(addition) parent directory of the model directories")
     p.add_argument("--math_mode", choices=sorted(MATH_MODES), default="3xtf32",
                    help="(addition) arithmetic of the ConvVAE's conv2-4 / deconv1-3 layers: 3xtf32 (fp32-accurate), "
-                        "tf32 (one TF32 tensor-core pass, not fp32-accurate) or simt (fp32 FMA)")
+                        "tf32 (one TF32 tensor-core pass, not fp32-accurate) or simt (fp32 FMA).  The MlpVAE "
+                        "(--model_type mlp) runs fp32 SIMT under simt and 3xtf32; tf32 runs its encoder/dense and "
+                        "decoder/dense_2 products (forward and gradients) as one TF32 tensor-core pass")
     return p
 
 

@@ -150,6 +150,13 @@ int32_t cpb_vae_train_step_host(const cpb_vae_config* cfg, float* params, float*
  * above (flat parameter buffer described by cpb_mlpvae_layout, caller-owned workspace, same loss / flag semantics); the
  * optimiser is cpb_adam_apply(_guarded) on the flat buffers.  14 variables: encoder/dense{,_1}, mean, logstd_sqare,
  * decoder/dense{,_1,_2}, each {kernel [in,out], bias}.
+ * Arithmetic: fp32 SIMT in math modes 0 and 1.  In math mode 2 (cpb_set_math_mode) the five frame-wide products --
+ * encoder/dense forward and weight gradient, decoder/dense_2 forward, data gradient and weight gradient (99 % of the
+ * step's multiply-adds) -- run as ONE TF32 wgmma pass with both operands rounded to nearest; everything else
+ * (encoder/dense_1, the heads, decoder/dense, decoder/dense_1, sampling, loss, Adam) runs as in the other modes.
+ * Batches with batch * 38400 >= 2^31 run those five products on the fp32 kernels in every mode.
+ * cpb_mlpvae_workspace_bytes depends on the math mode at the time of the query: mode 2 adds the TF32 weight images
+ * and the split partials, and a mode-2 call given a smaller workspace fails with CPB_ERR_WORKSPACE_TOO_SMALL.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
     cpb_vae_config base;               /* batch, target_channels, z_dim, loss, dtypes, beta, kl_tolerance, loss_scale */
@@ -259,15 +266,20 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
  *               The comparable setting of cuDNN / TensorFlow on this hardware is their TF32 default.
  * Modes 1 and 2 cover the same layers of the ConvVAE: forward, data gradient and weight gradient of conv2-4 and
  * deconv1-3, in every entry point that runs them (encode, decode, forward, loss_grad, train_step(_host),
- * cpb_encode_predict).  conv1, deconv4, the heads, dense1, the dense weight gradients, the MlpVAE and PPO use the
- * fp32 kernels in every mode.  The mode is process-global and read when a call is enqueued; other values are
- * rejected (CPB_ERR_INVALID_ARGUMENT). */
+ * cpb_encode_predict).  conv1, deconv4, the heads, dense1, the dense weight gradients and PPO use the fp32 kernels
+ * in every mode.  The MlpVAE uses the fp32 kernels in modes 0 and 1; mode 2 also runs its five frame-wide products
+ * (encoder/dense forward + weight gradient, decoder/dense_2 forward + data gradient + weight gradient) as one TF32
+ * pass (see the MlpVAE section).  The mode is process-global and read when a call is enqueued (and by the MlpVAE
+ * workspace query); other values are rejected (CPB_ERR_INVALID_ARGUMENT). */
 int32_t cpb_set_math_mode(int32_t mode);
 /* Debug / test hooks (not part of the reference-facing surface): workspace buffer offsets in bytes for
  * [xp,a1,a2,a3,a4,heads,z,d1,b1,b2,b3,logits_p,gA,gB,frame_loss,kl_rows] (-1 = absent in that mode), and a dense
  * D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
 int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t target_channels, int32_t z_dim, int32_t mode,
                                      int64_t* offsets, int32_t capacity);
+/* The MlpVAE twin, in the current math mode: [x,h1,h2,heads,z,g1,g2,logits,ga,gb] (ga / gb: the backward pass's two
+ * gradient buffers; after loss_grad, gb holds d loss / d (encoder/dense pre-activation) and logits d loss / d logits). */
+int32_t cpb_debug_mlpvae_buffer_offsets(const cpb_mlpvae_config* cfg, int32_t mode, int64_t* offsets, int32_t capacity);
 int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int32_t m, int32_t i, int32_t j,
                            int32_t variant, float* partial, void* stream);
 int32_t cpb_debug_tc_gemm(const float* a, const float* bt, float* d, int32_t m, int32_t n, int32_t k,
