@@ -34,6 +34,20 @@ class MlpVaeConfig(C.Structure):
     _fields_ = [("base", VaeConfig), ("enc1", C.c_int32), ("enc2", C.c_int32), ("dec1", C.c_int32), ("dec2", C.c_int32)]
 
 
+MLP_MAX_LAYERS = 8
+
+
+class MlpVaeSpec(C.Structure):
+    _fields_ = [("base", VaeConfig), ("num_encoder", C.c_int32), ("encoder_sizes", C.c_int32 * MLP_MAX_LAYERS),
+                ("num_decoder", C.c_int32), ("decoder_sizes", C.c_int32 * MLP_MAX_LAYERS)]
+
+    @classmethod
+    def of(cls, base, encoder_sizes, decoder_sizes):
+        """The spec of an MlpVAE with these hidden-layer sizes (at most MLP_MAX_LAYERS per side)."""
+        return cls(base, len(encoder_sizes), (C.c_int32 * MLP_MAX_LAYERS)(*encoder_sizes), len(decoder_sizes),
+                   (C.c_int32 * MLP_MAX_LAYERS)(*decoder_sizes))
+
+
 class PpoConfig(C.Structure):
     _fields_ = [("state_dim", C.c_int32), ("num_actions", C.c_int32), ("hidden1", C.c_int32),
                 ("hidden2", C.c_int32), ("action_low", C.c_float * 4), ("action_high", C.c_float * 4),
@@ -44,6 +58,7 @@ _P = C.c_void_p
 _i32, _i64, _f32, _f64 = C.c_int32, C.c_int64, C.c_float, C.c_double
 _VC = C.POINTER(VaeConfig)
 _MC = C.POINTER(MlpVaeConfig)
+_MS = C.POINTER(MlpVaeSpec)
 _PC = C.POINTER(PpoConfig)
 
 # name -> (restype, argtypes); must list every symbol of include/carla_ppo_b200.h
@@ -71,6 +86,15 @@ PROTOTYPES = {
     "cpb_mlpvae_decode": (_i32, [_MC, _P, _P, _P, _P, _i64, _P]),
     "cpb_mlpvae_forward": (_i32, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
     "cpb_mlpvae_loss_grad": (_i32, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_mlpvae_spec_num_tensors": (_i32, [_MS]),
+    "cpb_mlpvae_spec_tensor_name": (C.c_char_p, [_MS, _i32]),
+    "cpb_mlpvae_spec_layout": (_i32, [_MS, _P, _P, _P, _P]),
+    "cpb_mlpvae_spec_workspace_bytes": (_i64, [_MS, _i32]),
+    "cpb_mlpvae_spec_encode": (_i32, [_MS, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_mlpvae_spec_decode": (_i32, [_MS, _P, _P, _P, _P, _i64, _P]),
+    "cpb_mlpvae_spec_forward": (_i32, [_MS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_mlpvae_spec_loss_grad": (_i32, [_MS, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_mlpvae_encode_predict": (_i32, [_MS, _P, _P, _P, _i32, _PC, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P, _i64, _P]),
     "cpb_ppo_num_tensors": (_i32, []),
     "cpb_ppo_tensor_name": (C.c_char_p, [_i32]),
     "cpb_ppo_layout": (_i32, [_PC, _P, _P, _P, _P]),
@@ -85,6 +109,7 @@ PROTOTYPES = {
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_mlpvae_buffer_offsets": (_i32, [_MC, _i32, _P, _i32]),
+    "cpb_debug_mlpvae_spec_buffer_offsets": (_i32, [_MS, _i32, _P, _i32]),
     "cpb_debug_tc_wgrad": (_i32, [_P, _P, _P, _i32, _i32, _i32, _i32, _P, _P]),
     "cpb_debug_tc_gemm": (_i32, [_P, _P, _P, _i32, _i32, _i32, _P, _P]),
     "cpb_get_math_mode": (_i32, []),

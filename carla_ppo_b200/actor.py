@@ -1,5 +1,5 @@
 """Fused per-step inference of the RL loop: camera frame -> VAE mean -> [latent | measurements] -> PPO action / value in
-ONE C call (cpb_encode_predict), one pinned H2D (frame + measurements + noise) and one D2H (state + action + value).
+ONE C call (cpb_encode_predict; cpb_mlpvae_encode_predict for an MlpVAE), one pinned H2D (frame + measurements + noise) and one D2H (state + action + value).
 
 In the reference every environment step costs two TensorFlow session runs with a host round trip in between:
 ``encode_state_fn(env)`` (vae_common.py:45-61: sess.run(vae.mean)) inside ``env.step`` and then ``model.predict(state)``
@@ -73,10 +73,11 @@ class FusedActor:
             ws_p = ppo._workspace(1)
             sd = ppo.state_dim
             out = self._out_dev.data_ptr()
-            _lib.check(vae._libh.cpb_encode_predict(
+            name = vae._API["encode_predict"]
+            _lib.check(getattr(vae._libh, name)(
                 C.byref(cfg), _lib.ptr(vae.params), base, base + nf, self._m, C.byref(ppo._c), _lib.ptr(ppo.params),
                 None if self.greedy else base + nf + 4 * self._m, _lib.ptr(self._latent), out, out + 4 * sd, out + 4 * (sd + a),
-                _lib.ptr(self._flags), _lib.ptr(ws_v), ws_v.numel(), _lib.ptr(ws_p), ws_p.numel(), vae._stream()), "cpb_encode_predict")
+                _lib.ptr(self._flags), _lib.ptr(ws_v), ws_v.numel(), _lib.ptr(ws_p), ws_p.numel(), vae._stream()), name)
             self._out_host.copy_(self._out_dev, non_blocking=True)
             torch.cuda.current_stream(vae._device).synchronize()
         res = self._out_host.numpy()

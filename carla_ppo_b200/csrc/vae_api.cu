@@ -688,61 +688,112 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
 
 
 // =============================================================================================
-// MlpVAE (reference vae/models.py:271-299): flatten -> dense E1 relu -> dense E2 relu -> [mean | logstd_sq] -> sample ->
-// dense D1 relu -> dense D2 relu -> dense 12800*Ct -> logits.  Same loss / sampling / Adam kernels as the ConvVAE; the
-// seven layers run on the fp32 SIMT tap-GEMM (dense form) and the SIMT weight-gradient kernel, except in math mode 2:
-// there the five frame-wide products -- encoder/dense forward and weight gradient, decoder/dense_2 forward, data
-// gradient and weight gradient, 99 % of the step's multiply-adds -- run as ONE TF32 wgmma pass with both operands
-// rounded to nearest (the forward passes and the data gradient on the tensor-core tap-GEMM, k-split where they reduce
-// over a frame, the weight gradients on tc_wgrad).
+// MlpVAE (reference vae/models.py:271-299, build_mlp): flatten -> one dense relu layer per encoder size -> [mean |
+// logstd_sq] -> sample -> one dense relu layer per decoder size -> the output layer, dense 12800*Ct -> logits.  Same loss /
+// sampling / Adam kernels as the ConvVAE; the layers run on the fp32 SIMT tap-GEMM (dense form) and the SIMT
+// weight-gradient kernel, except in math mode 2: there the five frame-wide products -- the first encoder layer's forward
+// and weight gradient, the output layer's forward, data gradient and weight gradient -- run as ONE TF32 wgmma pass with
+// both operands rounded to nearest (the forward passes and the data gradient on the tensor-core tap-GEMM, k-split where
+// they reduce over a frame, the weight gradients on tc_wgrad).  Profile labels call the output layer "dec2" at every
+// depth (its name in the default two-per-side model).
 // =============================================================================================
-enum MlpTensor { M_E1_K, M_E1_B, M_E2_K, M_E2_B, M_MEAN_K, M_MEAN_B, M_LOGVAR_K, M_LOGVAR_B, M_D1_K, M_D1_B, M_D2_K, M_D2_B, M_D3_K, M_D3_B, M_COUNT };
-static const char* kMlpNames[M_COUNT] = {
-    "encoder/dense/kernel", "encoder/dense/bias", "encoder/dense_1/kernel", "encoder/dense_1/bias",
-    "mean/kernel", "mean/bias", "logstd_sqare/kernel", "logstd_sqare/bias",
-    "decoder/dense/kernel", "decoder/dense/bias", "decoder/dense_1/kernel", "decoder/dense_1/bias",
-    "decoder/dense_2/kernel", "decoder/dense_2/bias"};
+constexpr int kMlpMaxLayers = 8;                                  // hidden layers per side
+constexpr int kMlpMaxTensors = 2 * (2 * kMlpMaxLayers + 3);
 
-struct MlpLayout { int64_t off[M_COUNT], size[M_COUNT]; int32_t shape[M_COUNT][2]; int64_t total; };
+// Tensor indices in TF creation order: encoder layer i {kernel, bias} at 2i, mean at 2L, logstd_sqare at 2L + 2, decoder
+// layer j at 2L + 4 + 2j (j = M: the output layer); a bias follows its kernel.
+struct MlpLayout {
+    int nenc, ndec, n;
+    int64_t off[kMlpMaxTensors], size[kMlpMaxTensors];
+    int32_t shape[kMlpMaxTensors][2];
+    int64_t total;
+    int enc(int i) const { return 2 * i; }
+    int mean() const { return 2 * nenc; }
+    int logvar() const { return 2 * nenc + 2; }
+    int dec(int j) const { return 2 * nenc + 4 + 2 * j; }
+};
 
-static int32_t check_mlp_cfg(const cpb_mlpvae_config* c) {
-    CPB_REQUIRE(c != nullptr, "mlp cfg is NULL");
+// The reference's tf.layers names: build_mlp numbers the dense layers of a scope dense, dense_1, dense_2, ...
+static const char* mlp_tensor_name(int nenc, int ndec, int i) {
+    static const char* heads[4] = {"mean/kernel", "mean/bias", "logstd_sqare/kernel", "logstd_sqare/bias"};
+    static char names[2][kMlpMaxLayers + 1][2][32];
+    static const bool ready = [] {
+        for (int d = 0; d < 2; ++d)
+            for (int l = 0; l <= kMlpMaxLayers; ++l)
+                for (int b = 0; b < 2; ++b) {
+                    char suffix[8] = "";
+                    if (l) snprintf(suffix, sizeof(suffix), "_%d", l);
+                    snprintf(names[d][l][b], sizeof(names[d][l][b]), "%s/dense%s/%s", d ? "decoder" : "encoder", suffix,
+                             b ? "bias" : "kernel");
+                }
+        return true;
+    }();
+    (void)ready;
+    if (i < 0 || i >= 2 * (nenc + ndec + 3)) return nullptr;
+    if (i < 2 * nenc) return names[0][i / 2][i % 2];
+    if (i < 2 * nenc + 4) return heads[i - 2 * nenc];
+    return names[1][(i - 2 * nenc - 4) / 2][i % 2];
+}
+
+static int32_t check_mlp_spec(const cpb_mlpvae_spec* c) {
+    CPB_REQUIRE(c != nullptr, "mlp spec is NULL");
     CPB_TRY(check_cfg(&c->base));
-    for (int v : {c->enc1, c->enc2, c->dec1, c->dec2})
+    // an empty side would make the y-batched heads or the first decoder layer reductions over a whole frame
+    CPB_REQUIRE(c->num_encoder >= 1 && c->num_encoder <= kMlpMaxLayers && c->num_decoder >= 1 && c->num_decoder <= kMlpMaxLayers,
+                "MlpVAE needs 1 to %d hidden layers per side (encoder_sizes / decoder_sizes), got %d and %d", kMlpMaxLayers,
+                c->num_encoder, c->num_decoder);
+    for (int i = 0; i < c->num_encoder + c->num_decoder; ++i) {
+        const int v = i < c->num_encoder ? c->encoder_sizes[i] : c->decoder_sizes[i - c->num_encoder];
         CPB_REQUIRE(v >= 32 && v % 32 == 0 && v <= 8192, "MlpVAE hidden sizes must be multiples of 32 in [32, 8192], got %d", v);
+    }
     return CPB_OK;
 }
 
-static MlpLayout make_mlp_layout(const cpb_mlpvae_config* c) {
+static MlpLayout make_mlp_layout(const cpb_mlpvae_spec* c) {
     const int IN = geo::NPIX * 3, OUT = geo::NPIX * c->base.target_channels, z = c->base.z_dim;
-    const int shp[M_COUNT][2] = {{IN, c->enc1}, {c->enc1, 0}, {c->enc1, c->enc2}, {c->enc2, 0}, {c->enc2, z}, {z, 0}, {c->enc2, z}, {z, 0},
-                                 {z, c->dec1}, {c->dec1, 0}, {c->dec1, c->dec2}, {c->dec2, 0}, {c->dec2, OUT}, {OUT, 0}};
-    // the two head kernels (and biases) adjacent: both heads run as one y-batched dense problem
-    static const int order[M_COUNT] = {M_E1_K, M_E1_B, M_E2_K, M_E2_B, M_MEAN_K, M_LOGVAR_K, M_MEAN_B, M_LOGVAR_B,
-                                       M_D1_K, M_D1_B, M_D2_K, M_D2_B, M_D3_K, M_D3_B};
     MlpLayout L;
-    for (int i = 0; i < M_COUNT; ++i) { L.shape[i][0] = shp[i][0]; L.shape[i][1] = shp[i][1]; L.size[i] = (int64_t)shp[i][0] * (shp[i][1] ? shp[i][1] : 1); }
+    L.nenc = c->num_encoder; L.ndec = c->num_decoder; L.n = 2 * (L.nenc + L.ndec + 3);
+    auto dense = [&](int t, int in, int out) {       // kernel [in, out] at t, bias [out] at t + 1
+        L.shape[t][0] = in; L.shape[t][1] = out; L.size[t] = (int64_t)in * out;
+        L.shape[t + 1][0] = out; L.shape[t + 1][1] = 0; L.size[t + 1] = out;
+    };
+    for (int i = 0; i < L.nenc; ++i) dense(L.enc(i), i ? c->encoder_sizes[i - 1] : IN, c->encoder_sizes[i]);
+    const int top = c->encoder_sizes[L.nenc - 1];
+    dense(L.mean(), top, z);
+    dense(L.logvar(), top, z);
+    for (int j = 0; j <= L.ndec; ++j) dense(L.dec(j), j ? c->decoder_sizes[j - 1] : z, j < L.ndec ? c->decoder_sizes[j] : OUT);
+    // storage: creation order, except that the two head kernels (and biases) are adjacent: both heads run as one
+    // y-batched dense problem
+    int order[kMlpMaxTensors], n = 0;
+    for (int t = 0; t < L.mean(); ++t) order[n++] = t;
+    for (int t : {L.mean(), L.logvar(), L.mean() + 1, L.logvar() + 1}) order[n++] = t;
+    for (int t = L.dec(0); t < L.n; ++t) order[n++] = t;
     int64_t o = 0;
-    for (int i = 0; i < M_COUNT; ++i) { L.off[order[i]] = o; o += align_up(L.size[order[i]], 64); }
+    for (int i = 0; i < L.n; ++i) { L.off[order[i]] = o; o += align_up(L.size[order[i]], 64); }
     L.total = o;
     return L;
 }
 
 struct MlpPlan {
-    int B, IN, OUT, z, zp, e1, e2, d1, d2;     // zp = z_pad(z), the row pitch of the latent buffers (as in VaePlan)
-    float *x, *y, *h1, *h2, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss, *g1, *g2, *logits;
+    int B, IN, OUT, z, zp;                   // zp = z_pad(z), the row pitch of the latent buffers (as in VaePlan)
+    int nenc, ndec, enc[kMlpMaxLayers], dec[kMlpMaxLayers];
+    float *x, *y, *h[kMlpMaxLayers], *heads, *zbuf, *kl_rows, *kl_active, *frame_loss, *g[kMlpMaxLayers], *logits;
     float *ga, *gb, *gz, *gheads, *partial, *colsum, *wT, *ksplit;
-    int64_t tE2, tHeads, tD1, tD2, tD3;      // float offsets of the transposed kernels inside wT
-    float* wP;                               // z < z_pad only: zero-padded heads [2][enc2][z_pad], biases [2][z_pad], D1 [z_pad][dec1]
+    // float offsets of the transposed kernels inside wT: encoder layers 1.. (tEnc[0] unused), the heads, decoder layers
+    // 0..M (tDec[M]: the output layer)
+    int64_t tEnc[kMlpMaxLayers], tHeads, tDec[kMlpMaxLayers + 1];
+    float* wP;                               // z < z_pad only: zero-padded heads [2][top][z_pad], biases [2][z_pad], decoder/dense [z_pad][dec0]
     int64_t pHeads, pHeadsB, pD1;
-    // math mode 2 only (tc): TF32 weight images of the frame-wide layers inside wTc -- encoder/dense K-major [e1][IN]
-    // (every mode), decoder/dense_2 K-major [OUT][d2] (forward and train) and as stored [d2][OUT] (train, data
-    // gradient) -- and tcScratch for the k-split partials and the tensor-core weight-gradient partials
+    // math mode 2 only (tc): TF32 weight images of the frame-wide layers inside wTc -- the first encoder layer K-major
+    // [enc0][IN] (every mode), the output layer K-major [OUT][dec_last] (forward and train) and as stored [dec_last][OUT]
+    // (train, data gradient) -- and tcScratch for the k-split partials and the tensor-core weight-gradient partials
     bool tc;
     float *wTc, *tcScratch;
     int64_t iE1, iD3f, iD3t;
     int64_t bytes;
     bool ok;
+    int top() const { return enc[nenc - 1]; }
+    int last() const { return dec[ndec - 1]; }
 };
 
 // The tensor-core kernels address a frame-wide operand with 32-bit offsets (B * 38 400 < 2^31, i.e. B <= 55 923):
@@ -751,58 +802,68 @@ static bool mlp_tc_batch_ok(int64_t b, int in) { return b * in < (1LL << 31); }
 
 static int64_t mlp_tc_scratch_floats(const MlpPlan& p, int mode) {
     const int64_t b = p.B;
-    int64_t n = (int64_t)tc_tapgemm_pick_ksplit(p.IN) * b * p.e1;                              // encoder/dense fwd
+    int64_t n = (int64_t)tc_tapgemm_pick_ksplit(p.IN) * b * p.enc[0];                              // first encoder layer fwd
     if (mode >= CPB_WS_TRAIN) {
-        n = std::max<int64_t>(n, (int64_t)tc_tapgemm_pick_ksplit(p.OUT) * b * p.d2);         // decoder/dense_2 dgrad
-        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.IN, p.e1, b) * p.IN * p.e1);
-        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.OUT, p.d2, b) * p.OUT * p.d2);
+        n = std::max<int64_t>(n, (int64_t)tc_tapgemm_pick_ksplit(p.OUT) * b * p.last());           // output layer dgrad
+        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.IN, p.enc[0], b) * p.IN * p.enc[0]);
+        n = std::max<int64_t>(n, (int64_t)tc_wgrad_pick_splits(p.OUT, p.last(), b) * p.OUT * p.last());
     }
     return n;
 }
 
-static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config* c, int mode) {
+static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_spec* c, int mode) {
     MlpPlan p;
     memset(&p, 0, sizeof(p));
     const int64_t b = c->base.batch;
     p.B = (int)b; p.IN = geo::NPIX * 3; p.OUT = geo::NPIX * c->base.target_channels; p.z = c->base.z_dim;
     p.zp = z_pad(p.z);
-    p.e1 = c->enc1; p.e2 = c->enc2; p.d1 = c->dec1; p.d2 = c->dec2;
+    p.nenc = c->num_encoder; p.ndec = c->num_decoder;
+    for (int i = 0; i < p.nenc; ++i) p.enc[i] = c->encoder_sizes[i];
+    for (int j = 0; j < p.ndec; ++j) p.dec[j] = c->decoder_sizes[j];
     const int64_t zp = p.zp;
     Arena a(ws, ws_bytes);
     p.x = a.take<float>(b * p.IN);
-    p.h1 = a.take<float>(b * p.e1);
-    p.h2 = a.take<float>(b * p.e2);
+    for (int i = 0; i < p.nenc; ++i) p.h[i] = a.take<float>(b * p.enc[i]);
     p.heads = a.take<float>(2 * b * zp);
     p.ksplit = a.take<float>((int64_t)kMaxKSplit * 2 * b * zp);
     if (p.zp != p.z) {
         int64_t o = 0;
         auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
-        p.pHeads = take(2LL * p.e2 * zp); p.pHeadsB = take(2LL * zp); p.pD1 = take(zp * p.d1);
+        p.pHeads = take(2LL * p.top() * zp); p.pHeadsB = take(2LL * zp); p.pD1 = take(zp * p.dec[0]);
         p.wP = a.take<float>(o);
     }
     if (mode >= CPB_WS_FORWARD) {
         p.y = a.take<float>(b * p.OUT);
         p.zbuf = a.take<float>(b * zp);
         p.kl_rows = a.take<float>(b); p.kl_active = a.take<float>(b); p.frame_loss = a.take<float>(b);
-        p.g1 = a.take<float>(b * p.d1);
-        p.g2 = a.take<float>(b * p.d2);
+        for (int j = 0; j < p.ndec; ++j) p.g[j] = a.take<float>(b * p.dec[j]);
         p.logits = a.take<float>(b * p.OUT);
     }
     if (mode >= CPB_WS_TRAIN) {
-        const int64_t widest = std::max<int64_t>(std::max(p.e1, p.e2), std::max(p.d1, p.d2));
+        int64_t widest = 0;
+        for (int i = 0; i < p.nenc; ++i) widest = std::max<int64_t>(widest, p.enc[i]);
+        for (int j = 0; j < p.ndec; ++j) widest = std::max<int64_t>(widest, p.dec[j]);
         p.ga = a.take<float>(b * widest);
         p.gb = a.take<float>(b * widest);
         p.gz = a.take<float>(b * zp);
         p.gheads = a.take<float>(2 * b * zp);
         int64_t o = 0;
         auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
-        p.tE2 = take((int64_t)p.e1 * p.e2); p.tHeads = take(2LL * p.e2 * zp); p.tD1 = take(zp * p.d1);
-        p.tD2 = take((int64_t)p.d1 * p.d2); p.tD3 = take((int64_t)p.d2 * p.OUT);
+        for (int i = 1; i < p.nenc; ++i) p.tEnc[i] = take((int64_t)p.enc[i - 1] * p.enc[i]);
+        p.tHeads = take(2LL * p.top() * zp);
+        for (int j = 0; j < p.ndec; ++j) p.tDec[j] = take((j ? (int64_t)p.dec[j - 1] : zp) * p.dec[j]);
+        p.tDec[p.ndec] = take((int64_t)p.last() * p.OUT);
         p.wT = a.take<float>(o);
-        struct P { int I, J; };
-        const P ps[] = {{p.IN, p.e1}, {p.e1, p.e2}, {p.e2, p.zp}, {p.zp, p.d1}, {p.d1, p.d2}, {p.d2, p.OUT}};
+        // the weight-gradient partials of every layer: consecutive widths of IN, enc..., z_pad, dec..., OUT
+        int widths[2 * kMlpMaxLayers + 3], nw = 0;
+        widths[nw++] = p.IN;
+        for (int i = 0; i < p.nenc; ++i) widths[nw++] = p.enc[i];
+        widths[nw++] = p.zp;
+        for (int j = 0; j < p.ndec; ++j) widths[nw++] = p.dec[j];
+        widths[nw++] = p.OUT;
         int64_t best = 0;
-        for (const P& q : ps) best = std::max<int64_t>(best, (int64_t)wgrad_pick_splits(q.I, q.J, b) * q.I * q.J);
+        for (int k = 0; k + 1 < nw; ++k)
+            best = std::max<int64_t>(best, (int64_t)wgrad_pick_splits(widths[k], widths[k + 1], b) * widths[k] * widths[k + 1]);
         p.partial = a.take<float>(best);
         p.colsum = a.take<float>(colsum_scratch_floats(b, p.OUT) + colsum_scratch_floats(b, (int)widest));
     }
@@ -811,9 +872,9 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_config
     if (p.tc) {
         int64_t o = 0;
         auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
-        p.iE1 = take(2LL * p.e1 * p.IN);
-        if (mode >= CPB_WS_FORWARD) p.iD3f = take(2LL * p.OUT * p.d2);
-        if (mode >= CPB_WS_TRAIN) p.iD3t = take(2LL * p.d2 * p.OUT);
+        p.iE1 = take(2LL * p.enc[0] * p.IN);
+        if (mode >= CPB_WS_FORWARD) p.iD3f = take(2LL * p.OUT * p.last());
+        if (mode >= CPB_WS_TRAIN) p.iD3t = take(2LL * p.last() * p.OUT);
         p.wTc = a.take<float>(o);
         p.tcScratch = a.take<float>(mlp_tc_scratch_floats(p, mode));
     }
@@ -827,10 +888,10 @@ static int32_t mlp_pad_weights(const MlpPlan& pl, const MlpLayout& L, const floa
     if (pl.zp == pl.z) return CPB_OK;
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    add_relayout(t, L.off[M_MEAN_K], pl.pHeads, 2, pl.e2, pl.z, 1, pl.e2, pl.zp);
-    add_relayout(t, L.off[M_MEAN_B], pl.pHeadsB, 1, 1, pl.z, 1, 1, pl.zp);
-    add_relayout(t, L.off[M_LOGVAR_B], pl.pHeadsB + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
-    add_relayout(t, L.off[M_D1_K], pl.pD1, 1, pl.z, pl.d1, 1, pl.zp, pl.d1);
+    add_relayout(t, L.off[L.mean()], pl.pHeads, 2, pl.top(), pl.z, 1, pl.top(), pl.zp);
+    add_relayout(t, L.off[L.mean() + 1], pl.pHeadsB, 1, 1, pl.z, 1, 1, pl.zp);
+    add_relayout(t, L.off[L.logvar() + 1], pl.pHeadsB + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
+    add_relayout(t, L.off[L.dec(0)], pl.pD1, 1, pl.z, pl.dec[0], 1, pl.zp, pl.dec[0]);
     return launch_relayout(params, pl.wP, t, s);
 }
 
@@ -845,9 +906,10 @@ static int32_t mlp_tc_weights(const MlpPlan& pl, const MlpLayout& L, const float
         j.src_off = L.off[tensor]; j.dst_hi = j.dst_lo = dst; j.mode = mode; j.N = N; j.C = C; j.round_nearest = 1;
         j.count = (long long)N * C; w.total += j.count;
     };
-    if (encoder) add(M_E1_K, pl.iE1, 3, pl.e1, pl.IN);       // [e1][IN] from the kernel [IN][e1]
-    if (decoder) add(M_D3_K, pl.iD3f, 3, pl.OUT, pl.d2);     // [OUT][d2] from the kernel [d2][OUT]
-    if (backward) add(M_D3_K, pl.iD3t, 0, pl.d2, pl.OUT);    // the kernel as stored: the data gradient's [N = d2][K = OUT]
+    const int out = L.dec(pl.ndec);
+    if (encoder) add(L.enc(0), pl.iE1, 3, pl.enc[0], pl.IN);       // [enc0][IN] from the kernel [IN][enc0]
+    if (decoder) add(out, pl.iD3f, 3, pl.OUT, pl.last());          // [OUT][dec_last] from the kernel [dec_last][OUT]
+    if (backward) add(out, pl.iD3t, 0, pl.last(), pl.OUT);         // the kernel as stored: the data gradient's [N = dec_last][K = OUT]
     ProfScope prof("mlp.tc_weights", s);
     return launch_tc_weights(params, pl.wTc, w, s);
 }
@@ -880,35 +942,44 @@ static int32_t run_tc_dense_wgrad(const char* label, const float* big, int I, co
     return launch_reduce_partials(partial, w.splits, I, J, I, I, J, out, s);
 }
 
-static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
+static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_spec* c, const float* params, const void* source,
                            int32_t* flags, cudaStream_t s) {
     const float sscale = c->base.source_dtype == CPB_FRAME_U8 ? 1.f / 255.f : 1.f;
     CPB_TRY(launch_prep_flat(source, c->base.source_dtype, sscale, (long long)pl.B * pl.IN, pl.x, flags, 1, s));
-    TapGemmParams p = dense_problem(pl.x, pl.B, pl.IN, params + L.off[M_E1_K], pl.e1, params + L.off[M_E1_B], nullptr, pl.h1, 1);
+    TapGemmParams p = dense_problem(pl.x, pl.B, pl.IN, params + L.off[L.enc(0)], pl.enc[0], params + L.off[L.enc(0) + 1],
+                                    nullptr, pl.h[0], 1);
     CPB_TRY(mlp_dense("mlp.enc.fwd", pl, p, pl.tc ? pl.wTc + pl.iE1 : nullptr, s));
-    p = dense_problem(pl.h1, pl.B, pl.e1, params + L.off[M_E2_K], pl.e2, params + L.off[M_E2_B], nullptr, pl.h2, 1);
-    CPB_TRY(launch_tapgemm(p, s));
+    for (int i = 1; i < pl.nenc; ++i) {
+        p = dense_problem(pl.h[i - 1], pl.B, pl.enc[i - 1], params + L.off[L.enc(i)], pl.enc[i], params + L.off[L.enc(i) + 1],
+                          nullptr, pl.h[i], 1);
+        CPB_TRY(launch_tapgemm(p, s));
+    }
     const bool padded = pl.zp != pl.z;
-    p = dense_problem(pl.h2, pl.B, pl.e2, padded ? pl.wP + pl.pHeads : params + L.off[M_MEAN_K], pl.zp,
-                      padded ? pl.wP + pl.pHeadsB : params + L.off[M_MEAN_B], nullptr, pl.heads, 0);
+    p = dense_problem(pl.h[pl.nenc - 1], pl.B, pl.top(), padded ? pl.wP + pl.pHeads : params + L.off[L.mean()], pl.zp,
+                      padded ? pl.wP + pl.pHeadsB : params + L.off[L.mean() + 1], nullptr, pl.heads, 0);
     p.ybatch = 2;
-    p.w_ystride = padded ? (long long)pl.e2 * pl.zp : L.off[M_LOGVAR_K] - L.off[M_MEAN_K];
-    p.bias_ystride = padded ? pl.zp : L.off[M_LOGVAR_B] - L.off[M_MEAN_B];
+    p.w_ystride = padded ? (long long)pl.top() * pl.zp : L.off[L.logvar()] - L.off[L.mean()];
+    p.bias_ystride = padded ? pl.zp : L.off[L.logvar() + 1] - L.off[L.mean() + 1];
     p.dst_ystride = (long long)pl.B * pl.zp;
     return launch_tapgemm(p, s);
 }
 
 static int32_t mlp_decoder(const MlpPlan& pl, const MlpLayout& L, const float* params, const float* zsrc, float* logits, cudaStream_t s) {
-    const float* w1 = pl.zp != pl.z ? pl.wP + pl.pD1 : params + L.off[M_D1_K];
-    TapGemmParams p = dense_problem(zsrc, pl.B, pl.zp, w1, pl.d1, params + L.off[M_D1_B], nullptr, pl.g1, 1);
-    CPB_TRY(launch_tapgemm(p, s));
-    p = dense_problem(pl.g1, pl.B, pl.d1, params + L.off[M_D2_K], pl.d2, params + L.off[M_D2_B], nullptr, pl.g2, 1);
-    CPB_TRY(launch_tapgemm(p, s));
-    p = dense_problem(pl.g2, pl.B, pl.d2, params + L.off[M_D3_K], pl.OUT, params + L.off[M_D3_B], nullptr, logits, 0);
+    const float* src = zsrc;
+    int k = pl.zp;
+    for (int j = 0; j < pl.ndec; ++j) {
+        const float* w = j == 0 && pl.zp != pl.z ? pl.wP + pl.pD1 : params + L.off[L.dec(j)];
+        TapGemmParams p = dense_problem(src, pl.B, k, w, pl.dec[j], params + L.off[L.dec(j) + 1], nullptr, pl.g[j], 1);
+        CPB_TRY(launch_tapgemm(p, s));
+        src = pl.g[j];
+        k = pl.dec[j];
+    }
+    const int out = L.dec(pl.ndec);
+    TapGemmParams p = dense_problem(src, pl.B, k, params + L.off[out], pl.OUT, params + L.off[out + 1], nullptr, logits, 0);
     return mlp_dense("mlp.dec2.fwd", pl, p, pl.tc ? pl.wTc + pl.iD3f : nullptr, s);
 }
 
-static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const void* source,
+static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_spec* c, const float* params, const void* source,
                                 const void* target, const float* eps, bool want_dlogits, int32_t* flags, cudaStream_t s) {
     CPB_TRY(mlp_encoder(pl, L, c, params, source, flags, s));
     CPB_TRY(launch_reparam(pl.heads, eps, pl.B, pl.z, pl.zp, c->base.kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
@@ -925,65 +996,84 @@ static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb
                                   want_dlogits ? pl.logits : nullptr, s);
 }
 
-static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_config* c, const float* params, const float* eps,
+static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpvae_spec* c, const float* params, const float* eps,
                             float* grads, cudaStream_t s) {
-    const int B = pl.B, z = pl.z, zp = pl.zp;
+    const int B = pl.B, z = pl.z, zp = pl.zp, ne = pl.nenc, nd = pl.ndec, out = L.dec(nd);
     float* dlog = pl.logits;
     float* cs = pl.colsum;
     CPB_TRY(launch_fill_zero(grads, L.total, s));
-    // transposed kernels for the data gradients ([in,out] -> [out,in]); the two head kernels are adjacent (2 "taps")
+    // transposed kernels for the data gradients ([in,out] -> [out,in]); the two head kernels are adjacent (2 "taps").
+    // One launch, or one per full table in deep models.
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols, int rows_pad, int cols_pad) {
-        add_relayout(t, src, dst, taps, rows, cols, 0, rows_pad, cols_pad);
+    auto add = [&](int tensor, int64_t dst, int taps, int rows, int cols, int rows_pad, int cols_pad) -> int32_t {
+        if (t.njobs == kMaxRelayoutJobs) {
+            CPB_TRY(launch_relayout(params, pl.wT, t, s));
+            memset(&t, 0, sizeof(t));
+        }
+        add_relayout(t, L.off[tensor], dst, taps, rows, cols, 0, rows_pad, cols_pad);
+        return CPB_OK;
     };
-    add(L.off[M_E2_K], pl.tE2, 1, pl.e1, pl.e2, pl.e1, pl.e2);
-    add(L.off[M_MEAN_K], pl.tHeads, 2, pl.e2, z, pl.e2, zp);      // [2][z_pad][enc2]
-    add(L.off[M_D1_K], pl.tD1, 1, z, pl.d1, zp, pl.d1);           // [dec1][z_pad]
-    add(L.off[M_D2_K], pl.tD2, 1, pl.d1, pl.d2, pl.d1, pl.d2);
-    if (!pl.tc) add(L.off[M_D3_K], pl.tD3, 1, pl.d2, pl.OUT, pl.d2, pl.OUT);    // mode 2 reads the TF32 image iD3t instead
+    for (int i = 1; i < ne; ++i) CPB_TRY(add(L.enc(i), pl.tEnc[i], 1, pl.enc[i - 1], pl.enc[i], pl.enc[i - 1], pl.enc[i]));
+    CPB_TRY(add(L.mean(), pl.tHeads, 2, pl.top(), z, pl.top(), zp));                // [2][z_pad][top]
+    CPB_TRY(add(L.dec(0), pl.tDec[0], 1, z, pl.dec[0], zp, pl.dec[0]));              // [dec0][z_pad]
+    for (int j = 1; j < nd; ++j) CPB_TRY(add(L.dec(j), pl.tDec[j], 1, pl.dec[j - 1], pl.dec[j], pl.dec[j - 1], pl.dec[j]));
+    if (!pl.tc) CPB_TRY(add(out, pl.tDec[nd], 1, pl.last(), pl.OUT, pl.last(), pl.OUT));    // mode 2 reads the TF32 image iD3t instead
     CPB_TRY(launch_relayout(params, pl.wT, t, s));
     TapGemmParams p;
-    // ---- decoder.  Mode 2: decoder/dense_2's weight gradient runs as its transpose dlog^T g2 (I = OUT >= 12 800 rows,
-    // J = dec2 columns: tc_wgrad needs I >= 128 and dec2 may be 32), transposed back in the split reduction.
+    // ---- output layer.  Mode 2: its weight gradient runs as its transpose dlog^T g_last (I = OUT >= 12 800 rows,
+    // J = dec_last columns: tc_wgrad needs I >= 128 and dec_last may be 32), transposed back in the split reduction.
     if (pl.tc)
-        CPB_TRY(run_tc_dense_wgrad("mlp.dec2.wgrad", dlog, pl.OUT, pl.g2, pl.d2, B, pl.tcScratch, grads + L.off[M_D3_K], true, s));
+        CPB_TRY(run_tc_dense_wgrad("mlp.dec2.wgrad", dlog, pl.OUT, pl.g[nd - 1], pl.last(), B, pl.tcScratch, grads + L.off[out], true, s));
     else
-        CPB_TRY(run_dense_wgrad("mlp.dec2.wgrad", pl.g2, pl.d2, pl.d2, dlog, B, pl.OUT, pl.OUT, pl.partial, grads + L.off[M_D3_K], s));
-    CPB_TRY(launch_colsum(dlog, B, pl.OUT, pl.OUT, grads + L.off[M_D3_B], cs, s));
-    p = dense_problem(dlog, B, pl.OUT, pl.wT + pl.tD3, pl.d2, nullptr, pl.g2, pl.ga, 0);                       // ga = g(g2 pre-activation)
+        CPB_TRY(run_dense_wgrad("mlp.dec2.wgrad", pl.g[nd - 1], pl.last(), pl.last(), dlog, B, pl.OUT, pl.OUT, pl.partial,
+                                grads + L.off[out], s));
+    CPB_TRY(launch_colsum(dlog, B, pl.OUT, pl.OUT, grads + L.off[out + 1], cs, s));
+    p = dense_problem(dlog, B, pl.OUT, pl.wT + pl.tDec[nd], pl.last(), nullptr, pl.g[nd - 1], pl.ga, 0);   // ga = g(g_last pre-activation)
     CPB_TRY(mlp_dense("mlp.dec2.dgrad", pl, p, pl.tc ? pl.wTc + pl.iD3t : nullptr, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.g1, pl.d1, pl.d1, pl.ga, B, pl.d2, pl.d2, pl.partial, grads + L.off[M_D2_K], s));
-    CPB_TRY(launch_colsum(pl.ga, B, pl.d2, pl.d2, grads + L.off[M_D2_B], cs, s));
-    p = dense_problem(pl.ga, B, pl.d2, pl.wT + pl.tD2, pl.d1, nullptr, pl.g1, pl.gb, 0);                         // gb = g(g1 pre-activation)
-    CPB_TRY(launch_tapgemm(p, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.zbuf, zp, z, pl.gb, B, pl.d1, pl.d1, pl.partial, grads + L.off[M_D1_K], s));
-    CPB_TRY(launch_colsum(pl.gb, B, pl.d1, pl.d1, grads + L.off[M_D1_B], cs, s));
-    p = dense_problem(pl.gb, B, pl.d1, pl.wT + pl.tD1, zp, nullptr, nullptr, pl.gz, 0);
-    CPB_TRY(launch_tapgemm(p, s));
+    // ---- decoder hidden layers, top down: the gradient alternates between ga and gb; decoder/dense's goes to gz
+    float* cur = pl.ga;
+    float* other = pl.gb;
+    for (int j = nd - 1; j >= 0; --j) {
+        const float* in = j ? pl.g[j - 1] : pl.zbuf;
+        const int k = j ? pl.dec[j - 1] : zp, k_real = j ? k : z;
+        CPB_TRY(run_dense_wgrad("mlp.wgrad", in, k, k_real, cur, B, pl.dec[j], pl.dec[j], pl.partial, grads + L.off[L.dec(j)], s));
+        CPB_TRY(launch_colsum(cur, B, pl.dec[j], pl.dec[j], grads + L.off[L.dec(j) + 1], cs, s));
+        p = dense_problem(cur, B, pl.dec[j], pl.wT + pl.tDec[j], k, nullptr, j ? pl.g[j - 1] : nullptr, j ? other : pl.gz, 0);
+        CPB_TRY(launch_tapgemm(p, s));
+        std::swap(cur, other);
+    }
     // ---- sampling + KL, heads
+    const float* htop = pl.h[ne - 1];
     CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, c->base.beta * c->base.loss_scale / (float)B, pl.gheads, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.e2, pl.gheads, B, zp, z, pl.partial, grads + L.off[M_MEAN_K], s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h2, pl.e2, pl.e2, pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
-                            grads + L.off[M_LOGVAR_K], s));
-    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[M_MEAN_B], cs, s));
-    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[M_LOGVAR_B], cs, s));
-    p = dense_problem(pl.gheads, B, zp, pl.wT + pl.tHeads, pl.e2, nullptr, pl.h2, pl.ga, 0);
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", htop, pl.top(), pl.top(), pl.gheads, B, zp, z, pl.partial, grads + L.off[L.mean()], s));
+    CPB_TRY(run_dense_wgrad("mlp.wgrad", htop, pl.top(), pl.top(), pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
+                            grads + L.off[L.logvar()], s));
+    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[L.mean() + 1], cs, s));
+    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[L.logvar() + 1], cs, s));
+    // the encoder's gradient alternates between ga and gb so that the first layer's lands in gb at every depth
+    cur = ne % 2 == 0 ? pl.ga : pl.gb;
+    other = ne % 2 == 0 ? pl.gb : pl.ga;
+    p = dense_problem(pl.gheads, B, zp, pl.wT + pl.tHeads, pl.top(), nullptr, htop, cur, 0);
     p.cls[0].ntaps = 2;
     p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
     p.cls[0].taps[1].src_off = (long long)B * zp;
-    p.cls[0].taps[1].w_off = (long long)zp * pl.e2;
-    CPB_TRY(launch_tapgemm(p, s));                                                                               // ga = g(h2 pre-activation)
-    // ---- encoder
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h1, pl.e1, pl.e1, pl.ga, B, pl.e2, pl.e2, pl.partial, grads + L.off[M_E2_K], s));
-    CPB_TRY(launch_colsum(pl.ga, B, pl.e2, pl.e2, grads + L.off[M_E2_B], cs, s));
-    p = dense_problem(pl.ga, B, pl.e2, pl.wT + pl.tE2, pl.e1, nullptr, pl.h1, pl.gb, 0);                         // gb = g(h1 pre-activation)
-    CPB_TRY(launch_tapgemm(p, s));
+    p.cls[0].taps[1].w_off = (long long)zp * pl.top();
+    CPB_TRY(launch_tapgemm(p, s));                                                                      // cur = g(h_top pre-activation)
+    // ---- encoder, top down
+    for (int i = ne - 1; i >= 1; --i) {
+        CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h[i - 1], pl.enc[i - 1], pl.enc[i - 1], cur, B, pl.enc[i], pl.enc[i], pl.partial,
+                                grads + L.off[L.enc(i)], s));
+        CPB_TRY(launch_colsum(cur, B, pl.enc[i], pl.enc[i], grads + L.off[L.enc(i) + 1], cs, s));
+        p = dense_problem(cur, B, pl.enc[i], pl.wT + pl.tEnc[i], pl.enc[i - 1], nullptr, pl.h[i - 1], other, 0);
+        CPB_TRY(launch_tapgemm(p, s));                                                                  // other = g(h_{i-1} pre-activation)
+        std::swap(cur, other);
+    }
     if (pl.tc)
-        CPB_TRY(run_tc_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, pl.gb, pl.e1, B, pl.tcScratch, grads + L.off[M_E1_K], false, s));
+        CPB_TRY(run_tc_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, cur, pl.enc[0], B, pl.tcScratch, grads + L.off[L.enc(0)], false, s));
     else
-        CPB_TRY(run_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, pl.IN, pl.gb, B, pl.e1, pl.e1, pl.partial, grads + L.off[M_E1_K], s));
-    return launch_colsum(pl.gb, B, pl.e1, pl.e1, grads + L.off[M_E1_B], cs, s);
+        CPB_TRY(run_dense_wgrad("mlp.enc.wgrad", pl.x, pl.IN, pl.IN, cur, B, pl.enc[0], pl.enc[0], pl.partial, grads + L.off[L.enc(0)], s));
+    return launch_colsum(cur, B, pl.enc[0], pl.enc[0], grads + L.off[L.enc(0) + 1], cs, s);
 }
 
 // [B, z_pad] latent rows of the workspace -> the caller's [B, z] rows
@@ -1216,20 +1306,40 @@ __global__ void assemble_state_kernel(const float* __restrict__ latent, const fl
     state[idx] = c < z ? latent[b * z + c] : meas[b * m + (c - z)];
 }
 
+// The VAE half of an encode_predict call: the mean of `frames` into latent [B, z]
+typedef int32_t (*EncodeMeanFn)(const void* vae, const float* params, const void* frames, float* latent, int32_t* flags,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+
+// cpb_encode_predict and cpb_mlpvae_encode_predict: `encode` on the VAE described by `vae` (whose common part is `base`),
+// then the state assembly and the PPO forward
+static int32_t encode_predict(const cpb_vae_config* base, const void* vae, EncodeMeanFn encode, const float* vae_params,
+                              const void* frames, const float* measurements, int32_t num_measurements, const cpb_ppo_config* ppo_cfg,
+                              const float* ppo_params, const float* noise, float* latent_tmp, float* state, float* action,
+                              float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes, void* ppo_workspace,
+                              int64_t ppo_workspace_bytes, void* stream) {
+    CPB_REQUIRE(base && ppo_cfg && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
+    CPB_REQUIRE(num_measurements >= 0 && (num_measurements == 0 || measurements != nullptr), "encode_predict: bad measurements");
+    CPB_REQUIRE(ppo_cfg->state_dim == base->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
+                ppo_cfg->state_dim, base->z_dim, num_measurements);
+    const int B = base->batch;
+    CPB_TRY(encode(vae, vae_params, frames, latent_tmp, flags, vae_workspace, vae_workspace_bytes, stream));
+    const int total = B * ppo_cfg->state_dim;
+    assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, base->z_dim, num_measurements, state);
+    CPB_LAUNCHED();
+    return cpb_ppo_forward(ppo_cfg, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
 int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_params, const void* frames, const float* measurements,
                            int32_t num_measurements, const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
                            float* latent_tmp, float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
                            int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
-    CPB_REQUIRE(vae_cfg && ppo_cfg && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
-    CPB_REQUIRE(num_measurements >= 0 && (num_measurements == 0 || measurements != nullptr), "encode_predict: bad measurements");
-    CPB_REQUIRE(ppo_cfg->state_dim == vae_cfg->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
-                ppo_cfg->state_dim, vae_cfg->z_dim, num_measurements);
-    const int B = vae_cfg->batch;
-    CPB_TRY(cpb_vae_encode(vae_cfg, vae_params, frames, latent_tmp, nullptr, flags, vae_workspace, vae_workspace_bytes, stream));
-    const int total = B * ppo_cfg->state_dim;
-    assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, vae_cfg->z_dim, num_measurements, state);
-    CPB_LAUNCHED();
-    return cpb_ppo_forward(ppo_cfg, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
+    EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
+                             int64_t ws_bytes, void* stream) {
+        return cpb_vae_encode((const cpb_vae_config*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
+    };
+    return encode_predict(vae_cfg, vae_cfg, encode, vae_params, frames, measurements, num_measurements, ppo_cfg, ppo_params, noise,
+                          latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes, ppo_workspace,
+                          ppo_workspace_bytes, stream);
 }
 
 static int64_t frame_bytes(int dtype, int channels) {
@@ -1281,13 +1391,19 @@ int32_t cpb_vae_train_step_host(const cpb_vae_config* cfg, float* params, float*
 }
 
 /* ---------------------------------------------------------------------------------------------------- MlpVAE */
-int32_t cpb_mlpvae_num_tensors(void) { return M_COUNT; }
-const char* cpb_mlpvae_tensor_name(int32_t i) { return (i >= 0 && i < M_COUNT) ? kMlpNames[i] : nullptr; }
+int32_t cpb_mlpvae_spec_num_tensors(const cpb_mlpvae_spec* spec) {
+    CPB_TRY(check_mlp_spec(spec));
+    return 2 * (spec->num_encoder + spec->num_decoder + 3);
+}
+const char* cpb_mlpvae_spec_tensor_name(const cpb_mlpvae_spec* spec, int32_t i) {
+    if (check_mlp_spec(spec) != CPB_OK) return nullptr;
+    return mlp_tensor_name(spec->num_encoder, spec->num_decoder, i);
+}
 
-int32_t cpb_mlpvae_layout(const cpb_mlpvae_config* cfg, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
-    CPB_TRY(check_mlp_cfg(cfg));
-    MlpLayout L = make_mlp_layout(cfg);
-    for (int i = 0; i < M_COUNT; ++i) {
+int32_t cpb_mlpvae_spec_layout(const cpb_mlpvae_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
+    CPB_TRY(check_mlp_spec(spec));
+    MlpLayout L = make_mlp_layout(spec);
+    for (int i = 0; i < L.n; ++i) {
         if (offsets) offsets[i] = L.off[i];
         if (sizes) sizes[i] = L.size[i];
         if (shapes) { shapes[i * 4] = L.shape[i][0]; shapes[i * 4 + 1] = L.shape[i][1]; shapes[i * 4 + 2] = 0; shapes[i * 4 + 3] = 0; }
@@ -1296,49 +1412,57 @@ int32_t cpb_mlpvae_layout(const cpb_mlpvae_config* cfg, int64_t* offsets, int64_
     return CPB_OK;
 }
 
-/* debug: byte offsets of the named MlpVAE workspace buffers for (cfg, mode) in the current math mode; returns the count */
-int32_t cpb_debug_mlpvae_buffer_offsets(const cpb_mlpvae_config* cfg, int32_t mode, int64_t* offsets, int32_t capacity) {
-    CPB_TRY(check_mlp_cfg(cfg));
+/* debug: byte offsets of the named MlpVAE workspace buffers for (spec, mode) in the current math mode; returns the count */
+int32_t cpb_debug_mlpvae_spec_buffer_offsets(const cpb_mlpvae_spec* spec, int32_t mode, int64_t* offsets, int32_t capacity) {
+    CPB_TRY(check_mlp_spec(spec));
     CPB_REQUIRE(mode >= CPB_WS_ENCODE && mode <= CPB_WS_TRAIN, "bad workspace mode %d", mode);
     char* base = (char*)4096;   // fake non-null base: only differences are used
-    MlpPlan pl = make_mlp_plan(base, (int64_t)1 << 60, cfg, mode);
-    const float* ptrs[] = {pl.x, pl.h1, pl.h2, pl.heads, pl.zbuf, pl.g1, pl.g2, pl.logits, pl.ga, pl.gb};
-    const int n = (int)(sizeof(ptrs) / sizeof(ptrs[0]));
+    MlpPlan pl = make_mlp_plan(base, (int64_t)1 << 60, spec, mode);
+    const float* ptrs[2 * kMlpMaxLayers + 6];
+    int n = 0;
+    ptrs[n++] = pl.x;
+    for (int i = 0; i < pl.nenc; ++i) ptrs[n++] = pl.h[i];
+    ptrs[n++] = pl.heads;
+    ptrs[n++] = pl.zbuf;
+    for (int j = 0; j < pl.ndec; ++j) ptrs[n++] = pl.g[j];
+    ptrs[n++] = pl.logits;
+    ptrs[n++] = pl.ga;
+    ptrs[n++] = pl.gb;
     for (int i = 0; i < n && i < capacity; ++i) offsets[i] = ptrs[i] ? (int64_t)((const char*)ptrs[i] - base) : -1;
     return n;
 }
 
-int64_t cpb_mlpvae_workspace_bytes(const cpb_mlpvae_config* cfg, int32_t mode) {
-    if (check_mlp_cfg(cfg) != CPB_OK || mode < 0 || mode > 2) return CPB_ERR_INVALID_ARGUMENT;
-    return make_mlp_plan(nullptr, 0, cfg, mode).bytes;
+int64_t cpb_mlpvae_spec_workspace_bytes(const cpb_mlpvae_spec* spec, int32_t mode) {
+    if (check_mlp_spec(spec) != CPB_OK || mode < 0 || mode > 2) return CPB_ERR_INVALID_ARGUMENT;
+    return make_mlp_plan(nullptr, 0, spec, mode).bytes;
 }
 
 #define CPB_MLP_PLAN(mode)                                                                           \
-    CPB_TRY(check_mlp_cfg(cfg));                                                                     \
+    CPB_TRY(check_mlp_spec(spec));                                                                   \
     CPB_TRY(ensure_init());                                                                          \
     CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                          \
-    MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, cfg, mode);                               \
+    MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, mode);                              \
     if (!pl.ok) {                                                                                    \
         cpb::set_error("workspace too small: need %lld bytes, got %lld", (long long)pl.bytes, (long long)workspace_bytes); \
         return CPB_ERR_WORKSPACE_TOO_SMALL;                                                          \
     }                                                                                                \
-    MlpLayout L = make_mlp_layout(cfg);                                                              \
+    MlpLayout L = make_mlp_layout(spec);                                                             \
     cudaStream_t s = (cudaStream_t)stream;
 
-int32_t cpb_mlpvae_encode(const cpb_mlpvae_config* cfg, const float* params, const void* source, float* mean, float* logvar,
-                          int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
+int32_t cpb_mlpvae_spec_encode(const cpb_mlpvae_spec* spec, const float* params, const void* source, float* mean, float* logvar,
+                               int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_ENCODE);
     CPB_REQUIRE(params && source && mean, "mlp encode: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_tc_weights(pl, L, params, true, false, false, s));
-    CPB_TRY(mlp_encoder(pl, L, cfg, params, source, flags, s));
+    CPB_TRY(mlp_encoder(pl, L, spec, params, source, flags, s));
     CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
     if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
     return CPB_OK;
 }
 
-int32_t cpb_mlpvae_decode(const cpb_mlpvae_config* cfg, const float* params, const float* z, float* reconstruction, void* workspace,
-                          int64_t workspace_bytes, void* stream) {
+int32_t cpb_mlpvae_spec_decode(const cpb_mlpvae_spec* spec, const float* params, const float* z, float* reconstruction, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && z && reconstruction, "mlp decode: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
@@ -1351,15 +1475,15 @@ int32_t cpb_mlpvae_decode(const cpb_mlpvae_config* cfg, const float* params, con
     return launch_sigmoid(pl.logits, reconstruction, (long long)pl.B * pl.OUT, s);
 }
 
-int32_t cpb_mlpvae_forward(const cpb_mlpvae_config* cfg, const float* params, const void* source, const void* target, const float* eps,
-                           float* losses, float* mean, float* logvar, float* z, float* reconstruction, int32_t* flags,
-                           void* workspace, int64_t workspace_bytes, void* stream) {
+int32_t cpb_mlpvae_spec_forward(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target, const float* eps,
+                                float* losses, float* mean, float* logvar, float* z, float* reconstruction, int32_t* flags,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_FORWARD);
     CPB_REQUIRE(params && source && target && losses, "mlp forward: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_tc_weights(pl, L, params, true, true, false, s));
-    CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, false, flags, s));
-    CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
+    CPB_TRY(mlp_forward_loss(pl, L, spec, params, source, target, eps, false, flags, s));
+    CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, spec->base.loss_scale, losses, s));
     if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
     if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
     if (z) CPB_TRY(copy_latent_out(pl.zbuf, z, pl.B, pl.z, pl.zp, s));
@@ -1367,15 +1491,87 @@ int32_t cpb_mlpvae_forward(const cpb_mlpvae_config* cfg, const float* params, co
     return CPB_OK;
 }
 
-int32_t cpb_mlpvae_loss_grad(const cpb_mlpvae_config* cfg, const float* params, const void* source, const void* target, const float* eps,
-                             float* grads, float* losses, int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
+int32_t cpb_mlpvae_spec_loss_grad(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target,
+                                  const float* eps, float* grads, float* losses, int32_t* flags, void* workspace,
+                                  int64_t workspace_bytes, void* stream) {
     CPB_MLP_PLAN(CPB_WS_TRAIN);
     CPB_REQUIRE(params && source && target && grads && losses, "mlp loss_grad: NULL pointer");
     CPB_TRY(mlp_pad_weights(pl, L, params, s));
     CPB_TRY(mlp_tc_weights(pl, L, params, true, true, true, s));
-    CPB_TRY(mlp_forward_loss(pl, L, cfg, params, source, target, eps, true, flags, s));
-    CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->base.loss_scale, losses, s));
-    return mlp_backward(pl, L, cfg, params, eps, grads, s);
+    CPB_TRY(mlp_forward_loss(pl, L, spec, params, source, target, eps, true, flags, s));
+    CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, spec->base.loss_scale, losses, s));
+    return mlp_backward(pl, L, spec, params, eps, grads, s);
+}
+
+int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
+                                  int32_t num_measurements, const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
+                                  float* latent_tmp, float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
+                                  int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
+    EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
+                             int64_t ws_bytes, void* stream) {
+        return cpb_mlpvae_spec_encode((const cpb_mlpvae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
+    };
+    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_cfg,
+                          ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
+                          ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+/* The two-per-side entry points: the spec entry points on {enc1, enc2} / {dec1, dec2} */
+static int32_t spec_of(const cpb_mlpvae_config* c, cpb_mlpvae_spec* spec) {
+    CPB_REQUIRE(c != nullptr, "mlp cfg is NULL");
+    memset(spec, 0, sizeof(*spec));
+    spec->base = c->base;
+    spec->num_encoder = 2; spec->encoder_sizes[0] = c->enc1; spec->encoder_sizes[1] = c->enc2;
+    spec->num_decoder = 2; spec->decoder_sizes[0] = c->dec1; spec->decoder_sizes[1] = c->dec2;
+    return CPB_OK;
+}
+#define CPB_MLP_SPEC_OF(cfg)   \
+    cpb_mlpvae_spec spec;      \
+    CPB_TRY(spec_of(cfg, &spec));
+
+int32_t cpb_mlpvae_num_tensors(void) { return 2 * (2 + 2 + 3); }
+const char* cpb_mlpvae_tensor_name(int32_t i) { return mlp_tensor_name(2, 2, i); }
+
+int32_t cpb_mlpvae_layout(const cpb_mlpvae_config* cfg, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_mlpvae_spec_layout(&spec, offsets, sizes, shapes, total);
+}
+
+int32_t cpb_debug_mlpvae_buffer_offsets(const cpb_mlpvae_config* cfg, int32_t mode, int64_t* offsets, int32_t capacity) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_debug_mlpvae_spec_buffer_offsets(&spec, mode, offsets, capacity);
+}
+
+int64_t cpb_mlpvae_workspace_bytes(const cpb_mlpvae_config* cfg, int32_t mode) {
+    cpb_mlpvae_spec spec;
+    if (spec_of(cfg, &spec) != CPB_OK) return CPB_ERR_INVALID_ARGUMENT;
+    return cpb_mlpvae_spec_workspace_bytes(&spec, mode);
+}
+
+int32_t cpb_mlpvae_encode(const cpb_mlpvae_config* cfg, const float* params, const void* source, float* mean, float* logvar,
+                          int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_mlpvae_spec_encode(&spec, params, source, mean, logvar, flags, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_decode(const cpb_mlpvae_config* cfg, const float* params, const float* z, float* reconstruction, void* workspace,
+                          int64_t workspace_bytes, void* stream) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_mlpvae_spec_decode(&spec, params, z, reconstruction, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_forward(const cpb_mlpvae_config* cfg, const float* params, const void* source, const void* target, const float* eps,
+                           float* losses, float* mean, float* logvar, float* z, float* reconstruction, int32_t* flags,
+                           void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_mlpvae_spec_forward(&spec, params, source, target, eps, losses, mean, logvar, z, reconstruction, flags, workspace,
+                                   workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_loss_grad(const cpb_mlpvae_config* cfg, const float* params, const void* source, const void* target, const float* eps,
+                             float* grads, float* losses, int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_MLP_SPEC_OF(cfg);
+    return cpb_mlpvae_spec_loss_grad(&spec, params, source, target, eps, grads, losses, flags, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

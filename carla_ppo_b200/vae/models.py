@@ -24,7 +24,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from .. import _lib
-from .._lib import CpbError, MlpVaeConfig, VaeConfig
+from .._lib import CpbError, MlpVaeConfig, MlpVaeSpec, VaeConfig
 
 
 # ----------------------------------------------------------------------------- loss selectors
@@ -92,9 +92,10 @@ class _Placeholder:
 class VAE:
     """Base class.  Geometry is the reference's only tested one: source [80,160,3], target [80,160,Ct]."""
 
-    # C entry points of the architecture (ConvVAE: cpb_vae_*, MlpVAE: cpb_mlpvae_*; identical argument lists)
+    # C entry points of the architecture (ConvVAE: cpb_vae_*, MlpVAE: cpb_mlpvae_spec_*; identical argument lists)
     _API = {"num_tensors": "cpb_vae_num_tensors", "tensor_name": "cpb_vae_tensor_name", "encode": "cpb_vae_encode",
-            "decode": "cpb_vae_decode", "forward": "cpb_vae_forward", "loss_grad": "cpb_vae_loss_grad"}
+            "decode": "cpb_vae_decode", "forward": "cpb_vae_forward", "loss_grad": "cpb_vae_loss_grad",
+            "encode_predict": "cpb_encode_predict"}
     _HOST_STEP = True        # cpb_vae_train_step_host exists for this architecture
 
     def __init__(self, source_shape, target_shape, build_encoder_fn=None, build_decoder_fn=None,
@@ -155,11 +156,11 @@ class VAE:
         if self._device.index is None:
             self._device = torch.device("cuda", torch.cuda.current_device())
         dev = self._device
-        n = getattr(lib, self._API["num_tensors"])()
+        self._names = self._tensor_names(lib)
+        n = len(self._names)
         offs = (C.c_int64 * n)(); sizes = (C.c_int64 * n)(); shapes = (C.c_int32 * (4 * n))()
         total = C.c_int64()
         self._query_layout(lib, offs, sizes, shapes, total)
-        self._names = [getattr(lib, self._API["tensor_name"])(i).decode() for i in range(n)]
         self._offsets = {self._names[i]: int(offs[i]) for i in range(n)}
         self._shapes = {self._names[i]: tuple(int(s) for s in shapes[4 * i:4 * i + 4] if s > 0) for i in range(n)}
         self._total = int(total.value)
@@ -183,6 +184,10 @@ class VAE:
         self.step_idx = 0
         if init_logging:
             self._init_logging()
+
+    def _tensor_names(self, lib):
+        n = getattr(lib, self._API["num_tensors"])()
+        return [getattr(lib, self._API["tensor_name"])(i).decode() for i in range(n)]
 
     def _query_layout(self, lib, offs, sizes, shapes, total):
         _lib.check(lib.cpb_vae_layout(self.target_shape[2], self.z_dim, offs, sizes, shapes, C.byref(total)), "cpb_vae_layout")
@@ -765,37 +770,55 @@ class ConvVAE(VAE):
 
 
 class MlpVAE(VAE):
-    """The reference's dense VAE (vae/models.py:271-299): flatten -> dense(encoder_sizes, relu) -> mean / logstd_sqare ->
-    sample -> dense(decoder_sizes, relu) -> dense(prod(target_shape)) = logits.  Same surface as ConvVAE; the seven
-    dense layers run on the fp32 SIMT kernels of the library (cpb_mlpvae_* entry points) in math modes 0 and 1.  In
-    math mode 2 (cpb_set_math_mode(2), ``train_vae.py --math_mode tf32``) the five frame-wide products --
-    encoder/dense forward and weight gradient, decoder/dense_2 forward, data gradient and weight gradient -- run as one
-    TF32 tensor-core pass with both operands rounded to nearest (not fp32-accurate); the rest runs as in mode 1.  The
+    """The reference's dense VAE (vae/models.py:271-299): flatten -> one dense relu layer per encoder size -> mean /
+    logstd_sqare -> sample -> one dense relu layer per decoder size -> dense(prod(target_shape)) = logits.  Same surface
+    as ConvVAE.  Each side takes 1 to 8 hidden sizes, each a multiple of 32 in [32, 8192]; the variables carry the
+    reference's names (encoder/dense, encoder/dense_1, ..., decoder/dense_M for the output layer).  The dense layers run
+    on the fp32 SIMT kernels of the library (cpb_mlpvae_spec_* entry points) in math modes 0 and 1.  In math mode 2
+    (cpb_set_math_mode(2), ``train_vae.py --math_mode tf32``) the five frame-wide products -- the first encoder layer's
+    forward and weight gradient, the output layer's forward, data gradient and weight gradient -- run as one TF32
+    tensor-core pass with both operands rounded to nearest (not fp32-accurate); the rest runs as in mode 1.  The
     workspace is re-sized on every call, so switching the mode between calls is safe."""
 
-    _API = {"num_tensors": "cpb_mlpvae_num_tensors", "tensor_name": "cpb_mlpvae_tensor_name", "encode": "cpb_mlpvae_encode",
-            "decode": "cpb_mlpvae_decode", "forward": "cpb_mlpvae_forward", "loss_grad": "cpb_mlpvae_loss_grad"}
+    _API = {"encode": "cpb_mlpvae_spec_encode", "decode": "cpb_mlpvae_spec_decode", "forward": "cpb_mlpvae_spec_forward",
+            "loss_grad": "cpb_mlpvae_spec_loss_grad", "encode_predict": "cpb_mlpvae_encode_predict"}
     _HOST_STEP = False
 
     def __init__(self, source_shape, target_shape=None, encoder_sizes=(512, 256), decoder_sizes=(256, 512), **kwargs):
         target_shape = source_shape if target_shape is None else target_shape
-        if len(encoder_sizes) != 2 or len(decoder_sizes) != 2:
-            raise ValueError("MlpVAE is built for two hidden layers per side (the reference's defaults (512,256)/(256,512))")
         self.encoder_sizes = tuple(int(v) for v in encoder_sizes)
         self.decoder_sizes = tuple(int(v) for v in decoder_sizes)
+        for name, sizes in (("encoder_sizes", self.encoder_sizes), ("decoder_sizes", self.decoder_sizes)):
+            if not 1 <= len(sizes) <= _lib.MLP_MAX_LAYERS or any(v < 32 or v > 8192 or v % 32 for v in sizes):
+                raise ValueError("MlpVAE %s must hold 1 to %d sizes, each a multiple of 32 in [32, 8192], got %r"
+                                 % (name, _lib.MLP_MAX_LAYERS, sizes))
         super().__init__(source_shape, target_shape, None, None, **kwargs)
         self.encoded_shape = (self.encoder_sizes[-1],)
 
+    def _spec(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
+        base = VAE._config(self, batch, source_dtype, target_dtype, loss_scale)
+        return MlpVaeSpec.of(base, self.encoder_sizes, self.decoder_sizes)
+
+    _config = _spec
+
     def _mlp_config(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
+        """The two-per-side MlpVaeConfig of the cpb_mlpvae_* entry points; only a model with two hidden layers per
+        side has one."""
+        if len(self.encoder_sizes) != 2 or len(self.decoder_sizes) != 2:
+            raise ValueError("MlpVaeConfig describes two hidden layers per side; this model has %d and %d"
+                             % (len(self.encoder_sizes), len(self.decoder_sizes)))
         base = VAE._config(self, batch, source_dtype, target_dtype, loss_scale)
         return MlpVaeConfig(base, self.encoder_sizes[0], self.encoder_sizes[1], self.decoder_sizes[0], self.decoder_sizes[1])
 
-    _config = _mlp_config
+    def _tensor_names(self, lib):
+        spec = self._spec(1)
+        n = _lib.check(lib.cpb_mlpvae_spec_num_tensors(C.byref(spec)), "cpb_mlpvae_spec_num_tensors")
+        return [lib.cpb_mlpvae_spec_tensor_name(C.byref(spec), i).decode() for i in range(n)]
 
     def _query_layout(self, lib, offs, sizes, shapes, total):
-        cfg = self._mlp_config(1)
-        _lib.check(lib.cpb_mlpvae_layout(C.byref(cfg), offs, sizes, shapes, C.byref(total)), "cpb_mlpvae_layout")
+        spec = self._spec(1)
+        _lib.check(lib.cpb_mlpvae_spec_layout(C.byref(spec), offs, sizes, shapes, C.byref(total)), "cpb_mlpvae_spec_layout")
 
     def _workspace_need(self, batch, mode):
-        cfg = self._mlp_config(batch)
-        return self._libh.cpb_mlpvae_workspace_bytes(C.byref(cfg), mode)
+        spec = self._spec(batch)
+        return self._libh.cpb_mlpvae_spec_workspace_bytes(C.byref(spec), mode)

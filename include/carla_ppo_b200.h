@@ -145,26 +145,55 @@ int32_t cpb_vae_train_step_host(const cpb_vae_config* cfg, float* params, float*
                                 void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * MlpVAE (vae/models.py:271-299): flatten(38400) -> dense enc1 relu -> dense enc2 relu -> mean / logstd_sqare heads ->
- * sample -> dense dec1 relu -> dense dec2 relu -> dense 12800*Ct (logits).  Same conventions as the ConvVAE entry points
- * above (flat parameter buffer described by cpb_mlpvae_layout, caller-owned workspace, same loss / flag semantics); the
- * optimiser is cpb_adam_apply(_guarded) on the flat buffers.  14 variables: encoder/dense{,_1}, mean, logstd_sqare,
- * decoder/dense{,_1,_2}, each {kernel [in,out], bias}.
- * Arithmetic: fp32 SIMT in math modes 0 and 1.  In math mode 2 (cpb_set_math_mode) the five frame-wide products --
- * encoder/dense forward and weight gradient, decoder/dense_2 forward, data gradient and weight gradient (99 % of the
- * step's multiply-adds) -- run as ONE TF32 wgmma pass with both operands rounded to nearest; everything else
- * (encoder/dense_1, the heads, decoder/dense, decoder/dense_1, sampling, loss, Adam) runs as in the other modes.
+ * MlpVAE (vae/models.py:271-299): flatten(38400) -> one dense relu layer per encoder size -> mean / logstd_sqare heads ->
+ * sample -> one dense relu layer per decoder size -> the output layer, dense 12800*Ct (logits).  Same conventions as the
+ * ConvVAE entry points above (flat parameter buffer described by the layout call, caller-owned workspace, same loss /
+ * flag semantics); the optimiser is cpb_adam_apply(_guarded) on the flat buffers.
+ * Shapes: 1 to 8 hidden layers per side, every width a multiple of 32 in [32, 8192] (an empty side is refused).
+ * Variables, in the reference's creation order (build_mlp, vae/models.py:283-296), each {kernel [in,out], bias}:
+ * encoder/dense, encoder/dense_1 ... encoder/dense_{L-1}, mean, logstd_sqare, decoder/dense ... decoder/dense_{M-1} and
+ * the output layer decoder/dense_M [dec_{M-1}, 12800*Ct]: 2 (L + M + 3) tensors.
+ * Arithmetic: fp32 SIMT in math modes 0 and 1.  In math mode 2 (cpb_set_math_mode) the five frame-wide products -- the
+ * first encoder layer's forward and weight gradient, the output layer's forward, data gradient and weight gradient --
+ * run as ONE TF32 wgmma pass with both operands rounded to nearest; everything else (the other hidden layers, the heads,
+ * sampling, loss, Adam) runs as in the other modes.
  * Batches with batch * 38400 >= 2^31 run those five products on the fp32 kernels in every mode.
- * cpb_mlpvae_workspace_bytes depends on the math mode at the time of the query: mode 2 adds the TF32 weight images
- * and the split partials, and a mode-2 call given a smaller workspace fails with CPB_ERR_WORKSPACE_TOO_SMALL.
+ * The workspace size depends on the math mode at the time of the query: mode 2 adds the TF32 weight images and the
+ * split partials, and a mode-2 call given a smaller workspace fails with CPB_ERR_WORKSPACE_TOO_SMALL.
  * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    cpb_vae_config base;               /* batch, target_channels, z_dim, loss, dtypes, beta, kl_tolerance, loss_scale */
+    int32_t num_encoder;               /* L = len(encoder_sizes), 1..8 */
+    int32_t encoder_sizes[8];          /* the first L are used */
+    int32_t num_decoder;               /* M = len(decoder_sizes), 1..8 */
+    int32_t decoder_sizes[8];          /* the first M are used */
+} cpb_mlpvae_spec;
+
+int32_t     cpb_mlpvae_spec_num_tensors(const cpb_mlpvae_spec* spec);          /* 2 (L + M + 3) */
+const char* cpb_mlpvae_spec_tensor_name(const cpb_mlpvae_spec* spec, int32_t index);
+int32_t cpb_mlpvae_spec_layout(const cpb_mlpvae_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes /* 4 per tensor */,
+                               int64_t* total_floats);
+int64_t cpb_mlpvae_spec_workspace_bytes(const cpb_mlpvae_spec* spec, int32_t mode);
+int32_t cpb_mlpvae_spec_encode(const cpb_mlpvae_spec* spec, const float* params, const void* source, float* mean, float* logvar,
+                               int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_mlpvae_spec_decode(const cpb_mlpvae_spec* spec, const float* params, const float* z, float* reconstruction,
+                               void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_mlpvae_spec_forward(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target,
+                                const float* eps, float* losses, float* mean, float* logvar, float* z, float* reconstruction,
+                                int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_mlpvae_spec_loss_grad(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target,
+                                  const float* eps, float* grads, float* losses, int32_t* flags, void* workspace,
+                                  int64_t workspace_bytes, void* stream);
+
+/* The reference's default shape, two hidden layers per side: the cpb_mlpvae_spec_* entry points on
+ * {enc1, enc2} / {dec1, dec2}, with the same meaning and results. */
 typedef struct {
     cpb_vae_config base;               /* batch, target_channels, z_dim, loss, dtypes, beta, kl_tolerance, loss_scale */
     int32_t enc1, enc2;                /* encoder_sizes (512, 256)   (vae/models.py:277) */
     int32_t dec1, dec2;                /* decoder_sizes (256, 512)   (vae/models.py:278) */
 } cpb_mlpvae_config;
 
-int32_t     cpb_mlpvae_num_tensors(void);
+int32_t     cpb_mlpvae_num_tensors(void);              /* 14 */
 const char* cpb_mlpvae_tensor_name(int32_t index);
 int32_t cpb_mlpvae_layout(const cpb_mlpvae_config* cfg, int64_t* offsets, int64_t* sizes, int32_t* shapes /* 4 per tensor */,
                           int64_t* total_floats);
@@ -256,6 +285,14 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
                            void* vae_workspace, int64_t vae_workspace_bytes,
                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
+/* cpb_encode_predict with an MlpVAE (cpb_mlpvae_spec) as the encoder; same arguments, outputs and noise use. */
+int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                  const float* measurements, int32_t num_measurements,
+                                  const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
+                                  float* latent_tmp, float* state, float* action, float* value, int32_t* flags,
+                                  void* vae_workspace, int64_t vae_workspace_bytes,
+                                  void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
+
 /* Arithmetic used for the dense conv / transposed-conv contractions of the VAE (modes 1 and 0 are fp32-accurate):
  *   1 (default) wgmma tf32 with the error-compensated 3xTF32 split, fp32 accumulators in registers;
  *   0           fp32 FMA (SIMT) tap-GEMM -- also used in modes 1 and 2 for the layers the tensor-core kernel does
@@ -268,7 +305,7 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
  * deconv1-3, in every entry point that runs them (encode, decode, forward, loss_grad, train_step(_host),
  * cpb_encode_predict).  conv1, deconv4, the heads, dense1, the dense weight gradients and PPO use the fp32 kernels
  * in every mode.  The MlpVAE uses the fp32 kernels in modes 0 and 1; mode 2 also runs its five frame-wide products
- * (encoder/dense forward + weight gradient, decoder/dense_2 forward + data gradient + weight gradient) as one TF32
+ * (first encoder layer forward + weight gradient, output layer forward + data gradient + weight gradient) as one TF32
  * pass (see the MlpVAE section).  The mode is process-global and read when a call is enqueued (and by the MlpVAE
  * workspace query); other values are rejected (CPB_ERR_INVALID_ARGUMENT). */
 int32_t cpb_set_math_mode(int32_t mode);
@@ -277,8 +314,10 @@ int32_t cpb_set_math_mode(int32_t mode);
  * D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
 int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t target_channels, int32_t z_dim, int32_t mode,
                                      int64_t* offsets, int32_t capacity);
-/* The MlpVAE twin, in the current math mode: [x,h1,h2,heads,z,g1,g2,logits,ga,gb] (ga / gb: the backward pass's two
- * gradient buffers; after loss_grad, gb holds d loss / d (encoder/dense pre-activation) and logits d loss / d logits). */
+/* The MlpVAE twin, in the current math mode: [x,h_0..h_{L-1},heads,z,g_0..g_{M-1},logits,ga,gb], L + M + 6 entries
+ * (ga / gb: the backward pass's two gradient buffers; after loss_grad, gb holds d loss / d (encoder/dense pre-activation)
+ * and logits d loss / d logits).  The two-per-side call returns [x,h1,h2,heads,z,g1,g2,logits,ga,gb]. */
+int32_t cpb_debug_mlpvae_spec_buffer_offsets(const cpb_mlpvae_spec* spec, int32_t mode, int64_t* offsets, int32_t capacity);
 int32_t cpb_debug_mlpvae_buffer_offsets(const cpb_mlpvae_config* cfg, int32_t mode, int64_t* offsets, int32_t capacity);
 int32_t cpb_debug_tc_wgrad(const float* big, const float* small, float* out, int32_t m, int32_t i, int32_t j,
                            int32_t variant, float* partial, void* stream);

@@ -1,18 +1,20 @@
 """Math mode 1 (fp32 SIMT for the MlpVAE) against math mode 2 (its five frame-wide products as one TF32 pass) on the
-MlpVAE train step (encoder 512/256, decoder 256/512, z = 64, rgb target), in one process.
+MlpVAE train step (by default encoder 512/256, decoder 256/512, z = 64, rgb target), in one process.
 
-    python scripts/mlp_tf32_bench.py [--rounds 5] [--train-steps 300] [--out DIR] [--dump DIR [--dump-only]]
+    python scripts/mlp_tf32_bench.py [--encoder_sizes 512 256] [--decoder_sizes 256 512] [--rounds 5] [--train-steps 300]
+                                     [--out DIR] [--dump DIR [--dump-only]]
 
 1. Step time.  Both modes are warmed at both batch sizes, then blocks of train steps (glorot init, seeded uniform
    frames, device-resident inputs) alternate between the modes at batch 4096 and 512 for --rounds rounds, the order of
    the two modes swapped every round; each block is timed with CUDA events.  Reported per mode: median ms/step and
    spread (max - min over the rounds).
 2. Profile.  The per-group device time (cpb_profile_*) of each mode at both batch sizes, and for the five frame-wide
-   groups the achieved TFLOP/s computed from the layer shapes (2 x multiply-adds / group time).
-3. Training.  --train-steps Adam steps from the same glorot init on the 128 committed frames (batch 32, BCE, seeded
+   groups the achieved TFLOP/s computed from the layer shapes (2 x multiply-adds / group time).  The labels name the
+   first encoder layer "enc" and the output layer "dec2" at every depth.
+3. Training (skipped with --train-steps 0).  --train-steps Adam steps from the same glorot init on the 128 committed frames (batch 32, BCE, seeded
    minibatches and noise) in each mode; both loss curves are printed.  Evidence that training behaves alike, not a gate.
 --dump DIR writes DIR/mlp_mode1_loss_grad.npz: the losses and the flat gradient of one mode-1 loss_grad (glorot seed 0,
-seeded batch of 64): running it against two builds shows whether mode 1 changed.  --package-root loads the package
+seeded batch of 64, the default sizes): running it against two builds shows whether mode 1 changed.  --package-root loads the package
 (and its library) from another tree, e.g. a checkout of the other build.
 The card (name, power limit, max SM clock) is read with a read-only nvidia-smi query.  Writes DIR/mlp_tf32_bench.json.
 """
@@ -30,9 +32,13 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = {"3xtf32": 1, "tf32": 2}
 ENC, DEC, Z, IN, OUT = (512, 256), (256, 512), 64, 38400, 38400
-# multiply-adds per frame of the five frame-wide products (profile labels of cpb_mlpvae_loss_grad)
-GROUP_MACS = {"mlp.enc.fwd": IN * ENC[0], "mlp.enc.wgrad": IN * ENC[0], "mlp.dec2.fwd": DEC[1] * OUT,
-              "mlp.dec2.dgrad": DEC[1] * OUT, "mlp.dec2.wgrad": DEC[1] * OUT}
+
+
+def group_macs(enc, dec):
+    """Multiply-adds per frame of the five frame-wide products (profile labels of the MlpVAE loss_grad): the first
+    encoder layer and the output layer."""
+    return {"mlp.enc.fwd": IN * enc[0], "mlp.enc.wgrad": IN * enc[0], "mlp.dec2.fwd": dec[-1] * OUT,
+            "mlp.dec2.dgrad": dec[-1] * OUT, "mlp.dec2.wgrad": dec[-1] * OUT}
 
 
 def card():
@@ -41,9 +47,9 @@ def card():
     return q.stdout.strip()
 
 
-def make_vae(loss="mse", seed=0):
+def make_vae(loss="mse", seed=0, enc=ENC, dec=DEC):
     from carla_ppo_b200.vae.models import MlpVAE
-    vae = MlpVAE((80, 160, 3), z_dim=Z, encoder_sizes=ENC, decoder_sizes=DEC, beta=1.0, learning_rate=1e-4, loss_fn=loss,
+    vae = MlpVAE((80, 160, 3), z_dim=Z, encoder_sizes=enc, decoder_sizes=dec, beta=1.0, learning_rate=1e-4, loss_fn=loss,
                  model_dir=tempfile.mkdtemp(), seed=seed)
     vae.init_session(init_logging=False)          # glorot-uniform init
     return vae
@@ -108,7 +114,10 @@ def main():
     ap.add_argument("--dump", default=None, help="write one mode-1 loss_grad's losses and gradient to this directory")
     ap.add_argument("--dump-only", action="store_true")
     ap.add_argument("--package-root", default=ROOT, help="tree to import carla_ppo_b200 from")
+    ap.add_argument("--encoder_sizes", type=int, nargs="+", default=list(ENC))
+    ap.add_argument("--decoder_sizes", type=int, nargs="+", default=list(DEC))
     args = ap.parse_args()
+    enc, dec = tuple(args.encoder_sizes), tuple(args.decoder_sizes)
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.abspath(args.package_root))
     import torch
@@ -120,10 +129,10 @@ def main():
         dump(lib, args.dump)
         if args.dump_only:
             return
-    result = {"card": card(), "rounds": args.rounds, "model": {"encoder": ENC, "decoder": DEC, "z": Z}}
+    result = {"card": card(), "rounds": args.rounds, "model": {"encoder": enc, "decoder": dec, "z": Z}}
 
     # ---- 1. step time
-    vae = make_vae()
+    vae = make_vae(enc=enc, dec=dec)
     g = torch.Generator(device="cuda"); g.manual_seed(1234)
     x = torch.rand(4096, 80, 160, 3, generator=g, device="cuda")
     eps = torch.randn(4096, Z, generator=g, device="cuda")
@@ -157,16 +166,19 @@ def main():
             prof = profile(lib, vae, xb, eb)
             result["profile_ms_per_step"]["B%d_%s" % (b, name)] = prof
             result["tflops"]["B%d_%s" % (b, name)] = {
-                k: round(2.0 * macs * b / (prof[k] * 1e-3) / 1e12, 1) for k, macs in GROUP_MACS.items() if prof.get(k)}
+                k: round(2.0 * macs * b / (prof[k] * 1e-3) / 1e12, 1) for k, macs in group_macs(enc, dec).items() if prof.get(k)}
     del vae, x, eps, batches
     torch.cuda.empty_cache()
 
     # ---- 3. training curves on the committed frames
+    if args.train_steps == 0:
+        finish(result, args.out)
+        return
     frames = torch.as_tensor(np.load(os.path.join(ROOT, "tests", "golden", "frames_u8.npz"))["rgb"], device="cuda")
     curves = {}
     for name, mode in MODES.items():
         set_mode(lib, mode)
-        v = make_vae(loss="bce")
+        v = make_vae(loss="bce", enc=enc, dec=dec)
         rs = np.random.RandomState(0)
         out = []
         for _ in range(args.train_steps):
@@ -183,11 +195,15 @@ def main():
     tail = max(1, args.train_steps // 6)
     result["training"] = {m: {"recon_kl_every_%d" % every: [round(float(c[s].sum()), 3) for s in range(0, len(c), every)],
                               "mean_last_%d" % tail: round(float(c[-tail:].sum(axis=1).mean()), 3)} for m, c in curves.items()}
+    finish(result, args.out)
+
+
+def finish(result, out):
     result["card_after"] = card()
     print(json.dumps({k: v for k, v in result.items() if k != "training"}, indent=1))
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "mlp_tf32_bench.json"), "w") as f:
+    if out:
+        os.makedirs(out, exist_ok=True)
+        with open(os.path.join(out, "mlp_tf32_bench.json"), "w") as f:
             json.dump(result, f, indent=1)
 
 
