@@ -256,7 +256,8 @@ int32_t cpb_ppo_train_step(const cpb_ppo_config* cfg, float* params, const float
 /* utils.compute_gae (utils.py:45-50) + train.py:176-177, float64 like the reference:
  *   delta_t = r_t + (1-d_t) gamma V_{t+1} - V_t ;  A_t = delta_t + gamma*lam*A_{t+1}  (no reset)
  *   returns = A + V ;  advantages_norm = (A - mean A) / (std A + 1e-8)
- * rewards, values, dones: double[T] (dones as 0/1); outputs double[T], any may be NULL. */
+ * rewards, values, dones: double[T] (dones as 0/1); outputs double[T]: advantages is required,
+ * returns and advantages_norm may be NULL. */
 int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_value,
                 const double* dones, int32_t T, double gamma, double lam,
                 double* advantages, double* returns, double* advantages_norm, void* stream);
