@@ -108,6 +108,7 @@ PROTOTYPES = {
                              _i32, _i32, _P, _P, _P, _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
+    "cpb_debug_vae_backward_stop": (_i32, [C.c_char_p]),
     "cpb_debug_mlpvae_buffer_offsets": (_i32, [_MC, _i32, _P, _i32]),
     "cpb_debug_mlpvae_spec_buffer_offsets": (_i32, [_MS, _i32, _P, _i32]),
     "cpb_debug_tc_wgrad": (_i32, [_P, _P, _P, _i32, _i32, _i32, _i32, _P, _P]),

@@ -595,6 +595,14 @@ static int32_t run_forward_loss(const VaePlan& pl, const VaeLayout& L, const cpb
     return CPB_OK;
 }
 
+// cpb_debug_vae_backward_stop: the layer groups of run_backward after which it may return early, in pass order.  Each
+// group is the layer's weight gradient, bias gradient and data gradient; the stop comes after all three.
+static const char* kBackwardStops[] = {"deconv4.dgrad", "deconv3.dgrad", "deconv2.dgrad", "deconv1.dgrad", "dense1.dgrad",
+                                       "heads.dgrad", "conv4.dgrad", "conv3.dgrad"};
+enum { STOP_DECONV4, STOP_DECONV3, STOP_DECONV2, STOP_DECONV1, STOP_DENSE1, STOP_HEADS, STOP_CONV4, STOP_CONV3 };
+static int g_backward_stop = -1;    // index into kBackwardStops, -1: run the whole pass
+#define CPB_BACKWARD_STOP(group) if (g_backward_stop == (group)) return CPB_OK
+
 static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae_config* cfg, const float* params,
                             const float* eps, float* grads, cudaStream_t s) {
     using namespace geo;
@@ -613,6 +621,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.frame_dsum, B, 4, pl.ct, grads + L.off[T_DECONV4_B], cs, s));
     { ProfScope prof("deconv4.dgrad", s);
       CPB_TRY(launch_edge_gather(dlog, pl.ct, params + L.off[T_DECONV4_K], nullptr, pl.b3, pl.gA, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
+    CPB_BACKWARD_STOP(STOP_DECONV4);
     TapGemmParams p;
     // ---- deconv3
     CPB_TRY(run_wgrad("deconv3.wgrad", pl.gA, W1, C1, (long long)H1 * W1 * C1, 5, pl.b2, B, H2, W2, C2, 5 * 5 * C1, 5 * 5 * C1,
@@ -621,6 +630,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p = gather_problem(pl.gA, B, H1, W1, C1, 5, params + L.off[T_DECONV3_K], C2, nullptr, pl.b2, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV3].f_hi, pl.relayout + pl.rl.tc[TC_DECONV3].f_lo);
     CPB_TRY(tg("deconv3.dgrad", p, s, 0));   // gB = g(b2)
+    CPB_BACKWARD_STOP(STOP_DECONV3);
     // ---- deconv2
     CPB_TRY(run_wgrad("deconv2.wgrad", pl.gB, W2, C2, (long long)H2 * W2 * C2, 4, pl.b1, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_DECONV2_K], s));
@@ -628,6 +638,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p = gather_problem(pl.gB, B, H2, W2, C2, 4, params + L.off[T_DECONV2_K], C3, nullptr, pl.b1, pl.gA, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV2].f_hi, pl.relayout + pl.rl.tc[TC_DECONV2].f_lo);
     CPB_TRY(tg("deconv2.dgrad", p, s, 0));   // gA = g(b1)
+    CPB_BACKWARD_STOP(STOP_DECONV2);
     // ---- deconv1
     CPB_TRY(run_wgrad("deconv1.wgrad", pl.gA, W3, C3, (long long)H3 * W3 * C3, 4, pl.d1, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
                       grads + L.off[T_DECONV1_K], s));
@@ -635,6 +646,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p = gather_problem(pl.gA, B, H3, W3, C3, 4, params + L.off[T_DECONV1_K], C4, nullptr, nullptr, pl.gB, 0,
                        pl.relayout + pl.rl.tc[TC_DECONV1].f_hi, pl.relayout + pl.rl.tc[TC_DECONV1].f_lo);
     CPB_TRY(tg("deconv1.dgrad", p, s, 0));                                   // gB = g(d1) [B, 6144]
+    CPB_BACKWARD_STOP(STOP_DECONV1);
     // ---- dense1
     CPB_TRY(run_dense_wgrad("dense1.wgrad", pl.zbuf, zp, z, pl.gB, B, FEAT, FEAT, pl.partial, grads + L.off[T_DENSE1_K], s));
     CPB_TRY(launch_colsum(pl.gB, B, FEAT, FEAT, grads + L.off[T_DENSE1_B], cs, s));
@@ -642,6 +654,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p.ksplit = tapgemm_pick_ksplit(B, zp, 1, FEAT);
     p.kpartial = pl.ksplit; p.kpartial_stride = (long long)B * zp;
     CPB_TRY(tg("dense1.dgrad", p, s));
+    CPB_BACKWARD_STOP(STOP_DENSE1);
     // ---- sampling + KL
     CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, cfg->beta * cfg->loss_scale / (float)B,
                                pl.gheads, s));
@@ -657,6 +670,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p.cls[0].taps[1].src_off = (long long)B * zp;
     p.cls[0].taps[1].w_off = (long long)zp * FEAT;
     CPB_TRY(tg("heads.dgrad", p, s));                                   // gA = g(a4 pre-activation)
+    CPB_BACKWARD_STOP(STOP_HEADS);
     // ---- conv4
     CPB_TRY(run_wgrad("conv4.wgrad", pl.a3, W3, C3, (long long)H3 * W3 * C3, 4, pl.gA, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
                       grads + L.off[T_CONV4_K], s));
@@ -664,6 +678,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p = scatter_problem(pl.gA, B, H4, W4, C4, 4, pl.relayout + pl.rl.conv4T, C3, nullptr, pl.a3, pl.gB, H3, W3, 0,
                         pl.relayout + pl.rl.tc[TC_CONV4].t_hi, pl.relayout + pl.rl.tc[TC_CONV4].t_lo);
     CPB_TRY(tg("conv4.dgrad", p, s, 4));   // gB = g(a3)
+    CPB_BACKWARD_STOP(STOP_CONV4);
     // ---- conv3
     CPB_TRY(run_wgrad("conv3.wgrad", pl.a2, W2, C2, (long long)H2 * W2 * C2, 4, pl.gB, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
                       grads + L.off[T_CONV3_K], s));
@@ -671,6 +686,7 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     p = scatter_problem(pl.gB, B, H3, W3, C3, 4, pl.relayout + pl.rl.conv3T, C2, nullptr, pl.a2, pl.gA, H2, W2, 0,
                         pl.relayout + pl.rl.tc[TC_CONV3].t_hi, pl.relayout + pl.rl.tc[TC_CONV3].t_lo);
     CPB_TRY(tg("conv3.dgrad", p, s, 4));   // gA = g(a2)
+    CPB_BACKWARD_STOP(STOP_CONV3);
     // ---- conv2
     CPB_TRY(run_wgrad("conv2.wgrad", pl.a1, W1, C1, (long long)H1 * W1 * C1, 4, pl.gA, B, H2, W2, C2, 16 * C1, 16 * C1, pl.partial,
                       grads + L.off[T_CONV2_K], s));
@@ -1104,10 +1120,27 @@ int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t ct, int32_t z, int32
     char* base = (char*)4096;   // fake non-null base: only differences are used
     VaePlan pl = make_plan(base, (int64_t)1 << 60, batch, ct, z, mode);
     const float* ptrs[] = {pl.xp, pl.a1, pl.a2, pl.a3, pl.a4, pl.heads, pl.zbuf, pl.d1, pl.b1, pl.b2, pl.b3, pl.logits_p, pl.gA, pl.gB,
-                           pl.frame_loss, pl.kl_rows};
+                           pl.frame_loss, pl.kl_rows, pl.gz, pl.gheads};
     const int n = (int)(sizeof(ptrs) / sizeof(ptrs[0]));
-    for (int i = 0; i < n && i < capacity; ++i) offsets[i] = ptrs[i] ? (int64_t)((const char*)ptrs[i] - base) : -1;
-    return n;
+    // the table only grows at its end: a caller that asks for the first `capacity` entries gets exactly those
+    const int written = n < capacity ? n : (capacity > 0 ? capacity : 0);
+    for (int i = 0; i < written; ++i) offsets[i] = ptrs[i] ? (int64_t)((const char*)ptrs[i] - base) : -1;
+    return written;
+}
+
+/* debug: make every later ConvVAE backward pass return right after the named layer group (NULL: run the whole pass) */
+int32_t cpb_debug_vae_backward_stop(const char* group) {
+    if (group == nullptr) {
+        g_backward_stop = -1;
+        return CPB_OK;
+    }
+    for (int i = 0; i < (int)(sizeof(kBackwardStops) / sizeof(kBackwardStops[0])); ++i)
+        if (strcmp(group, kBackwardStops[i]) == 0) {
+            g_backward_stop = i;
+            return CPB_OK;
+        }
+    cpb::set_error("cpb_debug_vae_backward_stop: unknown layer group '%s'", group);
+    return CPB_ERR_INVALID_ARGUMENT;
 }
 
 /* debug: D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core tap-GEMM (dense, one tap); the single-pass kernel in math

@@ -311,10 +311,19 @@ int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_
  * workspace query); other values are rejected (CPB_ERR_INVALID_ARGUMENT). */
 int32_t cpb_set_math_mode(int32_t mode);
 /* Debug / test hooks (not part of the reference-facing surface): workspace buffer offsets in bytes for
- * [xp,a1,a2,a3,a4,heads,z,d1,b1,b2,b3,logits_p,gA,gB,frame_loss,kl_rows] (-1 = absent in that mode), and a dense
- * D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
+ * [xp,a1,a2,a3,a4,heads,z,d1,b1,b2,b3,logits_p,gA,gB,frame_loss,kl_rows,gz,gheads] (-1 = absent in that mode; the
+ * first min(18, capacity) entries are written and their count returned; new entries are only ever appended), and a
+ * dense D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
 int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t target_channels, int32_t z_dim, int32_t mode,
                                      int64_t* offsets, int32_t capacity);
+/* Process-global, like the math mode: every later ConvVAE backward pass (loss_grad, train_step) returns CPB_OK right
+ * after the named layer group -- its weight, bias and data gradients -- has been enqueued.  Groups in pass order:
+ * "deconv4.dgrad", "deconv3.dgrad", "deconv2.dgrad", "deconv1.dgrad", "dense1.dgrad", "heads.dgrad", "conv4.dgrad",
+ * "conv3.dgrad" (the whole pass ends with conv2's data gradient and conv1's weight gradient).  At a stop, the
+ * workspace gradient buffer the group read (logits_p, gA, gB, gz or gheads) still holds its input gradient and the one
+ * it wrote its output gradient; gradients of the layers not reached yet are 0.  NULL runs the whole pass again; any
+ * other string is rejected (CPB_ERR_INVALID_ARGUMENT) and leaves the setting as it was. */
+int32_t cpb_debug_vae_backward_stop(const char* group);
 /* The MlpVAE twin, in the current math mode: [x,h_0..h_{L-1},heads,z,g_0..g_{M-1},logits,ga,gb], L + M + 6 entries
  * (ga / gb: the backward pass's two gradient buffers; after loss_grad, gb holds d loss / d (encoder/dense pre-activation)
  * and logits d loss / d logits).  The two-per-side call returns [x,h1,h2,heads,z,g1,g2,logits,ga,gb]. */
