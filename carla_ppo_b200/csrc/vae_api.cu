@@ -72,6 +72,7 @@ int32_t ensure_init() {
 // ---------------------------------------------------------------------------------------------
 // geometry (source 80x160x3, reference vae_common.py:18-20; layer table SURVEY appendix A.1)
 // ---------------------------------------------------------------------------------------------
+struct Side { int H, W, C; };
 namespace geo {
 constexpr int H0 = 80, W0 = 160;
 constexpr int H1 = 39, W1 = 79, C1 = 32;
@@ -80,6 +81,7 @@ constexpr int H3 = 8, W3 = 18, C3 = 128;
 constexpr int H4 = 3, W4 = 8, C4 = 256;
 constexpr int FEAT = H4 * W4 * C4;   // 6144
 constexpr int NPIX = H0 * W0;        // 12800
+constexpr Side S1{H1, W1, C1}, S2{H2, W2, C2}, S3{H3, W3, C3}, S4{H4, W4, C4};
 }  // namespace geo
 
 enum VaeTensor {
@@ -113,19 +115,81 @@ static void set_shape(VaeLayout& L, int t, int a, int b = 0, int c = 0, int d = 
     L.size[t] = n;
 }
 
+// ---------------------------------------------------------------------------------------------
+// workspace plan
+// ---------------------------------------------------------------------------------------------
+constexpr int kTcLayerCount = 6;
+struct TcW { int64_t f_hi, f_lo, t_hi, t_lo; };   // gather-form / quad-scatter-form K-major hi/lo copies of one kernel
+struct Relayout {
+    int64_t T[kTcLayerCount];       // scatter-form kernels [kh][kw][cs][cb] of the SIMT tap-GEMM, by TC_* slot
+    int64_t dense1T, headsT, conv1P, deconv4P;
+    TcW tc[kTcLayerCount];          // by TC_* slot
+    // z < z_pad only (empty otherwise): zero-padded copies of the z-sized weights, [2][6144][z_pad], [2][z_pad], [z_pad][6144]
+    int64_t headsP, headsBP, dense1P;
+    int64_t total;
+};
+enum { TC_CONV2, TC_CONV3, TC_CONV4, TC_DECONV1, TC_DECONV2, TC_DECONV3 };
+
+// Inside the library the latent has z_pad = 64 * ceil(z / 64) columns: the heads and dense1 then run the shapes of a
+// multiple-of-64 model (the k-split tap-GEMM needs N % 64 == 0).  The padded columns hold zeros.
+static int z_pad(int z) { return (int)align_up(z, 64); }
+
+struct VaePlan {
+    int B, ct, z, zp, mode;     // zp = z_pad(z): row pitch of every latent buffer (heads, zbuf, gz, gheads, ksplit)
+    Relayout rl;
+    float *relayout, *xp, *yp, *a1, *a2, *a3, *a4, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss;
+    float *d1, *b1, *b2, *b3, *logits_p;
+    float *gA, *gB, *gz, *gheads, *partial, *colsum;
+    float* cs_edge;     // per-CTA column sums of deconv4's data gradient (edge_gather), [edge_gather_blocks(B)][32]
+    float* frame_dsum;  // per-frame channel sums of d loss / d logits, [B][4]
+    float* ksplit;      // partial results of the k-split dense layers: kMaxKSplit x [2, B, z_pad]
+    int64_t bytes;
+};
+
+// ---------------------------------------------------------------------------------------------
+// The six stride-2 layers on the tap-GEMM, in the big/small notation of DESIGN §2 (kernel [k][k][Cb][Cs]): a conv maps its
+// big side to its small side, a deconv the other way round.  The gather form of a pass reads the big side and the kernel
+// as stored (TF32 image TcW::f_*), the scatter form the small side and Relayout::T (TF32 quad image TcW::t_*).  The form
+// rule (uses_scatter): a conv's forward pass runs the gather form and its data gradient the scatter form; a deconv's the
+// other way round.
+// ---------------------------------------------------------------------------------------------
+struct TcLayer {
+    const char *fwd, *wgrad, *dgrad;        // profile labels of the three passes; dgrad also names the backward stop
+    int kernel, bias, slot;                 // VaeTensor, VaeTensor, TC_*
+    bool deconv;
+    int k;
+    Side big, small;
+    float *VaePlan::*in, *VaePlan::*out;    // the forward pass's input and output activation
+    bool edge;                              // the bias gradient comes from the column sums edge_gather left in cs_edge
+    bool linear;                            // the input has no ReLU: the data gradient is not masked
+};
+
+#define CPB_TC_LABELS(name) name ".fwd", name ".wgrad", name ".dgrad"
+static const TcLayer kTcLayers[kTcLayerCount] = {
+    //                         kernel       bias         slot        deconv k  big      small    in            out           edge   linear
+    {CPB_TC_LABELS("conv2"),   T_CONV2_K,   T_CONV2_B,   TC_CONV2,   false, 4, geo::S1, geo::S2, &VaePlan::a1, &VaePlan::a2, false, false},
+    {CPB_TC_LABELS("conv3"),   T_CONV3_K,   T_CONV3_B,   TC_CONV3,   false, 4, geo::S2, geo::S3, &VaePlan::a2, &VaePlan::a3, false, false},
+    {CPB_TC_LABELS("conv4"),   T_CONV4_K,   T_CONV4_B,   TC_CONV4,   false, 4, geo::S3, geo::S4, &VaePlan::a3, &VaePlan::a4, false, false},
+    // d1, dense1's output, is linear
+    {CPB_TC_LABELS("deconv1"), T_DECONV1_K, T_DECONV1_B, TC_DECONV1, true,  4, geo::S3, geo::S4, &VaePlan::d1, &VaePlan::b1, false, true},
+    {CPB_TC_LABELS("deconv2"), T_DECONV2_K, T_DECONV2_B, TC_DECONV2, true,  4, geo::S2, geo::S3, &VaePlan::b1, &VaePlan::b2, false, false},
+    // deconv4's data gradient (edge_gather) leaves the column sums of deconv3's output gradient in cs_edge
+    {CPB_TC_LABELS("deconv3"), T_DECONV3_K, T_DECONV3_B, TC_DECONV3, true,  5, geo::S1, geo::S2, &VaePlan::b2, &VaePlan::b3, true,  false},
+};
+
+static bool uses_scatter(const TcLayer& l, bool dgrad) { return l.deconv != dgrad; }
+
 static VaeLayout make_layout(int ct, int z) {
     using namespace geo;
     VaeLayout L;
     set_shape(L, T_CONV1_K, 4, 4, 3, C1);    set_shape(L, T_CONV1_B, C1);
-    set_shape(L, T_CONV2_K, 4, 4, C1, C2);   set_shape(L, T_CONV2_B, C2);
-    set_shape(L, T_CONV3_K, 4, 4, C2, C3);   set_shape(L, T_CONV3_B, C3);
-    set_shape(L, T_CONV4_K, 4, 4, C3, C4);   set_shape(L, T_CONV4_B, C4);
+    for (const TcLayer& l : kTcLayers) {
+        set_shape(L, l.kernel, l.k, l.k, l.big.C, l.small.C);
+        set_shape(L, l.bias, l.deconv ? l.big.C : l.small.C);
+    }
     set_shape(L, T_MEAN_K, FEAT, z);         set_shape(L, T_MEAN_B, z);
     set_shape(L, T_LOGVAR_K, FEAT, z);       set_shape(L, T_LOGVAR_B, z);
     set_shape(L, T_DENSE1_K, z, FEAT);       set_shape(L, T_DENSE1_B, FEAT);
-    set_shape(L, T_DECONV1_K, 4, 4, C3, C4); set_shape(L, T_DECONV1_B, C3);
-    set_shape(L, T_DECONV2_K, 4, 4, C2, C3); set_shape(L, T_DECONV2_B, C2);
-    set_shape(L, T_DECONV3_K, 5, 5, C1, C2); set_shape(L, T_DECONV3_B, C1);
     set_shape(L, T_DECONV4_K, 4, 4, ct, C1); set_shape(L, T_DECONV4_B, ct);
     // storage order: TF creation order, except that the two head kernels (and the two head biases) are
     // adjacent so that both heads run as one y-batched tap-GEMM.
@@ -142,23 +206,6 @@ static VaeLayout make_layout(int ct, int z) {
     return L;
 }
 
-// ---------------------------------------------------------------------------------------------
-// workspace plan
-// ---------------------------------------------------------------------------------------------
-struct TcW { int64_t f_hi, f_lo, t_hi, t_lo; };   // gather-form / quad-scatter-form K-major hi/lo copies of one kernel
-struct Relayout {
-    int64_t conv2T, conv3T, conv4T, deconv1T, deconv2T, deconv3T, dense1T, headsT, conv1P, deconv4P;
-    TcW tc[6];          // conv2, conv3, conv4, deconv1, deconv2, deconv3
-    // z < z_pad only (empty otherwise): zero-padded copies of the z-sized weights, [2][6144][z_pad], [2][z_pad], [z_pad][6144]
-    int64_t headsP, headsBP, dense1P;
-    int64_t total;
-};
-enum { TC_CONV2, TC_CONV3, TC_CONV4, TC_DECONV1, TC_DECONV2, TC_DECONV3 };
-
-// Inside the library the latent has z_pad = 64 * ceil(z / 64) columns: the heads and dense1 then run the shapes of a
-// multiple-of-64 model (the k-split tap-GEMM needs N % 64 == 0).  The padded columns hold zeros.
-static int z_pad(int z) { return (int)align_up(z, 64); }
-
 static Relayout make_relayout(int z) {
     using namespace geo;
     const int zp = z_pad(z);
@@ -166,21 +213,16 @@ static Relayout make_relayout(int z) {
     Relayout r;
     int64_t o = 0;
     auto take = [&](int64_t n) { int64_t at = o; o += align_up(n, 64); return at; };
-    r.conv2T = take(16LL * C1 * C2);
-    r.conv3T = take(16LL * C2 * C3);
-    r.conv4T = take(16LL * C3 * C4);
-    r.deconv1T = take(16LL * C3 * C4);
-    r.deconv2T = take(16LL * C2 * C3);
-    r.deconv3T = take(25LL * C1 * C2);
+    for (const TcLayer& l : kTcLayers) r.T[l.slot] = take((int64_t)l.k * l.k * l.big.C * l.small.C);
     r.dense1T = take((int64_t)zp * FEAT);
     r.headsT = take(2LL * zp * FEAT);
     r.conv1P = take(16LL * 4 * C1);
     r.deconv4P = take(16LL * 4 * C1);
-    const int64_t sizes[6] = {16LL * C1 * C2, 16LL * C2 * C3, 16LL * C3 * C4, 16LL * C3 * C4, 16LL * C2 * C3, 25LL * C1 * C2};
-    const int64_t qsizes[6] = {16LL * C1 * C2, 16LL * C2 * C3, 16LL * C3 * C4, 16LL * C3 * C4, 16LL * C2 * C3, 36LL * C1 * C2};
-    for (int i = 0; i < 6; ++i) {
-        r.tc[i].f_hi = take(sizes[i]); r.tc[i].f_lo = take(sizes[i]);
-        r.tc[i].t_hi = take(qsizes[i]); r.tc[i].t_lo = take(qsizes[i]);
+    for (const TcLayer& l : kTcLayers) {
+        const int64_t n = (int64_t)l.k * l.k * l.big.C * l.small.C, win = (l.k + 1) / 2;
+        TcW& w = r.tc[l.slot];
+        w.f_hi = take(n); w.f_lo = take(n);
+        w.t_hi = take(win * win * 4 * l.big.C * l.small.C); w.t_lo = take(win * win * 4 * l.big.C * l.small.C);
     }
     r.headsP = take(padded ? 2LL * FEAT * zp : 0);
     r.headsBP = take(padded ? 2LL * zp : 0);
@@ -189,40 +231,18 @@ static Relayout make_relayout(int z) {
     return r;
 }
 
-struct VaePlan {
-    int B, ct, z, zp, mode;     // zp = z_pad(z): row pitch of every latent buffer (heads, zbuf, gz, gheads, ksplit)
-    Relayout rl;
-    float *relayout, *xp, *yp, *a1, *a2, *a3, *a4, *heads, *zbuf, *kl_rows, *kl_active, *frame_loss;
-    float *d1, *b1, *b2, *b3, *logits_p;
-    float *gA, *gB, *gz, *gheads, *partial, *colsum;
-    float* cs_edge;     // per-CTA column sums of deconv4's data gradient (edge_gather), [edge_gather_blocks(B)][32]
-    float* frame_dsum;  // per-frame channel sums of d loss / d logits, [B][4]
-    float* ksplit;      // partial results of the k-split dense layers: kMaxKSplit x [2, B, z_pad]
-    int64_t bytes;
-    bool ok;
-};
-
 static int64_t max_partial_floats(int B, int zp) {
     using namespace geo;
-    struct P { int I, J; long long M; };
-    const P ps[] = {
-        {64, C1, (long long)B * H1 * W1},          // conv1 / deconv4 (padded to 4 channels)
-        {16 * C1, C2, (long long)B * H2 * W2},     // conv2
-        {16 * C2, C3, (long long)B * H3 * W3},     // conv3 / deconv2
-        {16 * C3, C4, (long long)B * H4 * W4},     // conv4 / deconv1
-        {25 * C1, C2, (long long)B * H2 * W2},     // deconv3
-        {FEAT, zp, (long long)B},                   // heads
-        {zp, FEAT, (long long)B},                   // dense1
-    };
-    int64_t best = (int64_t)edge_wgrad_ctas(B) * 48 * C1;
     // the tensor-core weight gradient runs ONE wave of (i-tile, j-tile, split) CTAs with 128 x BN <= 128 x 64 tiles
-    if (best < (int64_t)kTcWaveCtas * 128 * 64) best = (int64_t)kTcWaveCtas * 128 * 64;
-    for (const P& p : ps) {
-        int64_t n = (int64_t)wgrad_pick_splits(p.I, p.J, p.M) * p.I * p.J;
-        if (n > best) best = n;
-        n = (int64_t)tc_wgrad_pick_splits(p.I, p.J, p.M) * p.I * p.J;
-        if (n > best) best = n;
-    }
+    int64_t best = std::max<int64_t>((int64_t)edge_wgrad_ctas(B) * 48 * C1, (int64_t)kTcWaveCtas * 128 * 64);
+    auto fit = [&](int I, int J, long long M) {
+        best = std::max<int64_t>(best, (int64_t)wgrad_pick_splits(I, J, M) * I * J);
+        best = std::max<int64_t>(best, (int64_t)tc_wgrad_pick_splits(I, J, M) * I * J);
+    };
+    fit(64, C1, (long long)B * H1 * W1);        // conv1 / deconv4 (padded to 4 channels)
+    for (const TcLayer& l : kTcLayers) fit(l.k * l.k * l.big.C, l.small.C, (long long)B * l.small.H * l.small.W);
+    fit(FEAT, zp, B);                           // heads
+    fit(zp, FEAT, B);                           // dense1
     return best;
 }
 
@@ -267,7 +287,6 @@ static VaePlan make_plan(void* ws, int64_t ws_bytes, int B, int ct, int z, int m
         p.frame_dsum = a.take<float>(b * 4);
     }
     p.bytes = a.off;
-    p.ok = ws == nullptr || !a.overflow;
     return p;
 }
 
@@ -385,18 +404,19 @@ static int32_t tg(const char* label, const TapGemmParams& p, cudaStream_t s, int
     return launch_tapgemm(p, s);
 }
 
-static int32_t run_wgrad(const char* label, const float* big, int Wb, int pitch, long long big_img, int k,
-                         const float* small, int B, int Ho, int Wo, int J, int c_pad, int c_real, float* partial,
-                         float* out, cudaStream_t s) {
-    ProfScope prof(label, s);
+// out[k][k][Cb][Cs] = the weight gradient of table layer l from its big-side and small-side operands
+static int32_t run_wgrad(const TcLayer& l, const float* big, const float* small, int B, float* partial, float* out,
+                         cudaStream_t s) {
+    ProfScope prof(l.wgrad, s);
     WgradParams w;
     memset(&w, 0, sizeof(w));
     w.big = big; w.small = small; w.partial = partial;
-    w.batch = B; w.Wb = Wb; w.big_pitch = pitch; w.big_img = big_img; w.Ho = Ho; w.Wo = Wo; w.sstride = 2;
-    w.ntaps = k; w.run = k * pitch;
-    for (int kh = 0; kh < k; ++kh) w.tap_off[kh] = (long long)kh * Wb * pitch;
-    w.I = k * k * pitch; w.J = J;
-    const long long M = (long long)B * Ho * Wo;
+    w.batch = B; w.Wb = l.big.W; w.big_pitch = l.big.C; w.big_img = (long long)l.big.H * l.big.W * l.big.C;
+    w.Ho = l.small.H; w.Wo = l.small.W; w.sstride = 2;
+    w.ntaps = l.k; w.run = l.k * l.big.C;
+    for (int kh = 0; kh < l.k; ++kh) w.tap_off[kh] = (long long)kh * l.big.W * l.big.C;
+    w.I = l.k * l.k * l.big.C; w.J = l.small.C;
+    const long long M = (long long)B * l.small.H * l.small.W;
     if (g_math_mode >= 1 && tc_wgrad_supported(w.I, w.J, w.run)) {
         w.passes = tc_passes();
         w.splits = tc_wgrad_pick_splits(w.I, w.J, M);
@@ -407,7 +427,7 @@ static int32_t run_wgrad(const char* label, const float* big, int Wb, int pitch,
         w.m_per_split = align_up((M + w.splits - 1) / w.splits, 16);
         CPB_TRY(launch_wgrad(w, s));
     }
-    return launch_reduce_partials(partial, w.splits, w.I, w.J, c_pad, c_real, w.J, out, s);
+    return launch_reduce_partials(partial, w.splits, w.I, w.J, w.I, w.I, w.J, out, s);
 }
 
 // out[k_real][j_real] = x[B, K]^T g[B, J], dropping the padded rows k >= k_real and columns j >= j_real
@@ -452,68 +472,133 @@ static void add_relayout(RelayoutTable& t, int64_t src, int64_t dst, int taps, i
     t.total += j.count;
 }
 
+// The latent block both VAEs share: the two heads (mean, logstd_sq) over a [B, K] layer, z_pad-column latent rows
+struct Latent {
+    int B, K, z, zp;
+    const int64_t* off;     // the VAE's parameter offsets
+    int mean;               // tensor index of mean/kernel; mean/bias, logstd_sqare/kernel and logstd_sqare/bias follow it
+};
+
+// Both heads as one y-batched dense problem over x [B, K]: heads[0] = mean, heads[1] = logstd_sq.  The weights are the
+// parameters (both kernels, and both biases, are adjacent) when z == z_pad, the zero-padded wp and bp otherwise.
+static TapGemmParams heads_fwd_problem(const Latent& h, const float* params, const float* x, const float* wp, const float* bp,
+                                       float* heads) {
+    const bool padded = h.zp != h.z;
+    TapGemmParams p = dense_problem(x, h.B, h.K, padded ? wp : params + h.off[h.mean], h.zp,
+                                    padded ? bp : params + h.off[h.mean + 1], nullptr, heads, 0);
+    p.ybatch = 2;
+    p.w_ystride = padded ? (long long)h.K * h.zp : h.off[h.mean + 2] - h.off[h.mean];
+    p.bias_ystride = padded ? h.zp : h.off[h.mean + 3] - h.off[h.mean + 1];
+    p.dst_ystride = (long long)h.B * h.zp;
+    return p;
+}
+
+// The heads' weight and bias gradients from gheads [2][B][z_pad], then their data gradient into gx = g(x pre-activation)
+// = gmean Wm^T + glogvar Wl^T with wt = both kernels transposed, [2][z_pad][K].  dgrad_label may be null: no profile scope.
+static int32_t heads_backward(const Latent& h, const char* wgrad_label, const char* dgrad_label, const float* x, const float* gheads,
+                              const float* wt, float* gx, float* partial, float* cs, float* grads, cudaStream_t s) {
+    const long long glogvar = (long long)h.B * h.zp;
+    CPB_TRY(run_dense_wgrad(wgrad_label, x, h.K, h.K, gheads, h.B, h.zp, h.z, partial, grads + h.off[h.mean], s));
+    CPB_TRY(run_dense_wgrad(wgrad_label, x, h.K, h.K, gheads + glogvar, h.B, h.zp, h.z, partial, grads + h.off[h.mean + 2], s));
+    CPB_TRY(launch_colsum(gheads, h.B, h.zp, h.z, grads + h.off[h.mean + 1], cs, s));
+    CPB_TRY(launch_colsum(gheads + glogvar, h.B, h.zp, h.z, grads + h.off[h.mean + 3], cs, s));
+    TapGemmParams p = dense_problem(gheads, h.B, h.zp, wt, h.K, nullptr, x, gx, 0);
+    p.cls[0].ntaps = 2;
+    p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
+    p.cls[0].taps[1].src_off = glogvar;
+    p.cls[0].taps[1].w_off = (long long)h.zp * h.K;
+    if (dgrad_label == nullptr) return launch_tapgemm(p, s);
+    ProfScope prof(dgrad_label, s);
+    return launch_tapgemm(p, s);
+}
+
+// z < z_pad: the zero-padded copies of the z-sized weights -- `heads`: both kernels [2][K][z_pad] at wp, both biases
+// [2][z_pad] at bp; `dec`: the first decoder layer's kernel [z][N] at parameter offset dec_off, as [z_pad][N] at dp
+static void add_z_padding(RelayoutTable& t, const Latent& h, bool heads, int64_t wp, int64_t bp, bool dec, int64_t dec_off,
+                          int N, int64_t dp) {
+    if (h.zp == h.z) return;
+    if (heads) {
+        add_relayout(t, h.off[h.mean], wp, 2, h.K, h.z, 1, h.K, h.zp);
+        add_relayout(t, h.off[h.mean + 1], bp, 1, 1, h.z, 1, 1, h.zp);
+        add_relayout(t, h.off[h.mean + 3], bp + h.zp, 1, 1, h.z, 1, 1, h.zp);
+    }
+    if (dec) add_relayout(t, dec_off, dp, 1, h.z, N, 1, h.zp, N);
+}
+
+// An rgb target that is the source itself (vae/train_vae.py:75) is read from the source's prepared, range-checked copy
+static bool target_is_source(const cpb_vae_config* c, const void* source, const void* target) {
+    return target == source && c->target_channels == 3 && c->target_dtype == c->source_dtype &&
+           (c->target_dtype == CPB_FRAME_F32 || c->target_u8_scale == 1.f / 255.f);
+}
+
+// [B, z_pad] latent rows of the workspace -> the caller's [B, z] rows of mean, logvar (heads) and z (zbuf), where given
+static int32_t copy_latents_out(const float* heads, const float* zbuf, int B, int z, int zp, float* mean, float* logvar,
+                                float* zout, cudaStream_t s) {
+    const float* src[3] = {heads, heads + (long long)B * zp, zbuf};
+    float* dst[3] = {mean, logvar, zout};
+    for (int i = 0; i < 3; ++i) {
+        if (dst[i] == nullptr) continue;
+        if (zp == z)
+            CPB_CUDA(cudaMemcpyAsync(dst[i], src[i], (size_t)B * z * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        else
+            CPB_TRY(launch_pitch_copy(src[i], zp, dst[i], z, B, s));
+    }
+    return CPB_OK;
+}
+
 static int32_t relayout_weights(const VaePlan& pl, const VaeLayout& L, const float* params, bool encoder, bool decoder,
                                 bool backward, cudaStream_t s) {
     using namespace geo;
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    auto add = [&](int64_t src, int64_t dst, int taps, int rows, int cols, int mode, int rows_pad, int cols_pad) {
-        add_relayout(t, src, dst, taps, rows, cols, mode, rows_pad, cols_pad);
-    };
-    if (decoder) {
-        add(L.off[T_DECONV1_K], pl.rl.deconv1T, 16, C3, C4, 0, C3, C4);
-        add(L.off[T_DECONV2_K], pl.rl.deconv2T, 16, C2, C3, 0, C2, C3);
-        add(L.off[T_DECONV3_K], pl.rl.deconv3T, 25, C1, C2, 0, C1, C2);
-    }
-    if (backward) {
-        add(L.off[T_CONV2_K], pl.rl.conv2T, 16, C1, C2, 0, C1, C2);
-        add(L.off[T_CONV3_K], pl.rl.conv3T, 16, C2, C3, 0, C2, C3);
-        add(L.off[T_CONV4_K], pl.rl.conv4T, 16, C3, C4, 0, C3, C4);
-    }
-    if (backward) {
-        add(L.off[T_DENSE1_K], pl.rl.dense1T, 1, pl.z, FEAT, 0, pl.zp, FEAT);      // [6144][z_pad]
-        add(L.off[T_MEAN_K], pl.rl.headsT, 2, FEAT, pl.z, 0, FEAT, pl.zp);        // [2][z_pad][6144]: mean and logvar kernels are adjacent
-    }
-    if (pl.zp != pl.z) {
-        if (encoder) {
-            add(L.off[T_MEAN_K], pl.rl.headsP, 2, FEAT, pl.z, 1, FEAT, pl.zp);
-            add(L.off[T_MEAN_B], pl.rl.headsBP, 1, 1, pl.z, 1, 1, pl.zp);
-            add(L.off[T_LOGVAR_B], pl.rl.headsBP + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
-        }
-        if (decoder) add(L.off[T_DENSE1_K], pl.rl.dense1P, 1, pl.z, FEAT, 1, pl.zp, FEAT);
-    }
-    ProfScope prof("relayout_weights", s);
-    CPB_TRY(launch_relayout(params, pl.relayout, t, s));
-    if (g_math_mode == 0) return CPB_OK;
     TcWeightTable w;
     memset(&w, 0, sizeof(w));
     const int round_nearest = tc_passes() == 1 ? 1 : 0;
-    auto addw = [&](int tensor, int slot, int k, int cb, int cs, bool gather, bool scatter) {
-        const long long n = (long long)k * k * cb * cs;
-        if (gather) {
-            TcWeightJob& j = w.jobs[w.njobs++];
-            j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].f_hi; j.dst_lo = pl.rl.tc[slot].f_lo;
-            j.round_nearest = round_nearest;
-            j.mode = 1; j.k = k; j.cb = cb; j.cs = cs; j.N = cs; j.C = k * cb; j.count = n; w.total += n;
-        }
-        if (scatter) {
-            TcWeightJob& j = w.jobs[w.njobs++];
-            j.src_off = L.off[tensor]; j.dst_hi = pl.rl.tc[slot].t_hi; j.dst_lo = pl.rl.tc[slot].t_lo;
-            j.round_nearest = round_nearest;
-            const int win = (k + 1) / 2;
-            j.mode = 2; j.k = k; j.cb = cb; j.cs = cs; j.N = 4 * cb; j.C = cs; j.count = (long long)win * win * 4 * cb * cs; w.total += j.count;
-        }
+    auto addw = [&](const TcLayer& l, bool scatter) {
+        const TcW& at = pl.rl.tc[l.slot];
+        const int win = (l.k + 1) / 2;
+        TcWeightJob& j = w.jobs[w.njobs++];
+        j.src_off = L.off[l.kernel]; j.round_nearest = round_nearest;
+        j.mode = scatter ? 2 : 1; j.k = l.k; j.cb = l.big.C; j.cs = l.small.C;
+        j.dst_hi = scatter ? at.t_hi : at.f_hi; j.dst_lo = scatter ? at.t_lo : at.f_lo;
+        j.N = scatter ? 4 * l.big.C : l.small.C; j.C = scatter ? l.small.C : l.k * l.big.C;
+        j.count = (long long)j.N * j.C * (scatter ? win * win : l.k); w.total += j.count;
     };
-    // conv layers run gather-form forward / scatter-form dgrad; deconv layers the other way round
-    addw(T_CONV2_K, TC_CONV2, 4, C1, C2, true, backward);
-    addw(T_CONV3_K, TC_CONV3, 4, C2, C3, true, backward);
-    addw(T_CONV4_K, TC_CONV4, 4, C3, C4, true, backward);
-    if (decoder) {
-        addw(T_DECONV1_K, TC_DECONV1, 4, C3, C4, backward, true);
-        addw(T_DECONV2_K, TC_DECONV2, 4, C2, C3, backward, true);
-        addw(T_DECONV3_K, TC_DECONV3, 5, C1, C2, backward, true);
+    // the forms of each layer that the call's passes run: the scatter form's SIMT transpose, and each form's TF32 image
+    for (const TcLayer& l : kTcLayers) {
+        const bool fwd = l.deconv ? decoder : encoder;
+        const bool scatter = (fwd && uses_scatter(l, false)) || (backward && uses_scatter(l, true));
+        const bool gather = (fwd && !uses_scatter(l, false)) || (backward && !uses_scatter(l, true));
+        if (scatter) add_relayout(t, L.off[l.kernel], pl.rl.T[l.slot], l.k * l.k, l.big.C, l.small.C, 0, l.big.C, l.small.C);
+        if (gather) addw(l, false);
+        if (scatter) addw(l, true);
     }
+    if (backward) {
+        add_relayout(t, L.off[T_DENSE1_K], pl.rl.dense1T, 1, pl.z, FEAT, 0, pl.zp, FEAT);      // [6144][z_pad]
+        add_relayout(t, L.off[T_MEAN_K], pl.rl.headsT, 2, FEAT, pl.z, 0, FEAT, pl.zp);        // [2][z_pad][6144]: mean and logvar kernels are adjacent
+    }
+    add_z_padding(t, Latent{pl.B, FEAT, pl.z, pl.zp, L.off, T_MEAN_K}, encoder, pl.rl.headsP, pl.rl.headsBP, decoder,
+                  L.off[T_DENSE1_K], FEAT, pl.rl.dense1P);
+    ProfScope prof("relayout_weights", s);
+    CPB_TRY(launch_relayout(params, pl.relayout, t, s));
+    if (g_math_mode == 0) return CPB_OK;
     return launch_tc_weights(params, pl.relayout, w, s);
+}
+
+// A table layer's forward pass (bias, ReLU) or data gradient (ReLU mask `mask`, if any) in the form uses_scatter gives:
+// src is the big side and dst the small side in the gather form, the other way round in the scatter form
+static int32_t run_layer_pass(const VaePlan& pl, const VaeLayout& L, const float* params, const TcLayer& l, bool dgrad,
+                              const float* src, const float* mask, float* dst, cudaStream_t s) {
+    const char* label = dgrad ? l.dgrad : l.fwd;
+    const float* bias = dgrad ? nullptr : params + L.off[l.bias];
+    const int relu = dgrad ? 0 : 1;
+    const float* rl = pl.relayout;
+    const TcW& w = pl.rl.tc[l.slot];
+    if (uses_scatter(l, dgrad))
+        return tg(label, scatter_problem(src, pl.B, l.small.H, l.small.W, l.small.C, l.k, rl + pl.rl.T[l.slot], l.big.C, bias,
+                                         mask, dst, l.big.H, l.big.W, relu, rl + w.t_hi, rl + w.t_lo), s, l.k);
+    return tg(label, gather_problem(src, pl.B, l.big.H, l.big.W, l.big.C, l.k, params + L.off[l.kernel], l.small.C, bias, mask,
+                                    dst, relu, rl + w.f_hi, rl + w.f_lo), s, 0);
 }
 
 static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_config* cfg, const float* params,
@@ -525,25 +610,10 @@ static int32_t run_encoder(const VaePlan& pl, const VaeLayout& L, const cpb_vae_
       CPB_TRY(launch_prep_frames(source, cfg->source_dtype, sscale, 3, (long long)B * NPIX, pl.xp, flags, 1, s)); }
     { ProfScope prof("conv1.fwd", s);
       CPB_TRY(launch_edge_gather(pl.xp, 3, params + L.off[T_CONV1_K], params + L.off[T_CONV1_B], nullptr, pl.a1, B, s)); }
-    TapGemmParams p;
-    p = gather_problem(pl.a1, B, H1, W1, C1, 4, params + L.off[T_CONV2_K], C2, params + L.off[T_CONV2_B], nullptr, pl.a2, 1,
-                       pl.relayout + pl.rl.tc[TC_CONV2].f_hi, pl.relayout + pl.rl.tc[TC_CONV2].f_lo);
-    CPB_TRY(tg("conv2.fwd", p, s, 0));
-    p = gather_problem(pl.a2, B, H2, W2, C2, 4, params + L.off[T_CONV3_K], C3, params + L.off[T_CONV3_B], nullptr, pl.a3, 1,
-                       pl.relayout + pl.rl.tc[TC_CONV3].f_hi, pl.relayout + pl.rl.tc[TC_CONV3].f_lo);
-    CPB_TRY(tg("conv3.fwd", p, s, 0));
-    p = gather_problem(pl.a3, B, H3, W3, C3, 4, params + L.off[T_CONV4_K], C4, params + L.off[T_CONV4_B], nullptr, pl.a4, 1,
-                       pl.relayout + pl.rl.tc[TC_CONV4].f_hi, pl.relayout + pl.rl.tc[TC_CONV4].f_lo);
-    CPB_TRY(tg("conv4.fwd", p, s, 0));
-    // both heads as one y-batched dense problem: heads[0] = mean, heads[1] = logstd_sq; z_pad columns (the weights
-    // are the parameters themselves when z == z_pad, their zero-padded copies otherwise)
-    const bool padded = pl.zp != pl.z;
-    p = dense_problem(pl.a4, B, FEAT, padded ? pl.relayout + pl.rl.headsP : params + L.off[T_MEAN_K], pl.zp,
-                      padded ? pl.relayout + pl.rl.headsBP : params + L.off[T_MEAN_B], nullptr, pl.heads, 0);
-    p.ybatch = 2;
-    p.w_ystride = padded ? (long long)FEAT * pl.zp : L.off[T_LOGVAR_K] - L.off[T_MEAN_K];
-    p.bias_ystride = padded ? pl.zp : L.off[T_LOGVAR_B] - L.off[T_MEAN_B];
-    p.dst_ystride = (long long)B * pl.zp;
+    for (int i = TC_CONV2; i <= TC_CONV4; ++i)
+        CPB_TRY(run_layer_pass(pl, L, params, kTcLayers[i], false, pl.*kTcLayers[i].in, nullptr, pl.*kTcLayers[i].out, s));
+    TapGemmParams p = heads_fwd_problem(Latent{B, FEAT, pl.z, pl.zp, L.off, T_MEAN_K}, params, pl.a4, pl.relayout + pl.rl.headsP,
+                                        pl.relayout + pl.rl.headsBP, pl.heads);
     p.ksplit = tapgemm_pick_ksplit(B, pl.zp, 2, FEAT);
     p.kpartial = pl.ksplit; p.kpartial_stride = 2LL * B * pl.zp;
     return tg("heads.fwd", p, s);
@@ -557,15 +627,8 @@ static int32_t run_decoder(const VaePlan& pl, const VaeLayout& L, const float* p
     const float* w1 = pl.zp != pl.z ? pl.relayout + pl.rl.dense1P : params + L.off[T_DENSE1_K];
     TapGemmParams p = dense_problem(zsrc, B, pl.zp, w1, FEAT, params + L.off[T_DENSE1_B], nullptr, pl.d1, 0);
     CPB_TRY(tg("dense1.fwd", p, s));
-    p = scatter_problem(pl.d1, B, H4, W4, C4, 4, pl.relayout + pl.rl.deconv1T, C3, params + L.off[T_DECONV1_B],
-                        nullptr, pl.b1, H3, W3, 1, pl.relayout + pl.rl.tc[TC_DECONV1].t_hi, pl.relayout + pl.rl.tc[TC_DECONV1].t_lo);
-    CPB_TRY(tg("deconv1.fwd", p, s, 4));
-    p = scatter_problem(pl.b1, B, H3, W3, C3, 4, pl.relayout + pl.rl.deconv2T, C2, params + L.off[T_DECONV2_B],
-                        nullptr, pl.b2, H2, W2, 1, pl.relayout + pl.rl.tc[TC_DECONV2].t_hi, pl.relayout + pl.rl.tc[TC_DECONV2].t_lo);
-    CPB_TRY(tg("deconv2.fwd", p, s, 4));
-    p = scatter_problem(pl.b2, B, H2, W2, C2, 5, pl.relayout + pl.rl.deconv3T, C1, params + L.off[T_DECONV3_B],
-                        nullptr, pl.b3, H1, W1, 1, pl.relayout + pl.rl.tc[TC_DECONV3].t_hi, pl.relayout + pl.rl.tc[TC_DECONV3].t_lo);
-    CPB_TRY(tg("deconv3.fwd", p, s, 5));
+    for (int i = TC_DECONV1; i <= TC_DECONV3; ++i)
+        CPB_TRY(run_layer_pass(pl, L, params, kTcLayers[i], false, pl.*kTcLayers[i].in, nullptr, pl.*kTcLayers[i].out, s));
     ProfScope prof("deconv4.fwd", s);
     return launch_deconv4_fwd(pl.b3, params + L.off[T_DECONV4_K], params + L.off[T_DECONV4_B], B, pl.ct, logits_p,
                               sigm, s);
@@ -579,11 +642,8 @@ static int32_t run_forward_loss(const VaePlan& pl, const VaeLayout& L, const cpb
     CPB_TRY(run_encoder(pl, L, cfg, params, source, flags, s));
     CPB_TRY(launch_reparam(pl.heads, eps, B, pl.z, pl.zp, cfg->kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
     CPB_TRY(run_decoder(pl, L, params, pl.zbuf, pl.logits_p, sigm, s));
-    const float* yp = pl.yp;
-    if (target == source && cfg->target_channels == 3 && cfg->target_dtype == cfg->source_dtype &&
-        (cfg->target_dtype == CPB_FRAME_F32 || cfg->target_u8_scale == 1.f / 255.f)) {
-        yp = pl.xp;   // rgb target == source (vae/train_vae.py:75): already prepared and range-checked
-    } else {
+    const float* yp = target_is_source(cfg, source, target) ? pl.xp : pl.yp;
+    if (yp == pl.yp) {
         const float tscale = cfg->target_dtype == CPB_FRAME_U8 ? cfg->target_u8_scale : 1.f;
         CPB_TRY(launch_prep_frames(target, cfg->target_dtype, tscale, cfg->target_channels, (long long)B * NPIX,
                                    pl.yp, flags, 2, s));
@@ -599,15 +659,27 @@ static int32_t run_forward_loss(const VaePlan& pl, const VaeLayout& L, const cpb
 // group is the layer's weight gradient, bias gradient and data gradient; the stop comes after all three.
 static const char* kBackwardStops[] = {"deconv4.dgrad", "deconv3.dgrad", "deconv2.dgrad", "deconv1.dgrad", "dense1.dgrad",
                                        "heads.dgrad", "conv4.dgrad", "conv3.dgrad"};
-enum { STOP_DECONV4, STOP_DECONV3, STOP_DECONV2, STOP_DECONV1, STOP_DENSE1, STOP_HEADS, STOP_CONV4, STOP_CONV3 };
-static int g_backward_stop = -1;    // index into kBackwardStops, -1: run the whole pass
-#define CPB_BACKWARD_STOP(group) if (g_backward_stop == (group)) return CPB_OK
+static const char* g_backward_stop = nullptr;    // the kBackwardStops entry run_backward stops after; null: none
+#define CPB_BACKWARD_STOP(group) if (g_backward_stop != nullptr && strcmp(g_backward_stop, group) == 0) return CPB_OK
+
+// A table layer's group of the backward pass: its weight gradient, bias gradient and data gradient.  g is the gradient at
+// the layer's output (pre-activation); gin receives the one at its input, masked by the input's ReLU.
+static int32_t run_layer_backward(const VaePlan& pl, const VaeLayout& L, const float* params, const TcLayer& l, const float* g,
+                                  float* gin, float* grads, cudaStream_t s) {
+    const float* in = pl.*l.in;
+    const Side& out = l.deconv ? l.big : l.small;
+    CPB_TRY(run_wgrad(l, l.deconv ? g : in, l.deconv ? in : g, pl.B, pl.partial, grads + L.off[l.kernel], s));
+    if (l.edge)
+        CPB_TRY(launch_colsum(pl.cs_edge, edge_gather_blocks(pl.B), out.C, out.C, grads + L.off[l.bias], pl.colsum, s));
+    else
+        CPB_TRY(launch_colsum(g, (long long)pl.B * out.H * out.W, out.C, out.C, grads + L.off[l.bias], pl.colsum, s));
+    return run_layer_pass(pl, L, params, l, true, g, l.linear ? nullptr : in, gin, s);
+}
 
 static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae_config* cfg, const float* params,
                             const float* eps, float* grads, cudaStream_t s) {
     using namespace geo;
-    const int B = pl.B;
-    const int z = pl.z, zp = pl.zp;
+    const int B = pl.B, z = pl.z, zp = pl.zp;
     float* dlog = pl.logits_p;   // overwritten in place by the loss kernel
     float* cs = pl.colsum;
     CPB_TRY(launch_fill_zero(grads, L.total, s));
@@ -621,79 +693,37 @@ static int32_t run_backward(const VaePlan& pl, const VaeLayout& L, const cpb_vae
     CPB_TRY(launch_colsum(pl.frame_dsum, B, 4, pl.ct, grads + L.off[T_DECONV4_B], cs, s));
     { ProfScope prof("deconv4.dgrad", s);
       CPB_TRY(launch_edge_gather(dlog, pl.ct, params + L.off[T_DECONV4_K], nullptr, pl.b3, pl.gA, B, s, pl.cs_edge)); }   // gA = g(b3 pre-activation)
-    CPB_BACKWARD_STOP(STOP_DECONV4);
-    TapGemmParams p;
-    // ---- deconv3
-    CPB_TRY(run_wgrad("deconv3.wgrad", pl.gA, W1, C1, (long long)H1 * W1 * C1, 5, pl.b2, B, H2, W2, C2, 5 * 5 * C1, 5 * 5 * C1,
-                      pl.partial, grads + L.off[T_DECONV3_K], s));
-    CPB_TRY(launch_colsum(pl.cs_edge, edge_gather_blocks(B), C1, C1, grads + L.off[T_DECONV3_B], cs, s));
-    p = gather_problem(pl.gA, B, H1, W1, C1, 5, params + L.off[T_DECONV3_K], C2, nullptr, pl.b2, pl.gB, 0,
-                       pl.relayout + pl.rl.tc[TC_DECONV3].f_hi, pl.relayout + pl.rl.tc[TC_DECONV3].f_lo);
-    CPB_TRY(tg("deconv3.dgrad", p, s, 0));   // gB = g(b2)
-    CPB_BACKWARD_STOP(STOP_DECONV3);
-    // ---- deconv2
-    CPB_TRY(run_wgrad("deconv2.wgrad", pl.gB, W2, C2, (long long)H2 * W2 * C2, 4, pl.b1, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
-                      grads + L.off[T_DECONV2_K], s));
-    CPB_TRY(launch_colsum(pl.gB, (long long)B * H2 * W2, C2, C2, grads + L.off[T_DECONV2_B], cs, s));
-    p = gather_problem(pl.gB, B, H2, W2, C2, 4, params + L.off[T_DECONV2_K], C3, nullptr, pl.b1, pl.gA, 0,
-                       pl.relayout + pl.rl.tc[TC_DECONV2].f_hi, pl.relayout + pl.rl.tc[TC_DECONV2].f_lo);
-    CPB_TRY(tg("deconv2.dgrad", p, s, 0));   // gA = g(b1)
-    CPB_BACKWARD_STOP(STOP_DECONV2);
-    // ---- deconv1
-    CPB_TRY(run_wgrad("deconv1.wgrad", pl.gA, W3, C3, (long long)H3 * W3 * C3, 4, pl.d1, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
-                      grads + L.off[T_DECONV1_K], s));
-    CPB_TRY(launch_colsum(pl.gA, (long long)B * H3 * W3, C3, C3, grads + L.off[T_DECONV1_B], cs, s));
-    p = gather_problem(pl.gA, B, H3, W3, C3, 4, params + L.off[T_DECONV1_K], C4, nullptr, nullptr, pl.gB, 0,
-                       pl.relayout + pl.rl.tc[TC_DECONV1].f_hi, pl.relayout + pl.rl.tc[TC_DECONV1].f_lo);
-    CPB_TRY(tg("deconv1.dgrad", p, s, 0));                                   // gB = g(d1) [B, 6144]
-    CPB_BACKWARD_STOP(STOP_DECONV1);
+    CPB_BACKWARD_STOP("deconv4.dgrad");
+    // ---- deconv3, deconv2, deconv1: gA -> gB -> gA -> gB = g(d1) [B, 6144]
+    float *g = pl.gA, *gin = pl.gB;
+    for (int i = TC_DECONV3; i >= TC_DECONV1; --i) {
+        CPB_TRY(run_layer_backward(pl, L, params, kTcLayers[i], g, gin, grads, s));
+        CPB_BACKWARD_STOP(kTcLayers[i].dgrad);
+        std::swap(g, gin);
+    }
     // ---- dense1
     CPB_TRY(run_dense_wgrad("dense1.wgrad", pl.zbuf, zp, z, pl.gB, B, FEAT, FEAT, pl.partial, grads + L.off[T_DENSE1_K], s));
     CPB_TRY(launch_colsum(pl.gB, B, FEAT, FEAT, grads + L.off[T_DENSE1_B], cs, s));
-    p = dense_problem(pl.gB, B, FEAT, pl.relayout + pl.rl.dense1T, zp, nullptr, nullptr, pl.gz, 0);
+    TapGemmParams p = dense_problem(pl.gB, B, FEAT, pl.relayout + pl.rl.dense1T, zp, nullptr, nullptr, pl.gz, 0);
     p.ksplit = tapgemm_pick_ksplit(B, zp, 1, FEAT);
     p.kpartial = pl.ksplit; p.kpartial_stride = (long long)B * zp;
     CPB_TRY(tg("dense1.dgrad", p, s));
-    CPB_BACKWARD_STOP(STOP_DENSE1);
+    CPB_BACKWARD_STOP("dense1.dgrad");
     // ---- sampling + KL
     CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, cfg->beta * cfg->loss_scale / (float)B,
                                pl.gheads, s));
-    // ---- heads
-    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, FEAT, pl.gheads, B, zp, z, pl.partial, grads + L.off[T_MEAN_K], s));
-    CPB_TRY(run_dense_wgrad("heads.wgrad", pl.a4, FEAT, FEAT, pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
-                            grads + L.off[T_LOGVAR_K], s));
-    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[T_MEAN_B], cs, s));
-    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[T_LOGVAR_B], cs, s));
-    p = dense_problem(pl.gheads, B, zp, pl.relayout + pl.rl.headsT, FEAT, nullptr, pl.a4, pl.gA, 0);
-    p.cls[0].ntaps = 2;                                              // g(a4) = gmean Wm^T + glogvar Wl^T
-    p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
-    p.cls[0].taps[1].src_off = (long long)B * zp;
-    p.cls[0].taps[1].w_off = (long long)zp * FEAT;
-    CPB_TRY(tg("heads.dgrad", p, s));                                   // gA = g(a4 pre-activation)
-    CPB_BACKWARD_STOP(STOP_HEADS);
-    // ---- conv4
-    CPB_TRY(run_wgrad("conv4.wgrad", pl.a3, W3, C3, (long long)H3 * W3 * C3, 4, pl.gA, B, H4, W4, C4, 16 * C3, 16 * C3, pl.partial,
-                      grads + L.off[T_CONV4_K], s));
-    CPB_TRY(launch_colsum(pl.gA, (long long)B * H4 * W4, C4, C4, grads + L.off[T_CONV4_B], cs, s));
-    p = scatter_problem(pl.gA, B, H4, W4, C4, 4, pl.relayout + pl.rl.conv4T, C3, nullptr, pl.a3, pl.gB, H3, W3, 0,
-                        pl.relayout + pl.rl.tc[TC_CONV4].t_hi, pl.relayout + pl.rl.tc[TC_CONV4].t_lo);
-    CPB_TRY(tg("conv4.dgrad", p, s, 4));   // gB = g(a3)
-    CPB_BACKWARD_STOP(STOP_CONV4);
-    // ---- conv3
-    CPB_TRY(run_wgrad("conv3.wgrad", pl.a2, W2, C2, (long long)H2 * W2 * C2, 4, pl.gB, B, H3, W3, C3, 16 * C2, 16 * C2, pl.partial,
-                      grads + L.off[T_CONV3_K], s));
-    CPB_TRY(launch_colsum(pl.gB, (long long)B * H3 * W3, C3, C3, grads + L.off[T_CONV3_B], cs, s));
-    p = scatter_problem(pl.gB, B, H3, W3, C3, 4, pl.relayout + pl.rl.conv3T, C2, nullptr, pl.a2, pl.gA, H2, W2, 0,
-                        pl.relayout + pl.rl.tc[TC_CONV3].t_hi, pl.relayout + pl.rl.tc[TC_CONV3].t_lo);
-    CPB_TRY(tg("conv3.dgrad", p, s, 4));   // gA = g(a2)
-    CPB_BACKWARD_STOP(STOP_CONV3);
-    // ---- conv2
-    CPB_TRY(run_wgrad("conv2.wgrad", pl.a1, W1, C1, (long long)H1 * W1 * C1, 4, pl.gA, B, H2, W2, C2, 16 * C1, 16 * C1, pl.partial,
-                      grads + L.off[T_CONV2_K], s));
-    CPB_TRY(launch_colsum(pl.gA, (long long)B * H2 * W2, C2, C2, grads + L.off[T_CONV2_B], cs, s));
-    p = scatter_problem(pl.gA, B, H2, W2, C2, 4, pl.relayout + pl.rl.conv2T, C1, nullptr, pl.a1, pl.gB, H1, W1, 0,
-                        pl.relayout + pl.rl.tc[TC_CONV2].t_hi, pl.relayout + pl.rl.tc[TC_CONV2].t_lo);
-    CPB_TRY(tg("conv2.dgrad", p, s, 4));   // gB = g(a1)
+    // ---- heads: gA = g(a4 pre-activation)
+    CPB_TRY(heads_backward(Latent{B, FEAT, z, zp, L.off, T_MEAN_K}, "heads.wgrad", "heads.dgrad", pl.a4, pl.gheads,
+                           pl.relayout + pl.rl.headsT, pl.gA, pl.partial, cs, grads, s));
+    CPB_BACKWARD_STOP("heads.dgrad");
+    // ---- conv4 (from the heads' data gradient in gA), conv3, conv2: gA -> gB -> gA -> gB = g(a1)
+    g = pl.gA;
+    gin = pl.gB;
+    for (int i = TC_CONV4; i >= TC_CONV2; --i) {
+        CPB_TRY(run_layer_backward(pl, L, params, kTcLayers[i], g, gin, grads, s));
+        CPB_BACKWARD_STOP(kTcLayers[i].dgrad);
+        std::swap(g, gin);
+    }
     // ---- conv1 (its input gradient is never used: the reference computes and discards it)
     { ProfScope prof("conv1.wgrad", s);
       CPB_TRY(launch_edge_wgrad(pl.xp, 3, pl.gB, B, pl.partial, s));
@@ -807,7 +837,6 @@ struct MlpPlan {
     float *wTc, *tcScratch;
     int64_t iE1, iD3f, iD3t;
     int64_t bytes;
-    bool ok;
     int top() const { return enc[nenc - 1]; }
     int last() const { return dec[ndec - 1]; }
 };
@@ -895,25 +924,18 @@ static MlpPlan make_mlp_plan(void* ws, int64_t ws_bytes, const cpb_mlpvae_spec* 
         p.tcScratch = a.take<float>(mlp_tc_scratch_floats(p, mode));
     }
     p.bytes = a.off;
-    p.ok = ws == nullptr || !a.overflow;
     return p;
 }
 
-// z < z_pad: the zero-padded copies of the z-sized weights that the forward pass reads (one launch)
-static int32_t mlp_pad_weights(const MlpPlan& pl, const MlpLayout& L, const float* params, cudaStream_t s) {
-    if (pl.zp == pl.z) return CPB_OK;
+// The weights a call reads besides the parameters: z < z_pad, the zero-padded copies of the z-sized weights (one launch);
+// math mode 2, the TF32 weight images (rounded to nearest) of the frame-wide products the call runs (one launch)
+static int32_t mlp_relayout_weights(const MlpPlan& pl, const MlpLayout& L, const float* params, bool encoder, bool decoder,
+                                    bool backward, cudaStream_t s) {
     RelayoutTable t;
     memset(&t, 0, sizeof(t));
-    add_relayout(t, L.off[L.mean()], pl.pHeads, 2, pl.top(), pl.z, 1, pl.top(), pl.zp);
-    add_relayout(t, L.off[L.mean() + 1], pl.pHeadsB, 1, 1, pl.z, 1, 1, pl.zp);
-    add_relayout(t, L.off[L.logvar() + 1], pl.pHeadsB + pl.zp, 1, 1, pl.z, 1, 1, pl.zp);
-    add_relayout(t, L.off[L.dec(0)], pl.pD1, 1, pl.z, pl.dec[0], 1, pl.zp, pl.dec[0]);
-    return launch_relayout(params, pl.wP, t, s);
-}
-
-// math mode 2: the TF32 weight images (rounded to nearest) of the frame-wide products the call runs (one launch)
-static int32_t mlp_tc_weights(const MlpPlan& pl, const MlpLayout& L, const float* params, bool encoder, bool decoder,
-                              bool backward, cudaStream_t s) {
+    add_z_padding(t, Latent{pl.B, pl.top(), pl.z, pl.zp, L.off, L.mean()}, true, pl.pHeads, pl.pHeadsB, true, L.off[L.dec(0)],
+                  pl.dec[0], pl.pD1);
+    CPB_TRY(launch_relayout(params, pl.wP, t, s));
     if (!pl.tc) return CPB_OK;
     TcWeightTable w;
     memset(&w, 0, sizeof(w));
@@ -970,14 +992,8 @@ static int32_t mlp_encoder(const MlpPlan& pl, const MlpLayout& L, const cpb_mlpv
                           nullptr, pl.h[i], 1);
         CPB_TRY(launch_tapgemm(p, s));
     }
-    const bool padded = pl.zp != pl.z;
-    p = dense_problem(pl.h[pl.nenc - 1], pl.B, pl.top(), padded ? pl.wP + pl.pHeads : params + L.off[L.mean()], pl.zp,
-                      padded ? pl.wP + pl.pHeadsB : params + L.off[L.mean() + 1], nullptr, pl.heads, 0);
-    p.ybatch = 2;
-    p.w_ystride = padded ? (long long)pl.top() * pl.zp : L.off[L.logvar()] - L.off[L.mean()];
-    p.bias_ystride = padded ? pl.zp : L.off[L.logvar() + 1] - L.off[L.mean() + 1];
-    p.dst_ystride = (long long)pl.B * pl.zp;
-    return launch_tapgemm(p, s);
+    return launch_tapgemm(heads_fwd_problem(Latent{pl.B, pl.top(), pl.z, pl.zp, L.off, L.mean()}, params, pl.h[pl.nenc - 1],
+                                            pl.wP + pl.pHeads, pl.wP + pl.pHeadsB, pl.heads), s);
 }
 
 static int32_t mlp_decoder(const MlpPlan& pl, const MlpLayout& L, const float* params, const float* zsrc, float* logits, cudaStream_t s) {
@@ -1000,11 +1016,8 @@ static int32_t mlp_forward_loss(const MlpPlan& pl, const MlpLayout& L, const cpb
     CPB_TRY(mlp_encoder(pl, L, c, params, source, flags, s));
     CPB_TRY(launch_reparam(pl.heads, eps, pl.B, pl.z, pl.zp, c->base.kl_tolerance, pl.zbuf, pl.kl_rows, pl.kl_active, s));
     CPB_TRY(mlp_decoder(pl, L, params, pl.zbuf, pl.logits, s));
-    const float* y = pl.y;
-    if (target == source && c->base.target_channels == 3 && c->base.target_dtype == c->base.source_dtype &&
-        (c->base.target_dtype == CPB_FRAME_F32 || c->base.target_u8_scale == 1.f / 255.f)) {
-        y = pl.x;
-    } else {
+    const float* y = target_is_source(&c->base, source, target) ? pl.x : pl.y;
+    if (y == pl.y) {
         const float tscale = c->base.target_dtype == CPB_FRAME_U8 ? c->base.target_u8_scale : 1.f;
         CPB_TRY(launch_prep_flat(target, c->base.target_dtype, tscale, (long long)pl.B * pl.OUT, pl.y, flags, 2, s));
     }
@@ -1062,20 +1075,11 @@ static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlp
     // ---- sampling + KL, heads
     const float* htop = pl.h[ne - 1];
     CPB_TRY(launch_reparam_bwd(pl.heads, eps, pl.gz, pl.kl_active, B, z, zp, c->base.beta * c->base.loss_scale / (float)B, pl.gheads, s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", htop, pl.top(), pl.top(), pl.gheads, B, zp, z, pl.partial, grads + L.off[L.mean()], s));
-    CPB_TRY(run_dense_wgrad("mlp.wgrad", htop, pl.top(), pl.top(), pl.gheads + (long long)B * zp, B, zp, z, pl.partial,
-                            grads + L.off[L.logvar()], s));
-    CPB_TRY(launch_colsum(pl.gheads, B, zp, z, grads + L.off[L.mean() + 1], cs, s));
-    CPB_TRY(launch_colsum(pl.gheads + (long long)B * zp, B, zp, z, grads + L.off[L.logvar() + 1], cs, s));
     // the encoder's gradient alternates between ga and gb so that the first layer's lands in gb at every depth
     cur = ne % 2 == 0 ? pl.ga : pl.gb;
     other = ne % 2 == 0 ? pl.gb : pl.ga;
-    p = dense_problem(pl.gheads, B, zp, pl.wT + pl.tHeads, pl.top(), nullptr, htop, cur, 0);
-    p.cls[0].ntaps = 2;
-    p.cls[0].taps[1].dy = p.cls[0].taps[1].dx = 0;
-    p.cls[0].taps[1].src_off = (long long)B * zp;
-    p.cls[0].taps[1].w_off = (long long)zp * pl.top();
-    CPB_TRY(launch_tapgemm(p, s));                                                                      // cur = g(h_top pre-activation)
+    CPB_TRY(heads_backward(Latent{B, pl.top(), z, zp, L.off, L.mean()}, "mlp.wgrad", nullptr, htop, pl.gheads, pl.wT + pl.tHeads,
+                           cur, pl.partial, cs, grads, s));                                           // cur = g(h_top pre-activation)
     // ---- encoder, top down
     for (int i = ne - 1; i >= 1; --i) {
         CPB_TRY(run_dense_wgrad("mlp.wgrad", pl.h[i - 1], pl.enc[i - 1], pl.enc[i - 1], cur, B, pl.enc[i], pl.enc[i], pl.partial,
@@ -1092,13 +1096,13 @@ static int32_t mlp_backward(const MlpPlan& pl, const MlpLayout& L, const cpb_mlp
     return launch_colsum(cur, B, pl.enc[0], pl.enc[0], grads + L.off[L.enc(0) + 1], cs, s);
 }
 
-// [B, z_pad] latent rows of the workspace -> the caller's [B, z] rows
-static int32_t copy_latent_out(const float* src, float* dst, int B, int z, int zp, cudaStream_t s) {
-    if (zp == z) {
-        CPB_CUDA(cudaMemcpyAsync(dst, src, (size_t)B * z * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        return CPB_OK;
-    }
-    return launch_pitch_copy(src, zp, dst, z, B, s);
+// every VAE entry point, once its configuration is valid: the device is set up, the workspace given and `need` bytes large
+static int32_t check_workspace(const void* workspace, int64_t workspace_bytes, int64_t need) {
+    CPB_TRY(ensure_init());
+    CPB_REQUIRE(workspace != nullptr, "workspace is NULL");
+    if (need <= workspace_bytes) return CPB_OK;
+    set_error("workspace too small: need %lld bytes, got %lld", (long long)need, (long long)workspace_bytes);
+    return CPB_ERR_WORKSPACE_TOO_SMALL;
 }
 
 }  // namespace cpb
@@ -1131,12 +1135,12 @@ int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t ct, int32_t z, int32
 /* debug: make every later ConvVAE backward pass return right after the named layer group (NULL: run the whole pass) */
 int32_t cpb_debug_vae_backward_stop(const char* group) {
     if (group == nullptr) {
-        g_backward_stop = -1;
+        g_backward_stop = nullptr;
         return CPB_OK;
     }
-    for (int i = 0; i < (int)(sizeof(kBackwardStops) / sizeof(kBackwardStops[0])); ++i)
-        if (strcmp(group, kBackwardStops[i]) == 0) {
-            g_backward_stop = i;
+    for (const char* stop : kBackwardStops)
+        if (strcmp(group, stop) == 0) {
+            g_backward_stop = stop;
             return CPB_OK;
         }
     cpb::set_error("cpb_debug_vae_backward_stop: unknown layer group '%s'", group);
@@ -1243,33 +1247,26 @@ int64_t cpb_vae_workspace_bytes(int32_t batch, int32_t ct, int32_t z, int32_t mo
     return make_plan(nullptr, 0, batch, ct, z, mode).bytes;
 }
 
-#define CPB_PLAN(mode)                                                                              \
-    CPB_TRY(check_cfg(cfg));                                                                        \
-    CPB_TRY(ensure_init());                                                                         \
-    CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                         \
-    VaePlan pl = make_plan(workspace, workspace_bytes, cfg->batch, cfg->target_channels, cfg->z_dim, mode); \
-    if (!pl.ok) {                                                                                   \
-        cpb::set_error("workspace too small: need %lld bytes, got %lld", (long long)pl.bytes,       \
-                       (long long)workspace_bytes);                                                 \
-        return CPB_ERR_WORKSPACE_TOO_SMALL;                                                         \
-    }                                                                                               \
-    VaeLayout L = make_layout(cfg->target_channels, cfg->z_dim);                                    \
-    cudaStream_t s = (cudaStream_t)stream;
-
 int32_t cpb_vae_encode(const cpb_vae_config* cfg, const float* params, const void* source, float* mean,
                        float* logvar, int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_PLAN(CPB_WS_ENCODE);
+    CPB_TRY(check_cfg(cfg));
+    const VaePlan pl = make_plan(workspace, workspace_bytes, cfg->batch, cfg->target_channels, cfg->z_dim, CPB_WS_ENCODE);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const VaeLayout L = make_layout(cfg->target_channels, cfg->z_dim);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && mean, "encode: NULL pointer");
     CPB_TRY(relayout_weights(pl, L, params, true, false, false, s));
     CPB_TRY(run_encoder(pl, L, cfg, params, source, flags, s));
-    CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
-    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
-    return CPB_OK;
+    return copy_latents_out(pl.heads, pl.zbuf, pl.B, pl.z, pl.zp, mean, logvar, nullptr, s);
 }
 
 int32_t cpb_vae_decode(const cpb_vae_config* cfg, const float* params, const float* z, float* reconstruction,
                        void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_PLAN(CPB_WS_FORWARD);
+    CPB_TRY(check_cfg(cfg));
+    const VaePlan pl = make_plan(workspace, workspace_bytes, cfg->batch, cfg->target_channels, cfg->z_dim, CPB_WS_FORWARD);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const VaeLayout L = make_layout(cfg->target_channels, cfg->z_dim);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && z && reconstruction, "decode: NULL pointer");
     CPB_TRY(relayout_weights(pl, L, params, false, true, false, s));
     if (pl.zp != pl.z) {
@@ -1283,21 +1280,26 @@ int32_t cpb_vae_forward(const cpb_vae_config* cfg, const float* params, const vo
                         const float* eps, float* losses, float* mean, float* logvar, float* z,
                         float* reconstruction, int32_t* flags, void* workspace, int64_t workspace_bytes,
                         void* stream) {
-    CPB_PLAN(CPB_WS_FORWARD);
+    CPB_TRY(check_cfg(cfg));
+    const VaePlan pl = make_plan(workspace, workspace_bytes, cfg->batch, cfg->target_channels, cfg->z_dim, CPB_WS_FORWARD);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const VaeLayout L = make_layout(cfg->target_channels, cfg->z_dim);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && target && losses, "forward: NULL pointer");
     CPB_TRY(relayout_weights(pl, L, params, true, true, false, s));
     CPB_TRY(run_forward_loss(pl, L, cfg, params, source, target, eps, false, reconstruction, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, cfg->loss_scale, losses, s));
-    if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
-    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
-    if (z) CPB_TRY(copy_latent_out(pl.zbuf, z, pl.B, pl.z, pl.zp, s));
-    return CPB_OK;
+    return copy_latents_out(pl.heads, pl.zbuf, pl.B, pl.z, pl.zp, mean, logvar, z, s);
 }
 
 int32_t cpb_vae_loss_grad(const cpb_vae_config* cfg, const float* params, const void* source, const void* target,
                           const float* eps, float* grads, float* losses, int32_t* flags, void* workspace,
                           int64_t workspace_bytes, void* stream) {
-    CPB_PLAN(CPB_WS_TRAIN);
+    CPB_TRY(check_cfg(cfg));
+    const VaePlan pl = make_plan(workspace, workspace_bytes, cfg->batch, cfg->target_channels, cfg->z_dim, CPB_WS_TRAIN);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const VaeLayout L = make_layout(cfg->target_channels, cfg->z_dim);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && target && grads && losses, "loss_grad: NULL pointer");
     CPB_TRY(relayout_weights(pl, L, params, true, true, true, s));
     CPB_TRY(run_forward_loss(pl, L, cfg, params, source, target, eps, true, nullptr, flags, s));
@@ -1470,36 +1472,28 @@ int64_t cpb_mlpvae_spec_workspace_bytes(const cpb_mlpvae_spec* spec, int32_t mod
     return make_mlp_plan(nullptr, 0, spec, mode).bytes;
 }
 
-#define CPB_MLP_PLAN(mode)                                                                           \
-    CPB_TRY(check_mlp_spec(spec));                                                                   \
-    CPB_TRY(ensure_init());                                                                          \
-    CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                          \
-    MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, mode);                              \
-    if (!pl.ok) {                                                                                    \
-        cpb::set_error("workspace too small: need %lld bytes, got %lld", (long long)pl.bytes, (long long)workspace_bytes); \
-        return CPB_ERR_WORKSPACE_TOO_SMALL;                                                          \
-    }                                                                                                \
-    MlpLayout L = make_mlp_layout(spec);                                                             \
-    cudaStream_t s = (cudaStream_t)stream;
-
 int32_t cpb_mlpvae_spec_encode(const cpb_mlpvae_spec* spec, const float* params, const void* source, float* mean, float* logvar,
                                int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_MLP_PLAN(CPB_WS_ENCODE);
+    CPB_TRY(check_mlp_spec(spec));
+    const MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, CPB_WS_ENCODE);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const MlpLayout L = make_mlp_layout(spec);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && mean, "mlp encode: NULL pointer");
-    CPB_TRY(mlp_pad_weights(pl, L, params, s));
-    CPB_TRY(mlp_tc_weights(pl, L, params, true, false, false, s));
+    CPB_TRY(mlp_relayout_weights(pl, L, params, true, false, false, s));
     CPB_TRY(mlp_encoder(pl, L, spec, params, source, flags, s));
-    CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
-    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
-    return CPB_OK;
+    return copy_latents_out(pl.heads, pl.zbuf, pl.B, pl.z, pl.zp, mean, logvar, nullptr, s);
 }
 
 int32_t cpb_mlpvae_spec_decode(const cpb_mlpvae_spec* spec, const float* params, const float* z, float* reconstruction, void* workspace,
                                int64_t workspace_bytes, void* stream) {
-    CPB_MLP_PLAN(CPB_WS_FORWARD);
+    CPB_TRY(check_mlp_spec(spec));
+    const MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, CPB_WS_FORWARD);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const MlpLayout L = make_mlp_layout(spec);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && z && reconstruction, "mlp decode: NULL pointer");
-    CPB_TRY(mlp_pad_weights(pl, L, params, s));
-    CPB_TRY(mlp_tc_weights(pl, L, params, false, true, false, s));
+    CPB_TRY(mlp_relayout_weights(pl, L, params, false, true, false, s));
     if (pl.zp != pl.z) {
         CPB_TRY(launch_pitch_copy(z, pl.z, pl.zbuf, pl.zp, pl.B, s));
         z = pl.zbuf;
@@ -1511,15 +1505,16 @@ int32_t cpb_mlpvae_spec_decode(const cpb_mlpvae_spec* spec, const float* params,
 int32_t cpb_mlpvae_spec_forward(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target, const float* eps,
                                 float* losses, float* mean, float* logvar, float* z, float* reconstruction, int32_t* flags,
                                 void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_MLP_PLAN(CPB_WS_FORWARD);
+    CPB_TRY(check_mlp_spec(spec));
+    const MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, CPB_WS_FORWARD);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const MlpLayout L = make_mlp_layout(spec);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && target && losses, "mlp forward: NULL pointer");
-    CPB_TRY(mlp_pad_weights(pl, L, params, s));
-    CPB_TRY(mlp_tc_weights(pl, L, params, true, true, false, s));
+    CPB_TRY(mlp_relayout_weights(pl, L, params, true, true, false, s));
     CPB_TRY(mlp_forward_loss(pl, L, spec, params, source, target, eps, false, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, spec->base.loss_scale, losses, s));
-    if (mean) CPB_TRY(copy_latent_out(pl.heads, mean, pl.B, pl.z, pl.zp, s));
-    if (logvar) CPB_TRY(copy_latent_out(pl.heads + (long long)pl.B * pl.zp, logvar, pl.B, pl.z, pl.zp, s));
-    if (z) CPB_TRY(copy_latent_out(pl.zbuf, z, pl.B, pl.z, pl.zp, s));
+    CPB_TRY(copy_latents_out(pl.heads, pl.zbuf, pl.B, pl.z, pl.zp, mean, logvar, z, s));
     if (reconstruction) CPB_TRY(launch_sigmoid(pl.logits, reconstruction, (long long)pl.B * pl.OUT, s));
     return CPB_OK;
 }
@@ -1527,10 +1522,13 @@ int32_t cpb_mlpvae_spec_forward(const cpb_mlpvae_spec* spec, const float* params
 int32_t cpb_mlpvae_spec_loss_grad(const cpb_mlpvae_spec* spec, const float* params, const void* source, const void* target,
                                   const float* eps, float* grads, float* losses, int32_t* flags, void* workspace,
                                   int64_t workspace_bytes, void* stream) {
-    CPB_MLP_PLAN(CPB_WS_TRAIN);
+    CPB_TRY(check_mlp_spec(spec));
+    const MlpPlan pl = make_mlp_plan(workspace, workspace_bytes, spec, CPB_WS_TRAIN);
+    CPB_TRY(check_workspace(workspace, workspace_bytes, pl.bytes));
+    const MlpLayout L = make_mlp_layout(spec);
+    cudaStream_t s = (cudaStream_t)stream;
     CPB_REQUIRE(params && source && target && grads && losses, "mlp loss_grad: NULL pointer");
-    CPB_TRY(mlp_pad_weights(pl, L, params, s));
-    CPB_TRY(mlp_tc_weights(pl, L, params, true, true, true, s));
+    CPB_TRY(mlp_relayout_weights(pl, L, params, true, true, true, s));
     CPB_TRY(mlp_forward_loss(pl, L, spec, params, source, target, eps, true, flags, s));
     CPB_TRY(launch_finalize_losses(pl.frame_loss, pl.kl_rows, pl.B, spec->base.loss_scale, losses, s));
     return mlp_backward(pl, L, spec, params, eps, grads, s);
