@@ -106,6 +106,9 @@ PROTOTYPES = {
     "cpb_gae": (_i32, [_P, _P, _f64, _P, _i32, _f64, _f64, _P, _P, _P, _P]),
     "cpb_ppo_learn": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
                              _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_gae_segments": (_i32, [_P, _P, _P, _P, _P, _i32, _i32, _f64, _f64, _P, _P, _P, _P]),
+    "cpb_ppo_learn_segments": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32, _f64, _f64,
+                                      _i32, _i32, _P, _P, _P, _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_vae_backward_stop": (_i32, [C.c_char_p]),

@@ -416,15 +416,15 @@ __device__ __forceinline__ Affine compose(const Affine& first, const Affine& sec
     return Affine{first.a * second.a, first.b * second.a + second.b};   // second(first(y))
 }
 
-__global__ void __launch_bounds__(1024)
-gae_kernel(const double* __restrict__ rewards, const double* __restrict__ values, double bootstrap,
-           const double* __restrict__ dones, int T, double gamma, double lam, double* __restrict__ adv_out,
-           double* __restrict__ ret_out, double* __restrict__ advn_out, float* __restrict__ ret32,
-           float* __restrict__ advn32, double* __restrict__ scratch /* [T] when adv_out is null */) {
+constexpr int kGaeThreads = 1024;   // the scan's grouping (and so its rounding) depends on it: every GAE kernel uses it
+
+// adv[0..T) of one rollout by the CTA's kGaeThreads threads: the reference's backward recursion as an affine scan.
+// Ends with a barrier, so the CTA may read all of adv afterwards.
+__device__ __forceinline__ void gae_scan(const double* __restrict__ rewards, const double* __restrict__ values,
+                                         double bootstrap, const double* __restrict__ dones, int T, double gamma,
+                                         double lam, double* __restrict__ adv) {
     __shared__ Affine warp_tot[32];
     __shared__ double carry_s;
-    __shared__ double red[32];
-    double* adv = adv_out != nullptr ? adv_out : scratch;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const double c = gamma * lam;
     if (tid == 0) carry_s = 0.0;
@@ -467,7 +467,15 @@ gae_kernel(const double* __restrict__ rewards, const double* __restrict__ values
         if (tid == 1023) carry_s = y;
         __syncthreads();
     }
-    // mean / population std (numpy: mean, then mean of squared deviations)
+}
+
+// returns = adv + values, advantages normalised by the mean and population std of adv[0..T) (numpy: mean, then mean of
+// squared deviations), by the CTA's kGaeThreads threads; each output may be null
+__device__ __forceinline__ void gae_normalise(const double* __restrict__ adv, const double* __restrict__ values, int T,
+                                              double* __restrict__ ret_out, double* __restrict__ advn_out,
+                                              float* __restrict__ ret32, float* __restrict__ advn32) {
+    __shared__ double red[32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     double s = 0.0;
     for (int i = tid; i < T; i += 1024) s += adv[i];
     s = warp_sum(s);
@@ -502,6 +510,44 @@ gae_kernel(const double* __restrict__ rewards, const double* __restrict__ values
         if (ret32 != nullptr) ret32[i] = (float)r;
         if (advn32 != nullptr) advn32[i] = (float)an;
     }
+}
+
+__global__ void __launch_bounds__(kGaeThreads)
+gae_kernel(const double* __restrict__ rewards, const double* __restrict__ values, double bootstrap,
+           const double* __restrict__ dones, int T, double gamma, double lam, double* __restrict__ adv_out,
+           double* __restrict__ ret_out, double* __restrict__ advn_out, float* __restrict__ ret32,
+           float* __restrict__ advn32, double* __restrict__ scratch /* [T] when adv_out is null */) {
+    double* adv = adv_out != nullptr ? adv_out : scratch;
+    gae_scan(rewards, values, bootstrap, dones, T, gamma, lam, adv);
+    gae_normalise(adv, values, T, ret_out, advn_out, ret32, advn32);
+}
+
+// Segmented GAE, step 1: CTA s scans rows [offsets[s], offsets[s+1]) with bootstrap[s] after its last row
+__global__ void __launch_bounds__(kGaeThreads)
+gae_segments_scan_kernel(const double* __restrict__ rewards, const double* __restrict__ values,
+                         const double* __restrict__ bootstrap, const double* __restrict__ dones,
+                         const int32_t* __restrict__ offsets, double gamma, double lam, double* __restrict__ adv) {
+    const int s = blockIdx.x;
+    const int begin = offsets[s], T = offsets[s + 1] - begin;
+    gae_scan(rewards + begin, values + begin, bootstrap[s], dones + begin, T, gamma, lam, adv + begin);
+}
+
+// Segmented GAE, step 2: one normalisation over all rows of the update
+__global__ void __launch_bounds__(kGaeThreads)
+gae_normalise_kernel(const double* __restrict__ adv, const double* __restrict__ values, int rows,
+                     double* __restrict__ ret_out, double* __restrict__ advn_out, float* __restrict__ ret32,
+                     float* __restrict__ advn32) {
+    gae_normalise(adv, values, rows, ret_out, advn_out, ret32, advn32);
+}
+
+int32_t launch_gae_segments(const double* rewards, const double* values, const double* bootstrap, const double* dones,
+                            const int32_t* offsets, int num_segments, int rows, double gamma, double lam, double* adv,
+                            double* ret_out, double* advn_out, float* ret32, float* advn32, cudaStream_t s) {
+    gae_segments_scan_kernel<<<num_segments, kGaeThreads, 0, s>>>(rewards, values, bootstrap, dones, offsets, gamma, lam, adv);
+    CPB_LAUNCHED();
+    gae_normalise_kernel<<<1, kGaeThreads, 0, s>>>(adv, values, rows, ret_out, advn_out, ret32, advn32);
+    CPB_LAUNCHED();
+    return CPB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -794,6 +840,45 @@ int32_t learn_persistent_init() {
     return CPB_OK;
 }
 
+// Everything of the driver's update block after GAE (train.py:178-207): theta_old <- theta, the old policy's
+// log-probabilities, and num_epochs x ceil(T / batch_size) minibatch Adam steps reading pl.ret32 / pl.adv32.
+int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
+                     float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                     const float* states, const float* actions, int T, int num_epochs, int batch_size,
+                     const int32_t* perms, float* metrics, cudaStream_t s) {
+    // theta_old <- theta (PPO.update_old_policy, ppo.py:275-276)
+    CPB_CUDA(cudaMemcpyAsync(params_old, params, L.total * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    // log pi_old(a_t|s_t) is constant during the update: evaluate it once for all T samples
+    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, nullptr, T, s));
+    CPB_TRY(launch_fill_zero(grads, L.total, s));
+    const int nmb = cdiv(T, batch_size);
+    CPB_TRY(learn_persistent_init());
+    if (g_learn_grid > 0 && num_epochs > 0) {
+        // all minibatch steps in ONE cooperative launch
+        LearnArgs a;
+        memset(&a, 0, sizeof(a));
+        a.cfg = *cfg; a.L = L; a.pl = pl;
+        a.params = params; a.grads = grads; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_powers = adam_powers; a.lr_dev = lr_dev;
+        a.states = states; a.actions = actions; a.perms = perms; a.metrics = metrics;
+        a.T = T; a.batch_size = batch_size; a.num_epochs = num_epochs; a.nmb = nmb;
+        void* args[] = {&a};
+        CPB_CUDA(cudaLaunchCooperativeKernel((void*)ppo_learn_persistent_kernel, dim3((unsigned)g_learn_grid), dim3(kLearnThreads), args, kLearnSmem, s));
+        CPB_LAUNCHED();
+        return CPB_OK;
+    }
+    for (int e = 0; e < num_epochs; ++e)
+        for (int i = 0; i < nmb; ++i) {
+            const int begin = i * batch_size;
+            const int B = begin + batch_size <= T ? batch_size : T - begin;
+            const int32_t* idx = perms + (long long)e * T + begin;
+            float* mt = metrics ? metrics + ((long long)e * nmb + i) * 5 : nullptr;
+            CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
+                                  grads, mt, s));
+            CPB_TRY(launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s));
+        }
+    return CPB_OK;
+}
+
 }  // namespace
 }  // namespace cpb
 
@@ -897,37 +982,38 @@ int32_t cpb_ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_ol
     gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
                                   pl.ret32, pl.adv32, pl.gae_scratch);
     CPB_LAUNCHED();
-    // theta_old <- theta (PPO.update_old_policy, ppo.py:275-276)
-    CPB_CUDA(cudaMemcpyAsync(params_old, params, L.total * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    // log pi_old(a_t|s_t) is constant during the update: evaluate it once for all T samples
-    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, nullptr, T, s));
-    CPB_TRY(launch_fill_zero(grads, L.total, s));
-    const int nmb = cdiv(T, batch_size);
-    CPB_TRY(learn_persistent_init());
-    if (g_learn_grid > 0 && num_epochs > 0) {
-        // all minibatch steps in ONE cooperative launch
-        LearnArgs a;
-        memset(&a, 0, sizeof(a));
-        a.cfg = *cfg; a.L = L; a.pl = pl;
-        a.params = params; a.grads = grads; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_powers = adam_powers; a.lr_dev = lr_dev;
-        a.states = states; a.actions = actions; a.perms = perms; a.metrics = metrics;
-        a.T = T; a.batch_size = batch_size; a.num_epochs = num_epochs; a.nmb = nmb;
-        void* args[] = {&a};
-        CPB_CUDA(cudaLaunchCooperativeKernel((void*)ppo_learn_persistent_kernel, dim3((unsigned)g_learn_grid), dim3(kLearnThreads), args, kLearnSmem, s));
-        CPB_LAUNCHED();
-        return CPB_OK;
-    }
-    for (int e = 0; e < num_epochs; ++e)
-        for (int i = 0; i < nmb; ++i) {
-            const int begin = i * batch_size;
-            const int B = begin + batch_size <= T ? batch_size : T - begin;
-            const int32_t* idx = perms + (long long)e * T + begin;
-            float* mt = metrics ? metrics + ((long long)e * nmb + i) * 5 : nullptr;
-            CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
-                                  grads, mt, s));
-            CPB_TRY(launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s));
-        }
-    return CPB_OK;
+    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
+                        num_epochs, batch_size, perms, metrics, s);
+}
+
+int32_t cpb_gae_segments(const double* rewards, const double* values, const double* bootstrap_values, const double* dones,
+                         const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma, double lam,
+                         double* advantages, double* returns, double* advantages_norm, void* stream) {
+    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments, "gae_segments: need 1 <= num_segments <= rows");
+    CPB_REQUIRE(rewards && values && bootstrap_values && dones && segment_offsets, "gae_segments: NULL pointer");
+    CPB_REQUIRE(advantages != nullptr, "gae_segments: advantages output is required");
+    return launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                               advantages, returns, advantages_norm, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+                               float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                               const float* actions, const double* rewards, const double* values,
+                               const double* bootstrap_values, const double* dones, const int32_t* segment_offsets,
+                               int32_t num_segments, int32_t rows, double gamma, double lam, int32_t num_epochs,
+                               int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments && batch_size >= 1 && num_epochs >= 0,
+                "ppo_learn_segments: bad sizes");
+    CPB_PPO_PLAN(batch_size < rows ? batch_size : rows, rows);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                rewards && values && bootstrap_values && dones && segment_offsets, "ppo_learn_segments: NULL pointer");
+    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn_segments: perms is NULL");
+    // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
+    CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                                pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
+    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
+                        num_epochs, batch_size, perms, metrics, s);
 }
 
 }  // extern "C"

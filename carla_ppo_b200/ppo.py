@@ -372,10 +372,22 @@ class PPO:
         self.params_old.copy_(self.params)
 
     def learn(self, states, actions, values, rewards, dones, last_value, gamma=0.99, lam=0.95, num_epochs=3,
-              batch_size=32, perms=None, return_metrics=False):
+              batch_size=32, perms=None, return_metrics=False, segment_lengths=None):
         """train.py:171-207 in one C call: compute_gae -> returns -> normalised advantages ->
         update_old_policy -> num_epochs x ceil(T/batch_size) minibatch steps.  ``perms`` ([num_epochs, T]
-        index orders) defaults to np.random permutations like the reference's np.random.shuffle."""
+        index orders) defaults to np.random permutations like the reference's np.random.shuffle.
+
+        ``segment_lengths`` (S lengths, each >= 1, summing to T): the rows are S environments' rollouts concatenated in
+        that order and ``last_value`` holds their S bootstrap values.  GAE runs per segment, the advantages are
+        normalised once over all T rows, and the minibatches draw from all of them (cpb_ppo_learn_segments)."""
+        if segment_lengths is not None:
+            rows = int(np.prod(states.shape if hasattr(states, "shape") else np.shape(states))) // self.state_dim
+            lengths = [int(n) for n in segment_lengths]
+            if not lengths or min(lengths) < 1 or sum(lengths) != rows:
+                raise ValueError("learn(): segment_lengths must be >= 1 each and sum to the %d rows, got %r" % (rows, lengths))
+            boot = np.asarray(last_value, np.float64).reshape(-1)
+            if boot.shape[0] != len(lengths):
+                raise ValueError("learn(): %d segments need as many bootstrap values, got %d" % (len(lengths), boot.shape[0]))
         self._require_session()
         torch = self._torch
         s = self._dev(states, torch.float32).reshape(-1, self.state_dim)
@@ -395,12 +407,22 @@ class PPO:
         nmb = -(-t_len // batch_size)
         metrics = torch.empty(max(num_epochs * nmb, 1), 5, dtype=torch.float32, device=self._device)
         ws = self._workspace(min(batch_size, t_len), t_len)
-        self._call("cpb_ppo_learn", 
-            C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
-            _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
-            _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), float(last_value), _lib.ptr(d), t_len, float(gamma),
-            float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics), _lib.ptr(ws), ws.numel(),
-            self._stream())
+        if segment_lengths is None:
+            self._call("cpb_ppo_learn",
+                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+                _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
+                _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), float(last_value), _lib.ptr(d), t_len, float(gamma),
+                float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics), _lib.ptr(ws), ws.numel(),
+                self._stream())
+        else:
+            b = self._dev(boot, torch.float64)
+            offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
+            self._call("cpb_ppo_learn_segments",
+                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+                _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
+                _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
+                len(lengths), t_len, float(gamma), float(lam), int(num_epochs), int(batch_size), _lib.ptr(p),
+                _lib.ptr(metrics), _lib.ptr(ws), ws.numel(), self._stream())
         self.train_step_counter += num_epochs * nmb
         self._pending_metrics.append(metrics[:num_epochs * nmb])
         if return_metrics:

@@ -8,6 +8,9 @@ hyper-parameter flags and TensorBoard tags, with the neural work on the H100 lib
                              num_epochs x ceil(T/batch) minibatch Adam steps in one C call (train.py:171-207);
                              ``--reference_loop`` runs the reference's own Python loop over PPO.train instead
                              (numerically identical: tests/test_integration_gpu.py)
+  * ``--num_envs N``:        N replay environments (seeded seed + i) in lockstep: one batched encode + predict per step
+                             (B = number of active environments) and one update per rollout over one trajectory segment
+                             per environment (PPO.learn(segment_lengths=...)); N = 1 is the reference's loop
 """
 from __future__ import annotations
 
@@ -69,19 +72,27 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     print("")
 
     measurements_to_include = set(["steer", "throttle", "speed"])
+    num_envs = int(params.get("num_envs", 1))
+    if num_envs < 1:
+        raise ValueError("num_envs must be >= 1")
     if env is None:
         print("Creating environment")
-        env = ReplayEnv(load_replay_frames(params.get("replay_data", "vae/data")), obs_res=(160, 80),
-                        action_smoothing=params["action_smoothing"], encode_state_fn=None,
-                        reward_fn=reward_functions[params["reward_fn"]], synchronous=params["synchronous"], fps=params["fps"],
-                        start_carla=False, episode_length=params.get("episode_length", 256))
+        frames = load_replay_frames(params.get("replay_data", "vae/data"))
+        envs = [ReplayEnv(frames, obs_res=(160, 80), action_smoothing=params["action_smoothing"], encode_state_fn=None,
+                          reward_fn=reward_functions[params["reward_fn"]], synchronous=params["synchronous"], fps=params["fps"],
+                          start_carla=False, episode_length=params.get("episode_length", 256)) for _ in range(num_envs)]
+    else:
+        envs = list(env) if isinstance(env, (list, tuple)) else [env]
+        if len(envs) != num_envs:
+            raise ValueError("num_envs = %d but %d environments were given" % (num_envs, len(envs)))
     if isinstance(seed, int):
-        env.seed(seed)
+        for i, e in enumerate(envs):
+            e.seed(seed + i)
     best_eval_reward = -float("inf")
 
     input_shape = np.array([vae.z_dim + len(measurements_to_include)])
     print("Creating model")
-    model = PPO(input_shape, env.action_space, learning_rate=learning_rate, lr_decay=lr_decay, epsilon=ppo_epsilon,
+    model = PPO(input_shape, envs[0].action_space, learning_rate=learning_rate, lr_decay=lr_decay, epsilon=ppo_epsilon,
                 initial_std=initial_std, value_scale=value_scale, entropy_scale=entropy_scale,
                 model_dir=os.path.join(models_root, model_name), seed=seed if isinstance(seed, int) else None)
     if not restart and interactive:
@@ -100,56 +111,97 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
         model.load_latest_checkpoint()
     model.write_dict_to_summary("hyperparameters", params, 0)
 
+    # Training steps every environment, then encodes all of their new frames and predicts their actions in one batched
+    # call (actor.encode_predict); the environments' own encode_state_fn does nothing meanwhile.  Evaluation runs the
+    # single-environment callback on envs[0].
     actor = None
     if fused:
         from .actor import FusedActor
         actor = FusedActor(vae, model, measurements_to_include)
-        env.encode_state_fn = actor.encode_state_fn
-        predict = actor.predict
+        vec_actor, eval_encode_state_fn = actor, actor.encode_state_fn
     else:
-        env.encode_state_fn = create_encode_state_fn(vae, measurements_to_include)
-        predict = model.predict
+        from .actor import UnfusedActor
+        vec_actor, eval_encode_state_fn = UnfusedActor(vae, model, measurements_to_include), create_encode_state_fn(vae, measurements_to_include)
+    for e in envs:
+        e.encode_state_fn = _deferred_encode
 
-    def log_episode(prefix, episode_idx):
-        model.write_value_to_summary(prefix + "/distance_traveled", env.distance_traveled, episode_idx)
-        model.write_value_to_summary(prefix + "/average_speed", 3.6 * env.speed_accum / max(env.step_count, 1), episode_idx)
-        model.write_value_to_summary(prefix + "/center_lane_deviation", env.center_lane_deviation, episode_idx)
-        model.write_value_to_summary(prefix + "/average_center_lane_deviation", env.center_lane_deviation / max(env.step_count, 1), episode_idx)
-        model.write_value_to_summary(prefix + "/distance_over_deviation", env.distance_traveled / max(env.center_lane_deviation, 1e-9), episode_idx)
+    def log_episode(prefix, episode_idx, logged):
+        mean = lambda f: float(np.mean([f(e) for e in logged]))
+        model.write_value_to_summary(prefix + "/distance_traveled", mean(lambda e: e.distance_traveled), episode_idx)
+        model.write_value_to_summary(prefix + "/average_speed", mean(lambda e: 3.6 * e.speed_accum / max(e.step_count, 1)), episode_idx)
+        model.write_value_to_summary(prefix + "/center_lane_deviation", mean(lambda e: e.center_lane_deviation), episode_idx)
+        model.write_value_to_summary(prefix + "/average_center_lane_deviation", mean(lambda e: e.center_lane_deviation / max(e.step_count, 1)), episode_idx)
+        model.write_value_to_summary(prefix + "/distance_over_deviation", mean(lambda e: e.distance_traveled / max(e.center_lane_deviation, 1e-9)), episode_idx)
+
+    def log_sampled_actions(actions):
+        """What predict(state, write_to_summary=True) records for each action taken (ppo.py:248)."""
+        for act in actions:
+            if model.train_writer is not None:
+                for k in range(model.num_actions):
+                    model.train_writer.add_scalar("predict_actor/action_%d/sampled_action" % k, float(act[k]), model.predict_step_counter)
+            model.predict_step_counter += 1
 
     history = []
+    # One round = every environment plays one training episode (the reference's episode at num_envs = 1).  A rollout
+    # steps the still-active environments in lockstep for up to `horizon` steps; an environment that terminates stops
+    # collecting for the rest of the round (the reference's `break`).  Each rollout ends in ONE update over one trajectory
+    # segment per environment that collected rows, in environment order.
     while num_episodes <= 0 or model.get_episode_idx() < num_episodes:
         episode_idx = model.get_episode_idx()
         if episode_idx % eval_interval == 0:
             video_filename = os.path.join(model.video_dir, "episode{}.avi".format(episode_idx)) if params.get("record_eval") else None
-            eval_reward = run_eval(env, model, video_filename=video_filename, actor=actor)
+            envs[0].encode_state_fn = eval_encode_state_fn
+            eval_reward = run_eval(envs[0], model, video_filename=video_filename, actor=actor)
+            envs[0].encode_state_fn = _deferred_encode
             model.write_value_to_summary("eval/reward", eval_reward, episode_idx)
-            log_episode("eval", episode_idx)
+            log_episode("eval", episode_idx, envs[:1])
             if eval_reward > best_eval_reward:
                 model.save()
                 best_eval_reward = eval_reward
 
-        state, terminal_state, total_reward = env.reset(), False, 0
+        for e in envs:
+            e.reset()
+        # state / action / value of every environment: the prediction for its current state
+        state, action, value = (list(x) for x in vec_actor.encode_predict(envs))
+        total_reward = [0.0] * num_envs
+        active = list(range(num_envs))
         print(f"Episode {episode_idx} (Step {model.get_train_step_idx()})")
-        while not terminal_state:
-            states, taken_actions, values, rewards, dones = [], [], [], [], []
+        first_rollout = True
+        while active:
+            if not first_rollout:                     # the reference predicts again on the state it bootstrapped from
+                a, v = model.predict(np.stack([state[i] for i in active]))
+                a, v = np.reshape(a, (len(active), -1)), np.reshape(v, (len(active),))
+                for j, i in enumerate(active):
+                    action[i], value[i] = a[j], v[j]
+            first_rollout = False
+            rollout = {i: ([], [], [], [], []) for i in active}      # states, taken_actions, values, rewards, dones
             for _ in range(horizon):
-                action, value = predict(state, write_to_summary=True)
-                new_state, reward, terminal_state, info = env.step(action)
-                if info["closed"]:
-                    return model
-                env.extra_info.extend(["Episode {}".format(episode_idx), "Training...", "", "Value:  % 20.2f" % value])
-                env.render()
-                total_reward += reward
-                states.append(state); taken_actions.append(action); values.append(value)
-                rewards.append(reward); dones.append(terminal_state)
-                state = new_state
-                if terminal_state:
+                log_sampled_actions([action[i] for i in active])
+                stepped, terminal = list(active), {}
+                for i in stepped:
+                    _, reward, terminal[i], info = envs[i].step(action[i])
+                    if info["closed"]:
+                        return model
+                    envs[i].extra_info.extend(["Episode {}".format(episode_idx), "Training...", "", "Value:  % 20.2f" % value[i]])
+                    envs[i].render()
+                    total_reward[i] += reward
+                    for buf, x in zip(rollout[i], (state[i], action[i], value[i], reward, terminal[i])):
+                        buf.append(x)
+                new_state, new_action, new_value = vec_actor.encode_predict([envs[i] for i in stepped])
+                for j, i in enumerate(stepped):
+                    state[i], action[i], value[i] = new_state[j], new_action[j], new_value[j]
+                active = [i for i in stepped if not terminal[i]]
+                if not active:
                     break
-            _, last_values = predict(state)                              # bootstrap value (train.py:172)
+            # bootstrap values (train.py:172): the predictions on each environment's current state
+            segments = [i for i in sorted(rollout) if rollout[i][3]]
+            states, taken_actions, values, rewards, dones = ([x for i in segments for x in rollout[i][k]] for k in range(5))
+            last_values = [value[i] for i in segments]
+            lengths = [len(rollout[i][3]) for i in segments]
             T = len(rewards)
             if reference_loop:
-                advantages = compute_gae(rewards, values, last_values, dones, discount_factor, gae_lambda)
+                advantages = np.concatenate([compute_gae(rollout[i][3], rollout[i][2], value[i], rollout[i][4], discount_factor, gae_lambda)
+                                             for i in segments])
                 returns = advantages + values
                 advantages = (advantages - advantages.mean()) / (advantages.std() + 1e-8)
                 s_arr, a_arr = np.array(states), np.array(taken_actions)
@@ -166,14 +218,25 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
                     indices = np.arange(T)
                     np.random.shuffle(indices)
                     perms.append(indices)
-                model.learn(np.array(states), np.array(taken_actions), values, rewards, dones, last_values, gamma=discount_factor,
-                            lam=gae_lambda, num_epochs=num_epochs, batch_size=batch_size, perms=np.stack(perms) if perms else None)
-        model.write_value_to_summary("train/reward", total_reward, episode_idx)
-        log_episode("train", episode_idx)
+                if num_envs == 1:
+                    model.learn(np.array(states), np.array(taken_actions), values, rewards, dones, last_values[0],
+                                gamma=discount_factor, lam=gae_lambda, num_epochs=num_epochs, batch_size=batch_size,
+                                perms=np.stack(perms) if perms else None)
+                else:
+                    model.learn(np.array(states), np.array(taken_actions), values, rewards, dones, last_values,
+                                gamma=discount_factor, lam=gae_lambda, num_epochs=num_epochs, batch_size=batch_size,
+                                perms=np.stack(perms) if perms else None, segment_lengths=lengths)
+        model.write_value_to_summary("train/reward", float(np.mean(total_reward)), episode_idx)
+        log_episode("train", episode_idx, envs)
         model.write_episodic_summaries()
-        history.append(total_reward)
+        history.append(float(np.mean(total_reward)))
     model.reward_history = history
     return model
+
+
+def _deferred_encode(env):
+    """encode_state_fn of the training environments: the loop encodes all stepped environments in one call afterwards."""
+    return None
 
 
 def main(argv=None):
@@ -210,6 +273,8 @@ def main(argv=None):
     parser.add_argument("--models_root", type=str, default="models")
     parser.add_argument("--unfused", action="store_true", help="separate encode / predict calls per step, like the reference")
     parser.add_argument("--reference_loop", action="store_true", help="the reference's Python minibatch loop over PPO.train instead of PPO.learn")
+    parser.add_argument("--num_envs", type=int, default=1, help="replay environments stepped in lockstep (seeded seed + i); "
+                        "one batched encode + predict per step and one PPO update over all their rollouts")
     params = vars(parser.parse_args(argv))
     start_carla = params.pop("start_carla")
     restart = params.pop("restart")

@@ -45,18 +45,29 @@ def create_encode_state_fn(vae, measurements_to_include):
     """Returns fn(env) -> np.float64[z_dim + M]: VAE mean of the current camera frame with the selected
     measurements appended (vae_common.py:33-62).  A uint8 observation is uploaded as uint8 and scaled by
     1/255 inside the conv1 loader -- numerically the same as preprocess_frame followed by a float feed."""
+    encode_states = create_encode_states_fn(vae, measurements_to_include)
+    return lambda env: encode_states([env])[0]
+
+
+def create_encode_states_fn(vae, measurements_to_include):
+    """create_encode_state_fn for several environments: fn(envs) -> [state of envs[i]], with ONE vae.encode on all their
+    frames."""
     measure_flags = ["steer" in measurements_to_include, "throttle" in measurements_to_include,
                      "speed" in measurements_to_include, "orientation" in measurements_to_include]
 
-    def encode_state(env):
-        obs = env.observation
-        frame = obs if getattr(obs, "dtype", None) == np.uint8 else preprocess_frame(obs)
-        encoded_state = vae.encode([frame])[0]
-        measurements = []
-        if measure_flags[0]: measurements.append(env.vehicle.control.steer)
-        if measure_flags[1]: measurements.append(env.vehicle.control.throttle)
-        if measure_flags[2]: measurements.append(env.vehicle.get_speed())
-        if measure_flags[3]: measurements.extend(_vector(env.vehicle.get_forward_vector()))
-        return np.append(encoded_state, measurements)
+    def encode_states(envs):
+        frames = [env.observation for env in envs]
+        if any(getattr(obs, "dtype", None) != np.uint8 for obs in frames):
+            frames = [preprocess_frame(np.asarray(obs)) for obs in frames]
+        encoded_states = vae.encode(frames)
+        states = []
+        for env, encoded_state in zip(envs, encoded_states):
+            measurements = []
+            if measure_flags[0]: measurements.append(env.vehicle.control.steer)
+            if measure_flags[1]: measurements.append(env.vehicle.control.throttle)
+            if measure_flags[2]: measurements.append(env.vehicle.get_speed())
+            if measure_flags[3]: measurements.extend(_vector(env.vehicle.get_forward_vector()))
+            states.append(np.append(encoded_state, measurements))
+        return states
 
-    return encode_state
+    return encode_states

@@ -347,6 +347,38 @@ void    cpb_profile_enable(int32_t on);
 void    cpb_profile_reset(void);
 int64_t cpb_profile_report(char* buf, int64_t capacity);
 
+/* ------------------------------------------------------------------------------------------
+ * PPO over several trajectory segments (N environments stepped in lockstep)
+ *
+ * A segment is the contiguous run of rows [segment_offsets[s], segment_offsets[s+1]) that one environment produced
+ * between two updates; segment_offsets[S+1] (int32, device) runs from 0 to rows and increases strictly, and its contents
+ * are trusted like perms.  Within a segment the GAE is utils.compute_gae on that rollout (utils.py:45-50,
+ * train.py:171-177): delta masks the bootstrap term by (1 - d), the accumulation is not reset inside the segment, and
+ * bootstrap_values[s] follows its last row.  Returns are A + V per row; the advantages are normalised ONCE over all rows
+ * (population std + 1e-8).  With S = 1 the results are bit-identical to cpb_gae / cpb_ppo_learn.
+ * S >= 1, rows >= S and the required pointers are checked before any launch (CPB_ERR_INVALID_ARGUMENT).
+ * ---------------------------------------------------------------------------------------- */
+
+/* cpb_gae over S segments (utils.py:45-50 + train.py:176-177 per segment, one normalisation): rewards, values, dones
+ * double[rows], bootstrap_values double[S]; advantages double[rows] is required, returns / advantages_norm may be NULL. */
+int32_t cpb_gae_segments(const double* rewards, const double* values, const double* bootstrap_values,
+                         const double* dones, const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                         double gamma, double lam, double* advantages, double* returns, double* advantages_norm,
+                         void* stream);
+
+/* cpb_ppo_learn (train.py:171-207) over S segments: the segmented GAE above, then theta_old <- theta, one old-policy
+ * log-prob pass over all rows and num_epochs x ceil(rows/batch) minibatch Adam steps following perms[num_epochs][rows]
+ * (launch-per-kernel, or the persistent kernel under CPB_PPO_PERSISTENT=1, as in cpb_ppo_learn).
+ * Workspace: cpb_ppo_workspace_bytes(cfg, min(batch_size, rows), rows). */
+int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+                               float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                               const float* states, const float* actions, const double* rewards,
+                               const double* values, const double* bootstrap_values, const double* dones,
+                               const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                               double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                               const int32_t* perms, float* metrics, void* workspace,
+                               int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
