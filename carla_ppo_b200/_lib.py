@@ -30,6 +30,11 @@ class VaeConfig(C.Structure):
                 ("loss_scale", C.c_float)]
 
 
+class VaeSpec(C.Structure):
+    """A ConvVAE at frame size height x width (each a multiple of 16 in [48, 512])."""
+    _fields_ = [("base", VaeConfig), ("height", C.c_int32), ("width", C.c_int32)]
+
+
 class MlpVaeConfig(C.Structure):
     _fields_ = [("base", VaeConfig), ("enc1", C.c_int32), ("enc2", C.c_int32), ("dec1", C.c_int32), ("dec2", C.c_int32)]
 
@@ -57,6 +62,7 @@ class PpoConfig(C.Structure):
 _P = C.c_void_p
 _i32, _i64, _f32, _f64 = C.c_int32, C.c_int64, C.c_float, C.c_double
 _VC = C.POINTER(VaeConfig)
+_VS = C.POINTER(VaeSpec)
 _MC = C.POINTER(MlpVaeConfig)
 _MS = C.POINTER(MlpVaeSpec)
 _PC = C.POINTER(PpoConfig)
@@ -78,6 +84,16 @@ PROTOTYPES = {
     "cpb_vae_train_step": (_i32, [_VC, _P, _P, _P, _P, _P, _f32, _P, _P, _P, _P, _P, _P, _i64, _P]),
     "cpb_vae_staging_bytes": (_i64, [_VC]),
     "cpb_vae_train_step_host": (_i32, [_VC, _P, _P, _P, _P, _P, _f32, _P, _P, _P, _P, _P, _P, _i64, _P, _i64, _P]),
+    "cpb_vae_spec_layout": (_i32, [_VS, _P, _P, _P, _P]),
+    "cpb_vae_spec_workspace_bytes": (_i64, [_VS, _i32]),
+    "cpb_vae_spec_encode": (_i32, [_VS, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_vae_spec_decode": (_i32, [_VS, _P, _P, _P, _P, _i64, _P]),
+    "cpb_vae_spec_forward": (_i32, [_VS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_vae_spec_loss_grad": (_i32, [_VS, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_vae_spec_train_step": (_i32, [_VS, _P, _P, _P, _P, _P, _f32, _P, _P, _P, _P, _P, _P, _i64, _P]),
+    "cpb_vae_spec_staging_bytes": (_i64, [_VS]),
+    "cpb_vae_spec_train_step_host": (_i32, [_VS, _P, _P, _P, _P, _P, _f32, _P, _P, _P, _P, _P, _P, _i64, _P, _i64, _P]),
+    "cpb_vae_spec_encode_predict": (_i32, [_VS, _P, _P, _P, _i32, _PC, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P, _i64, _P]),
     "cpb_mlpvae_num_tensors": (_i32, []),
     "cpb_mlpvae_tensor_name": (C.c_char_p, [_i32]),
     "cpb_mlpvae_layout": (_i32, [_MC, _P, _P, _P, _P]),
@@ -111,6 +127,7 @@ PROTOTYPES = {
                                       _i32, _i32, _P, _P, _P, _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
+    "cpb_debug_vae_spec_buffer_offsets": (_i32, [_VS, _i32, _P, _i32]),
     "cpb_debug_vae_backward_stop": (_i32, [C.c_char_p]),
     "cpb_debug_mlpvae_buffer_offsets": (_i32, [_MC, _i32, _P, _i32]),
     "cpb_debug_mlpvae_spec_buffer_offsets": (_i32, [_MS, _i32, _P, _i32]),

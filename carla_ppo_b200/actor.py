@@ -32,17 +32,18 @@ class FusedActor:
         if str(vae._device) != str(ppo._device):
             raise ValueError("VAE and PPO must live on the same device")
         self._torch = vae._torch
+        self._frame_bytes = int(np.prod(vae.source_shape))     # one uint8 frame at the VAE's frame size
         self._capacity = 0           # environments the pinned / device buffers hold
         self.greedy = False          # run_eval sets this: no sampling noise (ppo.py:244-247, run_eval.py:51)
         self._cached = None
         self.calls = 0
 
     def _buffers(self, n):
-        """Pinned host / device buffers for n environments: in = uint8 frames [n] | float32 measurements [n, M] | float32
-        noise [n, A]; out = float32 states [n, state_dim] | actions [n, A] | values [n]."""
+        """Pinned host / device buffers for n environments: in = uint8 frames [n, H, W, 3] | float32 measurements [n, M] |
+        float32 noise [n, A]; out = float32 states [n, state_dim] | actions [n, A] | values [n]."""
         if n > self._capacity:
             torch, dev, ppo = self._torch, self.vae._device, self.ppo
-            n_in = n * (80 * 160 * 3 + 4 * (self._m + ppo.num_actions))
+            n_in = n * (self._frame_bytes + 4 * (self._m + ppo.num_actions))
             n_out = n * (ppo.state_dim + ppo.num_actions + 1)
             self._in_host = torch.empty(n_in, dtype=torch.uint8).pin_memory()
             self._in_dev = torch.empty(n_in, dtype=torch.uint8, device=dev)
@@ -66,7 +67,7 @@ class FusedActor:
         encode_state_fn(envs[i]) returns.  The noise is ppo._rng.randn(n, A), rows in environment order (none when
         greedy)."""
         vae, ppo, torch = self.vae, self.ppo, self._torch
-        n, a, sd, nf = len(envs), ppo.num_actions, ppo.state_dim, 80 * 160 * 3
+        n, a, sd, nf = len(envs), ppo.num_actions, ppo.state_dim, self._frame_bytes
         self._buffers(n)
         host = self._in_host.numpy()
         fview = host[n * nf:n * (nf + 4 * (self._m + a))].view(np.float32)

@@ -67,6 +67,11 @@ struct ProfScope {
 static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// The tensor-core kernels (tc_tapgemm, tc_wgrad) address an activation tensor of `batch` images of `img` floats with
+// 32-bit offsets.  Their launchers refuse a problem outside this rule; the ConvVAE planner derives its batch bound from it.
+static inline bool tc_offsets_fit(int64_t batch, int64_t img) { return batch * img < (1ll << 31); }
+static inline int64_t tc_max_batch(int64_t img) { return ((1ll << 31) - 1) / img; }
+
 // ---- workspace bump allocator ---------------------------------------------------------------
 struct Arena {
     char* base;

@@ -1,4 +1,5 @@
-// The two 3-channel "edge" layers of the ConvVAE (conv1: 80x160x3 -> 39x79x32, and deconv4's gradient side).
+// The two 3-channel "edge" layers of the ConvVAE (conv1: HxWx3 -> H1xW1x32 with H1 = H/2 - 1, W1 = W/2 - 1 -- 80x160x3 ->
+// 39x79x32 by default -- and deconv4's gradient side).  The frame size is a run-time argument (FrameGeo).
 // Their contraction is short (K = 4*4*Cb = 48, N = 32): the generic tap-GEMM spends its time in pipeline
 // prologues, and per frame they only move ~360 KB -- they should run near the HBM roofline.  Dedicated kernels:
 //
@@ -18,18 +19,20 @@ namespace cpb {
 
 namespace {
 
-constexpr int EH = 80, EW = 160, SH = 39, SW = 79, SC = 32;   // big image (pixels), small image, small channels
+constexpr int SC = 32;   // small-side channels
 
 // One thread = 4 horizontally adjacent output pixels x 16 of the 32 channels (lane parity picks the half).  The
 // weights are read from shared memory as warp-broadcast LDS.128; such a load still writes 512 bytes of registers,
 // i.e. occupies the 128 B/clk shared-memory return path for 4 cycles, so what matters is FMAs per LDS.128:
 // 4 pixels x 4 channels = 16 (two pixels x 32 channels per thread gave 8 and left the kernel LDS-bound at twice
 // its FMA time).
-template <int CB, int EPI>   // EPI 0: bias + ReLU, 1: multiply by (mask > 0)
+template <int CB, int EPI, int FH, int FW>   // EPI 0: bias + ReLU, 1: multiply by (mask > 0); FH, FW: FrameExtents
 __global__ void __launch_bounds__(128)
 edge_gather_kernel(const float4* __restrict__ big4, const float* __restrict__ w, const float* __restrict__ bias,
-                   const float* __restrict__ mask, float* __restrict__ small, long long nwork,
+                   const float* __restrict__ mask, float* __restrict__ small, long long nwork, FrameGeo g,
                    float* __restrict__ cs_partial) {
+    const FrameExtents<FH, FW> e(g);
+    const int EH = e.H, EW = e.W, SH = e.H1, SW = e.W1;      // big image (pixels), small image
     __shared__ __align__(16) float ws[16 * CB * SC];
     for (int i = threadIdx.x; i < 16 * CB * SC; i += blockDim.x) ws[i] = w[i];
     __syncthreads();
@@ -43,14 +46,14 @@ edge_gather_kernel(const float4* __restrict__ big4, const float* __restrict__ w,
     if (t < nwork) {
     constexpr int NPX = 4;                               // output pixels per thread
     constexpr int HC = SC / 2;                           // channels per thread: the float4 groups 2*j4 + par, so that
-    constexpr int GW = (SW + NPX - 1) / NPX;             // a lane pair's stores fill whole 32-byte sectors
+    const int GW = (SW + NPX - 1) / NPX;                 // a lane pair's stores fill whole 32-byte sectors
     const int par = (int)(t & 1);
     const long long grp = t >> 1;
     const int gx = (int)(grp % GW);
     const int oy = (int)((grp / GW) % SH);
     const long long n = grp / (GW * SH);
     const int ox = gx * NPX;
-    const int nvalid = SW - ox < NPX ? SW - ox : NPX;    // 4, or 3 in the last group of a row
+    const int nvalid = SW - ox < NPX ? SW - ox : NPX;    // 4, or 3 in the last group of a row (W1 = 3 mod 4)
 
     float acc[NPX][HC];
 #pragma unroll
@@ -128,19 +131,32 @@ edge_gather_kernel(const float4* __restrict__ big4, const float* __restrict__ w,
 
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int WG_WARPS = 8;
-constexpr int BIG_ROW_FLOATS = EW * 4;            // 640 floats per padded big row
-constexpr int SMALL_ROW_FLOATS = SW * SC;         // 2528 floats per small row
+// shared-memory rows of edge_wgrad_kernel: a padded big row of W float4 pixels (the pitch + 4 puts the 4 kernel-row lane
+// groups on different banks) and a small row of W1 x 32 floats (+ 32)
+__host__ __device__ inline int wg_big_pitch(const FrameGeo& g) { return g.W * 4 + 4; }
+__host__ __device__ inline int wg_small_pitch(const FrameGeo& g) { return g.W1 * SC + 32; }
+// 2 x 4 big rows and 2 small rows (double buffer); at W = 48 the 8 big rows (1568 floats) still hold the combined
+// [48 x 32] tile that reuses them
+inline int wg_smem_bytes(const FrameGeo& g) { return (int)sizeof(float) * (8 * wg_big_pitch(g) + 2 * wg_small_pitch(g)); }
 
-template <int CB>
+template <int CB, int FH, int FW>
 __global__ void __launch_bounds__(WG_WARPS * 32)
 edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ small, long long nrows, int rows_per_cta,
-                  float* __restrict__ partial) {
+                  FrameGeo geo, float* __restrict__ partial) {
     // micro-tile: lane = (ig, jg): ig in [0, NI) owns TI rows of the [16*CB x 32] tile, jg in [0, 8) owns 4 columns
     constexpr int I = 16 * CB;                     // 48 or 16 rows: i = (kh*4 + kw)*CB + c
     constexpr int NI = 4, TI = I / NI;             // 12 or 4 rows per lane
-    constexpr int BIGP = BIG_ROW_FLOATS + 4;       // padded row pitch: the 4 kernel-row lane groups hit different banks
-    __shared__ __align__(16) float sbig[2][4 * BIGP];
-    __shared__ __align__(16) float ssmall[2][SMALL_ROW_FLOATS + 32];
+    const FrameExtents<FH, FW> e(geo);
+    const int EH = e.H, EW = e.W, SH = e.H1, SW = e.W1;
+    const int BIG_ROW_FLOATS = EW * 4, SMALL_ROW_FLOATS = SW * SC;
+    const int BIGP = EW * 4 + 4, SMALLP = SW * SC + 32;            // wg_big_pitch, wg_small_pitch
+    // the 80x160 instantiation keeps its rows in static shared memory (41 KB), the run-time one in dynamic
+    constexpr int kStaticFloats = FW ? 8 * (FW * 4 + 4) + 2 * ((FW / 2 - 1) * SC + 32) : 1;
+    __shared__ __align__(16) float wg_static[kStaticFloats];
+    extern __shared__ __align__(16) float wg_dynamic[];
+    float* const wg_smem = FW ? wg_static : wg_dynamic;
+    auto sbig = [&](int b) { return wg_smem + b * 4 * BIGP; };                 // [2][4 * BIGP]
+    auto ssmall = [&](int b) { return wg_smem + 8 * BIGP + b * SMALLP; };      // [2][SMALLP]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ig = lane >> 3, jg = lane & 7;
@@ -157,13 +173,13 @@ edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ smal
     auto stage_row = [&](int buf, long long r) {
         const long long n = r / SH;
         const int oy = (int)(r - n * SH);
-        const float* gb = big4 + ((n * EH + 2 * oy) * EW) * 4;           // 4 consecutive padded rows of 640 floats
+        const float* gb = big4 + ((n * EH + 2 * oy) * EW) * 4;           // 4 consecutive padded rows of W float4 pixels
         for (int f = tid; f < 4 * BIG_ROW_FLOATS / 4; f += WG_WARPS * 32) {
             const int kh = f / (BIG_ROW_FLOATS / 4), q = f - kh * (BIG_ROW_FLOATS / 4);
-            cp_async16(&sbig[buf][kh * BIGP + q * 4], gb + f * 4, true);
+            cp_async16(&sbig(buf)[kh * BIGP + q * 4], gb + f * 4, true);
         }
         const float* gs = small + r * SMALL_ROW_FLOATS;
-        for (int f = tid; f < SMALL_ROW_FLOATS / 4; f += WG_WARPS * 32) cp_async16(&ssmall[buf][f * 4], gs + f * 4, true);
+        for (int f = tid; f < SMALL_ROW_FLOATS / 4; f += WG_WARPS * 32) cp_async16(&ssmall(buf)[f * 4], gs + f * 4, true);
     };
 
     if (r_begin < r_end) stage_row(0, r_begin);
@@ -176,9 +192,9 @@ edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ smal
         __syncthreads();
         // this warp's positions of the row: ox = warp, warp + 8, ...
         for (int ox = warp; ox < SW; ox += WG_WARPS) {
-            const float4 g = *reinterpret_cast<const float4*>(&ssmall[buf][ox * SC + jg * 4]);
+            const float4 g = *reinterpret_cast<const float4*>(&ssmall(buf)[ox * SC + jg * 4]);
             // lane group ig owns kernel row kh = ig: its TI = 4*CB values are the window row's 4 pixels x CB channels
-            const float4* wp = reinterpret_cast<const float4*>(&sbig[buf][ig * BIGP + 2 * ox * 4]);
+            const float4* wp = reinterpret_cast<const float4*>(&sbig(buf)[ig * BIGP + 2 * ox * 4]);
             float a[TI];
 #pragma unroll
             for (int kw = 0; kw < 4; ++kw) {
@@ -196,7 +212,7 @@ edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ smal
     }
     cp_async_wait<0>();
     // ---- combine the 8 warps: each warp adds its tile into shared memory in turn (fixed order -> deterministic)
-    float* tile = &sbig[0][0];                                  // reuse: I*32 floats <= 1536 < 4*BIGP
+    float* tile = wg_smem;                                      // reuse: I*32 floats <= 1536 <= 8*BIGP
     __syncthreads();
     for (int w8 = 0; w8 < WG_WARPS; ++w8) {
         if (warp == w8) {
@@ -215,42 +231,59 @@ edge_wgrad_kernel(const float* __restrict__ big4, const float* __restrict__ smal
 
 }  // namespace
 
-long long edge_gather_blocks(int batch) { return cdiv(2LL * batch * SH * ((SW + 3) / 4), 128); }
+long long edge_gather_blocks(int batch, const FrameGeo& g) { return cdiv(2LL * batch * g.H1 * ((g.W1 + 3) / 4), 128); }
 
 int32_t launch_edge_gather(const float* big4, int cb, const float* w, const float* bias, const float* mask,
-                           float* small, int batch, cudaStream_t stream, float* cs_partial) {
+                           float* small, int batch, const FrameGeo& g, cudaStream_t stream, float* cs_partial) {
     CPB_REQUIRE(cb == 1 || cb == 3, "edge_gather: channels must be 1 or 3");
     CPB_REQUIRE(cs_partial == nullptr || mask != nullptr, "edge_gather: column sums exist for the mask form only");
-    const long long npairs = 2LL * batch * SH * ((SW + 3) / 4);      // (4-pixel group, channel half) work items
+    const long long npairs = 2LL * batch * g.H1 * ((g.W1 + 3) / 4);  // (4-pixel group, channel half) work items
     if (npairs == 0) return CPB_OK;
     const unsigned blocks = (unsigned)cdiv(npairs, 128);
     const float4* b4 = reinterpret_cast<const float4*>(big4);
+    auto launch = [&](auto kernel) {
+        kernel<<<blocks, 128, 0, stream>>>(b4, w, mask ? nullptr : bias, mask, small, npairs, g, mask ? cs_partial : nullptr);
+    };
+    const bool fixed = is_default_frame(g);
     if (mask == nullptr) {
-        if (cb == 3) edge_gather_kernel<3, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, npairs, nullptr);
-        else edge_gather_kernel<1, 0><<<blocks, 128, 0, stream>>>(b4, w, bias, nullptr, small, npairs, nullptr);
+        if (cb == 3) launch(fixed ? edge_gather_kernel<3, 0, 80, 160> : edge_gather_kernel<3, 0, 0, 0>);
+        else launch(fixed ? edge_gather_kernel<1, 0, 80, 160> : edge_gather_kernel<1, 0, 0, 0>);
     } else {
-        if (cb == 3) edge_gather_kernel<3, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, npairs, cs_partial);
-        else edge_gather_kernel<1, 1><<<blocks, 128, 0, stream>>>(b4, w, nullptr, mask, small, npairs, cs_partial);
+        if (cb == 3) launch(fixed ? edge_gather_kernel<3, 1, 80, 160> : edge_gather_kernel<3, 1, 0, 0>);
+        else launch(fixed ? edge_gather_kernel<1, 1, 80, 160> : edge_gather_kernel<1, 1, 0, 0>);
     }
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
-int edge_wgrad_ctas(int batch) {
-    const long long nrows = (long long)batch * SH;
+int edge_wgrad_ctas(int batch, const FrameGeo& g) {
+    const long long nrows = (long long)batch * g.H1;
     long long ctas = 132 * 2;                     // two CTAs per SM of an H100 SXM
     if (ctas > nrows) ctas = nrows;
     return (int)(ctas < 1 ? 1 : ctas);
 }
 
-int32_t launch_edge_wgrad(const float* big4, int cb, const float* small, int batch, float* partial, cudaStream_t stream) {
+int32_t edge_init() {
+    const FrameGeo widest = frame_geo(kMaxFrameSide, kMaxFrameSide);
+    // (the 80x160 instantiations use 41 KB of static shared memory)
+    CPB_CUDA(cudaFuncSetAttribute(edge_wgrad_kernel<3, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem_bytes(widest)));
+    CPB_CUDA(cudaFuncSetAttribute(edge_wgrad_kernel<1, 0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem_bytes(widest)));
+    return CPB_OK;
+}
+
+int32_t launch_edge_wgrad(const float* big4, int cb, const float* small, int batch, const FrameGeo& g, float* partial,
+                          cudaStream_t stream) {
     CPB_REQUIRE(cb == 1 || cb == 3, "edge_wgrad: channels must be 1 or 3");
-    const long long nrows = (long long)batch * SH;
+    CPB_REQUIRE(g.W <= kMaxFrameSide, "edge_wgrad: frame width %d above %d", g.W, kMaxFrameSide);
+    const long long nrows = (long long)batch * g.H1;
     if (nrows == 0) return CPB_OK;
-    const int ctas = edge_wgrad_ctas(batch);
+    const int ctas = edge_wgrad_ctas(batch, g);
     const int rows_per_cta = (int)((nrows + ctas - 1) / ctas);
-    if (cb == 3) edge_wgrad_kernel<3><<<ctas, WG_WARPS * 32, 0, stream>>>(big4, small, nrows, rows_per_cta, partial);
-    else edge_wgrad_kernel<1><<<ctas, WG_WARPS * 32, 0, stream>>>(big4, small, nrows, rows_per_cta, partial);
+    const bool fixed = is_default_frame(g);
+    const int smem = fixed ? 0 : wg_smem_bytes(g);
+    auto launch = [&](auto kernel) { kernel<<<ctas, WG_WARPS * 32, smem, stream>>>(big4, small, nrows, rows_per_cta, g, partial); };
+    if (cb == 3) launch(fixed ? edge_wgrad_kernel<3, 80, 160> : edge_wgrad_kernel<3, 0, 0>);
+    else launch(fixed ? edge_wgrad_kernel<1, 80, 160> : edge_wgrad_kernel<1, 0, 0>);
     CPB_LAUNCHED();
     return CPB_OK;
 }

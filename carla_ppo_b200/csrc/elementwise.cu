@@ -53,11 +53,14 @@ __global__ void sigmoid_kernel(const float* __restrict__ x, float* __restrict__ 
 // ------------------------------------------------------------------------------------------
 // One thread = NQ horizontally adjacent 2x2 output quads.  Every weight float4 read from shared memory
 // (warp-broadcast LDS.128, which occupies the 128 B/clk return path for 4 cycles) feeds NQ x 4 FMAs.
-template <int CT, int NQ>
+template <int CT, int NQ, int FH, int FW>   // FH, FW: FrameExtents
 __global__ void __launch_bounds__(128)
 deconv4_fwd_kernel(const float* __restrict__ small, const float* __restrict__ w, const float* __restrict__ bias,
-                   long long nwork, float* __restrict__ logits_p, float* __restrict__ sigm) {
-    constexpr int HS = 39, WS = 79, CS = 32, QH = 40, QW = 80, HB = 80, WB = 160, PW = QW / NQ;
+                   long long nwork, FrameGeo g, float* __restrict__ logits_p, float* __restrict__ sigm) {
+    // small [HS, WS] = [H1, W1]; output quads [QH, QW] = [H/2, W/2] (W/2 is a multiple of 8: NQ divides a quad row)
+    constexpr int CS = 32;
+    const FrameExtents<FH, FW> e(g);
+    const int HS = e.H1, WS = e.W1, QH = e.H / 2, QW = e.W / 2, HB = e.H, WB = e.W, PW = QW / NQ;
     __shared__ __align__(16) float ws[16 * CT * CS];
     for (int i = threadIdx.x; i < 16 * CT * CS; i += blockDim.x) ws[i] = w[i];
     __syncthreads();
@@ -224,7 +227,7 @@ recon_loss_kernel(const float4* logits_p, const float4* __restrict__ target_p, i
     // logits_p and dlogits_p MAY ALIAS (the training path overwrites the logits with d loss / d logits in place): neither
     // is __restrict__, each element is read before it is written by the same thread.
     // frame_dsum (optional): [batch][4] per-frame channel sums of d loss / d logits -- the last layer's bias gradient is their
-    // column sum, which saves a separate pass over the [B, 80, 160, 4] gradient image
+    // column sum, which saves a separate pass over the [B, H, W, 4] gradient image
     const long long base = (long long)blockIdx.x * npix;
     float sum = 0.f;
     float ds[4] = {0.f, 0.f, 0.f, 0.f};
@@ -440,15 +443,18 @@ int32_t launch_prep_frames(const void* src, int dtype, float scale, int cin, lon
     return CPB_OK;
 }
 
-int32_t launch_deconv4_fwd(const float* small, const float* w, const float* bias, int batch, int ct,
+int32_t launch_deconv4_fwd(const float* small, const float* w, const float* bias, int batch, int ct, const FrameGeo& g,
                            float* logits_p, float* sigm, cudaStream_t stream) {
     constexpr int nq = 4;                                          // 8 quads per thread measured 2x slower (254 registers)
-    const long long npairs = (long long)batch * 40 * (80 / nq);     // groups of nq horizontally adjacent 2x2 output quads
+    CPB_REQUIRE(g.W % (2 * nq) == 0, "deconv4: frame width %d is not a multiple of %d", g.W, 2 * nq);
+    const long long npairs = (long long)batch * (g.H / 2) * (g.W / 2 / nq);   // groups of nq horizontally adjacent 2x2 output quads
     if (npairs == 0) return CPB_OK;
     const unsigned blocks = (unsigned)cdiv(npairs, 128);
-    if (ct == 3) deconv4_fwd_kernel<3, nq><<<blocks, 128, 0, stream>>>(small, w, bias, npairs, logits_p, sigm);
-    else if (ct == 1) deconv4_fwd_kernel<1, nq><<<blocks, 128, 0, stream>>>(small, w, bias, npairs, logits_p, sigm);
-    else CPB_REQUIRE(false, "deconv4: target_channels must be 1 or 3");
+    CPB_REQUIRE(ct == 1 || ct == 3, "deconv4: target_channels must be 1 or 3");
+    auto launch = [&](auto kernel) { kernel<<<blocks, 128, 0, stream>>>(small, w, bias, npairs, g, logits_p, sigm); };
+    const bool fixed = is_default_frame(g);
+    if (ct == 3) launch(fixed ? deconv4_fwd_kernel<3, nq, 80, 160> : deconv4_fwd_kernel<3, nq, 0, 0>);
+    else launch(fixed ? deconv4_fwd_kernel<1, nq, 80, 160> : deconv4_fwd_kernel<1, nq, 0, 0>);
     CPB_LAUNCHED();
     return CPB_OK;
 }
@@ -482,9 +488,8 @@ int32_t launch_pitch_copy(const float* src, int src_pitch, float* dst, int dst_p
 }
 
 template <int LOSS>
-static int32_t launch_recon_loss_t(const float* logits_p, const float* target_p, int batch, int ct, float gscale,
+static int32_t launch_recon_loss_t(const float* logits_p, const float* target_p, int batch, int npix, int ct, float gscale,
                                    float* frame_loss, float* dlogits_p, float* frame_dsum, cudaStream_t stream) {
-    const int npix = 80 * 160;
     if (ct == 3)
         recon_loss_kernel<LOSS, 3><<<batch, 256, 0, stream>>>((const float4*)logits_p, (const float4*)target_p, npix,
                                                               gscale, frame_loss, (float4*)dlogits_p, frame_dsum);
@@ -495,14 +500,14 @@ static int32_t launch_recon_loss_t(const float* logits_p, const float* target_p,
     return CPB_OK;
 }
 
-int32_t launch_recon_loss(const float* logits_p, const float* target_p, int batch, int ct, int loss_type,
+int32_t launch_recon_loss(const float* logits_p, const float* target_p, int batch, int npix, int ct, int loss_type,
                           float gscale, float* frame_loss, float* dlogits_p, cudaStream_t stream, float* frame_dsum) {
     CPB_REQUIRE(ct == 1 || ct == 3, "recon_loss: target_channels must be 1 or 3");
     if (batch == 0) return CPB_OK;
     switch (loss_type) {
-        case CPB_LOSS_MSE: return launch_recon_loss_t<CPB_LOSS_MSE>(logits_p, target_p, batch, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
-        case CPB_LOSS_BCE: return launch_recon_loss_t<CPB_LOSS_BCE>(logits_p, target_p, batch, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
-        case CPB_LOSS_BCE_V2: return launch_recon_loss_t<CPB_LOSS_BCE_V2>(logits_p, target_p, batch, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
+        case CPB_LOSS_MSE: return launch_recon_loss_t<CPB_LOSS_MSE>(logits_p, target_p, batch, npix, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
+        case CPB_LOSS_BCE: return launch_recon_loss_t<CPB_LOSS_BCE>(logits_p, target_p, batch, npix, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
+        case CPB_LOSS_BCE_V2: return launch_recon_loss_t<CPB_LOSS_BCE_V2>(logits_p, target_p, batch, npix, ct, gscale, frame_loss, dlogits_p, frame_dsum, stream);
     }
     CPB_REQUIRE(false, "recon_loss: unknown loss_type %d", loss_type);
 }

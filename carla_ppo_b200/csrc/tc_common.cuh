@@ -12,6 +12,12 @@ constexpr int kMaxBN = 64;                    // widest N tile: 1.5 x BN fp32 ac
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// Row division by the output width d without a divide: rem / d = umulhi(2 rem, ceil(2^31 / d)), exact for rem < 65536 and
+// d < 32768 (the rounding of the magic adds less than 2^-15 to a quotient whose fraction is at most 1 - 1/d).  The
+// magic fits in 32 bits for every d, one-pixel-wide images (d = 1) included, where ceil(2^32 / d) would not.
+__host__ __device__ __forceinline__ uint32_t row_magic(int d) { return (uint32_t)((0x80000000ull + (uint32_t)d - 1) / (uint32_t)d); }
+__device__ __forceinline__ int row_of(int rem, uint32_t magic) { return (int)__umulhi((uint32_t)rem << 1, magic); }
+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }

@@ -160,7 +160,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             ntapsA = clsA->ntaps;
             const int Wo = clsA->Wo, HoWo = clsA->Ho * Wo;
             const long long M = (long long)p.batch * HoWo;
-            const uint32_t wo_magic = (uint32_t)((0x100000000ull + (uint32_t)Wo - 1) / (uint32_t)Wo);   // exact for rem < 65536
+            const uint32_t wo_magic = row_magic(Wo);
             // first row by division, the others are 16 positions apart
             long long m = st_m0(stA) + (tl >> 3);
             int n = (int)(m / HoWo);
@@ -168,7 +168,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
 #pragma unroll
             for (int i = 0; i < RPT; ++i) {
                 const bool ok = m < M;
-                const int oy = (int)__umulhi((uint32_t)rem, wo_magic);
+                const int oy = row_of(rem, wo_magic);
                 const int ox = rem - oy * Wo;
                 const int iy = oy * p.sstride, ix = ox * p.sstride;
                 a_base[i] = (uint32_t)n * (uint32_t)p.src_img + (uint32_t)((iy * p.Ws + ix) * p.src_pitch + a_chunk * 4);
@@ -457,7 +457,7 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     const long long total_w = mgroups * (p.N / BN) * p.nclass * p.ksplit;
     const int resident = g_tc_clusters[tc_passes_slot(PASSES)][tc_bn_slot(BN)];
     CPB_REQUIRE(total_w < (1ll << 30) && resident > 0, "tc_tapgemm: bad tile count");
-    CPB_REQUIRE((long long)p.batch * p.src_img < (1ll << 31) && (long long)p.batch * p.dst_img < (1ll << 31),
+    CPB_REQUIRE(tc_offsets_fit(p.batch, p.src_img) && tc_offsets_fit(p.batch, p.dst_img),
                 "tc_tapgemm: tensors too large for 32-bit row offsets");
     for (int c = 0; c < p.nclass; ++c) CPB_REQUIRE(p.cls[c].ntaps <= 32, "tc_tapgemm: more than 32 taps");
     if (p.quad) {

@@ -100,8 +100,8 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
         }
         const uint32_t a_dst0 = (uint32_t)(8 * pg * 512);
         // position cursor of this thread's NEXT copy: image n, position rem = oy*Wo + ox inside it.  Advancing by a
-        // k-block (32 positions) needs no division: oy comes from a multiply-high by ceil(2^32 / Wo).
-        const uint32_t wo_magic = (uint32_t)((0x100000000ull + (uint32_t)p.Wo - 1) / (uint32_t)p.Wo);
+        // k-block (32 positions) needs no division: oy comes from a multiply-high (row_of).
+        const uint32_t wo_magic = row_magic(p.Wo);
         const int dx = p.sstride * p.big_pitch;                              // next position in the row
         const int drow = (p.sstride * p.Wb - p.Wo * p.sstride) * p.big_pitch;   // ... wrapping to the next row
         const int dimg = (int)(p.big_img - (long long)p.Ho * p.sstride * p.Wb * p.big_pitch);   // ... to the next image
@@ -112,7 +112,7 @@ tc_wgrad_kernel(const __grid_constant__ WgradParams p) {
             remA = (int)(m - (long long)nA * HoWo);
         }
         auto issue_a = [&](uint32_t stage, uint64_t* full) {
-            int oy = (int)__umulhi((uint32_t)remA, wo_magic);
+            int oy = row_of(remA, wo_magic);
             int ox = remA - oy * p.Wo;
             uint32_t off = (uint32_t)nA * (uint32_t)p.big_img + (uint32_t)((oy * p.sstride * p.Wb + ox * p.sstride) * p.big_pitch) + (uint32_t)a_coloff;
 #pragma unroll
@@ -340,7 +340,7 @@ int tc_wgrad_pick_splits(int I, int J, long long M) {
 int32_t launch_tc_wgrad(const WgradParams& p, cudaStream_t stream) {
     CPB_REQUIRE(tc_wgrad_supported(p.I, p.J, p.run) && p.I == p.ntaps * p.run, "tc_wgrad: unsupported problem (I=%d J=%d)", p.I, p.J);
     CPB_REQUIRE(p.m_per_split % TBK == 0 && p.splits >= 1, "tc_wgrad: bad split");
-    CPB_REQUIRE((long long)p.batch * p.big_img < (1ll << 31) && p.m_per_split < (1ll << 30) && p.Wo < 65536 && p.Ho * p.Wo < 65536,
+    CPB_REQUIRE(tc_offsets_fit(p.batch, p.big_img) && p.m_per_split < (1ll << 30) && p.Wo < 65536 && p.Ho * p.Wo < 65536,
                 "tc_wgrad: tensor too large for 32-bit offsets");
     CPB_REQUIRE(p.passes == 3 || p.passes == 1, "tc_wgrad: passes must be 3 or 1, got %d", p.passes);
     if (p.passes == 1) return tc_wg_bn(p.J) == 64 ? tc_wg_launch<64, 1>(p, stream) : tc_wg_launch<32, 1>(p, stream);

@@ -70,7 +70,8 @@ def main(argv=None):
 
     vae = load_vae(args.vae_model, args.vae_z_dim, args.vae_model_type)
     measurements_to_include = set(["steer", "throttle", "speed"])
-    env = ReplayEnv(load_replay_frames(args.replay_data), obs_res=(160, 80), action_smoothing=args.action_smoothing,
+    obs_res = (vae.source_shape[1], vae.source_shape[0])                  # (width, height) of the frames the VAE takes
+    env = ReplayEnv(load_replay_frames(args.replay_data), obs_res=obs_res, action_smoothing=args.action_smoothing,
                     encode_state_fn=create_encode_state_fn(vae, measurements_to_include), reward_fn=reward_functions[args.reward_fn],
                     synchronous=args.synchronous, fps=args.fps, start_carla=False)
     np.random.seed(0)

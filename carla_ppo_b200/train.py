@@ -28,7 +28,7 @@ from .vae_common import create_encode_state_fn, load_vae
 
 
 def load_replay_frames(path, limit=None):
-    """uint8 [N,80,160,3] frames from a directory laid out like the reference's vae/data (rgb/{i}.png), a .npz with an
+    """uint8 [N,H,W,3] frames from a directory laid out like the reference's vae/data (rgb/{i}.png), a .npz with an
     'rgb' array (tests/golden/frames_u8.npz), or an array."""
     if not isinstance(path, str):
         return np.asarray(path)
@@ -78,7 +78,8 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     if env is None:
         print("Creating environment")
         frames = load_replay_frames(params.get("replay_data", "vae/data"))
-        envs = [ReplayEnv(frames, obs_res=(160, 80), action_smoothing=params["action_smoothing"], encode_state_fn=None,
+        obs_res = (vae.source_shape[1], vae.source_shape[0])          # (width, height) of the frames the VAE takes
+        envs = [ReplayEnv(frames, obs_res=obs_res, action_smoothing=params["action_smoothing"], encode_state_fn=None,
                           reward_fn=reward_functions[params["reward_fn"]], synchronous=params["synchronous"], fps=params["fps"],
                           start_carla=False, episode_length=params.get("episode_length", 256)) for _ in range(num_envs)]
     else:

@@ -24,7 +24,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from .. import _lib
-from .._lib import CpbError, MlpVaeConfig, MlpVaeSpec, VaeConfig
+from .._lib import CpbError, MlpVaeConfig, MlpVaeSpec, VaeConfig, VaeSpec
 
 
 # ----------------------------------------------------------------------------- loss selectors
@@ -81,6 +81,41 @@ def dp_shared_permutation(torch, dist, indices, device):
     return perm.cpu().numpy()
 
 
+FRAME_MIN, FRAME_MAX = 48, 512
+
+
+def frame_rule_error(height, width):
+    """None when the ConvVAE takes frames of height x width, else the refusal text (the library's, cpb_vae_spec_*): the
+    reference's decoder maps the encoder output back to exactly H x W only for multiples of 16 (vae/models.py:265)."""
+    if all(FRAME_MIN <= v <= FRAME_MAX and v % 16 == 0 for v in (height, width)):
+        return None
+    return "frame %dx%d: height and width must each be a multiple of 16 in [48, 512]" % (height, width)
+
+
+def encoded_hw(height, width):
+    """The encoder's output [H4, W4] (four 4x4 stride-2 VALID convolutions)."""
+    for _ in range(4):
+        height, width = (height - 4) // 2 + 1, (width - 4) // 2 + 1
+    return height, width
+
+
+def recorded_source_shape(checkpoint_dir):
+    """The source_shape the latest .npz checkpoint under checkpoint_dir recorded (``vae/source_shape``), or None: no
+    checkpoint, a TF bundle, or a checkpoint written before the shape was recorded."""
+    state = os.path.join(checkpoint_dir, "checkpoint")
+    if not os.path.isfile(state):
+        return None
+    with open(state) as f:
+        m = re.search(r'^model_checkpoint_path:\s*"(.*)"', f.read(), re.M)
+    if not m:
+        return None
+    prefix = m.group(1) if os.path.isabs(m.group(1)) else os.path.join(checkpoint_dir, m.group(1))
+    if not os.path.isfile(prefix + ".npz"):
+        return None
+    with np.load(prefix + ".npz") as blob:
+        return tuple(int(v) for v in blob["vae/source_shape"]) if "vae/source_shape" in blob else None
+
+
 class _Placeholder:
     """Stands in for the TF tensors callers only inspect (``vae.sample.shape[1]``, inspect_vae.py:100)."""
 
@@ -90,12 +125,13 @@ class _Placeholder:
 
 
 class VAE:
-    """Base class.  Geometry is the reference's only tested one: source [80,160,3], target [80,160,Ct]."""
+    """Base class.  Frames are source [H,W,3], target [H,W,Ct]: the ConvVAE takes every H and W that are multiples of 16
+    in [48, 512], the MlpVAE the reference's 80x160."""
 
-    # C entry points of the architecture (ConvVAE: cpb_vae_*, MlpVAE: cpb_mlpvae_spec_*; identical argument lists)
-    _API = {"num_tensors": "cpb_vae_num_tensors", "tensor_name": "cpb_vae_tensor_name", "encode": "cpb_vae_encode",
-            "decode": "cpb_vae_decode", "forward": "cpb_vae_forward", "loss_grad": "cpb_vae_loss_grad",
-            "encode_predict": "cpb_encode_predict"}
+    # C entry points of the architecture (ConvVAE: cpb_vae_spec_*, MlpVAE: cpb_mlpvae_spec_*; identical argument lists)
+    _API = {"num_tensors": "cpb_vae_num_tensors", "tensor_name": "cpb_vae_tensor_name", "encode": "cpb_vae_spec_encode",
+            "decode": "cpb_vae_spec_decode", "forward": "cpb_vae_spec_forward", "loss_grad": "cpb_vae_spec_loss_grad",
+            "encode_predict": "cpb_vae_spec_encode_predict"}
     _HOST_STEP = True        # cpb_vae_train_step_host exists for this architecture
 
     def __init__(self, source_shape, target_shape, build_encoder_fn=None, build_decoder_fn=None,
@@ -105,11 +141,7 @@ class VAE:
         # unknown kwargs (e.g. models_dir="vae", vae_common.py:21) are swallowed like the reference does
         self.source_shape = tuple(int(v) for v in source_shape)
         self.target_shape = tuple(int(v) for v in (source_shape if target_shape is None else target_shape))
-        if self.source_shape != (80, 160, 3):
-            raise ValueError("ConvVAE is built for source_shape (80,160,3) (reference vae/models.py:243-244), got %r"
-                             % (self.source_shape,))
-        if self.target_shape[:2] != (80, 160) or self.target_shape[2] not in (1, 3):
-            raise ValueError("target_shape must be (80,160,1) or (80,160,3), got %r" % (self.target_shape,))
+        self._check_shapes()
         self.z_dim = int(z_dim)
         self.beta = float(beta)
         self.kl_tolerance = float(kl_tolerance)
@@ -134,7 +166,7 @@ class VAE:
         self.source_states = _Placeholder((None,) + self.source_shape, "source_state_placeholder")
         self.target_states = _Placeholder((None,) + self.target_shape, "target_state_placeholder")
         self.sample = _Placeholder((None, self.z_dim), "sample")
-        self.encoded_shape = (3, 8, 256)
+        self.encoded_shape = encoded_hw(*self.source_shape[:2]) + (256,)
 
         self.sess = None
         self.step_idx = 0
@@ -185,17 +217,29 @@ class VAE:
         if init_logging:
             self._init_logging()
 
+    def _check_shapes(self):
+        if len(self.source_shape) != 3 or self.source_shape[2] != 3:
+            raise ValueError("source_shape must be (height, width, 3), got %r" % (self.source_shape,))
+        err = frame_rule_error(*self.source_shape[:2])
+        if err is not None:
+            raise ValueError(err)
+        h, w = self.source_shape[:2]
+        if len(self.target_shape) != 3 or self.target_shape[:2] != (h, w) or self.target_shape[2] not in (1, 3):
+            raise ValueError("target_shape must be (%d,%d,1) or (%d,%d,3), got %r" % (h, w, h, w, self.target_shape))
+
     def _tensor_names(self, lib):
         n = getattr(lib, self._API["num_tensors"])()
         return [getattr(lib, self._API["tensor_name"])(i).decode() for i in range(n)]
 
     def _query_layout(self, lib, offs, sizes, shapes, total):
-        _lib.check(lib.cpb_vae_layout(self.target_shape[2], self.z_dim, offs, sizes, shapes, C.byref(total)), "cpb_vae_layout")
+        spec = self._config(1)
+        _lib.check(lib.cpb_vae_spec_layout(C.byref(spec), offs, sizes, shapes, C.byref(total)), "cpb_vae_spec_layout")
 
     def _workspace_need(self, batch, mode):
         # on this instance's device: the size query initialises the library there (the plan depends on the kernel family)
+        spec = self._config(batch)
         with self._on_device():
-            return self._libh.cpb_vae_workspace_bytes(batch, self.target_shape[2], self.z_dim, mode)
+            return self._libh.cpb_vae_spec_workspace_bytes(C.byref(spec), mode)
 
     def _initial_weights(self) -> Dict[str, np.ndarray]:
         rng = np.random.RandomState(self._seed if self._seed is not None else np.random.randint(0, 2 ** 31 - 1))
@@ -315,6 +359,8 @@ class VAE:
             from ..tf_bundle import write_bundle
             write_bundle(prefix, {k: np.asarray(v) for k, v in blob.items()})
         else:
+            # the frame size the model was built for: load_vae rebuilds it from the checkpoint alone
+            blob["vae/source_shape"] = np.asarray(self.source_shape, np.int32)
             np.savez(prefix + ".npz", **blob)
         state = os.path.join(self.checkpoint_dir, "checkpoint")
         kept = []
@@ -359,6 +405,10 @@ class VAE:
                 blob = BundleReader(prefix).all()
             else:
                 return None
+            recorded = tuple(int(v) for v in blob["vae/source_shape"]) if "vae/source_shape" in blob else None
+            if recorded is not None and recorded != self.source_shape:
+                raise ValueError("checkpoint %s was written by a model with source_shape %r, this one has %r"
+                                 % (prefix, recorded, self.source_shape))
             weights = {n: blob["vae/" + n] for n in self._names}
             m_, v_, pw = None, None, None
             if self.training and ("vae/vae/%s/Adam" % self._names[0]) in blob:
@@ -385,13 +435,20 @@ class VAE:
             self._ws[key] = ws
         return ws
 
-    def _config(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
+    def _base_config(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
         tscale = 1.0 / 255.0 if self.target_shape[2] == 3 else 1.0 / 12.0
         return VaeConfig(batch, self.target_shape[2], self.z_dim, self.loss_type, source_dtype, target_dtype,
                          tscale, self.beta, self.kl_tolerance, loss_scale)
 
+    def _config(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
+        """The VaeSpec of the cpb_vae_spec_* entry points: the config at this model's frame size."""
+        return VaeSpec(self._base_config(batch, source_dtype, target_dtype, loss_scale), *self.source_shape[:2])
+
+    def _frame_shape(self, channels):
+        return tuple(self.source_shape[:2]) + (channels,)
+
     def _to_device_frames(self, frames, channels):
-        """numpy / list / torch -> contiguous CUDA tensor [B,80,160,channels], float32 or uint8."""
+        """numpy / list / torch -> contiguous CUDA tensor [B,H,W,channels] (source_shape's H, W), float32 or uint8."""
         torch = self._torch
         if not isinstance(frames, torch.Tensor):
             arr = np.asarray(frames)
@@ -402,8 +459,8 @@ class VAE:
             frames = frames.to(torch.float32)
         if frames.dim() == 3:
             frames = frames.unsqueeze(0)
-        if tuple(frames.shape[1:]) != (80, 160, channels):
-            raise ValueError("expected frames of shape [B,80,160,%d], got %r" % (channels, tuple(frames.shape)))
+        if tuple(frames.shape[1:]) != self._frame_shape(channels):
+            raise ValueError("expected frames of shape [B,%d,%d,%d], got %r" % (self._frame_shape(channels) + (tuple(frames.shape),)))
         return frames.to(self._device, non_blocking=True).contiguous()
 
     @staticmethod
@@ -450,13 +507,13 @@ class VAE:
         return (mean, logvar) if return_logvar else mean
 
     def generate_from_latent(self, z):
-        """-> np.float32 [B, 80*160*Ct]: sigmoid of the decoder output, flattened (vae/models.py:188-191)."""
+        """-> np.float32 [B, H*W*Ct]: sigmoid of the decoder output, flattened (vae/models.py:188-191)."""
         self._require_session()
         torch = self._torch
         zt = torch.as_tensor(np.asarray(z, np.float32) if not isinstance(z, torch.Tensor) else z,
                              dtype=torch.float32, device=self._device).reshape(-1, self.z_dim).contiguous()
         b = zt.shape[0]
-        out = torch.empty(b, 80 * 160 * self.target_shape[2], dtype=torch.float32, device=self._device)
+        out = torch.empty(b, int(np.prod(self.target_shape)), dtype=torch.float32, device=self._device)
         ws = self._workspace(b, _lib.WS_FORWARD)
         cfg = self._config(b)
         self._call(self._API["decode"], C.byref(cfg), _lib.ptr(self.params), _lib.ptr(zt), _lib.ptr(out),
@@ -482,7 +539,7 @@ class VAE:
         torch = self._torch
         b = x.shape[0]
         if y is None:
-            y = torch.zeros(b, 80, 160, self.target_shape[2], dtype=torch.float32, device=self._device)
+            y = torch.zeros((b,) + self.target_shape, dtype=torch.float32, device=self._device)
         losses = torch.empty(2, dtype=torch.float32, device=self._device)
         mean = logvar = z = rec = None
         if want_latents:
@@ -490,7 +547,7 @@ class VAE:
             logvar = torch.empty_like(mean)
             z = torch.empty_like(mean)
         if want_reconstruction:
-            rec = torch.empty(b, 80 * 160 * self.target_shape[2], dtype=torch.float32, device=self._device)
+            rec = torch.empty(b, int(np.prod(self.target_shape)), dtype=torch.float32, device=self._device)
         ws = self._workspace(b, _lib.WS_FORWARD)
         cfg = self._config(b, self._frame_dtype(x), self._frame_dtype(y), loss_scale)
         self._call(self._API["forward"], C.byref(cfg), _lib.ptr(self.params), _lib.ptr(x), _lib.ptr(y),
@@ -577,15 +634,15 @@ class VAE:
         sd = _lib.FRAME_U8 if src.dtype == np.uint8 else _lib.FRAME_F32
         td = _lib.FRAME_U8 if tgt.dtype == np.uint8 else _lib.FRAME_F32
         cfg = self._config(b, sd, td)
-        need = self._libh.cpb_vae_staging_bytes(C.byref(cfg))
-        _lib.check(need, "cpb_vae_staging_bytes")
+        need = self._libh.cpb_vae_spec_staging_bytes(C.byref(cfg))
+        _lib.check(need, "cpb_vae_spec_staging_bytes")
         st = self._ws.get("staging")
         if st is None or st.numel() < need:
             st = self._ws["staging"] = torch.empty(int(need), dtype=torch.uint8, device=self._device)
         ws = self._workspace(b, _lib.WS_TRAIN)
         losses = np.zeros(2, np.float32)
         flags = np.zeros(1, np.int32)
-        self._call("cpb_vae_train_step_host", 
+        self._call("cpb_vae_spec_train_step_host",
             C.byref(cfg), _lib.ptr(self.params), _lib.ptr(self.grads), _lib.ptr(self.adam_m), _lib.ptr(self.adam_v),
             _lib.ptr(self.adam_powers), self.base_learning_rate, _lib.ptr(src), _lib.ptr(src if same else tgt),
             _lib.ptr(eps), _lib.ptr(losses), _lib.ptr(flags), _lib.ptr(st), st.numel(), _lib.ptr(ws), ws.numel(),
@@ -629,8 +686,8 @@ class VAE:
                 if arr.dtype != np.uint8:
                     arr = arr.astype(np.float32, copy=False)
                 a = torch.from_numpy(np.ascontiguousarray(arr))
-            if tuple(a.shape[1:]) != (80, 160, channels):
-                raise ValueError("expected frames of shape [B,80,160,%d], got %r" % (channels, tuple(a.shape)))
+            if tuple(a.shape[1:]) != self._frame_shape(channels):
+                raise ValueError("expected frames of shape [B,%d,%d,%d], got %r" % (self._frame_shape(channels) + (tuple(a.shape),)))
             return a
         same = target is None or target is source
         xs = as_cpu_tensor(source, 3)
@@ -642,8 +699,8 @@ class VAE:
             dev = self._device
             st = self._pipe = {
                 "key": key, "i": 0, "copy_stream": torch.cuda.Stream(device=dev),
-                "x": [torch.empty((b, 80, 160, 3), dtype=xs.dtype, device=dev) for _ in range(2)],
-                "y": [None, None] if same else [torch.empty((b, 80, 160, self.target_shape[2]), dtype=ys.dtype, device=dev) for _ in range(2)],
+                "x": [torch.empty((b,) + self.source_shape, dtype=xs.dtype, device=dev) for _ in range(2)],
+                "y": [None, None] if same else [torch.empty((b,) + self.target_shape, dtype=ys.dtype, device=dev) for _ in range(2)],
                 "eps": [torch.empty((b, self.z_dim), dtype=torch.float32, device=dev) for _ in range(2)],
                 "copied": [torch.cuda.Event() for _ in range(2)], "done": [torch.cuda.Event() for _ in range(2)],
                 "used": [False, False],
@@ -762,10 +819,19 @@ class VAE:
 
 
 class ConvVAE(VAE):
-    """Convolutional VAE (reference vae/models.py:233-268); tested, like the reference, with 160x80x3."""
+    """Convolutional VAE (reference vae/models.py:233-268) at any frame size the reference builds: source_shape (H, W, 3)
+    with H and W multiples of 16 in [48, 512] (80x160 in the reference's own data), target_shape (H, W, 1 or 3); the
+    target defaults to the source at 80x160 only.  encoded_shape is (H/16 - 2, W/16 - 2, 256)."""
 
     def __init__(self, source_shape, target_shape=None, **kwargs):
-        target_shape = source_shape if target_shape is None else target_shape
+        if target_shape is None:
+            # target_shape defaults to source_shape (an rgb target) at the reference's 80x160 only; a model built for
+            # another frame size names its target, (H, W, 3) or (H, W, 1), as train_vae.py and load_vae do
+            h, w = (int(v) for v in tuple(source_shape)[:2])
+            if (h, w) != (80, 160):
+                raise ValueError(frame_rule_error(h, w) or "ConvVAE at frame %dx%d: give target_shape, (%d, %d, 3) for an rgb "
+                                 "target or (%d, %d, 1) for a segmentation target" % (h, w, h, w, h, w))
+            target_shape = source_shape
         super().__init__(source_shape, target_shape, None, None, **kwargs)
 
 
@@ -795,8 +861,15 @@ class MlpVAE(VAE):
         super().__init__(source_shape, target_shape, None, None, **kwargs)
         self.encoded_shape = (self.encoder_sizes[-1],)
 
+    def _check_shapes(self):
+        if self.source_shape != (80, 160, 3):
+            raise ValueError("MlpVAE is built for source_shape (80,160,3) (reference vae/models.py:243-244), got %r"
+                             % (self.source_shape,))
+        if self.target_shape[:2] != (80, 160) or self.target_shape[2] not in (1, 3):
+            raise ValueError("target_shape must be (80,160,1) or (80,160,3), got %r" % (self.target_shape,))
+
     def _spec(self, batch, source_dtype=_lib.FRAME_F32, target_dtype=_lib.FRAME_F32, loss_scale=1.0):
-        base = VAE._config(self, batch, source_dtype, target_dtype, loss_scale)
+        base = self._base_config(batch, source_dtype, target_dtype, loss_scale)
         return MlpVaeSpec.of(base, self.encoder_sizes, self.decoder_sizes)
 
     _config = _spec
@@ -807,7 +880,7 @@ class MlpVAE(VAE):
         if len(self.encoder_sizes) != 2 or len(self.decoder_sizes) != 2:
             raise ValueError("MlpVaeConfig describes two hidden layers per side; this model has %d and %d"
                              % (len(self.encoder_sizes), len(self.decoder_sizes)))
-        base = VAE._config(self, batch, source_dtype, target_dtype, loss_scale)
+        base = self._base_config(batch, source_dtype, target_dtype, loss_scale)
         return MlpVaeConfig(base, self.encoder_sizes[0], self.encoder_sizes[1], self.decoder_sizes[0], self.decoder_sizes[1])
 
     def _tensor_names(self, lib):

@@ -20,7 +20,7 @@ from .. import _lib
 
 
 def read_png_dir(directory: str, channels: int) -> np.ndarray:
-    """All ``*.png`` of a directory (os.listdir order, like the reference) as one uint8 array [N,80,160,channels]."""
+    """All ``*.png`` of a directory (os.listdir order, like the reference) as one uint8 array [N,H,W,channels]."""
     from PIL import Image
     frames = []
     for name in os.listdir(directory):

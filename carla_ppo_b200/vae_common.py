@@ -8,19 +8,24 @@ import re
 
 import numpy as np
 
-from .vae.models import ConvVAE, MlpVAE
+from .vae.models import ConvVAE, MlpVAE, recorded_source_shape
 
 
-def load_vae(model_dir, z_dim=None, model_type=None):
+def load_vae(model_dir, z_dim=None, model_type=None, source_shape=None):
     """Loads a pretrained VAE; z_dim / model type / target depth are parsed from the directory name when
-    not given (vae_common.py:12-15).  Raises Exception("Failed to load VAE") like the reference."""
+    not given (vae_common.py:12-15).  The frame size is ``source_shape`` when given, else the one the checkpoint
+    recorded (ConvVAE.save writes it), else the reference's 80x160x3.  Raises Exception("Failed to load VAE") like the
+    reference."""
     if z_dim is None:
         z_dim = int(re.findall(r"zdim(\d+)", model_dir)[0])
     if model_type is None:
         model_type = "mlp" if "mlp" in model_dir else "cnn"
     vae_class = MlpVAE if model_type == "mlp" else ConvVAE
     target_depth = 1 if "seg_" in model_dir else 3
-    vae = vae_class(source_shape=np.array([80, 160, 3]), target_shape=np.array([80, 160, target_depth]),
+    if source_shape is None:
+        source_shape = recorded_source_shape("{}/checkpoints/".format(model_dir)) or (80, 160, 3)
+    h, w = int(source_shape[0]), int(source_shape[1])
+    vae = vae_class(source_shape=np.array([h, w, 3]), target_shape=np.array([h, w, target_depth]),
                     z_dim=z_dim, models_dir="vae", model_dir=model_dir, training=False)
     vae.init_session(init_logging=False)
     if not vae.load_latest_checkpoint():

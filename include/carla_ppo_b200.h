@@ -17,9 +17,12 @@
  *     caller; cpb_vae_layout / cpb_ppo_layout give each TF variable's offset in that buffer.
  *   - every function returns 0 on success or a negative cpb_status; cpb_last_error() returns a
  *     message for the calling thread.  Bad arguments never launch anything.
- *   - geometry: source frames are [B,80,160,3] (vae_common.py:18-20), targets [B,80,160,Ct] with
- *     Ct in {3,1}; z_dim must be a multiple of 4 in [4,1024] (ConvVAE and MlpVAE).  Every [B,z] latent
- *     row (eps, mean, logvar, z, latent) is dense at pitch z_dim.
+ *   - geometry: source frames are [B,H,W,3], targets [B,H,W,Ct] with Ct in {3,1}.  The ConvVAE takes
+ *     any H and W that are multiples of 16 in [48,512] through the cpb_vae_spec_* entry points (the
+ *     frame sizes the reference's ConvVAE builds, vae/models.py:233-268); the cpb_vae_config entry
+ *     points and the MlpVAE use the reference's default 80x160 (vae_common.py:18-20).  z_dim must be a
+ *     multiple of 4 in [4,1024] (ConvVAE and MlpVAE).  Every [B,z] latent row (eps, mean, logvar, z,
+ *     latent) is dense at pitch z_dim.
  */
 #ifndef CARLA_PPO_B200_H
 #define CARLA_PPO_B200_H
@@ -66,6 +69,21 @@ typedef struct {
     float   loss_scale;       /* multiplies both batch means and all gradients: 1 for a whole batch,
                                  shard/global for a data-parallel shard (sum over ranks = global mean) */
 } cpb_vae_config;
+
+/* A ConvVAE at any legal frame size: H = height and W = width, each a multiple of 16 in [48, 512].  The encoder's
+ * four 4x4 stride-2 VALID convolutions give H1 = H/2 - 1, H2 = H/4 - 2, H3 = H/8 - 2, H4 = H/16 - 2 (the same in W) and
+ * FEAT = H4*W4*256; the decoder maps H4 back to exactly H (any other height fails the reference's assert,
+ * vae/models.py:265).  The variables keep their names, TF shapes and storage order; only mean, logstd_sqare and
+ * dense1 grow with FEAT.  Every cpb_vae_* entry point below has a cpb_vae_spec_* twin with the same arguments, the spec
+ * in place of the config; the cpb_vae_* ones are the twins at {cfg, 80, 160}.  A frame outside the rule is refused
+ * (CPB_ERR_INVALID_ARGUMENT) before any launch.
+ * Batch bound: in math modes 1 and 2 the tensor-core kernels address a tensor with 32-bit offsets, which needs
+ * B * H1 * W1 * 32 < 2^31 (B <= 21781 at 80x160, 5342 at 160x320, 1032 at 512x512); a larger batch is refused with
+ * CPB_ERR_UNSUPPORTED before any launch.  Math mode 0 takes every batch. */
+typedef struct {
+    cpb_vae_config base;      /* batch, target_channels, z_dim, loss, dtypes, beta, kl_tolerance, loss_scale */
+    int32_t height, width;    /* H, W of the source and target frames */
+} cpb_vae_spec;
 
 /* Number of TF variables (22) and their names, in creation order ("encoder/conv1/kernel", ...,
  * without the leading "vae/" scope).  Replaces: tf.trainable_variables() of the "vae" scope. */
@@ -143,6 +161,33 @@ int32_t cpb_vae_train_step_host(const cpb_vae_config* cfg, float* params, float*
                                 const void* target_host, const float* eps_host, float* losses_host,
                                 int32_t* flags_host, void* staging, int64_t staging_bytes,
                                 void* workspace, int64_t workspace_bytes, void* stream);
+
+/* The cpb_vae_spec twins.  layout reads target_channels, z_dim, height and width; workspace_bytes also the batch. */
+int32_t cpb_vae_spec_layout(const cpb_vae_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes,
+                            int64_t* total_floats);
+int64_t cpb_vae_spec_workspace_bytes(const cpb_vae_spec* spec, int32_t mode);
+int32_t cpb_vae_spec_encode(const cpb_vae_spec* spec, const float* params, const void* source,
+                            float* mean, float* logvar, int32_t* flags,
+                            void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_vae_spec_decode(const cpb_vae_spec* spec, const float* params, const float* z,
+                            float* reconstruction, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_vae_spec_forward(const cpb_vae_spec* spec, const float* params, const void* source,
+                             const void* target, const float* eps, float* losses,
+                             float* mean, float* logvar, float* z, float* reconstruction, int32_t* flags,
+                             void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_vae_spec_loss_grad(const cpb_vae_spec* spec, const float* params, const void* source,
+                               const void* target, const float* eps, float* grads, float* losses,
+                               int32_t* flags, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_vae_spec_train_step(const cpb_vae_spec* spec, float* params, float* grads, float* adam_m,
+                                float* adam_v, float* adam_powers, float lr, const void* source,
+                                const void* target, const float* eps, float* losses, int32_t* flags,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+int64_t cpb_vae_spec_staging_bytes(const cpb_vae_spec* spec);
+int32_t cpb_vae_spec_train_step_host(const cpb_vae_spec* spec, float* params, float* grads, float* adam_m,
+                                     float* adam_v, float* adam_powers, float lr, const void* source_host,
+                                     const void* target_host, const float* eps_host, float* losses_host,
+                                     int32_t* flags_host, void* staging, int64_t staging_bytes,
+                                     void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * MlpVAE (vae/models.py:271-299): flatten(38400) -> one dense relu layer per encoder size -> mean / logstd_sqare heads ->
@@ -286,6 +331,14 @@ int32_t cpb_encode_predict(const cpb_vae_config* vae_cfg, const float* vae_param
                            void* vae_workspace, int64_t vae_workspace_bytes,
                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
+/* cpb_encode_predict with a ConvVAE at any legal frame size: frames [B,H,W,3] (spec->height, spec->width). */
+int32_t cpb_vae_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                    const float* measurements, int32_t num_measurements,
+                                    const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
+                                    float* latent_tmp, float* state, float* action, float* value, int32_t* flags,
+                                    void* vae_workspace, int64_t vae_workspace_bytes,
+                                    void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
+
 /* cpb_encode_predict with an MlpVAE (cpb_mlpvae_spec) as the encoder; same arguments, outputs and noise use. */
 int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
                                   const float* measurements, int32_t num_measurements,
@@ -316,6 +369,8 @@ int32_t cpb_set_math_mode(int32_t mode);
  * dense D[M,N] = A[M,K] * Bt[N,K]^T through the tensor-core kernel (scratch: at least 2*N*K floats, the weight image). */
 int32_t cpb_debug_vae_buffer_offsets(int32_t batch, int32_t target_channels, int32_t z_dim, int32_t mode,
                                      int64_t* offsets, int32_t capacity);
+/* The same for a ConvVAE at the spec's frame size (batch, target_channels, z_dim, height, width). */
+int32_t cpb_debug_vae_spec_buffer_offsets(const cpb_vae_spec* spec, int32_t mode, int64_t* offsets, int32_t capacity);
 /* Process-global, like the math mode: every later ConvVAE backward pass (loss_grad, train_step) returns CPB_OK right
  * after the named layer group -- its weight, bias and data gradients -- has been enqueued.  Groups in pass order:
  * "deconv4.dgrad", "deconv3.dgrad", "deconv2.dgrad", "deconv1.dgrad", "dense1.dgrad", "heads.dgrad", "conv4.dgrad",
