@@ -67,7 +67,8 @@ struct TapGemmParams {
     int quad_cb;
     int quad_lcb;         // log2(quad_cb), set by the launcher
     int cluster;          // tensor-core path: CTAs per cluster (set by the launcher)
-    int debug;            // tensor-core path: timing decomposition (CPB_TC_DEBUG): 2 no A copies, 4 A copies zero-fill only, 8 no weight copies
+    int debug;            // tensor-core path: timing decomposition (CPB_TC_DEBUG): 2 no A copies, 4 A copies zero-fill only, 8 no weight copies,
+                          // 16 no tile epilogue (tap-GEMM: nothing is stored)
     int passes;           // tensor-core path: 3 (3xTF32) or 1 (one TF32 pass; weights from jobs with round_nearest set)
     TapClass cls[4];
 };

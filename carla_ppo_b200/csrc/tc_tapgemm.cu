@@ -14,8 +14,10 @@
 //   * B (weights)                    : stored by tc_weights_kernel as ready-made swizzled tile images [hi | lo]; one
 //                                      cp.async.bulk per k-block (multicast to the CTAs of a cluster).
 // Persistent, warp-specialised kernel (see tc_tapgemm_kernel): two consumer warpgroups (64 tile rows each, 12 wgmma per
-// 32-wide k-block in one commit group: main (+)= a_hi x b_hi, cross (+)= a_hi x b_lo, cross += a_lo x b_hi) and four
-// A-loader warps, the first lane of which also issues the weight-tile copies.
+// 32-wide k-block in one commit group: main (+)= a_hi x b_hi, cross (+)= a_hi x b_lo, cross += a_lo x b_hi), four
+// A-loader warps, the first lane of which also issues the weight-tile copies, and four epilogue warps: the consumers
+// leave a finished tile's sums in a shared-memory buffer and start the next tile, the epilogue warps apply bias /
+// ReLU / ReLU mask and store it with 16-byte accesses meanwhile.
 //
 // Accumulation.  The tensor core adds into its fp32 accumulator with truncation, which shrinks a long running sum
 // systematically (relative bias growing linearly with K).  Two measures bring this back to fp32-FMA level:
@@ -23,7 +25,7 @@
 //     large accumulator;
 //   * wgmma accumulation only runs over chunks of 128 k (4 k-blocks); each finished chunk is added to per-thread fp32
 //     register accumulators (round-to-nearest).
-// The register accumulators feed the bias / ReLU / ReLU-mask epilogue directly.
+// The register accumulators are what the bias / ReLU / ReLU-mask epilogue receives.
 //
 // Single-pass variant (PASSES = 1, math mode 2): a*b ~= rna(a) * rna(b), both operands rounded to the nearest TF32
 // value (the A fragment in registers, the weights by tc_weights_kernel), ONE wgmma per 8-wide k-step into the chunk
@@ -43,16 +45,25 @@ struct TcCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
     static constexpr int B_IMAGES = PASSES == 3 ? 2 : 1;                    // weight images per k-block: [hi | lo] or [hi]
     static constexpr int STAGE_BYTES = A_TILE_BYTES + B_IMAGES * B_TILE_BYTES;   // raw A rows | weight image(s)
-    static constexpr int STAGES = 200 * 1024 / STAGE_BYTES;                 // 3 passes: BN 64: 6, BN 32: 8; 1 pass: 8, 10
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // +1024: manual 1 KB alignment
+    static constexpr int OUT_BYTES = TBM * BN * 4;                          // the finished tile's raw sums, for the epilogue warps
+    static constexpr int STAGES = (224 * 1024 - OUT_BYTES) / STAGE_BYTES;   // 3 passes: BN 64: 6, BN 32: 8; 1 pass: 8, 10
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_BYTES + 1024;   // +1024: manual 1 KB alignment
 };
 constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 register accumulators
 
-constexpr int kConsumerWarps = 8;                     // warps 0-7: two wgmma warpgroups + epilogue
+constexpr int kConsumerWarps = 8;                     // warps 0-7: two wgmma warpgroups
 constexpr int kLoaderWarp0 = 8;                       // warps 8-11: A loaders (cp.async)
 constexpr int kLoaderWarps = 4;
 constexpr int kLoaderThreads = kLoaderWarps * 32;
-constexpr int kTcThreads = 384;                       // a multiple of 4 warps: registers are granted per 4 warps
+constexpr int kEpilogueWarp0 = 12;                    // warps 12-15: tile epilogue (bias / ReLU / mask, global stores)
+constexpr int kEpilogueWarps = 4;
+constexpr int kEpilogueThreads = kEpilogueWarps * 32;
+constexpr int kTcThreads = 512;                       // four warpgroups: setmaxnreg moves registers between whole warpgroups
+// 512 threads start with 128 registers each; the loader and epilogue warpgroups give theirs back down to kSideRegs and
+// the two consumer warpgroups grow to kConsumerRegs: 256 * 168 + 256 * 80 <= 65 536
+constexpr int kLaunchRegs = 128, kConsumerRegs = 168, kSideRegs = 80;
+template <int R> __device__ __forceinline__ void reg_grow() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void reg_shrink() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 int g_tc_cluster = 1;         // CTAs per cluster = multicast width of the weight tiles (CPB_TC_CLUSTER, 1/2/4/8)
 int g_tc_clusters[2][2] = {{0, 0}, {0, 0}};   // co-resident clusters of the persistent grid, per instantiation [passes 3/1][BN 32/64]
@@ -91,7 +102,7 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 // KSPLIT the work items are the super-tiles and the split bookkeeping compiles away: the per-k-block loop of the
 // unsplit kernels keeps its instructions and registers.
 template <int BN, int PASSES, bool KSPLIT>
-__global__ void __maxnreg__(168)     // 12 warps x 32 x 168 registers fit one SM
+__global__ void __maxnreg__(kLaunchRegs)
 tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, const int total_w) {
     static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or a single TF32 pass");
     using Cfg = TcCfg<BN, PASSES>;
@@ -102,6 +113,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t full_bar[STAGES];     // A loader threads (cp.async completion) + weight bytes -> consumers
     __shared__ uint64_t empty_bar[STAGES];    // consumer warps of ALL CTAs of the cluster -> producers: stage is free everywhere
+    __shared__ uint64_t out_full;             // consumer warps -> epilogue warps: the tile's sums are in the output buffer
+    __shared__ uint64_t out_empty;            // epilogue warps -> consumers: the output buffer has been read (CTA-local, both)
 
     const int tid = threadIdx.x;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform for the compiler
@@ -114,10 +127,17 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     // the dynamic shared window starts at the same offset in every CTA of the kernel, so the 1 KB-aligned base is
     // the same offset everywhere -- which the multicast copies rely on
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    // Output buffer (behind the stage ring): the tile's 128 x BN raw fp32 sums, rows of BN * 4 bytes, the 16-byte chunk
+    // index of row r XORed with 2 * (r % 4).  A consumer warp's float2 fragment store covers rows g .. g+3 (per half
+    // warp) x 32 bytes at the same columns, which the XOR spreads over all 32 banks; an epilogue thread's float4 read
+    // stays inside one row, whose chunks the XOR only permutes.  Neither access has a bank conflict.
+    const uint32_t out_base = smem_base + STAGES * STAGE_BYTES;
 
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], kLoaderThreads + 1); mbar_init(&empty_bar[s], (uint32_t)(kConsumerWarps * CS)); }
+        mbar_init(&out_full, kConsumerWarps);
+        mbar_init(&out_empty, kEpilogueWarps);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -132,7 +152,121 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     // first k-block of split ks of a tile with nkb k-blocks
     auto split_kb = [&](int nkb, int ks) { return (int)((long long)nkb * ks / ksplit); };
 
-    if (warp >= kLoaderWarp0) {
+    if (warp >= kEpilogueWarp0) {
+        reg_shrink<kSideRegs>();
+        // ================================ tile epilogue ================================
+        // The epilogue warps walk the same work items as the consumers.  Thread et owns 16-byte column chunk et % CPR of
+        // tile rows et / CPR + RPP * i: a row's BN columns are contiguous in the destination (quad form: each parity
+        // class's quad_cb >= 8 columns are), so a warp's stores and ReLU-mask loads are whole 128-byte lines.  The
+        // destination offsets and the mask's sign bits of item w are computed / fetched while the consumers are still
+        // accumulating w; once the sums arrive only shared loads, the arithmetic and the stores remain.
+        constexpr int CPR = BN / 4;                        // 16-byte chunks per tile row
+        constexpr int RPP = kEpilogueThreads / CPR;        // tile rows per pass of the four warps: 8 (BN 64) / 16 (BN 32)
+        constexpr int NR = TBM / RPP;                      // rows per thread: 16 / 8
+        constexpr uint32_t SKIP = 0xffffffffu;             // no destination: row beyond M or quad position outside the image
+        const int et = tid - kEpilogueWarp0 * 32;
+        const int ec = et % CPR, er = et / CPR;
+        const uint32_t o_src = out_base + (uint32_t)(er * (BN * 4) + ((ec ^ ((er & 3) << 1)) << 4));   // RPP % 4 == 0: the XOR is the same for every i
+        uint32_t phO = 0;                                  // parity of out_full's current phase
+        for (int w = cl_id; w < total_w && !(p.debug & 16); w += cl_n) {
+            const int st = KSPLIT ? w / ksplit : w, ks = KSPLIT ? w - st * ksplit : 0;
+            const TapClass& cls = p.cls[st_z(st)];
+            float* const dst = KSPLIT ? p.dst + (long long)ks * p.kpartial_stride : p.dst;
+            const int Wo = cls.Wo, HoWo = cls.Ho * Wo;
+            const uint32_t M = (uint32_t)p.batch * (uint32_t)HoWo;      // destination offsets fit 32 bits (checked at launch), so rows do
+            const uint32_t wo_magic = row_magic(Wo);
+            const int col = st_y(st) * BN + ec * 4;
+            int ch = col, qy = 0, qx = 0;                  // quad form: column inside the parity class (qy, qx)
+            if (p.quad) {
+                const int c = col >> p.quad_lcb;
+                ch = col & (p.quad_cb - 1);
+                qy = c >> 1; qx = c & 1;
+            }
+            // row cursor: the first row by division, the others are RPP positions apart.  next_off returns the float
+            // offset of the thread's chunk in the cursor's row (or SKIP) and moves the cursor on one pass
+            const uint32_t m0 = (uint32_t)st_m0(st) + (uint32_t)er;
+            const int n0 = (int)(m0 / (uint32_t)HoWo);
+            const int rem0 = (int)(m0 - (uint32_t)n0 * (uint32_t)HoWo);
+            uint32_t m = m0;
+            int n = n0, rem = rem0;
+            auto next_off = [&]() {
+                const int oy = row_of(rem, wo_magic);
+                const int ox = rem - oy * Wo;
+                const uint32_t img = (uint32_t)n * (uint32_t)p.dst_img;
+                bool ok = m < M;
+                uint32_t off;
+                if (p.quad) {
+                    const int y = oy * 2 + qy, x = ox * 2 + qx;
+                    ok = ok && y < p.Hd && x < p.Wd;
+                    off = img + (uint32_t)((y * p.Wd + x) * p.dst_pitch + ch);
+                } else {
+                    off = img + (uint32_t)(((oy * p.dstride + cls.py) * p.Wd + (ox * p.dstride + cls.px)) * p.dst_pitch + col);
+                }
+                m += RPP; rem += RPP;
+                while (rem >= HoWo) { rem -= HoWo; ++n; }
+                return ok ? off : SKIP;
+            };
+            // ReLU mask: only the sign tests are kept, one word per eight rows, bit 4 * u + e = (mask element e of row u
+            // of the eight) > 0.  keep[] is a queue: every trip pushes its words at the back, so that after the last
+            // trip keep[0] belongs to the first eight rows (the loops stay rolled: a few hundred instructions, and a
+            // bounded number of loads' registers at a time)
+            uint32_t keep[NR / 8];
+            if (p.mask) {
+#pragma unroll 1
+                for (int b = 0; b < NR / 8; ++b) {         // eight rows' loads in flight, one word per trip
+                    uint32_t offs[8];
+                    float4 mk[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) offs[u] = next_off();
+#pragma unroll
+                    for (int u = 0; u < 8; ++u)
+                        mk[u] = offs[u] != SKIP ? __ldg(reinterpret_cast<const float4*>(p.mask + offs[u])) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    uint32_t bits = 0u;
+#pragma unroll
+                    for (int u = 0; u < 8; ++u)
+                        bits |= ((mk[u].x > 0.f ? 1u : 0u) | (mk[u].y > 0.f ? 2u : 0u) | (mk[u].z > 0.f ? 4u : 0u) | (mk[u].w > 0.f ? 8u : 0u)) << (4 * u);
+#pragma unroll
+                    for (int q = 0; q < NR / 8 - 1; ++q) keep[q] = keep[q + 1];
+                    keep[NR / 8 - 1] = bits;
+                }
+                m = m0; n = n0; rem = rem0;
+            }
+            float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (p.bias) bias = __ldg(reinterpret_cast<const float4*>(p.bias + ch));
+
+            mbar_wait(&out_full, phO);
+            phO ^= 1u;
+#pragma unroll 1
+            for (int b = 0; b < NR / 8; ++b) {
+                uint32_t offs[8];
+                float4 sums[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u)
+                    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(sums[u].x), "=f"(sums[u].y), "=f"(sums[u].z), "=f"(sums[u].w)
+                                 : "r"(o_src + (uint32_t)((8 * b + u) * RPP * BN * 4)));
+#pragma unroll
+                for (int u = 0; u < 8; ++u) offs[u] = next_off();
+                const uint32_t bits = p.mask ? keep[0] : 0u;
+#pragma unroll
+                for (int q = 0; q < NR / 8 - 1; ++q) keep[q] = keep[q + 1];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                    if (offs[u] == SKIP) continue;
+                    float4 o = sums[u];
+                    if (p.bias) { o.x += bias.x; o.y += bias.y; o.z += bias.z; o.w += bias.w; }
+                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                    if (p.mask) {
+                        const uint32_t k = bits >> (4 * u);
+                        o.x = (k & 1u) ? o.x : 0.f; o.y = (k & 2u) ? o.y : 0.f; o.z = (k & 4u) ? o.z : 0.f; o.w = (k & 8u) ? o.w : 0.f;
+                    }
+                    *reinterpret_cast<float4*>(dst + offs[u]) = o;
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&out_empty);         // this warp has read its part of the buffer
+        }
+    } else if (warp >= kLoaderWarp0) {
+        reg_shrink<kSideRegs>();
         // ================================ A loaders ================================
         // The raw fp32 activation rows are copied global -> swizzled shared memory with cp.async (16 B per thread and
         // row, zero-filled outside the image); the consumers split them into TF32 hi / lo in registers.  Completion is
@@ -142,7 +276,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         const int a_chunk = tl & 7;
         // row r = tl/8 + 16*i lives at (r/8)*1024 + (r%8)*128 + ((chunk ^ r%8) * 16): i only moves the 1 KB group (2 per i)
         const uint32_t a_soff0 = (uint32_t)((tl >> 6) * 1024 + ((tl >> 3) & 7) * 128 + ((a_chunk ^ ((tl >> 3) & 7)) << 4));
-        constexpr int RPT = TBM / (kLoaderThreads / 8);     // rows per thread: 8
+        constexpr int RPP = kLoaderThreads / 8;             // rows per pass: 16
+        constexpr int RPT = TBM / RPP;                      // rows per thread: 8
 
         // ---- A cursor: 8 threads cover the 128 bytes of one row, 16 rows per pass, 8 passes
         int wA = cl_id, stA = 0, tapA = 0, cA = 0;   // work item, its super-tile, tap and k offset inside the tap
@@ -161,26 +296,34 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             const int Wo = clsA->Wo, HoWo = clsA->Ho * Wo;
             const long long M = (long long)p.batch * HoWo;
             const uint32_t wo_magic = row_magic(Wo);
-            // first row by division, the others are 16 positions apart
+            // first row by division, the others are RPP positions apart
             long long m = st_m0(stA) + (tl >> 3);
             int n = (int)(m / HoWo);
             int rem = (int)(m - (long long)n * HoWo);
+            int iy[RPT], ix[RPT];
 #pragma unroll
             for (int i = 0; i < RPT; ++i) {
-                const bool ok = m < M;
                 const int oy = row_of(rem, wo_magic);
                 const int ox = rem - oy * Wo;
-                const int iy = oy * p.sstride, ix = ox * p.sstride;
-                a_base[i] = (uint32_t)n * (uint32_t)p.src_img + (uint32_t)((iy * p.Ws + ix) * p.src_pitch + a_chunk * 4);
-                uint32_t bits = 0xffffffffu;
-                if (p.check) {
-                    bits = 0u;
-                    for (int t = 0; t < ntapsA; ++t)
-                        if ((unsigned)(iy + clsA->taps[t].dy) < (unsigned)p.Hs && (unsigned)(ix + clsA->taps[t].dx) < (unsigned)p.Ws) bits |= 1u << t;
-                }
-                a_taps[i] = ok ? bits : 0u;
-                m += 16; rem += 16;
+                iy[i] = oy * p.sstride; ix[i] = ox * p.sstride;
+                a_base[i] = (uint32_t)n * (uint32_t)p.src_img + (uint32_t)((iy[i] * p.Ws + ix[i]) * p.src_pitch + a_chunk * 4);
+                a_taps[i] = m < M ? 0xffffffffu : 0u;
+                m += RPP; rem += RPP;
                 while (rem >= HoWo) { rem -= HoWo; ++n; }
+            }
+            if (p.check) {
+                // taps outside, rows inside: a tap's displacement is read once for the thread's RPT rows
+                uint32_t in[RPT];
+#pragma unroll
+                for (int i = 0; i < RPT; ++i) in[i] = 0u;
+                for (int t = 0; t < ntapsA; ++t) {
+                    const int dy = clsA->taps[t].dy, dx = clsA->taps[t].dx;
+#pragma unroll
+                    for (int i = 0; i < RPT; ++i)
+                        if ((unsigned)(iy[i] + dy) < (unsigned)p.Hs && (unsigned)(ix[i] + dx) < (unsigned)p.Ws) in[i] |= 1u << t;
+                }
+#pragma unroll
+                for (int i = 0; i < RPT; ++i) a_taps[i] &= in[i];
             }
             if constexpr (KSPLIT) {
                 const int nkb = ntapsA * kb_per_tap;
@@ -256,7 +399,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             if (++sS == STAGES) { sS = 0; phS ^= 1u; }
         }
     } else {
-        // ================================ wgmma consumers + epilogue ================================
+        // ================================ wgmma consumers ================================
+        reg_grow<kConsumerRegs>();
         // warpgroup wg owns tile rows [64*wg, 64*wg + 64); thread layout of the accumulators: see wgmma_tf32
         constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
         const int wg = warp >> 2;
@@ -264,69 +408,6 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         float dm[HALF], dc[HALF];                    // chunk accumulators of the main and the cross terms (3 passes)
 #pragma unroll
         for (int i = 0; i < HALF; ++i) { acc[i] = 0.f; dm[i] = 0.f; dc[i] = 0.f; }
-
-        auto epilogue = [&](int st, int ks) {        // bias / ReLU / mask -> global, from the register accumulators
-            const TapClass& cls = p.cls[st_z(st)];
-            float* const dst = KSPLIT ? p.dst + (long long)ks * p.kpartial_stride : p.dst;
-            const int Wo = cls.Wo, HoWo = cls.Ho * Wo;
-            const int col0 = st_y(st) * BN + 2 * (lane & 3);
-            const int lcb = p.quad_lcb;              // log2(quad_cb)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const long long m = st_m0(st) + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-                if (m >= (long long)p.batch * HoWo) continue;
-                const int n = (int)(m / HoWo);
-                const int rem = (int)(m - (long long)n * HoWo);
-                const int oy = rem / Wo;
-                const int ox = rem - oy * Wo;
-                // destination float offsets fit 32 bits (checked at launch)
-                const uint32_t img = (uint32_t)n * (uint32_t)p.dst_img;
-                const uint32_t off_plain = img + (uint32_t)(((oy * p.dstride + cls.py) * p.Wd + (ox * p.dstride + cls.px)) * p.dst_pitch);
-                // groups of 4 column pairs, so that the ReLU-mask loads of a group are in flight together
-                constexpr int NG = BN / 8;
-                constexpr int GB = NG < 4 ? NG : 4;
-#pragma unroll
-                for (int j0 = 0; j0 < NG; j0 += GB) {
-                    uint32_t offs[GB];
-                    int chs[GB];
-                    bool oks[GB];
-                    float2 mks[GB];
-#pragma unroll
-                    for (int u = 0; u < GB; ++u) {
-                        const int col = col0 + (j0 + u) * 8;
-                        oks[u] = true;
-                        if (p.quad) {
-                            const int c = col >> lcb;
-                            chs[u] = col & (p.quad_cb - 1);
-                            const int y = oy * 2 + (c >> 1), x = ox * 2 + (c & 1);
-                            oks[u] = y < p.Hd && x < p.Wd;
-                            offs[u] = img + (uint32_t)((y * p.Wd + x) * p.dst_pitch + chs[u]);
-                        } else {
-                            chs[u] = col;
-                            offs[u] = off_plain + (uint32_t)col;
-                        }
-                    }
-                    if (p.mask) {
-#pragma unroll
-                        for (int u = 0; u < GB; ++u)
-                            mks[u] = oks[u] ? __ldg(reinterpret_cast<const float2*>(p.mask + offs[u])) : make_float2(0.f, 0.f);
-                    }
-#pragma unroll
-                    for (int u = 0; u < GB; ++u) {
-                        if (!oks[u]) continue;
-                        const int r = 4 * (j0 + u) + 2 * h;
-                        float2 o = make_float2(acc[r], acc[r + 1]);
-                        if (p.bias) {
-                            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + chs[u]));
-                            o.x += b.x; o.y += b.y;
-                        }
-                        if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-                        if (p.mask) { o.x = mks[u].x > 0.f ? o.x : 0.f; o.y = mks[u].y > 0.f ? o.y : 0.f; }
-                        *reinterpret_cast<float2*>(dst + offs[u]) = o;
-                    }
-                }
-            }
-        };
 
         // stage s is free in this CTA's consumers: lane r < CS arrives on the stage's empty barrier of cluster CTA r
         auto release = [&](int s) {
@@ -342,6 +423,24 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
         const uint32_t a_row = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + (lane & 3) * 4);
         const uint32_t a_swz = (uint32_t)((r0 & 7) << 4);
+
+        // The finished tile goes to the epilogue warps through the output buffer: acc[4*j + 2*h + c] is row r0 + 8*h,
+        // columns 8*j + 2*(lane%4) + c, i.e. bytes 8*(lane%4) of the 32-byte pair of chunks j XOR r0%4 (layout: see
+        // out_base).  The consumers then go straight on to the next item's first k-block.
+        const uint32_t o_dst = (uint32_t)(r0 * (BN * 4) + ((r0 & 3) << 5) + (lane & 3) * 8);
+        uint32_t phE = 1;                            // parity out_empty shows once free (fresh barrier: 1 counts as complete)
+        auto hand_off = [&]() {
+            mbar_wait(&out_empty, phE);
+            phE ^= 1u;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(out_base + (uint32_t)(h * 8 * BN * 4) + (o_dst ^ (uint32_t)(j << 5))),
+                                 "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1]) : "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&out_full);
+        };
 
         int g = 0;                                   // k-blocks consumed so far (all tiles)
         for (int w = cl_id; w < total_w; w += cl_n) {
@@ -413,7 +512,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                     }
                 }
             }
-            epilogue(st, ks);
+            if (!(p.debug & 16)) hand_off();         // timing decomposition: no epilogue
 #pragma unroll
             for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
         }
@@ -459,6 +558,11 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     CPB_REQUIRE(total_w < (1ll << 30) && resident > 0, "tc_tapgemm: bad tile count");
     CPB_REQUIRE(tc_offsets_fit(p.batch, p.src_img) && tc_offsets_fit(p.batch, p.dst_img),
                 "tc_tapgemm: tensors too large for 32-bit row offsets");
+    // the epilogue warps store (and read the bias and the ReLU mask) 16 bytes at a time
+    auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; };
+    CPB_REQUIRE(al16(p.dst) && al16(p.mask) && al16(p.bias) && p.dst_pitch % 4 == 0 && p.dst_img % 4 == 0 &&
+                    (p.ksplit == 1 || (al16(p.kpartial) && p.kpartial_stride % 4 == 0)),
+                "tc_tapgemm: destination, mask and bias must be 16-byte aligned");
     for (int c = 0; c < p.nclass; ++c) CPB_REQUIRE(p.cls[c].ntaps <= 32, "tc_tapgemm: more than 32 taps");
     if (p.quad) {
         CPB_REQUIRE((p.quad_cb & (p.quad_cb - 1)) == 0, "tc_tapgemm: quad form needs a power-of-two channel count");
