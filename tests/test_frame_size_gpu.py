@@ -193,6 +193,7 @@ class GeoCase(L.Case):
         h, w = hw
         self.s = sides(h, w)
         self.lib, self.mode, self.B, self.ct, self.z, self.zp = lib, mode, B, ct, z, 64 * ((z + 63) // 64)
+        self.frames = B
         self.j = L.Judge("%dx%d mode %d B=%d ct=%d z=%d" % (h, w, mode, B, ct, z))
         _lib.check(lib.cpb_set_math_mode(mode))
         wts = vo.glorot_init(B + 10 * ct + h, (h, w, 3), ct, z)
@@ -244,12 +245,17 @@ class GeoCase(L.Case):
         out["g"] = {"gA": ws[offs[L.BUFFERS.index("gA")]:], "gB": ws[offs[L.BUFFERS.index("gB")]:]} if offs[12] >= 0 else {}
         return out
 
-    def forward(self):
+    def forward(self, encode_only=False):
+        """encode_only: an encode call, its encoder passes and heads checked in the encode workspace."""
         from carla_ppo_b200 import _lib
-        self._poisoned(_lib.WS_FORWARD)
-        self.vae.forward_device(self.x, self.y, self.eps)
+        ws_mode = _lib.WS_ENCODE if encode_only else _lib.WS_FORWARD
+        self._poisoned(ws_mode)
+        if encode_only:
+            self.vae.encode_device(self.x)
+        else:
+            self.losses = self.vae.forward_device(self.x, self.y, self.eps)["losses"]
         torch.cuda.synchronize()
-        v = self._views(_lib.WS_FORWARD)
+        v = self._views(ws_mode)
         j, B, z, op, wt, s = self.j, self.B, self.z, self._op, self._wt, self.s
         R, relu = L.R, torch.relu
 
@@ -268,23 +274,25 @@ class GeoCase(L.Case):
                 return relu(r) if act else r
             return ref
 
-        L.check_frames(j, "conv1.fwd", v["a1"], conv("conv1", "xp", False), B)
-        L.check_frames(j, "conv2.fwd", v["a2"], conv("conv2", "a1", True), B)
-        L.check_frames(j, "conv3.fwd", v["a3"], conv("conv3", "a2", True), B)
-        L.check_frames(j, "conv4.fwd", v["a4"], conv("conv4", "a3", True), B)
+        L.check_frames(j, "conv1.fwd", v["a1"], conv("conv1", "xp", False), self.frames)
+        L.check_frames(j, "conv2.fwd", v["a2"], conv("conv2", "a1", True), self.frames)
+        L.check_frames(j, "conv3.fwd", v["a3"], conv("conv3", "a2", True), self.frames)
+        L.check_frames(j, "conv4.fwd", v["a4"], conv("conv4", "a3", True), self.frames)
         for i, (kn, bn) in enumerate((("mean/kernel", "mean/bias"), ("logstd_sqare/kernel", "logstd_sqare/bias"))):
             with self.feat_floor():
                 L.check_frames(j, "heads.fwd %d" % i, v["heads"][i, :, :z], lambda dt, f0, f1, kn=kn, bn=bn: (
-                    op(v["a4"], False, dt, f0, f1).reshape(f1 - f0, -1) @ wt(kn, False, dt) + self.w[bn].to(dt)), B)
+                    op(v["a4"], False, dt, f0, f1).reshape(f1 - f0, -1) @ wt(kn, False, dt) + self.w[bn].to(dt)), self.frames)
         if not bool((v["heads"][:, :, z:] == 0).all()):
             j.failures.append("heads.fwd %s: padded columns are not 0" % j.tag)
+        if encode_only:
+            return
         L.check_frames(j, "dense1.fwd", v["d1"], lambda dt, f0, f1: (
             R.dense1_fwd(op(v["z"], False, dt, f0, f1), wt("decoder/dense1/kernel", False, dt))
-            + self.w["decoder/dense1/bias"].to(dt)).reshape((f1 - f0,) + s[4] + (256,)), B)
-        L.check_frames(j, "deconv1.fwd", v["b1"], deconv("deconv1", "d1", True, s[3]), B)
-        L.check_frames(j, "deconv2.fwd", v["b2"], deconv("deconv2", "b1", True, s[2]), B)
-        L.check_frames(j, "deconv3.fwd", v["b3"], deconv("deconv3", "b2", True, s[1]), B)
-        L.check_frames(j, "deconv4.fwd", v["logits_p"][..., :self.ct], deconv("deconv4", "b3", False, s[0], act=False), B)
+            + self.w["decoder/dense1/bias"].to(dt)).reshape((f1 - f0,) + s[4] + (256,)), self.frames)
+        L.check_frames(j, "deconv1.fwd", v["b1"], deconv("deconv1", "d1", True, s[3]), self.frames)
+        L.check_frames(j, "deconv2.fwd", v["b2"], deconv("deconv2", "b1", True, s[2]), self.frames)
+        L.check_frames(j, "deconv3.fwd", v["b3"], deconv("deconv3", "b2", True, s[1]), self.frames)
+        L.check_frames(j, "deconv4.fwd", v["logits_p"][..., :self.ct], deconv("deconv4", "b3", False, s[0], act=False), self.frames)
 
     def _group_deconv4(self, v, grads):
         ct, op, wt, R = self.ct, self._op, self._wt, L.R
@@ -311,11 +319,11 @@ class GeoCase(L.Case):
         gin = self._grad_view(v["g"]["gB"], (B, feat))
         j.finite("dense1 input gradient", gin)
         L.check_reduction(j, "dense1.wgrad", grads["decoder/dense1/kernel"],
-                          lambda dt, f0, f1: op(v["z"], False, dt, f0, f1)[:, :z].T @ gin[f0:f1].to(dt), B, taps=False)
-        L.check_reduction(j, "dense1.bias", grads["decoder/dense1/bias"], lambda dt, f0, f1: gin[f0:f1].to(dt).sum(0), B, taps=False)
+                          lambda dt, f0, f1: op(v["z"], False, dt, f0, f1)[:, :z].T @ gin[f0:f1].to(dt), self.frames, taps=False)
+        L.check_reduction(j, "dense1.bias", grads["decoder/dense1/bias"], lambda dt, f0, f1: gin[f0:f1].to(dt).sum(0), self.frames, taps=False)
         with self.feat_floor():
             L.check_frames(j, "dense1.dgrad", v["gz"][:, :z],
-                           lambda dt, f0, f1: gin[f0:f1].to(dt) @ wt("decoder/dense1/kernel", False, dt).T, B)
+                           lambda dt, f0, f1: gin[f0:f1].to(dt) @ wt("decoder/dense1/kernel", False, dt).T, self.frames)
         if not bool((v["gz"][:, z:] == 0).all()):
             j.failures.append("dense1.dgrad %s: padded columns of gz are not 0" % j.tag)
 
@@ -326,13 +334,13 @@ class GeoCase(L.Case):
         a4 = v["a4"].reshape(B, -1)
         for i, name in enumerate(("mean", "logstd_sqare")):
             L.check_reduction(j, "heads.wgrad (%s)" % name, grads[name + "/kernel"],
-                              lambda dt, f0, f1, i=i: a4[f0:f1].to(dt).T @ gh[i, f0:f1, :z].to(dt), B, taps=False)
+                              lambda dt, f0, f1, i=i: a4[f0:f1].to(dt).T @ gh[i, f0:f1, :z].to(dt), self.frames, taps=False)
             L.check_reduction(j, "heads.bias (%s)" % name, grads[name + "/bias"],
-                              lambda dt, f0, f1, i=i: gh[i, f0:f1, :z].to(dt).sum(0), B, taps=False)
+                              lambda dt, f0, f1, i=i: gh[i, f0:f1, :z].to(dt).sum(0), self.frames, taps=False)
         out = self._grad_view(v["g"]["gA"], self.shape(4, 256))
         L.check_frames(j, "heads.dgrad", out, lambda dt, f0, f1: (
             L.R.heads_dgrad(gh[:, f0:f1].to(dt), wt("mean/kernel", False, dt), wt("logstd_sqare/kernel", False, dt))
-            .reshape((f1 - f0,) + self.s[4] + (256,)) * (v["a4"][f0:f1] > 0)), B)
+            .reshape((f1 - f0,) + self.s[4] + (256,)) * (v["a4"][f0:f1] > 0)), self.frames)
 
     def _group_conv4(self, v, grads):
         self._enc_group(v, grads, "conv4", "gA", self.shape(4, 256), "a3", "gB", self.shape(3, 128))

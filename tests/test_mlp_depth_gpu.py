@@ -78,8 +78,9 @@ def buffer_names(vae):
             ["g%d" % j for j in range(len(vae.decoder_sizes))] + ["logits", "ga", "gb"])
 
 
-def read_ws(vae, batch, ws_mode, widths):
-    """Named buffers of the last call that used workspace `ws_mode`, read back from the device as [batch, width]."""
+def read_ws(vae, batch, ws_mode, widths, frames=None, host=True):
+    """Named buffers of the last call that used workspace `ws_mode`, read back from the device as [batch, width] float64
+    arrays -- only the rows `frames` when given; host=False: the float32 device views, all rows."""
     import torch
     from carla_ppo_b200 import _lib
     names = buffer_names(vae)
@@ -90,16 +91,19 @@ def read_ws(vae, batch, ws_mode, widths):
     out = {}
     for nm, width in widths.items():
         o = offs[names.index(nm)]
-        out[nm] = ws[o:o + 4 * batch * width].view(torch.float32).cpu().numpy().astype(np.float64).reshape(batch, width)
+        t = ws[o:o + 4 * batch * width].view(torch.float32).view(batch, width)
+        if host:
+            t = (t if frames is None else t[frames]).cpu().numpy().astype(np.float64)
+        out[nm] = t
     return out
 
 
-def relu_masks(vae, batch):
-    """The device's ReLU activity pattern of every hidden layer after a loss_grad call."""
+def relu_masks(vae, batch, frames=None):
+    """The device's ReLU activity pattern of every hidden layer after a loss_grad call (of the rows `frames` if given)."""
     from carla_ppo_b200 import _lib
     widths = {"h%d" % i: v for i, v in enumerate(vae.encoder_sizes)}
     widths.update({"g%d" % j: v for j, v in enumerate(vae.decoder_sizes)})
-    return {k: v > 0 for k, v in read_ws(vae, batch, _lib.WS_TRAIN, widths).items()}
+    return {k: v > 0 for k, v in read_ws(vae, batch, _lib.WS_TRAIN, widths, frames).items()}
 
 
 def _gate(approx, ref):
@@ -173,6 +177,41 @@ def test_mode_2_matches_float64_within_twice_the_tf32_restatement(tmp_path, lib,
     _check_model(tmp_path, lib, shape, case, _lib.MATH_TF32)
 
 
+def forward_products(vae, w, batch, frames=None):
+    """After a mode-2 forward call: the first encoder layer's and the output layer's forward products on the device's
+    own rows (`frames`, or all) against the fp32-summed product of the rounded operands -> {name: rel err}."""
+    from carla_ppo_b200 import _lib
+    r = round_tf32
+    enc, dec = vae.encoder_sizes, vae.decoder_sizes
+    out_name = "decoder/dense_%d" % len(dec)
+    last = "g%d" % (len(dec) - 1)
+    t = read_ws(vae, batch, _lib.WS_FORWARD, {"x": IN, "h0": enc[0], last: dec[-1], "logits": IN}, frames)
+    return {"first encoder layer fwd": rel_l2(t["h0"], np.maximum(r(t["x"]) @ r(w["encoder/dense/kernel"]) + w["encoder/dense/bias"], 0.0)),
+            "output layer fwd": rel_l2(t["logits"], r(t[last]) @ r(w[out_name + "/kernel"]) + w[out_name + "/bias"])}
+
+
+def backward_products(vae, w, batch, frames=None):
+    """After a mode-2 loss_grad call: the first encoder layer's and the output layer's weight gradients, and the output
+    layer's data gradient through the weight gradient of the last hidden decoder layer (which the fp32 SIMT kernels
+    compute from it), against the same products over the rows `frames` (all of them when None; a batch whose other
+    rows are exactly 0 otherwise) -> {name: rel err}."""
+    from carla_ppo_b200 import _lib
+    r = round_tf32
+    enc, dec = vae.encoder_sizes, vae.decoder_sizes
+    out_name = "decoder/dense_%d" % len(dec)
+    last = "g%d" % (len(dec) - 1)
+    got = vae.get_grads()
+    below = "z" if len(dec) == 1 else "g%d" % (len(dec) - 2)
+    t = read_ws(vae, batch, _lib.WS_TRAIN, {"x": IN, below: 64 if len(dec) == 1 else dec[-2], last: dec[-1], "logits": IN,
+                                            "gb": enc[0]}, frames)
+    dlog = t["logits"]                             # d loss / d logits after loss_grad
+    g_last = (r(dlog) @ r(w[out_name + "/kernel"]).T) * (t[last] > 0)
+    return {"first encoder layer wgrad": rel_l2(got["encoder/dense/kernel"], r(t["x"]).T @ r(t["gb"])),
+            "output layer wgrad": rel_l2(got[out_name + "/kernel"], r(t[last]).T @ r(dlog)),
+            "output layer dgrad": rel_l2(got["decoder/dense_%d/kernel" % (len(dec) - 1) if len(dec) > 1 else "decoder/dense/kernel"],
+                                         t[below].T @ g_last)}
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("batch", [6, 512])
 @pytest.mark.parametrize("shape", sorted(SHAPES))
@@ -181,35 +220,18 @@ def test_mode_2_frame_wide_products_on_the_devices_own_inputs(tmp_path, lib, sha
     fp32-summed product of the rounded operands; the output layer's data gradient through the weight gradient of the
     last hidden decoder layer, which the fp32 SIMT kernels compute from it."""
     from carla_ppo_b200 import _lib
-    r = round_tf32
     enc, dec = SHAPES[shape]
     _lib.check(lib.cpb_set_math_mode(_lib.MATH_TF32))
     w = mlp_weights(1, encoder_sizes=enc, decoder_sizes=dec)
     vae = make_mlp(tmp_path, w, enc, dec)
     x, _, eps = inputs(batch)
-    out_name = "decoder/dense_%d" % len(dec)
-    last = "g%d" % (len(dec) - 1)
     vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps))
-    t = read_ws(vae, batch, _lib.WS_FORWARD, {"x": IN, "h0": enc[0], last: dec[-1], "logits": IN})
-    assert np.array_equal(t["x"], x.reshape(batch, -1))
-    err = rel_l2(t["h0"], np.maximum(r(t["x"]) @ r(w["encoder/dense/kernel"]) + w["encoder/dense/bias"], 0.0))
-    assert err < UNIT_TOL, ("first encoder layer fwd", err)
-    err = rel_l2(t["logits"], r(t[last]) @ r(w[out_name + "/kernel"]) + w[out_name + "/bias"])
-    assert err < UNIT_TOL, ("output layer fwd", err)
-
+    assert np.array_equal(read_ws(vae, batch, _lib.WS_FORWARD, {"x": IN})["x"], x.reshape(batch, -1))
+    for what, err in forward_products(vae, w, batch).items():
+        assert err < UNIT_TOL, (what, err)
     vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
-    got = vae.get_grads()
-    below = "z" if len(dec) == 1 else "g%d" % (len(dec) - 2)
-    t = read_ws(vae, batch, _lib.WS_TRAIN, {"x": IN, below: 64 if len(dec) == 1 else dec[-2], last: dec[-1], "logits": IN,
-                                            "gb": enc[0]})
-    dlog = t["logits"]                             # d loss / d logits after loss_grad
-    err = rel_l2(got["encoder/dense/kernel"], r(t["x"]).T @ r(t["gb"]))
-    assert err < UNIT_TOL, ("first encoder layer wgrad", err)
-    err = rel_l2(got[out_name + "/kernel"], r(t[last]).T @ r(dlog))
-    assert err < UNIT_TOL, ("output layer wgrad", err)
-    g_last = (r(dlog) @ r(w[out_name + "/kernel"]).T) * (t[last] > 0)
-    err = rel_l2(got["decoder/dense_%d/kernel" % (len(dec) - 1) if len(dec) > 1 else "decoder/dense/kernel"], t[below].T @ g_last)
-    assert err < UNIT_TOL, ("output layer dgrad", err)
+    for what, err in backward_products(vae, w, batch).items():
+        assert err < UNIT_TOL, (what, err)
 
 
 @pytest.mark.gpu

@@ -26,6 +26,7 @@ pytestmark = pytest.mark.gpu
 
 FLOOR = 2e-6
 CHUNK = 256          # frames per reference evaluation (the float64 im2col of deconv3's data gradient: 1.1 GB)
+ZCHUNK = 1 << 26     # elements per step of Judge.zeros
 
 # Batches and the edge each hits (M = B x positions per frame; tile and split rules in tapgemm.cu, tc_tapgemm.cu,
 # wgrad.cu, tc_wgrad.cu):
@@ -85,6 +86,22 @@ class Judge:
         self.tag = tag
         self.failures = []
         self.worst = {}
+        self.live = None
+
+    def zeros(self, what, t):
+        """Placed-frame batches (self.live: the sorted live frames): every null frame of t [B, ...] exactly 0 (a NaN
+        left by a missed write is not 0), every live frame finite.  Reduced per frame, in chunks, on the device."""
+        live = torch.zeros(t.shape[0], dtype=torch.bool, device=t.device)
+        live[self.live] = True
+        step = max(1, ZCHUNK // max(1, t[0].numel()))
+        for f0 in range(0, t.shape[0], step):
+            c = t[f0:f0 + step].reshape(min(step, t.shape[0] - f0), -1)
+            bad = torch.where(live[f0:f0 + step], ~torch.isfinite(c).all(1), (c != 0).any(1))
+            if bool(bad.any()):
+                frames = (torch.nonzero(bad)[:, 0] + f0).tolist()
+                self.failures.append("%s %s: frames %s%s are %s" % (what, self.tag, frames[:8], " ..." if len(frames) > 8 else "",
+                                     "not finite (live)" if frames[0] in self.live else "not 0 (null frame)"))
+                return
 
     def finite(self, what, t):
         if not bool(torch.isfinite(t).all()):
@@ -115,14 +132,24 @@ def _sq(a, b, dims):
     return (d * d).sum(dims)
 
 
+def spans(frames):
+    """The frame ranges (f0, f1) a check visits: chunks of CHUNK frames over a whole batch of `frames`, or the given list
+    of ranges (the live frames of a placed-frame batch)."""
+    if isinstance(frames, int):
+        return [(f0, min(frames, f0 + CHUNK)) for f0 in range(0, frames, CHUNK)]
+    return frames
+
+
 def check_frames(j, what, dev, ref, B):
     """dev: the device's [B, ...] output; ref(dtype, f0, f1): the reference for frames f0:f1.  Gates the whole tensor,
-    every frame and, for images, the first / last row and column of every frame."""
+    every frame and, for images, the first / last row and column of every frame, over the frames spans(B) names; in a
+    placed-frame batch (j.live) every other frame must be exactly 0."""
     image = dev.dim() == 4
     names = ["frame"] + (["first row", "last row", "first column", "last column"] if image else [])
     sums = {n: [[], [], []] for n in names}
-    for f0 in range(0, B, CHUNK):
-        f1 = min(B, f0 + CHUNK)
+    if j.live is not None:
+        j.zeros(what, dev)
+    for f0, f1 in spans(B):
         d = dev[f0:f1]
         j.finite(what, d)
         r64 = ref(torch.float64, f0, f1)
@@ -146,11 +173,10 @@ def check_frames(j, what, dev, ref, B):
 
 def check_reduction(j, what, dev, ref, B, taps):
     """dev: the device's weight or bias gradient; ref(dtype, f0, f1): the contribution of frames f0:f1 (summed over
-    the chunks in that dtype).  Gates the whole tensor and, for a conv kernel [k, k, Cb, Cs], every tap block."""
+    spans(B) in that dtype: in a placed-frame batch, whose null frames contribute exactly 0, the live frames alone).  Gates the whole tensor and, for a conv kernel [k, k, Cb, Cs], every tap block."""
     j.finite(what, dev)
     r64 = r32 = 0
-    for f0 in range(0, B, CHUNK):
-        f1 = min(B, f0 + CHUNK)
+    for f0, f1 in spans(B):
         r64 = r64 + ref(torch.float64, f0, f1)
         r32 = r32 + ref(torch.float32, f0, f1)
     dims = tuple(range(dev.dim()))
@@ -160,11 +186,14 @@ def check_reduction(j, what, dev, ref, B, taps):
 
 
 class Case:
+    dgrad = True         # False: backward() checks the weight and bias gradients only (the reductions over the batch)
+
     def __init__(self, lib, tmp_path, mode, B, ct, z):
         from carla_ppo_b200 import _lib
         from carla_ppo_b200.vae.models import ConvVAE
         from oracle import vae_oracle as vo
         self.lib, self.mode, self.B, self.ct, self.z, self.zp = lib, mode, B, ct, z, 64 * ((z + 63) // 64)
+        self.frames = B      # what the checks visit (spans): the whole batch, or the live frames of a placed-frame batch
         self.j = Judge("mode %d B=%d ct=%d z=%d" % (mode, B, ct, z))
         _lib.check(lib.cpb_set_math_mode(mode))
         w = vo.glorot_init(B + 10 * ct, target_channels=ct, z_dim=z)
@@ -230,7 +259,7 @@ class Case:
     def forward(self):
         from carla_ppo_b200 import _lib
         self._poisoned(_lib.WS_FORWARD)
-        self.vae.forward_device(self.x, self.y, self.eps)
+        self.losses = self.vae.forward_device(self.x, self.y, self.eps)["losses"]
         torch.cuda.synchronize()
         v = self._views(_lib.WS_FORWARD)
         j, B, z, op, wt = self.j, self.B, self.z, self._op, self._wt
@@ -251,26 +280,26 @@ class Case:
                 return relu(r) if act else r
             return ref
 
-        check_frames(j, "conv1.fwd", v["a1"], conv("conv1", "xp", False), B)
-        check_frames(j, "conv2.fwd", v["a2"], conv("conv2", "a1", True), B)
-        check_frames(j, "conv3.fwd", v["a3"], conv("conv3", "a2", True), B)
-        check_frames(j, "conv4.fwd", v["a4"], conv("conv4", "a3", True), B)
+        check_frames(j, "conv1.fwd", v["a1"], conv("conv1", "xp", False), self.frames)
+        check_frames(j, "conv2.fwd", v["a2"], conv("conv2", "a1", True), self.frames)
+        check_frames(j, "conv3.fwd", v["a3"], conv("conv3", "a2", True), self.frames)
+        check_frames(j, "conv4.fwd", v["a4"], conv("conv4", "a3", True), self.frames)
 
         def heads(i):
             kn, bn = ("mean/kernel", "mean/bias") if i == 0 else ("logstd_sqare/kernel", "logstd_sqare/bias")
             return lambda dt, f0, f1: op(v["a4"], False, dt, f0, f1).reshape(f1 - f0, -1) @ wt(kn, False, dt) + self.w[bn].to(dt)
-        check_frames(j, "heads.fwd (mean)", v["heads"][0, :, :z], heads(0), B)
-        check_frames(j, "heads.fwd (logstd_sq)", v["heads"][1, :, :z], heads(1), B)
+        check_frames(j, "heads.fwd (mean)", v["heads"][0, :, :z], heads(0), self.frames)
+        check_frames(j, "heads.fwd (logstd_sq)", v["heads"][1, :, :z], heads(1), self.frames)
         if not bool((v["heads"][:, :, z:] == 0).all()):
             j.failures.append("heads.fwd %s: padded columns are not 0" % j.tag)
 
         check_frames(j, "dense1.fwd", v["d1"], lambda dt, f0, f1: (
             R.dense1_fwd(op(v["z"], False, dt, f0, f1), wt("decoder/dense1/kernel", False, dt))
-            + self.w["decoder/dense1/bias"].to(dt)).reshape(f1 - f0, 3, 8, 256), B)
-        check_frames(j, "deconv1.fwd", v["b1"], deconv("deconv1", "d1", True, (8, 18)), B)
-        check_frames(j, "deconv2.fwd", v["b2"], deconv("deconv2", "b1", True, (18, 38)), B)
-        check_frames(j, "deconv3.fwd", v["b3"], deconv("deconv3", "b2", True, (39, 79)), B)
-        check_frames(j, "deconv4.fwd", v["logits_p"][..., :self.ct], deconv("deconv4", "b3", False, (80, 160), act=False), B)
+            + self.w["decoder/dense1/bias"].to(dt)).reshape(f1 - f0, 3, 8, 256), self.frames)
+        check_frames(j, "deconv1.fwd", v["b1"], deconv("deconv1", "d1", True, (8, 18)), self.frames)
+        check_frames(j, "deconv2.fwd", v["b2"], deconv("deconv2", "b1", True, (18, 38)), self.frames)
+        check_frames(j, "deconv3.fwd", v["b3"], deconv("deconv3", "b2", True, (39, 79)), self.frames)
+        check_frames(j, "deconv4.fwd", v["logits_p"][..., :self.ct], deconv("deconv4", "b3", False, (80, 160), act=False), self.frames)
 
     # -------------------------------------------------------------- backward
     def backward(self):
@@ -295,11 +324,11 @@ class Case:
         input gradient gin, and (if given) the data gradient dgrad = (device output, ref)."""
         j, B, k = self.j, self.B, self.w[prefix + "/kernel"].shape[0]
         check_reduction(j, name + ".wgrad", grads[prefix + "/kernel"],
-                        lambda dt, f0, f1: R.wgrad(*wgrad_ops(dt, f0, f1), k), B, taps=True)
+                        lambda dt, f0, f1: R.wgrad(*wgrad_ops(dt, f0, f1), k), self.frames, taps=True)
         check_reduction(j, name + ".bias", grads[prefix + "/bias"],
-                        lambda dt, f0, f1: gin[f0:f1].to(dt).sum((0, 1, 2)), B, taps=False)
-        if dgrad is not None:
-            check_frames(j, name + ".dgrad", dgrad[0], dgrad[1], B)
+                        lambda dt, f0, f1: gin[f0:f1].to(dt).sum((0, 1, 2)), self.frames, taps=False)
+        if dgrad is not None and self.dgrad:
+            check_frames(j, name + ".dgrad", dgrad[0], dgrad[1], self.frames)
 
     def _group_deconv4(self, v, grads):
         ct, op, wt, B = self.ct, self._op, self._wt, self.B
@@ -337,10 +366,11 @@ class Case:
         gin = self._grad_view(v["g"]["gB"], (B, 6144))
         j.finite("dense1 input gradient", gin)
         check_reduction(j, "dense1.wgrad", grads["decoder/dense1/kernel"],
-                        lambda dt, f0, f1: op(v["z"], False, dt, f0, f1)[:, :z].T @ gin[f0:f1].to(dt), B, taps=False)
-        check_reduction(j, "dense1.bias", grads["decoder/dense1/bias"], lambda dt, f0, f1: gin[f0:f1].to(dt).sum(0), B, taps=False)
-        check_frames(j, "dense1.dgrad", v["gz"][:, :z],
-                     lambda dt, f0, f1: gin[f0:f1].to(dt) @ wt("decoder/dense1/kernel", False, dt).T, B)
+                        lambda dt, f0, f1: op(v["z"], False, dt, f0, f1)[:, :z].T @ gin[f0:f1].to(dt), self.frames, taps=False)
+        check_reduction(j, "dense1.bias", grads["decoder/dense1/bias"], lambda dt, f0, f1: gin[f0:f1].to(dt).sum(0), self.frames, taps=False)
+        if self.dgrad:
+            check_frames(j, "dense1.dgrad", v["gz"][:, :z],
+                         lambda dt, f0, f1: gin[f0:f1].to(dt) @ wt("decoder/dense1/kernel", False, dt).T, self.frames)
         if not bool((v["gz"][:, z:] == 0).all()):
             j.failures.append("dense1.dgrad %s: padded columns of gz are not 0" % j.tag)
 
@@ -351,13 +381,14 @@ class Case:
         a4 = v["a4"].reshape(B, -1)
         for i, name in enumerate(("mean", "logstd_sqare")):
             check_reduction(j, "heads.wgrad (%s)" % name, grads[name + "/kernel"],
-                            lambda dt, f0, f1, i=i: a4[f0:f1].to(dt).T @ gh[i, f0:f1, :z].to(dt), B, taps=False)
+                            lambda dt, f0, f1, i=i: a4[f0:f1].to(dt).T @ gh[i, f0:f1, :z].to(dt), self.frames, taps=False)
             check_reduction(j, "heads.bias (%s)" % name, grads[name + "/bias"],
-                            lambda dt, f0, f1, i=i: gh[i, f0:f1, :z].to(dt).sum(0), B, taps=False)
+                            lambda dt, f0, f1, i=i: gh[i, f0:f1, :z].to(dt).sum(0), self.frames, taps=False)
         out = self._grad_view(v["g"]["gA"], (B, 3, 8, 256))
-        check_frames(j, "heads.dgrad", out, lambda dt, f0, f1: (
+        if self.dgrad:
+            check_frames(j, "heads.dgrad", out, lambda dt, f0, f1: (
             R.heads_dgrad(gh[:, f0:f1].to(dt), wt("mean/kernel", False, dt), wt("logstd_sqare/kernel", False, dt))
-            .reshape(f1 - f0, 3, 8, 256) * (v["a4"][f0:f1] > 0)), B)
+            .reshape(f1 - f0, 3, 8, 256) * (v["a4"][f0:f1] > 0)), self.frames)
 
     def _enc_group(self, v, grads, name, gin_name, gin_shape, src, out_name, out_shape):
         op, wt, B = self._op, self._wt, self.B
