@@ -7,17 +7,9 @@ import re
 
 import numpy as np
 import pytest
+from harness import lib, library_state  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
 
 
 def header_functions():

@@ -3,24 +3,15 @@ cpb_vae_spec_* layout against the oracle's variable shapes, the legacy 80x160 en
 refusals that happen before any memory is touched, the oracle's backward against torch autograd away from 80x160, and
 the Python classes' constructor rule.  No compute entry point reaches the device here."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 from helpers import rel_l2
+from harness import lib, library_state, math_mode  # noqa: F401
 
 SIDES = list(range(48, 513, 16))
 FAKE = 0x1000          # never dereferenced: every call below must be refused before it touches memory
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
 
 
 def spec_of(h, w, batch=1, ct=3, z=64, loss=0):
@@ -174,9 +165,7 @@ def test_batch_bound_table():
 def test_batch_over_the_bound_is_refused_before_any_launch(lib, hw, mode):
     h, w = hw
     bound = tc_bound(h, w)
-    old = lib.cpb_get_math_mode()
-    assert lib.cpb_set_math_mode(mode) == 0
-    try:
+    with math_mode(lib, mode):
         before = lib.cpb_launch_count()
         for name, call in _compute_calls(lib, spec_of(h, w, batch=bound + 1)).items():
             assert call() == -4, name                                       # CPB_ERR_UNSUPPORTED
@@ -192,18 +181,12 @@ def test_batch_over_the_bound_is_refused_before_any_launch(lib, hw, mode):
         assert lib.cpb_launch_count() == before
         # the query calls take any batch: they do not depend on the math mode
         assert lib.cpb_vae_spec_workspace_bytes(C.byref(spec_of(h, w, batch=bound + 1)), 2) > 0
-    finally:
-        lib.cpb_set_math_mode(old)
 
 
 def test_mode_0_takes_batches_above_the_tensor_core_bound(lib):
-    old = lib.cpb_get_math_mode()
-    assert lib.cpb_set_math_mode(0) == 0
-    try:
+    with math_mode(lib, 0):
         sp = spec_of(512, 512, batch=tc_bound(512, 512) + 1)
         assert lib.cpb_vae_spec_encode(C.byref(sp), FAKE, FAKE, FAKE, None, None, FAKE, 0, None) not in (0, -4)
-    finally:
-        lib.cpb_set_math_mode(old)
 
 
 @pytest.mark.parametrize("hw", [(48, 48), (64, 96), (112, 208)])

@@ -7,13 +7,14 @@ import numpy as np
 import pytest
 
 from helpers import committed_frames, rel_l2, shipped_vae_weights
+from ppo_cases import shipped_vae, train_params
 
 pytestmark = pytest.mark.gpu
 
 RGB_DIR = "rgb_bce_cnn_zdim64_beta1_kl_tolerance0.0_data"
 
 
-def lay_out_shipped_vae(root):
+def lay_outshipped_vae(root):
     """Writes the shipped rgb checkpoint-232 (committed golden npz) as a TF-V2 tensor bundle under the reference's
     directory convention vae/models/<name>/checkpoints/model.ckpt-232.* + the ``checkpoint`` state file."""
     from carla_ppo_b200.tf_bundle import write_bundle
@@ -47,7 +48,7 @@ def test_vae_common_load_and_encode_state(tmp_path):
     uint8 observations and preprocess_frame()'d float observations (reference vae_common.py:6-62)."""
     from carla_ppo_b200 import vae_common
     from oracle import vae_oracle as vo
-    model_dir = lay_out_shipped_vae(str(tmp_path))
+    model_dir = lay_outshipped_vae(str(tmp_path))
     vae = vae_common.load_vae(model_dir, z_dim=None, model_type=None)
     assert vae.z_dim == 64 and vae.target_shape == (80, 160, 3) and vae.training is False
     assert vae.get_step_idx() == 232
@@ -99,31 +100,13 @@ def test_checkpoints_written_in_tf_format_round_trip(tmp_path):
 
 
 # ----------------------------------------------------------------------------- train.py / run_eval.py over the replay env
-def _train_params(name, **over):
-    p = dict(learning_rate=1e-4, lr_decay=1.0, discount_factor=0.99, gae_lambda=0.95, ppo_epsilon=0.2, initial_std=0.4,
-             value_scale=1.0, entropy_scale=0.01, horizon=16, num_epochs=2, num_episodes=2, batch_size=8,
-             vae_model="unused", vae_model_type=None, vae_z_dim=None, synchronous=True, fps=30, action_smoothing=0.0,
-             model_name=name, reward_fn="reward_speed_centering_angle_multiply", seed=0, eval_interval=1, record_eval=False,
-             logging=False)
-    p.update(over)
-    return p
-
-
-def _shipped_vae(tmp_path, tag):
-    from carla_ppo_b200.vae.models import ConvVAE
-    vae = ConvVAE(source_shape=(80, 160, 3), z_dim=64, model_dir=str(tmp_path / ("vae_" + tag)), training=False, seed=0)
-    vae.init_session(init_logging=False)
-    vae.set_weights(shipped_vae_weights()[0])
-    return vae
-
-
 def _run_training(tmp_path, tag, **over):
     from carla_ppo_b200.replay_env import ReplayEnv
     from carla_ppo_b200.train import train
     rgb, _ = committed_frames()
     env = ReplayEnv(rgb, episode_length=24, seed=0)
-    vae = _shipped_vae(tmp_path, tag)
-    model = train(_train_params(tag, **over), restart=False, env=env, vae=vae, models_root=str(tmp_path / "models"), interactive=False)
+    vae = shipped_vae(tmp_path, tag)
+    model = train(train_params(tag, **over), restart=False, env=env, vae=vae, models_root=str(tmp_path / "models"), interactive=False)
     return model, env
 
 
@@ -202,7 +185,7 @@ def test_run_eval_is_greedy_and_deterministic(tmp_path):
     from carla_ppo_b200.vae_common import create_encode_state_fn
     from helpers import shipped_ppo
     rgb, _ = committed_frames()
-    vae = _shipped_vae(tmp_path, "eval")
+    vae = shipped_vae(tmp_path, "eval")
     env = ReplayEnv(rgb, episode_length=20, seed=3)
     model = PPO((67,), env.action_space, model_dir=str(tmp_path / "agent"), seed=0)
     model.init_session(init_logging=False)

@@ -1,20 +1,11 @@
 """The large-batch cases without a GPU: where the live frames of a placed-frame batch sit, and the batches and workspace
 sizes of every case of tests/test_large_batch_gpu.py."""
 import ctypes as C
-import os
 
 import pytest
 
 import large_batch as LB
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
+from harness import lib, library_state, math_mode  # noqa: F401
 
 
 def base(batch, ct=3, z=64):
@@ -24,15 +15,11 @@ def base(batch, ct=3, z=64):
 
 def workspace_bytes(lib, case, mode):
     from carla_ppo_b200 import _lib
-    old = lib.cpb_get_math_mode()
-    assert lib.cpb_set_math_mode(mode) == 0
-    try:
+    with math_mode(lib, mode):
         if "hw" in case:
             return lib.cpb_vae_spec_workspace_bytes(C.byref(_lib.VaeSpec(base(case["batch"]), *case["hw"])), case["ws"])
         spec = _lib.MlpVaeSpec.of(base(case["batch"]), *case["mlp"])
         return lib.cpb_mlpvae_spec_workspace_bytes(C.byref(spec), case["ws"])
-    finally:
-        lib.cpb_set_math_mode(old)
 
 
 def test_live_frames_at_80x160():

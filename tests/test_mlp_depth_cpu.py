@@ -4,7 +4,6 @@ legacy ones, malformed specs are refused before anything launches, and the any-d
 matches torch autograd and, at two layers per side, oracle.vae_oracle and the TF32 restatement bit for bit.  No compute
 entry point runs a kernel here."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -12,21 +11,11 @@ import pytest
 import mlp_depth_oracle as mdo
 import mlp_tf32_oracle
 from helpers import rel_l2
+from harness import lib, library_state, math_mode  # noqa: F401
 
 DEFAULT = ((512, 256), (256, 512))
 SHAPES = {"1x1": ((512,), (512,)), "3x2": ((1024, 512, 256), (256, 512)),
           "8x8": ((256, 224, 192, 160, 128, 96, 64, 32), (32, 64, 96, 128, 160, 192, 224, 256))}
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    lib = _lib.load()
-    yield lib
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
 
 
 def _base(batch, ct=3, z=64):
@@ -89,15 +78,14 @@ def test_two_per_side_spec_is_the_legacy_model(lib, z, ct):
         assert offs == list(lo) and sizes == list(ls) and total == lt.value
         assert shapes == [tuple(s for s in lsh[4 * i:4 * i + 4] if s > 0) for i in range(n)]
         for mode in (_lib.MATH_SIMT, _lib.MATH_3XTF32, _lib.MATH_TF32):
-            _lib.check(lib.cpb_set_math_mode(mode))
-            for ws in range(3):
-                a = lib.cpb_mlpvae_spec_workspace_bytes(C.byref(spec), ws)
-                assert a > 0 and a == lib.cpb_mlpvae_workspace_bytes(C.byref(cfg), ws), (mode, ws)
-                so = (C.c_int64 * 10)(); lo2 = (C.c_int64 * 10)()
-                assert lib.cpb_debug_mlpvae_spec_buffer_offsets(C.byref(spec), ws, so, 10) == 10
-                assert lib.cpb_debug_mlpvae_buffer_offsets(C.byref(cfg), ws, lo2, 10) == 10
-                assert list(so) == list(lo2)
-        _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
+            with math_mode(lib, mode):
+                for ws in range(3):
+                    a = lib.cpb_mlpvae_spec_workspace_bytes(C.byref(spec), ws)
+                    assert a > 0 and a == lib.cpb_mlpvae_workspace_bytes(C.byref(cfg), ws), (mode, ws)
+                    so = (C.c_int64 * 10)(); lo2 = (C.c_int64 * 10)()
+                    assert lib.cpb_debug_mlpvae_spec_buffer_offsets(C.byref(spec), ws, so, 10) == 10
+                    assert lib.cpb_debug_mlpvae_buffer_offsets(C.byref(cfg), ws, lo2, 10) == 10
+                    assert list(so) == list(lo2)
 
 
 def test_buffer_offsets_name_every_hidden_layer(lib):

@@ -2,25 +2,14 @@
 nothing is rounded and rounds exactly the five frame-wide products; the workspace grows by exactly the TF32 weight
 images and split partials in mode 2 and not at all in modes 0 and 1.  No compute entry point is called here."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 import mlp_tf32_oracle
+from harness import lib, library_state, math_mode  # noqa: F401
 
 IN, TBK, WAVE = 38400, 32, 132
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    lib = _lib.load()
-    yield lib
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
 
 
 def _cfg(batch, ct=3, z=64, sizes=(512, 256, 256, 512)):
@@ -92,9 +81,8 @@ def test_workspace_grows_by_the_tf32_images_and_partials_in_mode_2_only(lib, bat
     cfg = _cfg(batch, ct, z, sizes)
     size = {}
     for mode in (_lib.MATH_SIMT, _lib.MATH_3XTF32, _lib.MATH_TF32):
-        _lib.check(lib.cpb_set_math_mode(mode))
-        size[mode] = [lib.cpb_mlpvae_workspace_bytes(C.byref(cfg), ws) for ws in range(3)]
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
+        with math_mode(lib, mode):
+            size[mode] = [lib.cpb_mlpvae_workspace_bytes(C.byref(cfg), ws) for ws in range(3)]
     assert size[_lib.MATH_SIMT] == size[_lib.MATH_3XTF32]
     for ws in range(3):
         assert size[_lib.MATH_TF32][ws] - size[_lib.MATH_3XTF32][ws] == _mode2_extra(batch, ct, sizes, ws), ws
@@ -105,12 +93,11 @@ def test_buffer_offsets_hook_names_the_mlp_buffers_and_ignores_the_math_mode(lib
     cfg = _cfg(16)
     got = {}
     for mode in (_lib.MATH_3XTF32, _lib.MATH_TF32):
-        _lib.check(lib.cpb_set_math_mode(mode))
-        for ws in range(3):
-            offs = (C.c_int64 * 10)()
-            assert lib.cpb_debug_mlpvae_buffer_offsets(C.byref(cfg), ws, offs, 10) == 10
-            got[mode, ws] = list(offs)
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
+        with math_mode(lib, mode):
+            for ws in range(3):
+                offs = (C.c_int64 * 10)()
+                assert lib.cpb_debug_mlpvae_buffer_offsets(C.byref(cfg), ws, offs, 10) == 10
+                got[mode, ws] = list(offs)
     for ws in range(3):
         assert got[_lib.MATH_3XTF32, ws] == got[_lib.MATH_TF32, ws]
     x, h1, h2, heads, z, g1, g2, logits, ga, gb = got[_lib.MATH_3XTF32, 2]

@@ -4,25 +4,12 @@ parameters; gradients <= max(2 x fp32-CPU-restatement error, 2e-5) per tensor.""
 import numpy as np
 import pytest
 
-from helpers import Box, rel_l2, shipped_ppo
+from helpers import rel_l2, shipped_ppo
+from ppo_cases import HIGH, LOW, baseline_config3, make_ppo
 
 pytestmark = pytest.mark.gpu
 
-LOW, HIGH = np.array([-1.0, 0.0]), np.array([1.0, 1.0])
 TOL = 1e-5
-
-
-def make_ppo(tmp_path, policy=None, old=None, **kw):
-    from carla_ppo_b200.ppo import PPO
-    kw.setdefault("learning_rate", 1e-4)
-    kw.setdefault("value_scale", 1.0)
-    kw.setdefault("entropy_scale", 0.01)
-    kw.setdefault("epsilon", 0.2)
-    m = PPO((67,), Box(LOW, HIGH), model_dir=str(tmp_path / "ppo"), seed=0, **kw)
-    m.init_session(init_logging=False)
-    if policy is not None:
-        m.set_weights(policy, old if old is not None else policy)
-    return m
 
 
 def rollout(T, seed=0):
@@ -146,20 +133,6 @@ def test_checkpoint_round_trip_and_lr_decay(tmp_path):
     assert all(np.array_equal(w1[k], w2[k]) for k in w1)
 
 
-def _baseline_config3(T=2048, E=4):
-    """SURVEY section 8(d) config 3 / BASELINE configs[2]: T=2048 rollout, 4 epochs x 8 minibatches of 256,
-    shipped agent ckpt-705 (policy, policy_old, warm Adam slots and beta powers), permutations from RandomState(0)."""
-    rs = np.random.RandomState(0)
-    states = rs.randn(T, 67).astype(np.float32)
-    actions = np.clip(rs.randn(T, 2), LOW, HIGH).astype(np.float32)
-    rewards = rs.rand(T)
-    values = rs.randn(T).astype(np.float32)
-    dones = np.zeros(T, bool); dones[-1] = True
-    prs = np.random.RandomState(0)
-    perms = np.stack([prs.permutation(T) for _ in range(E)])
-    return states, actions, rewards, values, dones, perms
-
-
 def test_learn_at_baseline_config3_matches_oracle(tmp_path):
     """The driver's update block (reference train.py:171-207) at EXACTLY BASELINE configs[2]: parameters, theta_old and
     the 32 per-minibatch losses vs the float64 restatement; gate = max(1e-5, 2 x the error of the float32 CPU
@@ -173,7 +146,7 @@ def test_learn_at_baseline_config3_matches_oracle(tmp_path):
     m = make_ppo(tmp_path, pol, old)
     m.set_weights(pol, old, adam_m, adam_v, powers)
     T, E, B = 2048, 4, 256
-    s, a, r, v, d, perms = _baseline_config3(T, E)
+    s, a, r, v, d, perms = baseline_config3(T, E)
     metrics = m.learn(s, a, v, r, d, 0.3, gamma=0.99, lam=0.95, num_epochs=E, batch_size=B, perms=perms, return_metrics=True)
 
     def restate(dtype):
@@ -223,13 +196,13 @@ def test_persistent_learn_kernel_matches_launch_per_kernel_path(tmp_path):
     snippet = r"""
 import sys, numpy as np
 sys.path.insert(0, %r); sys.path.insert(0, %r)
-import test_ppo_gpu as t
+import ppo_cases as t
 from helpers import shipped_ppo
 from pathlib import Path
 pol, z = shipped_ppo("policy")
 m = t.make_ppo(Path(%r), pol, pol)
 m.set_weights(pol, pol, {k: z["adam_m/" + k] for k in pol}, {k: z["adam_v/" + k] for k in pol}, (float(z["beta1_power"]), float(z["beta2_power"])))
-s, a, r, v, d, perms = t._baseline_config3(2048, 2)
+s, a, r, v, d, perms = t.baseline_config3(2048, 2)
 m.learn(s, a, v, r, d, 0.3, num_epochs=2, batch_size=200, perms=perms)       # ragged last minibatch (2048 = 10 x 200 + 48)
 np.savez(%r, **m.get_weights())
 """

@@ -9,34 +9,12 @@ import numpy as np
 import pytest
 
 import single_env_train
+from harness import lib, library_state  # noqa: F401
 from helpers import Box
-from test_ppo_shapes_cpu import _cfg
+from ppo_cases import ppo_config, segment_inputs, segmented_gae
 
 
 # ------------------------------------------------------------------------------------------------ float64 restatement
-def segmented_gae(rewards, values, bootstrap_values, dones, lengths, gamma, lam):
-    """oracle compute_gae on each segment, concatenated; returns = A + V; advantages normalised once over all rows
-    (train.py:175-177).  -> (returns, normalised advantages, advantages), float64."""
-    from oracle import ppo_oracle as po
-    offs = np.concatenate([[0], np.cumsum(lengths)]).astype(int)
-    adv = np.concatenate([po.compute_gae(np.asarray(rewards)[a:b], np.asarray(values)[a:b], bootstrap_values[s],
-                                         np.asarray(dones)[a:b], gamma, lam)
-                          for s, (a, b) in enumerate(zip(offs[:-1], offs[1:]))])
-    returns = adv + np.asarray(values, np.float64)
-    return returns, (adv - adv.mean()) / (adv.std() + 1e-8), adv
-
-
-def segment_inputs(lengths, seed=0):
-    """rewards, values, dones over the concatenated segments and one bootstrap value per segment.  Every other segment
-    ends in a terminal, and a few rows inside segments carry done = 1 (the reference masks their bootstrap term and does
-    not reset the accumulation)."""
-    rs = np.random.RandomState(seed)
-    rows = int(np.sum(lengths))
-    rewards, values = rs.rand(rows), rs.randn(rows)
-    dones = (rs.rand(rows) < 0.02).astype(np.float64)
-    ends = np.cumsum(lengths) - 1
-    dones[ends] = np.arange(len(lengths)) % 2 == 0
-    return rewards, values, rs.randn(len(lengths)), dones
 
 
 def test_one_segment_is_the_single_rollout_computation_bit_for_bit():
@@ -62,15 +40,6 @@ def test_segments_do_not_leak_into_each_other():
 
 
 # ------------------------------------------------------------------------------------------------ C ABI refusals
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
-
-
 FAKE = 0x1000          # never dereferenced: every call below must be refused before it touches memory
 
 
@@ -109,14 +78,14 @@ def _learn_args(cfg, **over):
                          + [{k: None} for k in LEARN_POINTERS],
                          ids=lambda d: "_".join("%s%s" % kv for kv in d.items()))
 def test_learn_segments_refuses_bad_arguments_without_a_launch(lib, over):
-    cfg = _cfg(67, 2, 500, 300)
+    cfg = ppo_config(67, 2, 500, 300)
     before = lib.cpb_launch_count()
     assert lib.cpb_ppo_learn_segments(*_learn_args(cfg, **over)) == -1
     assert lib.cpb_launch_count() == before
 
 
 def test_learn_segments_refuses_a_small_workspace(lib):
-    cfg = _cfg(67, 2, 500, 300)
+    cfg = ppo_config(67, 2, 500, 300)
     need = lib.cpb_ppo_workspace_bytes(C.byref(cfg), 16, 40)
     args = list(_learn_args(cfg))
     args[-2] = need - 1

@@ -9,11 +9,15 @@ import types
 import numpy as np
 import pytest
 
+from harness import lib, library_state, make_conv_vae, make_mlp, math_mode  # noqa: F401
 from helpers import committed_frames, rel_l2, shipped_ppo, shipped_vae_weights
-from test_ppo_gpu import LOW, HIGH, TOL, _baseline_config3, make_ppo
-from test_ppo_segments_cpu import segment_inputs, segmented_gae
+from ppo_cases import (HIGH, LOW, baseline_config3, make_ppo, segment_inputs, segmented_gae, shipped_vae,
+                       train_params)
+from vae_checks import mlp_weights
 
 pytestmark = pytest.mark.gpu
+
+TOL = 1e-5             # tests/test_ppo_gpu.py's
 
 LENGTHS = (1, 31, 32, 33, 1023, 1024, 1025, 4097)
 
@@ -69,7 +73,7 @@ def _state(m):
 _SNIPPET = r"""
 import sys, numpy as np
 sys.path.insert(0, %r); sys.path.insert(0, %r)
-import test_ppo_gpu as t
+import ppo_cases as t
 from helpers import shipped_ppo
 from pathlib import Path
 pol, z = shipped_ppo("policy")
@@ -78,7 +82,7 @@ out = {}
 for tag, seg in (("one", None), ("seg", [2048])):
     m = t.make_ppo(Path(%r) / tag, pol, old)
     m.set_weights(pol, old, {k: z["adam_m/" + k] for k in pol}, {k: z["adam_v/" + k] for k in pol}, (float(z["beta1_power"]), float(z["beta2_power"])))
-    s, a, r, v, d, perms = t._baseline_config3(2048, 2)
+    s, a, r, v, d, perms = t.baseline_config3(2048, 2)
     last = 0.3 if seg is None else [0.3]
     met = m.learn(s, a, v, r, d, last, num_epochs=2, batch_size=200, perms=perms, return_metrics=True, segment_lengths=seg)
     for k, x in dict(params=m.params, old=m.params_old, m=m.adam_m, v=m.adam_v, powers=m.adam_powers).items():
@@ -135,7 +139,7 @@ def test_learn_segments_match_the_oracle(tmp_path, lengths, E, B):
     m = make_ppo(tmp_path, pol, old)
     m.set_weights(pol, old, *adam)
     T = int(np.sum(lengths))
-    s, a, r, v, _, perms = _baseline_config3(T, E)
+    s, a, r, v, _, perms = baseline_config3(T, E)
     d = np.zeros(T, bool)
     ends = np.cumsum(lengths) - 1
     d[ends[::2]] = True                                     # every other segment ends in a terminal
@@ -170,13 +174,8 @@ def _fake_envs(n):
 
 def _vae(tmp_path, kind):
     if kind == "conv":
-        from carla_ppo_b200.vae.models import ConvVAE
-        vae = ConvVAE(source_shape=(80, 160, 3), z_dim=64, model_dir=str(tmp_path / "vae"), training=False, seed=0)
-        vae.init_session(init_logging=False)
-        vae.set_weights(shipped_vae_weights()[0])
-        return vae
-    from test_mlp_depth_gpu import SHAPES, make_mlp, mlp_weights
-    enc, dec = SHAPES["3x2"]
+        return make_conv_vae(tmp_path, shipped_vae_weights()[0], loss="bce", tag="vae", training=False)
+    enc, dec = (96, 256, 64), (160, 64)
     return make_mlp(tmp_path, mlp_weights(2, encoder_sizes=enc, decoder_sizes=dec), enc, dec, tag="vec", training=False)
 
 
@@ -192,18 +191,15 @@ def _oracle_mean(vae, kind, frames):
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("kind", ["conv", "mlp"])
 @pytest.mark.parametrize("n", [2, 8, 33])
-def test_batched_encode_predict(tmp_path, n, kind, mode):
+def test_batched_encode_predict(tmp_path, lib, n, kind, mode):
     """FusedActor.encode_predict at B = n: bit for bit the batched unfused calls (one vae.encode, one ppo.predict, the same
     noise), latents within max(1e-5, 2 x the single-frame calls' error) of float64, and actions / values within 1e-5 of
     the oracle's PPO on the device's states with the same noise."""
-    from carla_ppo_b200 import _lib
     from carla_ppo_b200.actor import FusedActor, UnfusedActor
     from carla_ppo_b200.ppo import PPO
     from oracle import ppo_oracle as po
     from helpers import Box
-    lib = _lib.load()
-    _lib.check(lib.cpb_set_math_mode(mode))
-    try:
+    with math_mode(lib, mode):
         vae = _vae(tmp_path, kind)
         meas = ("steer", "throttle", "speed")
         models = []
@@ -228,12 +224,9 @@ def test_batched_encode_predict(tmp_path, n, kind, mode):
         p64 = {k: w.astype(np.float64) for k, w in shipped_ppo("policy")[0].items()}
         ract, rval = po.predict(p64, np.stack(fs).astype(np.float32), LOW, HIGH, noise=noise)
         assert rel_l2(fa, ract) < TOL and rel_l2(fv, rval) < TOL
-    finally:
-        _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
 
 
 # ------------------------------------------------------------------------------------------------ train.train --num_envs
-from test_integration_gpu import _shipped_vae, _train_params       # noqa: E402
 
 
 def _train(tmp_path, tag, num_envs, fn=None, **over):
@@ -241,8 +234,8 @@ def _train(tmp_path, tag, num_envs, fn=None, **over):
     from carla_ppo_b200.train import train
     rgb, _ = committed_frames()
     envs = [ReplayEnv(rgb, episode_length=24 + 5 * i, seed=0) for i in range(num_envs)]
-    vae = _shipped_vae(tmp_path, tag)
-    params = _train_params(tag, num_envs=num_envs, **over)
+    vae = shipped_vae(tmp_path, tag)
+    params = train_params(tag, num_envs=num_envs, **over)
     model = (fn or train)(params, restart=False, env=envs if fn is None else envs[0], vae=vae,
                           models_root=str(tmp_path / "models"), interactive=False)
     return model, envs

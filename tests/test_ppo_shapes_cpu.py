@@ -1,170 +1,15 @@
 """The PPO at every shape the C ABI accepts, without a GPU: the float64 oracle against torch autograd at each shape of
-CASES on inputs where the clipped surrogate takes both branches, the weight initialiser and input builders that
-tests/test_ppo_shapes_gpu.py uses, and the parameter layout / workspace queries at A = 1..4 and odd sizes."""
+CASES on inputs where the clipped surrogate takes both branches, the weight initialiser and input builders
+(tests/ppo_cases.py), and the parameter layout / workspace queries at A = 1..4 and odd sizes."""
 import ctypes as C
-import os
-from collections import OrderedDict
 
 import numpy as np
 import pytest
 
+from harness import lib, library_state  # noqa: F401
 from helpers import Box, rel_l2
-
-# name -> (state_dim, num_actions, hidden1, hidden2).  state_dim = z_dim + measurements (train.py: z_dim any multiple of 4
-# in [4, 1024], 0-6 measurements); the small GEMM reads the first-layer reduction in 64-wide chunks.
-CASES = OrderedDict([
-    ("z4", (7, 2, 500, 300)),               # smallest latent + 3 measurements: one partial chunk
-    ("z100_orient", (106, 2, 500, 300)),    # z not a multiple of 64, all 6 measurements
-    ("z1024", (1027, 2, 500, 300)),         # largest latent: 17 chunks
-    ("a1", (67, 1, 500, 300)),              # one action
-    ("a3_z32", (35, 3, 500, 300)),          # three actions, asymmetric bounds
-    ("a4", (67, 4, 500, 300)),              # the head kernel's kMaxActions
-    ("tiny", (1, 4, 1, 1)),                 # K = 1, one-wide trunks
-    ("odd", (65, 3, 33, 31)),               # one over and one under a 32-wide tile
-    ("wide", (130, 2, 1024, 512)),          # many tiles per GEMM
-])
-
-# every action gets its own bounds, so that a mixed-up action index changes the result
-LOW4 = np.array([-1.0, 0.0, -2.0, 0.5])
-HIGH4 = np.array([1.0, 1.0, 0.5, 3.0])
-CLIP_LO, CLIP_HI = float(np.float32(0.8)), float(np.float32(1.2))   # the graph's float32 clip constants (epsilon 0.2)
-KINK_MARGIN = 1e-4
-# make_batch shifts of the old policy that put about a fifth of the rows in each branch of the clipped surrogate
-CLIPPED = dict(mean_shift=0.2, logstd_shift=0.05)
-
-
-def bounds(num_actions):
-    return LOW4[:num_actions].copy(), HIGH4[:num_actions].copy()
-
-
-def init_params(state_dim, num_actions, hidden1, hidden2, seed=0, initial_std=0.4):
-    """PPO._initial_weights at any (S, A, H1, H2): glorot-uniform kernels, zero biases, the action-mean kernel from
-    variance_scaling(0.1) truncated normal, action_logstd = log(initial_std); same RandomState draws in the same order."""
-    from oracle.ppo_oracle import param_shapes
-    rng = np.random.RandomState(seed)
-    out = OrderedDict()
-    for name, shape in param_shapes(state_dim, num_actions, (hidden1, hidden2), (hidden1, hidden2)).items():
-        if name == "action_logstd":
-            out[name] = np.full(shape, np.log(initial_std), np.float32)
-        elif name.endswith("bias"):
-            out[name] = np.zeros(shape, np.float32)
-        elif name == "action_mean/kernel":
-            std = np.sqrt(0.1 / shape[0]) / 0.87962566103423978
-            t = rng.randn(*shape)
-            bad = np.abs(t) > 2
-            while bad.any():
-                t[bad] = rng.randn(int(bad.sum()))
-                bad = np.abs(t) > 2
-            out[name] = (t * std).astype(np.float32)
-        else:
-            limit = np.sqrt(6.0 / (shape[0] + shape[1]))
-            out[name] = rng.uniform(-limit, limit, size=shape).astype(np.float32)
-    return out
-
-
-TRUNKS = (("dense/kernel", "dense/bias", "dense_1/kernel", "dense_1/bias"),
-          ("dense_2/kernel", "dense_2/bias", "dense_3/kernel", "dense_3/bias"))
-
-
-def _gap_bias(z):
-    """Per column of z [n, H]: a float32 bias b in the middle of the widest gap of the sorted -z, so that z + b is as far
-    from zero as the rows allow.  The gap is looked for where a quarter to three quarters of the rows are active; where
-    that window has no usable gap (e.g. a column whose inactive-input rows are all exactly 0), over all interior gaps."""
-    n = z.shape[0]
-    u = np.sort(-z, axis=0)
-    if n < 4:
-        return (u[-1] + 0.5).astype(np.float32)       # every row active, 0.5 from the kink
-    cols = np.arange(z.shape[1])
-    gaps = u[1:] - u[:-1]
-    lo, hi = (n - 1) // 4, n - 1 - (n - 1) // 4
-    i = lo + np.argmax(gaps[lo:hi], axis=0)
-    narrow = gaps[i, cols] < 4 * KINK_MARGIN
-    i = np.where(narrow, np.argmax(gaps, axis=0), i)
-    return ((u[i, cols] + u[i + 1, cols]) / 2).astype(np.float32)
-
-
-def pre_activations(p, states):
-    """The four trunk pre-activations in float64 (the oracle's forward takes no ReLU masks of its own)."""
-    s = np.asarray(states, np.float64)
-    out = []
-    for w1, b1, w2, b2 in TRUNKS:
-        z1 = s @ p[w1].astype(np.float64) + p[b1]
-        z2 = np.maximum(z1, 0.0) @ p[w2].astype(np.float64) + p[b2]
-        out += [z1, z2]
-    return out
-
-
-def relu_margin(p, states):
-    return min(float(np.abs(z).min()) for z in pre_activations(p, states))
-
-
-def place_biases(params, states):
-    """params with the four trunk biases chosen so that no pre-activation on `states` lies near a ReLU kink."""
-    p = {k: v.copy() for k, v in params.items()}
-    s = np.asarray(states, np.float64)
-    for w1, b1, w2, b2 in TRUNKS:
-        z = s @ p[w1].astype(np.float64)
-        p[b1] = _gap_bias(z)
-        z = np.maximum(z + p[b1], 0.0) @ p[w2].astype(np.float64)
-        p[b2] = _gap_bias(z)
-    return p
-
-
-def clip_groups(ratio, adv):
-    """Row masks of the five branches of min(r * adv, clip(r, 0.8, 1.2) * adv)."""
-    r, a = np.asarray(ratio).ravel(), np.asarray(adv).ravel()
-    below, above = r < CLIP_LO, r > CLIP_HI
-    return OrderedDict([("below_pos", below & (a > 0)), ("below_neg", below & (a < 0)),
-                        ("above_pos", above & (a > 0)), ("above_neg", above & (a < 0)), ("inside", ~below & ~above)])
-
-
-def near_clip_bound(ratio):
-    """Rows whose ratio lies within 1e-4 relative of a float32 clip bound, where a float32 rounding could flip the branch."""
-    r = np.asarray(ratio).ravel()
-    return (np.abs(r / CLIP_LO - 1) < 1e-4) | (np.abs(r / CLIP_HI - 1) < 1e-4)
-
-
-def make_batch(params, batch, seed, mean_shift=0.02, logstd_shift=0.0):
-    """(p, old, states, actions, returns, advantages) for one loss evaluation.  p = params with kink-free trunk biases on
-    these states; old = p with action_mean/bias shifted by +-mean_shift and action_logstd by logstd_shift; actions drawn
-    around the midpoint of the two policies' means (clipped to the bounds), so the log-ratio takes both signs.  The default
-    mean_shift keeps the ratios near 1 (at 3-4 actions a few rows in a hundred leave the clip range), CLIPPED fills all
-    five branches.  Rows whose ratio lands near a clip bound are redrawn.  Returns lie above each state's value, so the
-    value-bias gradient (2 / B) sum(v - ret) cannot cancel: a cancelled sum turns the float32 rounding of v into an
-    arbitrary relative error (standard-normal returns cancelled it 126-fold at z100_orient, B = 9)."""
-    from oracle import ppo_oracle as po
-    S, A = params["dense/kernel"].shape[0], params["action_logstd"].shape[0]
-    low, high = bounds(A)
-    rs = np.random.RandomState(seed)
-    n = batch
-    s = rs.randn(n, S).astype(np.float32)
-    p = place_biases(params, s)
-    old = {k: v.copy() for k, v in p.items()}
-    old["action_mean/bias"] = (p["action_mean/bias"] + mean_shift * np.array([1.0, -1.0, 1.0, -1.0])[:A]).astype(np.float32)
-    old["action_logstd"] = (p["action_logstd"] + logstd_shift).astype(np.float32)
-    mu, value = po.forward({k: v.astype(np.float64) for k, v in p.items()}, s, low, high)
-    mu_old, _ = po.forward({k: v.astype(np.float64) for k, v in old.items()}, s, low, high)
-    mid, sigma = (mu + mu_old) / 2, np.exp(p["action_logstd"].astype(np.float64))
-    a = np.clip(mid + sigma * rs.randn(n, A), low, high).astype(np.float32)
-    ret = (value + 0.5 + np.abs(rs.randn(n))).astype(np.float32)
-    adv = rs.randn(n).astype(np.float32)
-    for _ in range(20):
-        ratio = po.loss_and_grads(p, old, s, a, ret, adv, low, high, want_grads=False)["ratio"]
-        bad = near_clip_bound(ratio)
-        if not bad.any():
-            break
-        a[bad] = np.clip(mid[bad] + sigma * rs.randn(int(bad.sum()), A), low, high).astype(np.float32)
-    return p, old, s, a, ret, adv
-
-
-def loss_refs(p, old, s, a, ret, adv, low, high, epsilon=0.2):
-    """float64 oracle and the float32 autograd restatement (whose distance from float64 sets the gradient gates)."""
-    import torch
-    from oracle import ppo_oracle as po, torch_ref
-    ref = po.loss_and_grads(p, old, s, a, ret, adv, low, high, epsilon, 1.0, 0.01)
-    ref32 = torch_ref.ppo_loss_and_grads(p, old, s, a, ret, adv, low, high, epsilon, 1.0, 0.01, dtype=torch.float32)
-    return ref, ref32
-
+from ppo_cases import (CASES, CLIPPED, KINK_MARGIN, bounds, clip_groups, init_params, make_batch, ppo_config,
+                       pre_activations, relu_margin)
 
 # ------------------------------------------------------------------------------------------------------------ tests
 @pytest.mark.parametrize("case", list(CASES))
@@ -214,26 +59,6 @@ def test_biases_keep_pre_activations_off_the_relu_kink(case):
                 assert (z > 0).any(axis=0).all() and (z < 0).any(axis=0).all(), batch
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
-
-
-def _cfg(S, A, H1, H2):
-    from carla_ppo_b200 import _lib
-    cfg = _lib.PpoConfig()
-    cfg.state_dim, cfg.num_actions, cfg.hidden1, cfg.hidden2 = S, A, H1, H2
-    low, high = bounds(max(1, min(A, 4)))
-    for k in range(len(low)):
-        cfg.action_low[k], cfg.action_high[k] = low[k], high[k]
-    cfg.epsilon, cfg.value_scale, cfg.entropy_scale = 0.2, 1.0, 0.01
-    return cfg
-
-
 LAYOUT_SHAPES = list(CASES.values()) + [(67, 1, 500, 300), (67, 3, 500, 300), (2, 4, 3, 2), (1030, 1, 1, 7)]
 
 
@@ -241,7 +66,7 @@ LAYOUT_SHAPES = list(CASES.values()) + [(67, 1, 500, 300), (67, 3, 500, 300), (2
 def test_layout_matches_oracle_shapes(lib, shape):
     from oracle.ppo_oracle import param_shapes, PPO_TENSORS
     S, A, H1, H2 = shape
-    cfg = _cfg(*shape)
+    cfg = ppo_config(*shape)
     n = lib.cpb_ppo_num_tensors()
     offs = (C.c_int64 * n)(); sizes = (C.c_int64 * n)(); shapes = (C.c_int32 * (2 * n))(); total = C.c_int64()
     assert lib.cpb_ppo_layout(C.byref(cfg), offs, sizes, shapes, C.byref(total)) == 0
@@ -263,7 +88,7 @@ def test_layout_and_workspace_refuse_bad_shapes(lib, bad):
     from carla_ppo_b200 import _lib
     shape = dict(S=67, A=2, H1=500, H2=300)
     shape.update(bad)
-    cfg = _cfg(shape["S"], shape["A"], shape["H1"], shape["H2"])
+    cfg = ppo_config(shape["S"], shape["A"], shape["H1"], shape["H2"])
     total = C.c_int64(-7)
     assert lib.cpb_ppo_layout(C.byref(cfg), None, None, None, C.byref(total)) == -1      # CPB_ERR_INVALID_ARGUMENT
     assert total.value == -7                                                             # nothing written
@@ -274,7 +99,7 @@ def test_layout_and_workspace_refuse_bad_shapes(lib, bad):
 
 def test_workspace_grows_with_batch_and_horizon(lib):
     for shape in (CASES["a4"], CASES["tiny"], CASES["wide"]):
-        cfg = C.byref(_cfg(*shape))
+        cfg = C.byref(ppo_config(*shape))
         # sizes are rounded up to an alignment, so neighbouring batch sizes may share one
         by_batch = [lib.cpb_ppo_workspace_bytes(cfg, b, 0) for b in (1, 2, 9, 256, 8192, 8200, 20000)]
         assert by_batch[0] > 0 and all(x <= y for x, y in zip(by_batch, by_batch[1:])), by_batch
@@ -287,5 +112,5 @@ def test_workspace_grows_with_batch_and_horizon(lib):
         assert base < by_horizon[1] < by_horizon[2] < by_horizon[3], by_horizon
         assert lib.cpb_ppo_workspace_bytes(cfg, 0, 0) == -1
         assert lib.cpb_ppo_workspace_bytes(cfg, 64, -1) == -1
-    big = lib.cpb_ppo_workspace_bytes(C.byref(_cfg(*CASES["wide"])), 8200, 8200)
+    big = lib.cpb_ppo_workspace_bytes(C.byref(ppo_config(*CASES["wide"])), 8200, 8200)
     assert 0 < big < 1 << 30

@@ -14,9 +14,9 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import Box, rel_l2
-from test_ppo_shapes_cpu import (CASES, CLIPPED, KINK_MARGIN, bounds, clip_groups, init_params, loss_refs, make_batch,
-                                 near_clip_bound, place_biases, relu_margin)
+from helpers import rel_l2
+from ppo_cases import (CASES, CLIPPED, KINK_MARGIN, PERSISTENT, bounds, clip_groups, init_params, learn_setup, loss_refs,
+                       make_batch, make_ppo, near_clip_bound, place_biases, relu_margin, warm_adam)
 
 pytestmark = pytest.mark.gpu
 
@@ -42,40 +42,6 @@ class Worst:
         print("\nGATE %s: worst %s %.3e of gate %.3e" % (name, self.what, self.err, self.gate))
 
 
-def make_ppo(tmp_path, shape, policy, old=None, **kw):
-    """The PPO class at hidden widths other than the reference's 500 / 300: everything but the config is shape-generic
-    (it reads cpb_ppo_layout)."""
-    from carla_ppo_b200.ppo import PPO
-    S, A, H1, H2 = shape
-
-    class ShapedPPO(PPO):
-        def _cfg(self):
-            cfg = super()._cfg()
-            cfg.hidden1, cfg.hidden2 = H1, H2
-            return cfg
-
-    kw.setdefault("learning_rate", 1e-4)
-    kw.setdefault("value_scale", 1.0)
-    kw.setdefault("entropy_scale", 0.01)
-    kw.setdefault("epsilon", 0.2)
-    m = ShapedPPO((S,), Box(*bounds(A)), model_dir=str(tmp_path / "ppo"), seed=0, **kw)
-    m.init_session(init_logging=False)
-    m.set_weights(policy, old if old is not None else policy)
-    return m
-
-
-def warm_adam(params, grads, seed):
-    """Adam slots and beta powers of a resumed run, scaled to these gradients: from zero slots the first update is
-    lr * g / (|g| + 1e-8), which moves elements with |g| ~ 1e-8 by an arbitrary fraction of lr in any float32 arithmetic."""
-    rs = np.random.RandomState(seed)
-    m, v = {}, {}
-    for k, g in grads.items():
-        scale = np.sqrt(np.mean(np.square(g))) + 1e-12
-        m[k] = (0.5 * scale * rs.uniform(-1, 1, g.shape)).astype(np.float32)
-        v[k] = (np.square(np.abs(g) + scale) * rs.uniform(0.5, 2.0, g.shape)).astype(np.float32)
-    return m, v, (float(np.float32(0.9 ** 50)), float(np.float32(0.999 ** 50)))
-
-
 def check_loss(worst, metrics, grads, ref, ref32, label):
     for got, key in zip(metrics, METRICS):
         gate = max(TOL * max(abs(ref[key]), 1e-3), 2 * abs(ref32[key] - ref[key]))
@@ -94,7 +60,7 @@ def test_predict_matches_oracle(tmp_path, case):
     S, A = shape[:2]
     low, high = bounds(A)
     p = place_biases(init_params(*shape, seed=1), np.random.RandomState(2).randn(33, S))
-    m = make_ppo(tmp_path, shape, p)
+    m = make_ppo(tmp_path, p, shape=shape)
     p64 = {k: v.astype(np.float64) for k, v in p.items()}
     worst, hit_low, hit_high = Worst(), False, False
     for b in (1, 9, 33):
@@ -122,7 +88,7 @@ def test_loss_and_gradients_match_oracle(tmp_path, case):
     low, high = bounds(shape[1])
     p, old, s, a, ret, adv = make_batch(init_params(*shape, seed=5), 256, seed=6)
     assert relu_margin(p, s) > KINK_MARGIN
-    m = make_ppo(tmp_path, shape, p, old)
+    m = make_ppo(tmp_path, p, old, shape=shape)
     worst = Worst()
     for b in (1, 8, 9, 256):                # B = 9: one row in the head kernel's second CTA
         metrics, grads = m.loss_and_grads(s[:b], a[:b], ret[:b], adv[:b])
@@ -137,7 +103,7 @@ def test_loss_and_gradients_beyond_8192_rows(tmp_path):
     low, high = bounds(2)
     p, old, s, a, ret, adv = make_batch(init_params(*DEFAULT, seed=7), 8200, seed=8)
     assert relu_margin(p, s) > KINK_MARGIN
-    m = make_ppo(tmp_path, DEFAULT, p, old)
+    m = make_ppo(tmp_path, p, old, shape=DEFAULT)
     metrics, grads = m.loss_and_grads(s, a, ret, adv)
     worst = Worst()
     check_loss(worst, metrics, grads, *loss_refs(p, old, s, a, ret, adv, low, high), "B=8200")
@@ -157,7 +123,7 @@ def test_clipped_surrogate_both_branches(tmp_path, case):
     groups = clip_groups(ref["ratio"], adv)
     assert all(g.mean() >= 0.1 for g in groups.values()), {k: float(g.mean()) for k, g in groups.items()}
     assert not near_clip_bound(ref["ratio"]).any()
-    m = make_ppo(tmp_path, shape, p, old)
+    m = make_ppo(tmp_path, p, old, shape=shape)
     metrics, grads = m.loss_and_grads(s, a, ret, adv)
     worst = Worst()
     check_loss(worst, metrics, grads, ref, ref32, "clipped")
@@ -181,7 +147,7 @@ def test_loss_grad_with_row_gather(tmp_path, case):
     p, old, s, a, ret, adv = make_batch(init_params(*shape, seed=13), T, seed=14, **CLIPPED)
     idx = np.random.RandomState(15).randint(0, T, B).astype(np.int32)
     assert len(np.unique(idx)) < B and (np.diff(idx) < 0).any() and idx.max() >= B
-    m = make_ppo(tmp_path, shape, p, old)
+    m = make_ppo(tmp_path, p, old, shape=shape)
     dev = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(m._device)
     sd, ad, rd, vd, ixd = dev(s), dev(a), dev(ret), dev(adv), dev(idx)
     metrics = torch.empty(5, dtype=torch.float32, device=m._device)
@@ -214,7 +180,7 @@ def test_two_train_steps_match_oracle(tmp_path, case):
     p, old, s, a, ret, adv = make_batch(init_params(*shape, seed=17), 64, seed=18, **CLIPPED)
     assert relu_margin(p, s) > KINK_MARGIN
     m_, v_, powers = warm_adam(p, po.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)["grads"], 19)
-    m = make_ppo(tmp_path, shape, p, old)
+    m = make_ppo(tmp_path, p, old, shape=shape)
     m.set_weights(p, old, m_, v_, powers)
     for _ in range(2):
         m.train(s, a, ret, adv)
@@ -231,33 +197,6 @@ def test_two_train_steps_match_oracle(tmp_path, case):
         worst.check(rel_l2(got[name], p64[name]), max(TOL, 2 * rel_l2(p32[name], p64[name])), name)
     assert m.get_train_step_idx() == 2
     worst.report(case)
-
-
-def rollout(shape, T, seed):
-    """A rollout of the policy with kink-free trunk biases on its states, terminals in the middle (not at the end)."""
-    S, A = shape[:2]
-    low, high = bounds(A)
-    rs = np.random.RandomState(seed)
-    s = rs.randn(T, S).astype(np.float32)
-    p = place_biases(init_params(*shape, seed=seed + 1), s)
-    from oracle import ppo_oracle as po
-    mu, _ = po.forward({k: v.astype(np.float64) for k, v in p.items()}, s, low, high)
-    a = np.clip(mu + np.exp(p["action_logstd"].astype(np.float64)) * rs.randn(T, A), low, high).astype(np.float32)
-    r = rs.rand(T)
-    v = rs.randn(T).astype(np.float32)
-    d = np.zeros(T, bool)
-    d[T // 3] = d[(2 * T) // 3] = True
-    return p, s, a, r, v, d
-
-
-def learn_setup(shape, T, batch, epochs, seed):
-    from oracle import ppo_oracle as po
-    p, s, a, r, v, d = rollout(shape, T, seed)
-    perms = np.stack([np.random.RandomState(seed + 10 + e).permutation(T) for e in range(epochs)])
-    ret, adv_n, _ = po.returns_and_normalised_advantages(r, v, 0.3, d, 0.99, 0.95)
-    low, high = bounds(shape[1])
-    g = po.loss_and_grads(p, p, s, a, ret, adv_n, low, high, 0.2, 1.0, 0.01)["grads"]
-    return p, (s, a, r, v, d), perms, warm_adam(p, g, seed + 2)
 
 
 def learn_refs(shape, p, data, perms, batch, adam):
@@ -295,7 +234,7 @@ def test_learn_matches_oracle(tmp_path, case):
     T, batch, epochs = LEARN[case]
     p, data, perms, adam = learn_setup(shape, T, batch, epochs, seed=20)
     assert relu_margin(p, data[0]) > KINK_MARGIN
-    m = make_ppo(tmp_path, shape, p)
+    m = make_ppo(tmp_path, p, shape=shape)
     m.set_weights(p, p, adam[0], adam[1], adam[2])
     s, a, r, v, d = data
     metrics = m.learn(s, a, v, r, d, 0.3, gamma=0.99, lam=0.95, num_epochs=epochs, batch_size=batch, perms=perms,
@@ -308,29 +247,13 @@ def test_learn_matches_oracle(tmp_path, case):
     worst.report(case)
 
 
-# a4, T = 2500 in minibatches of 1200: the persistent kernel's head loop deals rows out by gridDim.x * 8 (1056 on a
-# 132-SM H100 SXM), so each full minibatch takes that loop round twice
-PERSISTENT = ("a4", 2500, 1200, 2)
-
-
-def persistent_learn(model_dir):
-    """learn() at PERSISTENT; run in a fresh process because CPB_PPO_PERSISTENT is read once per process."""
-    case, T, batch, epochs = PERSISTENT
-    p, data, perms, adam = learn_setup(CASES[case], T, batch, epochs, seed=30)
-    m = make_ppo(model_dir, CASES[case], p)
-    m.set_weights(p, p, adam[0], adam[1], adam[2])
-    s, a, r, v, d = data
-    metrics = m.learn(s, a, v, r, d, 0.3, num_epochs=epochs, batch_size=batch, perms=perms, return_metrics=True)
-    return m.get_weights(), metrics
-
-
 def test_persistent_learn_kernel_matches_oracle(tmp_path):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     snippet = r"""
 import sys, numpy as np
 sys.path[:0] = [%r, %r]
 from pathlib import Path
-import test_ppo_shapes_gpu as t
+import ppo_cases as t
 w, metrics = t.persistent_learn(Path(%r))
 np.savez(%r, metrics=metrics, **w)
 """

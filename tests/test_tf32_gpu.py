@@ -7,8 +7,7 @@ TF32 wgmma pass with both operands rounded to the nearest TF32 value.  Not fp32-
   * the whole model is within max(1e-5, 2 x err_tf32) of float64, err_tf32 being the distance of the "TF32
     restatement" (tests/tf32_oracle.py: the float64 oracle with round_tf32 applied to the same operands) from
     float64 on the same inputs;
-  * switching modes leaves mode 1 bit-identical.
-Every test restores mode 1 when it ends."""
+  * switching modes leaves mode 1 bit-identical."""
 import os
 import subprocess
 import sys
@@ -17,6 +16,7 @@ import numpy as np
 import pytest
 
 import tf32_oracle
+from harness import conv_relu_masks, conv_workspace, dev, lib, library_state, make_conv_vae, math_mode  # noqa: F401
 from helpers import committed_frames, kat, rel_l2, shipped_vae_weights
 from tf32_oracle import round_tf32
 
@@ -25,25 +25,9 @@ UNIT_TOL = 2e-6          # the tensor-core unit bar (tests/test_tc_gpu.py): only
 FWD_TOL = 1e-5
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
-
-
-@pytest.fixture(autouse=True)
-def tf32_mode(lib):
-    from carla_ppo_b200 import _lib
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_TF32))
-    yield
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
-
-
 def test_math_mode_2_is_accepted_and_bad_modes_are_rejected(lib):
     from carla_ppo_b200 import _lib
+    _lib.check(lib.cpb_set_math_mode(_lib.MATH_TF32))
     assert lib.cpb_get_math_mode() == _lib.MATH_TF32
     for bad in (3, -1):
         assert lib.cpb_set_math_mode(bad) == -1
@@ -93,9 +77,10 @@ def _gemm(lib, a, bt):
     ta, tb = torch.tensor(a, device="cuda"), torch.tensor(bt, device="cuda")
     d = torch.full((m, n), float("nan"), device="cuda")
     scratch = torch.empty(2 * n * k, device="cuda")
-    _lib.check(lib.cpb_debug_tc_gemm(ta.data_ptr(), tb.data_ptr(), d.data_ptr(), m, n, k, scratch.data_ptr(),
-                                     _lib.current_stream_handle()))
-    torch.cuda.synchronize()
+    with math_mode(lib, _lib.MATH_TF32):
+        _lib.check(lib.cpb_debug_tc_gemm(ta.data_ptr(), tb.data_ptr(), d.data_ptr(), m, n, k, scratch.data_ptr(),
+                                         _lib.current_stream_handle()))
+        torch.cuda.synchronize()
     return d.cpu().numpy()
 
 
@@ -107,9 +92,10 @@ def _wgrad(lib, big, small):
     tb, ts = torch.tensor(big, device="cuda"), torch.tensor(small, device="cuda")
     out = torch.full((i, j), float("nan"), device="cuda")
     part = torch.zeros(2 * i * j, device="cuda")          # the debug entry uses 2 splits
-    _lib.check(lib.cpb_debug_tc_wgrad(tb.data_ptr(), ts.data_ptr(), out.data_ptr(), m, i, j, 0, part.data_ptr(),
-                                      _lib.current_stream_handle()))
-    torch.cuda.synchronize()
+    with math_mode(lib, _lib.MATH_TF32):
+        _lib.check(lib.cpb_debug_tc_wgrad(tb.data_ptr(), ts.data_ptr(), out.data_ptr(), m, i, j, 0, part.data_ptr(),
+                                          _lib.current_stream_handle()))
+        torch.cuda.synchronize()
     return out.cpu().numpy()
 
 
@@ -191,57 +177,24 @@ def test_tf32_gemm_is_bit_identical_across_cluster_sizes():
 
 
 # ----------------------------------------------------------------------------- model level
-def make_vae(tmp_path, weights, loss="mse"):
-    from carla_ppo_b200.vae.models import ConvVAE
-    vae = ConvVAE(source_shape=(80, 160, 3), z_dim=64, loss_fn=loss, model_dir=str(tmp_path / "m"), seed=0)
-    vae.init_session(init_logging=False)
-    vae.set_weights(weights)
-    return vae
-
-
 def config1_inputs(n=32):
     x = np.random.RandomState(0).rand(n, 80, 160, 3).astype(np.float32)
     eps = np.random.RandomState(1).randn(n, 64).astype(np.float32)
     return x, eps
 
 
-def dev(vae, a):
-    import torch
-    return torch.as_tensor(np.ascontiguousarray(a), device=vae._device)
-
-
-SHAPES = {"a1": (39, 79, 32), "a2": (18, 38, 64), "a3": (8, 18, 128), "a4": (3, 8, 256), "d1": (3, 8, 256),
-          "b1": (8, 18, 128), "b2": (18, 38, 64), "b3": (39, 79, 32)}
-BUFFERS = ["xp", "a1", "a2", "a3", "a4", "heads", "z", "d1", "b1", "b2", "b3", "logits_p", "gA", "gB", "frame_loss", "kl_rows"]
-
-
-def workspace_tensors(vae, batch, ws_mode, names):
-    """Named activations of the last call that used workspace `ws_mode`, read back from the device."""
-    import ctypes as C
-    import torch
-    from carla_ppo_b200 import _lib
-    offs = (C.c_int64 * len(BUFFERS))()
-    _lib.load().cpb_debug_vae_buffer_offsets(batch, vae.target_shape[2], vae.z_dim, ws_mode, offs, len(BUFFERS))
-    ws = vae._ws[ws_mode]
-    out = {}
-    for nm in names:
-        o = offs[BUFFERS.index(nm)]
-        cnt = batch * int(np.prod(SHAPES[nm]))
-        out[nm] = ws[o:o + 4 * cnt].view(torch.float32).cpu().numpy().astype(np.float64).reshape((batch,) + SHAPES[nm])
-    return out
-
-
 @pytest.mark.gpu
-def test_every_tensor_core_layer_on_the_devices_own_inputs(tmp_path):
+def test_every_tensor_core_layer_on_the_devices_own_inputs(tmp_path, lib):
     """One forward at B = 32; each interior layer's output against relu(contract(round_tf32(in), round_tf32(W)) + b)
     in float64 on the input the DEVICE computed, so no error of an earlier layer is carried into the comparison."""
     from carla_ppo_b200 import _lib
     from oracle import vae_oracle as vo
     w = shipped_vae_weights()[0]
-    vae = make_vae(tmp_path, w)
+    vae = make_conv_vae(tmp_path, w)
     x, eps = config1_inputs(32)
-    vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps))
-    t = workspace_tensors(vae, 32, _lib.WS_FORWARD, ["a1", "a2", "a3", "a4", "d1", "b1", "b2", "b3"])
+    with math_mode(lib, _lib.MATH_TF32):
+        vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps))
+    t = {k: v.cpu().numpy().astype(np.float64) for k, v in conv_workspace(vae, 32, _lib.WS_FORWARD).items() if k != "g"}
     r = round_tf32
     layers = [("encoder/conv2", vo.conv_gather, "a1", "a2"), ("encoder/conv3", vo.conv_gather, "a2", "a3"),
               ("encoder/conv4", vo.conv_gather, "a3", "a4"), ("decoder/deconv1", vo.conv_scatter, "d1", "b1"),
@@ -252,35 +205,30 @@ def test_every_tensor_core_layer_on_the_devices_own_inputs(tmp_path):
         assert err < UNIT_TOL, "%s: %.3e" % (name, err)
 
 
-def _device_relu_masks(vae, batch):
-    from carla_ppo_b200 import _lib
-    t = workspace_tensors(vae, batch, _lib.WS_TRAIN, ["a1", "a2", "a3", "a4", "b1", "b2", "b3"])
-    layer = {"a1": "conv1", "a2": "conv2", "a3": "conv3", "a4": "conv4", "b1": "deconv1", "b2": "deconv2", "b3": "deconv3"}
-    return {layer[k]: v > 0 for k, v in t.items()}
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("loss", ["mse", "bce"])
 @pytest.mark.parametrize("which", ["shipped", "glorot0"])
-def test_model_matches_float64_within_twice_the_tf32_restatement(tmp_path, which, loss):
+def test_model_matches_float64_within_twice_the_tf32_restatement(tmp_path, lib, which, loss):
     """BASELINE config 1 (32 random frames).  Forward tensors, losses and all 22 gradients against plain float64, gated
     at max(1e-5, 2 x err_tf32), err_tf32 = the TF32 restatement's own distance from float64 (gradients: both oracle
-    runs on the device's ReLU activity pattern, as tests/test_vae_gpu.py::_grad_check).  Plus: the device is closer
+    runs on the device's ReLU activity pattern, as tests/vae_checks.py::grad_check).  Plus: the device is closer
     to the TF32 restatement than to float64 for `mean`, and for each loss whose TF32 shift from float64 stands above
     the float32 rounding level (2 x the distance of the float32 CPU restatement from float64) -- below that level
     the comparison would measure float32 rounding, not the single pass."""
     import torch
+    from carla_ppo_b200 import _lib
     from oracle import torch_ref
     from oracle import vae_oracle as vo
     w = shipped_vae_weights()[0] if which == "shipped" else vo.glorot_init(0)
-    vae = make_vae(tmp_path, w, loss)
+    vae = make_conv_vae(tmp_path, w, loss=loss)
     x, eps = config1_inputs(32)
-    out = vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps), want_reconstruction=True, want_latents=True)
-    fwd = {k: out[k].cpu().numpy().astype(np.float64) for k in ("mean", "logvar", "z", "reconstruction")}
-    vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
-    got = vae.get_grads()
-    losses = vae._losses.cpu().numpy().astype(np.float64)
-    masks = _device_relu_masks(vae, 32)
+    with math_mode(lib, _lib.MATH_TF32):
+        out = vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps), want_reconstruction=True, want_latents=True)
+        fwd = {k: out[k].cpu().numpy().astype(np.float64) for k in ("mean", "logvar", "z", "reconstruction")}
+        vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
+        got = vae.get_grads()
+        losses = vae._losses.cpu().numpy().astype(np.float64)
+    masks = conv_relu_masks(vae, 32)
     ref = vo.loss_and_grads(w, x, x, eps, loss, relu_masks=masks)
     t32 = tf32_oracle.loss_and_grads(w, x, x, eps, loss, relu_masks=masks)
     for k in ("mean", "logvar", "z"):
@@ -306,15 +254,17 @@ def test_model_matches_float64_within_twice_the_tf32_restatement(tmp_path, which
 
 
 @pytest.mark.gpu
-def test_known_answer_shipped_checkpoint_in_tf32(tmp_path):
+def test_known_answer_shipped_checkpoint_in_tf32(tmp_path, lib):
     """KAT-1 in mode 2: shipped rgb checkpoint-232 on the 128 committed frames stays within the reference-held bars of
     tests/test_vae_gpu.py::test_known_answer_shipped_checkpoint_on_shipped_frames: 1 % (reconstruction) and 5 % (KL)
     of the reference's own logged validation losses."""
+    from carla_ppo_b200 import _lib
     w = shipped_vae_weights()[0]
     rgb, _ = committed_frames()
-    vae = make_vae(tmp_path, w, loss="bce")
+    vae = make_conv_vae(tmp_path, w, loss="bce")
     eps = np.random.RandomState(7).randn(rgb.shape[0], 64).astype(np.float32)
-    losses = vae.forward_device(dev(vae, rgb), dev(vae, rgb), dev(vae, eps))["losses"].cpu().numpy()
+    with math_mode(lib, _lib.MATH_TF32):
+        losses = vae.forward_device(dev(vae, rgb), dev(vae, rgb), dev(vae, eps))["losses"].cpu().numpy()
     k = kat()
     logged = np.mean([v for _, v in k["logged"]["val"]["vae/reconstruction_loss"]])
     logged_kl = np.mean([v for _, v in k["logged"]["val"]["vae/kl_loss"]])
@@ -329,12 +279,12 @@ def test_mode_1_is_untouched_by_mode_2(tmp_path, lib):
     import torch
     from carla_ppo_b200 import _lib
     from oracle import vae_oracle as vo
-    vae = make_vae(tmp_path, vo.glorot_init(0))
+    vae = make_conv_vae(tmp_path, vo.glorot_init(0))
     x, eps = config1_inputs(8)
     res = []
     for mode in (_lib.MATH_3XTF32, _lib.MATH_TF32, _lib.MATH_3XTF32):
-        _lib.check(lib.cpb_set_math_mode(mode))
-        vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
-        res.append((vae.grads.clone(), vae._losses.clone()))
+        with math_mode(lib, mode):
+            vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
+            res.append((vae.grads.clone(), vae._losses.clone()))
     assert torch.equal(res[0][0], res[2][0]) and torch.equal(res[0][1], res[2][1])
     assert not torch.equal(res[0][0], res[1][0])

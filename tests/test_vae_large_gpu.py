@@ -5,12 +5,12 @@ Tile scheduling (super-tile counts, m-groups, split-K factors) depends on the ba
 do not cover these launches.  Every gate is max(1e-5, 2 x the error the float32 CPU restatement of the reference graph
 makes on the same inputs) -- the float32 error is stored in the golden file next to each quantity (err32*).
 """
-import ctypes as C
 import os
 
 import numpy as np
 import pytest
 
+from harness import conv_workspace, lib, library_state, make_conv_vae, math_mode  # noqa: F401
 from helpers import GOLDEN, rel_l2, shipped_vae_weights
 
 pytestmark = pytest.mark.gpu
@@ -25,38 +25,17 @@ def large_inputs(n):
     return x, eps
 
 
-def workspace_views(vae, batch):
-    import torch
-    from carla_ppo_b200 import _lib
-    lib = _lib.load()
-    names = ["xp", "a1", "a2", "a3", "a4", "heads", "z", "d1", "b1", "b2", "b3", "logits_p", "gA", "gB", "frame_loss", "kl_rows"]
-    offs = (C.c_int64 * 16)()
-    n = lib.cpb_debug_vae_buffer_offsets(batch, vae.target_shape[2], vae.z_dim, _lib.WS_TRAIN, offs, 16)
-    assert n == 16
-    ws = vae._ws[_lib.WS_TRAIN]
-    off = dict(zip(names, offs))
-
-    def view(name, count):
-        return ws[off[name]:off[name] + 4 * count].view(torch.float32)
-    return view
-
-
 @pytest.mark.parametrize("batch", [512, 4096])
 @pytest.mark.parametrize("mode", [1, 0], ids=["tc3xtf32", "simt"])
-def test_shipping_batch_matches_float64_golden(tmp_path, batch, mode):
+def test_shipping_batch_matches_float64_golden(tmp_path, lib, batch, mode):
     import torch
     from carla_ppo_b200 import _lib
-    from carla_ppo_b200.vae.models import ConvVAE
     if mode == 0 and batch == 4096:
         pytest.skip("the fp32 SIMT path is the fallback arithmetic; its batch-dependent scheduling is covered at 512")
     g = np.load(os.path.join(GOLDEN, "large_B%d.npz" % batch))
-    lib = _lib.load()
-    _lib.check(lib.cpb_set_math_mode(mode))
-    try:
+    with math_mode(lib, mode):
         w = shipped_vae_weights()[0]
-        vae = ConvVAE((80, 160, 3), z_dim=64, loss_fn="mse", model_dir=str(tmp_path / "m"), seed=0)
-        vae.init_session(init_logging=False)
-        vae.set_weights(w)
+        vae = make_conv_vae(tmp_path, w)
         x, eps = large_inputs(batch)
         xd = torch.from_numpy(x).to(vae._device); ed = torch.from_numpy(eps).to(vae._device)
         vae.loss_grad_device(xd, xd, ed)
@@ -65,14 +44,14 @@ def test_shipping_batch_matches_float64_golden(tmp_path, batch, mode):
         assert abs(losses[0] - g["recon"]) / g["recon"] < max(TOL, 2 * float(g["err32_recon"]))
         assert abs(losses[1] - g["kl"]) / g["kl"] < TOL
         # per-frame forward quantities of the sampled frames
-        view = workspace_views(vae, batch)
+        view = conv_workspace(vae, batch, _lib.WS_TRAIN)
         idx = torch.from_numpy(g["sample_idx"]).to(vae._device)
-        heads = view("heads", 2 * batch * 64).reshape(2, batch, 64)
+        heads = view["heads"]
         assert rel_l2(heads[0].index_select(0, idx).cpu().numpy(), g["mean"]) < max(TOL, 2 * float(g["err32_mean"]))
         assert rel_l2(heads[1].index_select(0, idx).cpu().numpy(), g["logvar"]) < max(TOL, 2 * float(g["err32_logvar"]))
-        fl = view("frame_loss", batch).index_select(0, idx).cpu().numpy()
+        fl = view["frame_loss"].index_select(0, idx).cpu().numpy()
         assert rel_l2(fl, g["frame_recon"]) < max(TOL, 2 * float(g["err32_frame_recon"]))
-        kr = view("kl_rows", batch).index_select(0, idx).cpu().numpy()
+        kr = view["kl_rows"].index_select(0, idx).cpu().numpy()
         assert rel_l2(kr, g["frame_kl"]) < TOL
         # the full-batch gradient, every tensor (large ones on the committed fixed-stride subsample)
         got = vae.get_grads()
@@ -82,5 +61,3 @@ def test_shipping_batch_matches_float64_golden(tmp_path, batch, mode):
             err = np.linalg.norm(mine.astype(np.float64) - ref) / np.linalg.norm(ref)
             gate = max(TOL, 2 * float(g["err32/" + name]))
             assert err < gate, "%s: rel err %.3e, gate %.3e (fp32 CPU restatement %.3e)" % (name, err, gate, float(g["err32/" + name]))
-    finally:
-        _lib.check(lib.cpb_set_math_mode(1))

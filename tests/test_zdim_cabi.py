@@ -2,22 +2,13 @@
 by the ConvVAE and MlpVAE layout / workspace entry points with the reference's variable shapes, and everything else is
 rejected with an error that names z_dim.  No compute entry point is called here."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
+from harness import lib, library_state  # noqa: F401
 
 Z_GOOD = (4, 32, 100, 1024)
 Z_BAD = (0, 2, 65, 1028)
-
-
-@pytest.fixture(scope="module")
-def lib():
-    from carla_ppo_b200 import _lib
-    if not os.path.isfile(_lib.LIB_PATH):
-        import __graft_entry__
-        __graft_entry__.build()
-    return _lib.load()
 
 
 def _vae_shapes(lib, ct, z):

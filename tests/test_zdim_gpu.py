@@ -10,9 +10,12 @@ import os
 import numpy as np
 import pytest
 
+import harness
 import tf32_oracle
+from harness import conv_relu_masks, dev, lib, library_state, make_conv_vae  # noqa: F401
 from helpers import committed_frames, rel_l2
-from test_vae_gpu import _grad_check, _shift_away_from_zero
+from ppo_cases import train_params
+from vae_checks import grad_check, shift_away_from_zero
 
 pytestmark = pytest.mark.gpu
 
@@ -27,12 +30,9 @@ def oracle():
 
 
 @pytest.fixture(params=[1, 0], ids=["tc3xtf32", "simt"])
-def math_mode(request):
-    from carla_ppo_b200 import _lib
-    lib = _lib.load()
-    _lib.check(lib.cpb_set_math_mode(request.param))
-    yield request.param
-    _lib.check(lib.cpb_set_math_mode(1))
+def math_mode(request, lib):
+    with harness.math_mode(lib, request.param):
+        yield request.param
 
 
 def inputs(n, z, seed=0):
@@ -50,22 +50,8 @@ def weights(oracle, z):
             if k.endswith("bias"):
                 w[k] = (0.05 * np.random.RandomState(len(k)).randn(*w[k].shape)).astype(np.float32)
         x, eps = inputs(2, z)
-        _WEIGHTS[z] = _shift_away_from_zero(oracle, w, x, eps, margin=2e-5)
+        _WEIGHTS[z] = shift_away_from_zero(oracle, w, x, eps, margin=2e-5)
     return {k: v.copy() for k, v in _WEIGHTS[z].items()}
-
-
-def make_vae(tmp_path, z, w=None, name="m", loss="mse", **kw):
-    from carla_ppo_b200.vae.models import ConvVAE
-    vae = ConvVAE(source_shape=(80, 160, 3), z_dim=z, loss_fn=loss, model_dir=str(tmp_path / name), seed=0, **kw)
-    vae.init_session(init_logging=False)
-    if w is not None:
-        vae.set_weights(w)
-    return vae
-
-
-def dev(vae, a):
-    import torch
-    return torch.as_tensor(np.ascontiguousarray(a), device=vae._device)
 
 
 @pytest.mark.parametrize("z", [16, 32, 100])
@@ -73,7 +59,7 @@ def test_conv_vae_forward_gradients_and_adam_match_oracle(tmp_path, oracle, math
     import torch
     from oracle import torch_ref
     w = weights(oracle, z)
-    vae = make_vae(tmp_path, z, w, learning_rate=1e-4)
+    vae = make_conv_vae(tmp_path, w, z=z, learning_rate=1e-4)
     # forward: every tensor that crosses the boundary at [B, z]
     x, eps = inputs(6, z, seed=3)
     out = vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps), want_reconstruction=True, want_latents=True)
@@ -88,7 +74,7 @@ def test_conv_vae_forward_gradients_and_adam_match_oracle(tmp_path, oracle, math
     assert abs(losses[1] - ref["kl"]) < FWD_TOL          # KL ~ 0.1-0.9 here, a cancelling sum: absolute gate, as for glorot0
     # all 22 gradients, on the inputs the biases were shifted for
     x2, eps2 = inputs(2, z)
-    _grad_check(vae, oracle, w, x2, x2, eps2, "mse", floor=FWD_TOL)
+    grad_check(vae, oracle, w, x2, x2, eps2, "mse", floor=FWD_TOL)
     # two Adam steps
     p64 = {k: v.astype(np.float64) for k, v in w.items()}
     st = oracle.adam_init_state(p64)
@@ -116,11 +102,11 @@ def test_kl_tolerance_floor_at_z32(tmp_path, oracle, math_mode):
     rows = -0.5 * np.sum(1 + ref["logvar"] - ref["mean"] ** 2 - np.exp(ref["logvar"]), axis=1)
     tol = float(rows.mean()) / z                      # floor between the two rows
     assert (rows < tol * z).any() and (rows > tol * z).any()
-    vae = make_vae(tmp_path, z, w, kl_tolerance=tol)
+    vae = make_conv_vae(tmp_path, w, z=z, kl_tolerance=tol)
     out = vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps))["losses"].cpu().numpy()
     ref = oracle.loss_and_grads(w, x, x, eps, "mse", 1.0, tol, want_grads=False)
     assert abs(out[1] - ref["kl"]) / ref["kl"] < FWD_TOL
-    _grad_check(vae, oracle, w, x, x, eps, "mse", kl_tolerance=tol, floor=FWD_TOL)
+    grad_check(vae, oracle, w, x, x, eps, "mse", kl_tolerance=tol, floor=FWD_TOL)
 
 
 def test_mlp_vae_at_z32_matches_oracle(tmp_path, oracle):
@@ -173,26 +159,21 @@ def test_mlp_vae_at_z32_matches_oracle(tmp_path, oracle):
     assert np.array_equal(again.encode(x[:2]), vae.encode(x[:2]))
 
 
-def test_tf32_mode_at_z32_within_twice_the_tf32_restatement(tmp_path, oracle):
+def test_tf32_mode_at_z32_within_twice_the_tf32_restatement(tmp_path, lib, oracle):
     """Math mode 2 at z = 32: forward tensors, losses and all 22 gradients within max(1e-5, 2 x err_tf32) of float64,
     as tests/test_tf32_gpu.py::test_model_matches_float64_within_twice_the_tf32_restatement."""
     from carla_ppo_b200 import _lib
-    from test_tf32_gpu import _device_relu_masks
-    lib = _lib.load()
     z = 32
     w = weights(oracle, z)
     x, eps = inputs(8, z, seed=5)
-    _lib.check(lib.cpb_set_math_mode(_lib.MATH_TF32))
-    try:
-        vae = make_vae(tmp_path, z, w)
+    with harness.math_mode(lib, _lib.MATH_TF32):
+        vae = make_conv_vae(tmp_path, w, z=z)
         out = vae.forward_device(dev(vae, x), dev(vae, x), dev(vae, eps), want_reconstruction=True, want_latents=True)
         fwd = {k: out[k].cpu().numpy().astype(np.float64) for k in ("mean", "logvar", "z", "reconstruction")}
         vae.loss_grad_device(dev(vae, x), dev(vae, x), dev(vae, eps))
         got = vae.get_grads()
         losses = vae._losses.cpu().numpy().astype(np.float64)
-        masks = _device_relu_masks(vae, 8)
-    finally:
-        _lib.check(lib.cpb_set_math_mode(_lib.MATH_3XTF32))
+        masks = conv_relu_masks(vae, 8)
     ref = oracle.loss_and_grads(w, x, x, eps, "mse", relu_masks=masks)
     t32 = tf32_oracle.loss_and_grads(w, x, x, eps, "mse", relu_masks=masks)
     for k in ("mean", "logvar", "z"):
@@ -217,7 +198,7 @@ def test_batch_invariance_and_reference_surface_at_z32(tmp_path, oracle, math_mo
     import torch
     z = 32
     w = weights(oracle, z)
-    vae = make_vae(tmp_path, z, w, training=False)
+    vae = make_conv_vae(tmp_path, w, z=z, training=False)
     g = torch.Generator(device="cuda"); g.manual_seed(0)
     B = 1024
     x = torch.rand(B, 80, 160, 3, generator=g, device="cuda")
@@ -242,14 +223,13 @@ def test_fused_actor_with_a_z32_vae(tmp_path, oracle):
     (cpb_encode_predict) and the unfused encode + PPO.predict produce the same trajectory and weights, bit for bit."""
     from carla_ppo_b200.replay_env import ReplayEnv
     from carla_ppo_b200.train import train
-    from test_integration_gpu import _train_params
     rgb, _ = committed_frames()
     w = weights(oracle, 32)
     runs = []
     for tag, over in (("fused", {}), ("unfused", {"unfused": True})):
         env = ReplayEnv(rgb, episode_length=24, seed=0)
-        vae = make_vae(tmp_path, 32, w, name="vae_" + tag, training=False)
-        model = train(_train_params(tag, **over), restart=False, env=env, vae=vae, models_root=str(tmp_path / "models"),
+        vae = make_conv_vae(tmp_path, w, z=32, tag="vae_" + tag, training=False)
+        model = train(train_params(tag, **over), restart=False, env=env, vae=vae, models_root=str(tmp_path / "models"),
                       interactive=False)
         assert model.state_dim == 35 and env.step_count > 0
         runs.append(model)
@@ -264,7 +244,7 @@ def test_save_and_load_vae_from_a_zdim32_directory(tmp_path, oracle):
     from carla_ppo_b200 import vae_common
     w = weights(oracle, 32)
     name = "rgb_bce_cnn_zdim32_beta1_kl_tolerance0.0_data"
-    vae = make_vae(tmp_path, 32, w, name=name, loss="bce")
+    vae = make_conv_vae(tmp_path, w, z=32, tag=name, loss="bce")
     vae.save()
     again = vae_common.load_vae(str(tmp_path / name))
     assert type(again).__name__ == "ConvVAE" and again.z_dim == 32
