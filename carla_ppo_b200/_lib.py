@@ -59,6 +59,11 @@ class PpoConfig(C.Structure):
                 ("epsilon", C.c_float), ("value_scale", C.c_float), ("entropy_scale", C.c_float)]
 
 
+class PpoLearnOptions(C.Structure):
+    """cpb_ppo_learn_options: 0 turns a guard off."""
+    _fields_ = [("max_grad_norm", C.c_float), ("target_kl", C.c_float)]
+
+
 _P = C.c_void_p
 _i32, _i64, _f32, _f64 = C.c_int32, C.c_int64, C.c_float, C.c_double
 _VC = C.POINTER(VaeConfig)
@@ -66,6 +71,7 @@ _VS = C.POINTER(VaeSpec)
 _MC = C.POINTER(MlpVaeConfig)
 _MS = C.POINTER(MlpVaeSpec)
 _PC = C.POINTER(PpoConfig)
+_PO = C.POINTER(PpoLearnOptions)
 
 # name -> (restype, argtypes); must list every symbol of include/carla_ppo_b200.h
 PROTOTYPES = {
@@ -125,6 +131,12 @@ PROTOTYPES = {
     "cpb_gae_segments": (_i32, [_P, _P, _P, _P, _P, _i32, _i32, _f64, _f64, _P, _P, _P, _P]),
     "cpb_ppo_learn_segments": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32, _f64, _f64,
                                       _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_learn_opts": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
+                                  _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_ppo_learn_segments_opts": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32, _f64,
+                                           _f64, _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_ppo_train_step_opts": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _PO, _P, _P, _P,
+                                       _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_vae_spec_buffer_offsets": (_i32, [_VS, _i32, _P, _i32]),

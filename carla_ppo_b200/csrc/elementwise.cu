@@ -394,14 +394,18 @@ __global__ void relayout_kernel(const float* __restrict__ params, float* __restr
 __global__ void adam_kernel(float4* __restrict__ p, const float4* __restrict__ g, float4* __restrict__ m,
                             float4* __restrict__ v, long long n4, const float* __restrict__ powers, float lr,
                             const float* __restrict__ lr_dev, float beta1, float beta2, float epsilon,
-                            const uint32_t* __restrict__ guard) {
+                            const uint32_t* __restrict__ guard, const float* __restrict__ gscale) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n4) return;
     if (guard != nullptr && guard[0] != 0u) return;     // verify_range tripped: the reference's tf.Assert aborts BEFORE the update
     const float lr_t = lr_dev != nullptr ? lr_dev[0] : lr;
     const float alpha = lr_t * sqrtf(1.f - powers[1]) / (1.f - powers[0]);
     const float omb1 = 1.f - beta1, omb2 = 1.f - beta2;
-    const float4 gv = g[i];
+    float4 gv = g[i];
+    if (gscale != nullptr) {                            // PPO gradient-norm clipping: the coefficient is 1 when nothing clips
+        const float c = gscale[0];
+        gv.x *= c; gv.y *= c; gv.z *= c; gv.w *= c;
+    }
     float4 mv = m[i], vv = v[i], pv = p[i];
     mv.x += (gv.x - mv.x) * omb1; mv.y += (gv.y - mv.y) * omb1; mv.z += (gv.z - mv.z) * omb1; mv.w += (gv.w - mv.w) * omb1;
     vv.x += (gv.x * gv.x - vv.x) * omb2; vv.y += (gv.y * gv.y - vv.y) * omb2;
@@ -411,10 +415,12 @@ __global__ void adam_kernel(float4* __restrict__ p, const float4* __restrict__ g
     m[i] = mv; v[i] = vv; p[i] = pv;
 }
 
-__global__ void adam_powers_kernel(float* powers, float beta1, float beta2, const uint32_t* __restrict__ guard) {
+__global__ void adam_powers_kernel(float* powers, float beta1, float beta2, const uint32_t* __restrict__ guard,
+                                   int32_t* __restrict__ steps) {
     if (guard != nullptr && guard[0] != 0u) return;
     powers[0] *= beta1;
     powers[1] *= beta2;
+    if (steps != nullptr) steps[0] += 1;
 }
 
 __global__ void fill_zero_kernel(float4* p, long long n4) {
@@ -579,13 +585,14 @@ int32_t launch_relayout(const float* params, float* dst, const RelayoutTable& ta
 
 int32_t launch_adam(float* params, const float* grads, float* m, float* v, long long n, float* powers,
                     float lr, const float* lr_dev, float beta1, float beta2, float epsilon, cudaStream_t stream,
-                    const void* guard) {
+                    const void* guard, const float* gscale, int32_t* steps) {
     CPB_REQUIRE(n % 4 == 0, "adam: buffer length %lld is not a multiple of 4", n);
     if (n == 0) return CPB_OK;
     adam_kernel<<<cdiv(n / 4, 256), 256, 0, stream>>>((float4*)params, (const float4*)grads, (float4*)m, (float4*)v,
-                                                      n / 4, powers, lr, lr_dev, beta1, beta2, epsilon, (const uint32_t*)guard);
+                                                      n / 4, powers, lr, lr_dev, beta1, beta2, epsilon, (const uint32_t*)guard,
+                                                      gscale);
     CPB_LAUNCHED();
-    adam_powers_kernel<<<1, 1, 0, stream>>>(powers, beta1, beta2, (const uint32_t*)guard);
+    adam_powers_kernel<<<1, 1, 0, stream>>>(powers, beta1, beta2, (const uint32_t*)guard, steps);
     CPB_LAUNCHED();
     return CPB_OK;
 }

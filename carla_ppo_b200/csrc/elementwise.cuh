@@ -98,10 +98,12 @@ struct RelayoutTable {
 };
 int32_t launch_relayout(const float* params, float* dst, const RelayoutTable& table, cudaStream_t stream);
 
-// guard (nullable, device, one 32-bit word): when its bits are non-zero the update is skipped entirely (verify_range)
+// guard (nullable, device, one 32-bit word): when its bits are non-zero the update is skipped entirely (verify_range, the
+// PPO approximate-KL stop).  gscale (nullable, device float[1]): every gradient is multiplied by gscale[0] first (PPO
+// gradient-norm clipping).  steps (nullable, device int32[1]): incremented when the update is applied.
 int32_t launch_adam(float* params, const float* grads, float* m, float* v, long long n, float* powers,
                     float lr, const float* lr_dev, float beta1, float beta2, float epsilon, cudaStream_t stream,
-                    const void* guard = nullptr);
+                    const void* guard = nullptr, const float* gscale = nullptr, int32_t* steps = nullptr);
 
 int32_t launch_fill_zero(float* p, long long n, cudaStream_t stream);
 

@@ -5,6 +5,8 @@
 // over the two trunks (policy / value) so one minibatch step is ~11 launches with no host sync.
 #include <cooperative_groups.h>
 
+#include <cmath>
+
 #include "common.cuh"
 #include "elementwise.cuh"
 
@@ -248,9 +250,10 @@ struct HeadArgs {
     float* dv;             // [B]   gradient w.r.t. the value output
     float* dh2;            // [B,H2] masked gradient w.r.t. policy trunk output
     float* dg2;            // [B,H2] masked gradient w.r.t. value trunk output
-    float* partial;        // [nblocks][8]: policy, value, ratio sums, logstd grads...
+    float* partial;        // [nblocks][8]: policy, value, ratio sums, logstd grads (3..3+A), approx-KL sum (7)
     const float* noise;    // predict path: [B,A] or null
     float* action_out;     // predict path
+    int kl_term;           // training head: add (r - 1) - log r to slot 7 (options entry points only)
 };
 
 // mode 0: log-prob only (old policy); mode 1: full training head; mode 2: predict (mu / sampled action, value)
@@ -344,6 +347,7 @@ __device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, flo
 #pragma unroll
             for (int k = 0; k < kMaxActions; ++k)
                 if (k < a.A) vals[3 + k] += dlogp * (diff[k] * diff[k] - 1.f);
+            if (a.kl_term) vals[7] += (ratio - 1.f) - (logp - logp_old);   // approximate KL (Stable-Baselines3's estimator)
         }
     }
 }
@@ -375,9 +379,27 @@ ppo_head_kernel(const __grid_constant__ HeadArgs a) {
     if (MODE == 1) head_block_reduce(vals, red, a.partial + blockIdx.x * 8);
 }
 
+// The per-call guards of the cpb_ppo_*_opts entry points (cpb_ppo_learn_options).  stop == nullptr on every other entry
+// point: then none of the guard code runs and the metrics rows are 5 wide.
+//   stop: device word, 0 while the update runs.  ppo_finalize sets it to 1 at the minibatch whose approx_kl exceeds
+//         kl_limit and to 2 at every minibatch evaluated after that; Adam skips every step while it is non-zero.
+//   clip: device float[1], the current minibatch's gradient scale min(1, max_norm / (norm + 1e-6)) (1 when max_norm == 0).
+struct Guards {
+    uint32_t* stop;
+    float* clip;
+    float* norm_partial;   // [kMaxPersistentCtas] per-block sums of squares of the gradient
+    uint32_t* counter;     // blocks of grad_norm_kernel done (back to 0 when it ends)
+    int32_t* steps;        // Adam steps applied (nullable)
+    float max_norm;        // 0: no clipping
+    float kl_limit;        // 1.5 * target_kl; 0: no stop
+};
+
 // metrics[5] = policy_loss, value_loss, entropy_loss, loss, mean ratio; grads[logstd], value-bias etc.
+// With guards, metrics rows are 7 wide: [5] = approx_kl (written here), [6] = the pre-clip gradient norm (written by the
+// norm reduction); a minibatch evaluated after the stop gets a NaN row.
 __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, int B, int A, const float* logstd, float value_scale,
-                                             float entropy_scale, float* glogstd, float* metrics, float* tot /* shared [8] */) {
+                                             float entropy_scale, float* glogstd, float* metrics, float* tot /* shared [8] */,
+                                             const Guards& g) {
     if (threadIdx.x < 8) {
         float s = 0.f;
         for (int i = 0; i < nblocks; ++i) s += __ldcg(partial + i * 8 + threadIdx.x);
@@ -394,8 +416,19 @@ __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, 
         const float pl = tot[0] * inv_b;
         const float vl = tot[1] * inv_b * value_scale;
         const float el = ent * entropy_scale;
-        if (metrics != nullptr) {
-            metrics[0] = pl; metrics[1] = vl; metrics[2] = el; metrics[3] = -pl + vl - el; metrics[4] = tot[2] * inv_b;
+        if (g.stop != nullptr && __ldcg(g.stop) != 0u) {
+            *g.stop = 2u;
+            if (metrics != nullptr)
+                for (int k = 0; k < 7; ++k) metrics[k] = __int_as_float(0x7fc00000);
+        } else {
+            if (metrics != nullptr) {
+                metrics[0] = pl; metrics[1] = vl; metrics[2] = el; metrics[3] = -pl + vl - el; metrics[4] = tot[2] * inv_b;
+            }
+            if (g.stop != nullptr) {
+                const float kl = tot[7] * inv_b;
+                if (metrics != nullptr) metrics[5] = kl;
+                if (g.kl_limit > 0.f && kl > g.kl_limit) *g.stop = 1u;
+            }
         }
     }
     __syncthreads();
@@ -403,9 +436,71 @@ __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, 
 
 __global__ void ppo_finalize_kernel(const float* __restrict__ partial, int nblocks, int B, int A,
                                     const float* __restrict__ logstd, float value_scale, float entropy_scale,
-                                    float* __restrict__ glogstd, float* __restrict__ metrics) {
+                                    float* __restrict__ glogstd, float* __restrict__ metrics, const Guards g) {
     __shared__ float tot[8];
-    ppo_finalize(partial, nblocks, B, A, logstd, value_scale, entropy_scale, glogstd, metrics, tot);
+    ppo_finalize(partial, nblocks, B, A, logstd, value_scale, entropy_scale, glogstd, metrics, tot, g);
+}
+
+// ---------------------------------------------------------------------------------------------
+// global L2 norm of the gradient (torch.nn.utils.clip_grad_norm_ over the 13 policy/ tensors; the layout's zero padding
+// adds nothing).  Every sum has a fixed order, so a repeated call is bit-identical.
+// ---------------------------------------------------------------------------------------------
+constexpr int kNormBlocks = 256, kNormThreads = 256;
+
+// sum of v over the CTA's threads in a fixed order, returned to every thread; red: shared [blockDim.x / 32]
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    v = warp_sum(v);
+    __syncthreads();                  // red may still be read by a previous call
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[w];
+    return s;
+}
+
+// this thread's share of sum(g^2): float4 elements k = first, first + stride, ...
+__device__ __forceinline__ float sumsq_share(const float4* g, long long n4, long long first, long long stride) {
+    float s = 0.f;
+    for (long long k = first; k < n4; k += stride) {
+        const float4 v = __ldcg(g + k);
+        s = fmaf(v.x, v.x, s); s = fmaf(v.y, v.y, s); s = fmaf(v.z, v.z, s); s = fmaf(v.w, v.w, s);
+    }
+    return s;
+}
+
+__device__ __forceinline__ float clip_coefficient(float sumsq, float max_norm) {
+    if (max_norm <= 0.f) return 1.f;
+    const float c = max_norm / (sqrtf(sumsq) + 1e-6f);
+    return c < 1.f ? c : 1.f;
+}
+
+// partial sums per block, then the last block to finish sums the partials in block order: clip coefficient, metrics[6]
+__global__ void __launch_bounds__(kNormThreads)
+grad_norm_kernel(const float4* __restrict__ g, long long n4, const Guards gd, float* __restrict__ metrics) {
+    __shared__ float red[kNormThreads / 32];
+    __shared__ bool last;
+    const float s = block_sum(sumsq_share(g, n4, (long long)blockIdx.x * blockDim.x + threadIdx.x, (long long)gridDim.x * blockDim.x), red);
+    if (threadIdx.x == 0) {
+        gd.norm_partial[blockIdx.x] = s;
+        __threadfence();
+        last = atomicAdd(gd.counter, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    float t = 0.f;
+    for (int i = threadIdx.x; i < (int)gridDim.x; i += blockDim.x) t += __ldcg(gd.norm_partial + i);
+    t = block_sum(t, red);
+    if (threadIdx.x == 0) {
+        gd.clip[0] = clip_coefficient(t, gd.max_norm);
+        if (metrics != nullptr && __ldcg(gd.stop) != 2u) metrics[6] = sqrtf(t);
+        *gd.counter = 0u;
+    }
+}
+
+int32_t launch_grad_norm(const float* grads, long long n, const Guards& gd, float* metrics, cudaStream_t s) {
+    grad_norm_kernel<<<kNormBlocks, kNormThreads, 0, s>>>(reinterpret_cast<const float4*>(grads), n / 4, gd, metrics);
+    CPB_LAUNCHED();
+    return CPB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -561,6 +656,8 @@ struct PpoPlan {
     float *dpre, *dv, *partial;
     float *ret32, *adv32;  // [T]
     double* gae_scratch;   // [T]
+    float* norm_partial;   // [kMaxPersistentCtas]  guards of the options entry points (Guards)
+    uint32_t* guard_words; // [4]: stop, counter, clip (as float bits), unused
     int64_t bytes;
     bool ok;
 };
@@ -584,6 +681,8 @@ PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_config* c, int m
     p.ret32 = a.take<float>(rows);
     p.adv32 = a.take<float>(rows);
     p.gae_scratch = a.take<double>(rows);
+    p.norm_partial = a.take<float>(kMaxPersistentCtas);
+    p.guard_words = a.take<uint32_t>(4);
     p.bytes = a.off;
     p.ok = ws == nullptr || !a.overflow;
     return p;
@@ -639,7 +738,7 @@ int32_t run_trunks(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan& p
 int32_t run_loss_grad(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan& pl, const float* params,
                       const float* states, const float* actions, const float* returns, const float* adv,
                       const int32_t* idx, int B, const float* logp_old, int logp_old_gathered, float* grads,
-                      float* metrics, cudaStream_t s) {
+                      float* metrics, const Guards& gd, cudaStream_t s) {
     const int S = c->state_dim, H1 = c->hidden1, H2 = c->hidden2, A = c->num_actions;
     CPB_TRY(run_trunks(c, L, pl, params, states, idx, B, s));
     float* h1p = pl.h1; float* h1v = pl.h1 + (long long)B * H1;
@@ -650,11 +749,12 @@ int32_t run_loss_grad(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan
     h.h2 = h2p; h.g2 = h2v; h.actions = actions; h.returns = returns; h.adv = adv; h.idx = idx;
     h.logp_old_in = logp_old; h.logp_old_gathered = logp_old_gathered;
     h.dpre = pl.dpre; h.dv = pl.dv; h.dh2 = dh2p; h.dg2 = dh2v; h.partial = pl.partial;
+    h.kl_term = gd.stop != nullptr;
     const int nblocks = cdiv(B, 8);
     ppo_head_kernel<1><<<nblocks, 256, 0, s>>>(h);
     CPB_LAUNCHED();
     ppo_finalize_kernel<<<1, 32, 0, s>>>(pl.partial, nblocks, B, A, params + L.off[P_LOGSTD], c->value_scale,
-                                         c->entropy_scale, grads + L.off[P_LOGSTD], metrics);
+                                         c->entropy_scale, grads + L.off[P_LOGSTD], metrics, gd);
     CPB_LAUNCHED();
     GemmBatch gb;
     // everything that only needs the head kernel's outputs goes into ONE launch (6 independent GEMMs):
@@ -692,6 +792,7 @@ struct LearnArgs {
     const int32_t* perms;
     float* metrics;
     int T, batch_size, num_epochs, nmb;
+    Guards gd;             // gd.stop == nullptr: no guards, 5-wide metrics rows
 };
 
 constexpr int kGroupsPerCta = 2;
@@ -728,22 +829,27 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
     extern __shared__ __align__(16) float learn_smem[];
     __shared__ float red[8][8];
     __shared__ float tot[8];
+    __shared__ float nred[kLearnThreads / 32];
     const cpb_ppo_config& c = a.cfg;
     const PpoLayout& L = a.L;
     const PpoPlan& pl = a.pl;
+    const Guards& gd = a.gd;
     const int S = c.state_dim, H1 = c.hidden1, H2 = c.hidden2, A = c.num_actions;
     const int ngroups = gridDim.x * kGroupsPerCta;
     const int gid = blockIdx.x * kGroupsPerCta + threadIdx.x / kTileThreads;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int mcols = gd.stop != nullptr ? 7 : 5;
     float* params = a.params;
     float* grads = a.grads;
 
+    // Every CTA runs every minibatch and reaches every grid.sync: the guards only predicate the Adam step, on values every
+    // CTA reads after a grid.sync (the stop word ppo_finalize wrote two barriers earlier, the norm partials of all CTAs).
     for (int e = 0; e < a.num_epochs; ++e)
         for (int i = 0; i < a.nmb; ++i) {
             const int begin = i * a.batch_size;
             const int B = begin + a.batch_size <= a.T ? a.batch_size : a.T - begin;
             const int32_t* idx = a.perms + (long long)e * a.T + begin;
-            float* mt = a.metrics ? a.metrics + ((long long)e * a.nmb + i) * 5 : nullptr;
+            float* mt = a.metrics ? a.metrics + ((long long)e * a.nmb + i) * mcols : nullptr;
             float* h1p = pl.h1; float* h1v = pl.h1 + (long long)B * H1;
             float* h2p = pl.h2; float* h2v = pl.h2 + (long long)B * H2;
             float* dh2p = pl.dh2; float* dh2v = pl.dh2 + (long long)B * H2;
@@ -772,6 +878,7 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
                 h.logp_out = nullptr; h.mu_out = nullptr; h.v_out = nullptr;
                 h.dpre = pl.dpre; h.dv = pl.dv; h.dh2 = dh2p; h.dg2 = dh2v; h.partial = pl.partial;
                 h.noise = nullptr; h.action_out = nullptr;
+                h.kl_term = gd.stop != nullptr;
                 float vals[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
                 for (int b = blockIdx.x * 8 + warp; b < B; b += gridDim.x * 8) head_row<1>(h, b, lane, vals);
                 head_block_reduce(vals, red, pl.partial + blockIdx.x * 8);
@@ -779,7 +886,7 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
             grid.sync();
             // ---- loss metrics + logstd gradient (CTA 0), then everything that only needs the head's outputs
             if (blockIdx.x == 0)
-                ppo_finalize(pl.partial, gridDim.x, B, A, params + L.off[P_LOGSTD], c.value_scale, c.entropy_scale, grads + L.off[P_LOGSTD], mt, tot);
+                ppo_finalize(pl.partial, gridDim.x, B, A, params + L.off[P_LOGSTD], c.value_scale, c.entropy_scale, grads + L.off[P_LOGSTD], mt, tot, gd);
             jobs[0] = bwd_weight_job(h1p, nullptr, B, H1, dh2p, H2, grads + L.off[P_W2], grads + L.off[P_B2]);
             jobs[1] = bwd_weight_job(h1v, nullptr, B, H1, dh2v, H2, grads + L.off[P_V2], grads + L.off[P_VB2]);
             jobs[2] = bwd_data_job(dh2p, B, H2, params + L.off[P_W2], H1, h1p, dh1p);
@@ -792,8 +899,26 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
             jobs[1] = bwd_weight_job(a.states, idx, B, S, dh1v, H1, grads + L.off[P_V1], grads + L.off[P_VB1]);
             run_phase<2>(jobs, 2, learn_smem, gid, ngroups);
             grid.sync();
+            // ---- guards: per-CTA sums of g^2, a barrier, then the same fixed-order sum of all partials in every CTA
+            float gscale = 1.f;
+            bool apply = true;
+            if (gd.stop != nullptr) {
+                const long long n4 = L.total / 4;
+                const float s = block_sum(sumsq_share(reinterpret_cast<const float4*>(grads), n4,
+                                                      (long long)blockIdx.x * blockDim.x + threadIdx.x,
+                                                      (long long)gridDim.x * blockDim.x), nred);
+                if (threadIdx.x == 0) gd.norm_partial[blockIdx.x] = s;
+                grid.sync();
+                float t = 0.f;
+                for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) t += __ldcg(gd.norm_partial + k);
+                t = block_sum(t, nred);
+                gscale = clip_coefficient(t, gd.max_norm);
+                const uint32_t stop = __ldcg(gd.stop);
+                apply = stop == 0u;
+                if (blockIdx.x == 0 && threadIdx.x == 0 && mt != nullptr && stop != 2u) mt[6] = sqrtf(t);
+            }
             // ---- TF ApplyAdam (the arithmetic of adam_kernel), beta powers advanced after the barrier
-            {
+            if (apply) {
                 const float lr_t = a.lr_dev[0];
                 const float p0 = __ldcg(a.adam_powers), p1 = __ldcg(a.adam_powers + 1);
                 const float alpha = lr_t * sqrtf(1.f - p1) / (1.f - p0);
@@ -805,7 +930,8 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
                 float4* m4 = reinterpret_cast<float4*>(a.adam_m);
                 float4* v4 = reinterpret_cast<float4*>(a.adam_v);
                 for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n4; k += (long long)gridDim.x * blockDim.x) {
-                    const float4 gv = __ldcg(g4 + k);
+                    float4 gv = __ldcg(g4 + k);
+                    if (gd.stop != nullptr) { gv.x *= gscale; gv.y *= gscale; gv.z *= gscale; gv.w *= gscale; }
                     float4 mv = m4[k], vv = v4[k], pv = p4[k];
                     mv.x += (gv.x - mv.x) * omb1; mv.y += (gv.y - mv.y) * omb1; mv.z += (gv.z - mv.z) * omb1; mv.w += (gv.w - mv.w) * omb1;
                     vv.x += (gv.x * gv.x - vv.x) * omb2; vv.y += (gv.y * gv.y - vv.y) * omb2;
@@ -816,7 +942,10 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
                 }
             }
             grid.sync();
-            if (blockIdx.x == 0 && threadIdx.x == 0) { a.adam_powers[0] *= 0.9f; a.adam_powers[1] *= 0.999f; }
+            if (blockIdx.x == 0 && threadIdx.x == 0 && apply) {
+                a.adam_powers[0] *= 0.9f; a.adam_powers[1] *= 0.999f;
+                if (gd.steps != nullptr) gd.steps[0] += 1;
+            }
         }
 }
 
@@ -845,7 +974,8 @@ int32_t learn_persistent_init() {
 int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
                      float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
                      const float* states, const float* actions, int T, int num_epochs, int batch_size,
-                     const int32_t* perms, float* metrics, cudaStream_t s) {
+                     const int32_t* perms, float* metrics, const Guards& gd, cudaStream_t s) {
+    const int mcols = gd.stop != nullptr ? 7 : 5;
     // theta_old <- theta (PPO.update_old_policy, ppo.py:275-276)
     CPB_CUDA(cudaMemcpyAsync(params_old, params, L.total * sizeof(float), cudaMemcpyDeviceToDevice, s));
     // log pi_old(a_t|s_t) is constant during the update: evaluate it once for all T samples
@@ -861,6 +991,7 @@ int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPla
         a.params = params; a.grads = grads; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_powers = adam_powers; a.lr_dev = lr_dev;
         a.states = states; a.actions = actions; a.perms = perms; a.metrics = metrics;
         a.T = T; a.batch_size = batch_size; a.num_epochs = num_epochs; a.nmb = nmb;
+        a.gd = gd;
         void* args[] = {&a};
         CPB_CUDA(cudaLaunchCooperativeKernel((void*)ppo_learn_persistent_kernel, dim3((unsigned)g_learn_grid), dim3(kLearnThreads), args, kLearnSmem, s));
         CPB_LAUNCHED();
@@ -871,11 +1002,40 @@ int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPla
             const int begin = i * batch_size;
             const int B = begin + batch_size <= T ? batch_size : T - begin;
             const int32_t* idx = perms + (long long)e * T + begin;
-            float* mt = metrics ? metrics + ((long long)e * nmb + i) * 5 : nullptr;
+            float* mt = metrics ? metrics + ((long long)e * nmb + i) * mcols : nullptr;
             CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
-                                  grads, mt, s));
-            CPB_TRY(launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s));
+                                  grads, mt, gd, s));
+            if (gd.stop != nullptr) {
+                // the minibatches after a stop are still launched (the host cannot know); Adam skips them on the device
+                CPB_TRY(launch_grad_norm(grads, L.total, gd, mt, s));
+                CPB_TRY(launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s,
+                                    gd.stop, gd.clip, gd.steps));
+            } else {
+                CPB_TRY(launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s));
+            }
         }
+    return CPB_OK;
+}
+
+// cpb_ppo_learn_options -> Guards on the plan's guard scratch, refusing bad options before anything is enqueued.  stop:
+// the caller's stop word (train_step), or null for a zeroed word of the call's own (learn).  steps_applied is zeroed.
+int32_t make_guards(const cpb_ppo_learn_options* opts, const PpoPlan& pl, uint32_t* stop, int32_t* steps_applied,
+                    cudaStream_t s, Guards* gd) {
+    float max_norm = 0.f, target_kl = 0.f;
+    if (opts != nullptr) { max_norm = opts->max_grad_norm; target_kl = opts->target_kl; }
+    CPB_REQUIRE(std::isfinite(max_norm) && max_norm >= 0.f, "ppo options: max_grad_norm must be finite and >= 0 (0 = off)");
+    CPB_REQUIRE(std::isfinite(target_kl) && target_kl >= 0.f, "ppo options: target_kl must be finite and >= 0 (0 = off)");
+    memset(gd, 0, sizeof(*gd));
+    gd->stop = stop != nullptr ? stop : pl.guard_words;
+    gd->counter = pl.guard_words + 1;
+    gd->clip = reinterpret_cast<float*>(pl.guard_words + 2);
+    gd->norm_partial = pl.norm_partial;
+    gd->steps = steps_applied;
+    gd->max_norm = max_norm;
+    gd->kl_limit = (float)(1.5 * (double)target_kl);
+    // the plan's own stop word (used when the caller gives none) and the norm reduction's block counter start at 0
+    CPB_CUDA(cudaMemsetAsync(pl.guard_words, 0, 2 * sizeof(uint32_t), s));
+    if (steps_applied != nullptr) CPB_CUDA(cudaMemsetAsync(steps_applied, 0, sizeof(int32_t), s));
     return CPB_OK;
 }
 
@@ -942,7 +1102,7 @@ int32_t cpb_ppo_loss_grad(const cpb_ppo_config* cfg, const float* params, const 
     CPB_TRY(launch_fill_zero(grads, L.total, s));
     CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, idx, batch, s));
     return run_loss_grad(cfg, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
-                         metrics, s);
+                         metrics, Guards{}, s);
 }
 
 int32_t cpb_ppo_train_step(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
@@ -957,6 +1117,27 @@ int32_t cpb_ppo_train_step(const cpb_ppo_config* cfg, float* params, const float
                        (cudaStream_t)stream);
 }
 
+int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
+                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                const float* states, const float* actions, const float* returns,
+                                const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(batch >= 1, "ppo_train_step_opts: batch must be >= 1");
+    CPB_PPO_PLAN(batch, 0);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                returns && advantages, "ppo_train_step_opts: NULL pointer");
+    Guards gd;
+    CPB_TRY(make_guards(opts, pl, stop, steps_applied, s, &gd));
+    CPB_TRY(launch_fill_zero(grads, L.total, s));
+    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, idx, batch, s));
+    CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
+                          metrics, gd, s));
+    CPB_TRY(launch_grad_norm(grads, L.total, gd, metrics, s));
+    return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s, gd.stop,
+                       gd.clip, gd.steps);
+}
+
 int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_value, const double* dones, int32_t T,
                 double gamma, double lam, double* advantages, double* returns, double* advantages_norm, void* stream) {
     CPB_REQUIRE(rewards && values && dones && T >= 1, "gae: bad arguments");
@@ -967,23 +1148,50 @@ int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_va
     return CPB_OK;
 }
 
+// cpb_ppo_learn and its options twin (guarded: opts / steps_applied are used and the metrics rows are 7 wide)
+static int32_t ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+                         float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                         const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                         const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                         int32_t batch_size, const int32_t* perms, float* metrics, bool guarded,
+                         const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                         int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(T >= 1 && batch_size >= 1 && num_epochs >= 0, "ppo_learn: bad sizes");
+    CPB_PPO_PLAN(batch_size < T ? batch_size : T, T);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                rewards && values && dones, "ppo_learn: NULL pointer");
+    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn: perms is NULL");
+    Guards gd{};
+    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
+    // GAE, returns, normalised advantages (float64), rounded to float32 like the reference's feed
+    gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
+                                  pl.ret32, pl.adv32, pl.gae_scratch);
+    CPB_LAUNCHED();
+    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
+                        num_epochs, batch_size, perms, metrics, gd, s);
+}
+
 int32_t cpb_ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
                       float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
                       const float* actions, const double* rewards, const double* values, double bootstrap_value,
                       const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
                       int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
                       int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(T >= 1 && batch_size >= 1 && num_epochs >= 0, "ppo_learn: bad sizes");
-    CPB_PPO_PLAN(batch_size < T ? batch_size : T, T);
-    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
-                rewards && values && dones, "ppo_learn: NULL pointer");
-    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn: perms is NULL");
-    // GAE, returns, normalised advantages (float64), rounded to float32 like the reference's feed
-    gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
-                                  pl.ret32, pl.adv32, pl.gae_scratch);
-    CPB_LAUNCHED();
-    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
-                        num_epochs, batch_size, perms, metrics, s);
+    return ppo_learn(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
+                     bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, false, nullptr, nullptr,
+                     workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_learn_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+                           float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                           const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                           const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                           int32_t batch_size, const int32_t* perms, float* metrics,
+                           const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+    return ppo_learn(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
+                     bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, true, opts,
+                     steps_applied, workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_gae_segments(const double* rewards, const double* values, const double* bootstrap_values, const double* dones,
@@ -996,6 +1204,30 @@ int32_t cpb_gae_segments(const double* rewards, const double* values, const doub
                                advantages, returns, advantages_norm, nullptr, nullptr, (cudaStream_t)stream);
 }
 
+// cpb_ppo_learn_segments and its options twin
+static int32_t ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+                                  float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                  const float* states, const float* actions, const double* rewards,
+                                  const double* values, const double* bootstrap_values, const double* dones,
+                                  const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                  double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                  float* metrics, bool guarded, const cpb_ppo_learn_options* opts,
+                                  int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments && batch_size >= 1 && num_epochs >= 0,
+                "ppo_learn_segments: bad sizes");
+    CPB_PPO_PLAN(batch_size < rows ? batch_size : rows, rows);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                rewards && values && bootstrap_values && dones && segment_offsets, "ppo_learn_segments: NULL pointer");
+    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn_segments: perms is NULL");
+    Guards gd{};
+    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
+    // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
+    CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                                pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
+    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
+                        num_epochs, batch_size, perms, metrics, gd, s);
+}
+
 int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
                                float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
                                const float* actions, const double* rewards, const double* values,
@@ -1003,17 +1235,22 @@ int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* 
                                int32_t num_segments, int32_t rows, double gamma, double lam, int32_t num_epochs,
                                int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
                                int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments && batch_size >= 1 && num_epochs >= 0,
-                "ppo_learn_segments: bad sizes");
-    CPB_PPO_PLAN(batch_size < rows ? batch_size : rows, rows);
-    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
-                rewards && values && bootstrap_values && dones && segment_offsets, "ppo_learn_segments: NULL pointer");
-    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn_segments: perms is NULL");
-    // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
-    CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
-                                pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
-    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
-                        num_epochs, batch_size, perms, metrics, s);
+    return ppo_learn_segments(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
+                              batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_learn_segments_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const double* rewards,
+                                    const double* values, const double* bootstrap_values, const double* dones,
+                                    const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                    double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                    float* metrics, const cpb_ppo_learn_options* opts, int32_t* steps_applied,
+                                    void* workspace, int64_t workspace_bytes, void* stream) {
+    return ppo_learn_segments(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
+                              batch_size, perms, metrics, true, opts, steps_applied, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -11,6 +11,10 @@ Reference surface mirrored (paths relative to the reference repo root):
 Additive entry point: ``learn(...)`` = the driver's whole update block (train.py:171-207: GAE, returns,
 advantage normalisation, theta_old <- theta, epochs x shuffled minibatches) in one C call with no host
 round trips.
+
+Additive options of ``learn`` and ``train`` (off by default, which is the reference's update): ``max_grad_norm`` clips the
+global L2 norm of each minibatch gradient and ``target_kl`` stops the update once the approximate KL between the new and
+the old policy exceeds 1.5 x target_kl (include/carla_ppo_b200.h, "Bounded PPO updates").
 """
 from __future__ import annotations
 
@@ -26,6 +30,14 @@ from ._lib import CpbError, PpoConfig
 
 ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8
 _METRIC_NAMES = ("train_loss/policy", "train_loss/value", "train_loss/entropy", "train_loss/loss", "train/prob_ratio")
+_GUARD_METRIC_NAMES = ("train/approx_kl", "train/grad_norm")     # metric columns 5 and 6 of a guarded update
+
+
+def learn_options(max_grad_norm=None, target_kl=None):
+    """cpb_ppo_learn_options of the two guards (None = off, like 0), or None when both are None."""
+    if max_grad_norm is None and target_kl is None:
+        return None
+    return _lib.PpoLearnOptions(float(max_grad_norm or 0.0), float(target_kl or 0.0))
 
 
 class PPO:
@@ -65,6 +77,8 @@ class PPO:
         self.train_writer = None
         self._ws = None
         self._pending_metrics = []
+        self._pending_applied = []
+        self.last_steps_applied = None       # device int32[1]: Adam steps applied by the last guarded learn / train call
 
     # ------------------------------------------------------------------ session / state
     def _cfg(self):
@@ -292,9 +306,14 @@ class PPO:
         self._sync_lr()
 
     # ------------------------------------------------------------------ hot path
-    def train(self, input_states, taken_actions, returns, advantage):
+    def train(self, input_states, taken_actions, returns, advantage, max_grad_norm=None, target_kl=None, stop=None):
         """ONE minibatch Adam step (ppo.py:218-229).  Metrics stay on the device until the next
-        write_episodic_summaries()."""
+        write_episodic_summaries().
+
+        ``max_grad_norm`` / ``target_kl`` (None = off): the guards of learn() on this step; ``stop`` (a device int32[1]
+        from new_stop_word(), zeroed once per update) carries the KL stop from step to step, so that a loop of train calls
+        stops exactly as learn() does, without a host sync.  With any of the three, the metrics are 7 wide and the step
+        goes through cpb_ppo_train_step_opts."""
         self._require_session()
         torch = self._torch
         s = self._dev(input_states, torch.float32).reshape(-1, self.state_dim)
@@ -304,16 +323,34 @@ class PPO:
         b = s.shape[0]
         if not (a.shape[0] == r.shape[0] == adv.shape[0] == b):
             raise ValueError("train(): inconsistent batch sizes")
-        metrics = torch.empty(5, dtype=torch.float32, device=self._device)
+        opts = learn_options(max_grad_norm, target_kl)
+        if opts is None and stop is not None:
+            opts = learn_options(0.0, 0.0)
+        metrics = torch.empty(5 if opts is None else 7, dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
-        self._call("cpb_ppo_train_step", 
-            C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
-            _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
-            _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), _lib.ptr(ws),
-            ws.numel(), self._stream())
+        if opts is None:
+            self._call("cpb_ppo_train_step", 
+                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+                _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
+                _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), _lib.ptr(ws),
+                ws.numel(), self._stream())
+        else:
+            applied = torch.empty(1, dtype=torch.int32, device=self._device)
+            self._call("cpb_ppo_train_step_opts",
+                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+                _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
+                _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), C.byref(opts),
+                _lib.ptr(stop), _lib.ptr(applied), _lib.ptr(ws), ws.numel(), self._stream())
+            self._pending_applied.append(applied)
+            self.last_steps_applied = applied
         self._pending_metrics.append(metrics)
         self.train_step_counter += 1
         return metrics
+
+    def new_stop_word(self):
+        """A zeroed device stop word for one update of train(..., stop=...) steps."""
+        self._require_session()
+        return self._torch.zeros(1, dtype=self._torch.int32, device=self._device)
 
     def loss_and_grads(self, input_states, taken_actions, returns, advantage):
         """Loss + gradients only (no Adam): returns (metrics[5] ndarray, {name: grad})."""
@@ -372,14 +409,19 @@ class PPO:
         self.params_old.copy_(self.params)
 
     def learn(self, states, actions, values, rewards, dones, last_value, gamma=0.99, lam=0.95, num_epochs=3,
-              batch_size=32, perms=None, return_metrics=False, segment_lengths=None):
+              batch_size=32, perms=None, return_metrics=False, segment_lengths=None, max_grad_norm=None, target_kl=None):
         """train.py:171-207 in one C call: compute_gae -> returns -> normalised advantages ->
         update_old_policy -> num_epochs x ceil(T/batch_size) minibatch steps.  ``perms`` ([num_epochs, T]
         index orders) defaults to np.random permutations like the reference's np.random.shuffle.
 
         ``segment_lengths`` (S lengths, each >= 1, summing to T): the rows are S environments' rollouts concatenated in
         that order and ``last_value`` holds their S bootstrap values.  GAE runs per segment, the advantages are
-        normalised once over all T rows, and the minibatches draw from all of them (cpb_ppo_learn_segments)."""
+        normalised once over all T rows, and the minibatches draw from all of them (cpb_ppo_learn_segments).
+
+        ``max_grad_norm`` (clip the global L2 norm of each minibatch gradient) and ``target_kl`` (skip every Adam step from
+        the first minibatch whose approximate KL exceeds 1.5 x target_kl): None = off.  With either, the update runs
+        through the *_opts entry points, metrics rows are 7 wide (+ approx_kl, pre-clip grad_norm; NaN after a stop) and
+        ``last_steps_applied`` holds the number of Adam steps applied."""
         if segment_lengths is not None:
             rows = int(np.prod(states.shape if hasattr(states, "shape") else np.shape(states))) // self.state_dim
             lengths = [int(n) for n in segment_lengths]
@@ -405,9 +447,27 @@ class PPO:
         else:
             p = self._dev(np.asarray(perms).reshape(num_epochs, t_len), torch.int32)
         nmb = -(-t_len // batch_size)
-        metrics = torch.empty(max(num_epochs * nmb, 1), 5, dtype=torch.float32, device=self._device)
+        opts = learn_options(max_grad_norm, target_kl)
+        ncol = 5 if opts is None else 7
+        metrics = torch.empty(max(num_epochs * nmb, 1), ncol, dtype=torch.float32, device=self._device)
         ws = self._workspace(min(batch_size, t_len), t_len)
-        if segment_lengths is None:
+        if opts is not None:
+            applied = torch.empty(1, dtype=torch.int32, device=self._device)
+            common = (C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+                      _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
+                      _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v))
+            tail = (float(gamma), float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics),
+                    C.byref(opts), _lib.ptr(applied), _lib.ptr(ws), ws.numel(), self._stream())
+            if segment_lengths is None:
+                self._call("cpb_ppo_learn_opts", *common, float(last_value), _lib.ptr(d), t_len, *tail)
+            else:
+                b = self._dev(boot, torch.float64)
+                offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
+                self._call("cpb_ppo_learn_segments_opts", *common, _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
+                           len(lengths), t_len, *tail)
+            self._pending_applied.append(applied)
+            self.last_steps_applied = applied
+        elif segment_lengths is None:
             self._call("cpb_ppo_learn",
                 C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
@@ -426,7 +486,7 @@ class PPO:
         self.train_step_counter += num_epochs * nmb
         self._pending_metrics.append(metrics[:num_epochs * nmb])
         if return_metrics:
-            return metrics[:num_epochs * nmb].cpu().numpy().reshape(num_epochs * nmb, 5)
+            return metrics[:num_epochs * nmb].cpu().numpy().reshape(num_epochs * nmb, ncol)
         return None
 
     # ------------------------------------------------------------------ counters / summaries
@@ -449,14 +509,27 @@ class PPO:
 
     def write_episodic_summaries(self):
         """Episodic means of the per-minibatch metrics, then episode_counter += 1 (ppo.py:271-273) -- which is
-        what decays the learning rate."""
+        what decays the learning rate.  After guarded updates the means cover the evaluated rows only (a KL stop leaves
+        NaN rows), and train/approx_kl, train/grad_norm and train/updates_applied (Adam steps applied) are added."""
         if self._pending_metrics:
             torch = self._torch
-            allm = torch.cat([m.reshape(-1, 5) for m in self._pending_metrics]).double().mean(dim=0).cpu().numpy()
+            guarded = [m.reshape(-1, 7) for m in self._pending_metrics if m.shape[-1] == 7]
+            if not guarded:
+                allm = torch.cat([m.reshape(-1, 5) for m in self._pending_metrics]).double().mean(dim=0).cpu().numpy()
+                extra = []
+            else:
+                rows = torch.cat([m.reshape(-1, m.shape[-1])[:, :5] for m in self._pending_metrics]).double()
+                allm = rows[~torch.isnan(rows[:, 0])].mean(dim=0).cpu().numpy()
+                g = torch.cat(guarded).double()
+                kl_norm = g[~torch.isnan(g[:, 0])][:, 5:7].mean(dim=0).cpu().numpy()
+                unguarded_steps = sum(m.reshape(-1, 5).shape[0] for m in self._pending_metrics if m.shape[-1] == 5)
+                applied = int(torch.cat(self._pending_applied).sum().item()) + unguarded_steps
+                extra = list(zip(_GUARD_METRIC_NAMES, kl_norm)) + [("train/updates_applied", applied)]
             if self.train_writer is not None:
-                for name, val in zip(_METRIC_NAMES, allm):
+                for name, val in list(zip(_METRIC_NAMES, allm)) + extra:
                     self.train_writer.add_scalar(name, float(val), self.episode_counter)
                 self.train_writer.add_scalar("train/learning_rate", float(self.learning_rate), self.episode_counter)
             self._pending_metrics = []
+            self._pending_applied = []
         self.episode_counter += 1
         self._sync_lr()

@@ -11,6 +11,8 @@ hyper-parameter flags and TensorBoard tags, with the neural work on the H100 lib
   * ``--num_envs N``:        N replay environments (seeded seed + i) in lockstep: one batched encode + predict per step
                              (B = number of active environments) and one update per rollout over one trajectory segment
                              per environment (PPO.learn(segment_lengths=...)); N = 1 is the reference's loop
+  * ``--max_grad_norm`` / ``--target_kl``: bound each update (global gradient-norm clipping, approximate-KL early
+                             stopping) on the device, in both the learn and the --reference_loop path; off by default
 """
 from __future__ import annotations
 
@@ -56,6 +58,8 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     eval_interval = params["eval_interval"]
     fused = not params.get("unfused", False)
     reference_loop = params.get("reference_loop", False)
+    # update guards (None = off, the reference's update); only the ones given are passed on
+    guards = {k: params[k] for k in ("max_grad_norm", "target_kl") if params.get(k) is not None}
 
     if isinstance(seed, int):
         np.random.seed(seed)
@@ -207,12 +211,14 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
                 advantages = (advantages - advantages.mean()) / (advantages.std() + 1e-8)
                 s_arr, a_arr = np.array(states), np.array(taken_actions)
                 model.update_old_policy()
+                if guards:                                # one stop word per update: the KL stop lasts for this update only
+                    guards["stop"] = model.new_stop_word()
                 for _ in range(num_epochs):
                     indices = np.arange(T)
                     np.random.shuffle(indices)
                     for i in range(int(np.ceil(T / batch_size))):
                         mb_idx = indices[i * batch_size:(i + 1) * batch_size]
-                        model.train(s_arr[mb_idx], a_arr[mb_idx], returns[mb_idx], advantages[mb_idx])
+                        model.train(s_arr[mb_idx], a_arr[mb_idx], returns[mb_idx], advantages[mb_idx], **guards)
             else:
                 perms = []
                 for _ in range(num_epochs):                               # the same np.random.shuffle stream as the loop above
@@ -222,11 +228,11 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
                 if num_envs == 1:
                     model.learn(np.array(states), np.array(taken_actions), values, rewards, dones, last_values[0],
                                 gamma=discount_factor, lam=gae_lambda, num_epochs=num_epochs, batch_size=batch_size,
-                                perms=np.stack(perms) if perms else None)
+                                perms=np.stack(perms) if perms else None, **guards)
                 else:
                     model.learn(np.array(states), np.array(taken_actions), values, rewards, dones, last_values,
                                 gamma=discount_factor, lam=gae_lambda, num_epochs=num_epochs, batch_size=batch_size,
-                                perms=np.stack(perms) if perms else None, segment_lengths=lengths)
+                                perms=np.stack(perms) if perms else None, segment_lengths=lengths, **guards)
         model.write_value_to_summary("train/reward", float(np.mean(total_reward)), episode_idx)
         log_episode("train", episode_idx, envs)
         model.write_episodic_summaries()
@@ -276,6 +282,10 @@ def main(argv=None):
     parser.add_argument("--reference_loop", action="store_true", help="the reference's Python minibatch loop over PPO.train instead of PPO.learn")
     parser.add_argument("--num_envs", type=int, default=1, help="replay environments stepped in lockstep (seeded seed + i); "
                         "one batched encode + predict per step and one PPO update over all their rollouts")
+    parser.add_argument("--max_grad_norm", type=float, default=None, help="clip the global L2 norm of each minibatch "
+                        "gradient to this value (default: off, like the reference)")
+    parser.add_argument("--target_kl", type=float, default=None, help="stop an update once the approximate KL between the "
+                        "new and the old policy exceeds 1.5 x this value (default: off, like the reference)")
     params = vars(parser.parse_args(argv))
     start_carla = params.pop("start_carla")
     restart = params.pop("restart")

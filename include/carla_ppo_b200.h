@@ -434,6 +434,64 @@ int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* 
                                const int32_t* perms, float* metrics, void* workspace,
                                int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Bounded PPO updates: global gradient-norm clipping and approximate-KL early stopping on the device
+ *
+ * Additions over the reference (which has neither): the *_opts twins below take the arguments of their originals plus
+ * `opts` and `steps_applied` (and train_step a stop word), and write 7-wide metrics rows.  Options are per call; a NULL
+ * `opts` or a 0 field turns that guard off, and a negative, NaN or infinite field is refused (CPB_ERR_INVALID_ARGUMENT)
+ * before anything is enqueued.  With both guards off the parameters, theta_old, Adam m / v, beta powers and metric
+ * columns 0-4 are bit-identical to the original entry point's.
+ *
+ *   max_grad_norm > 0 (torch.nn.utils.clip_grad_norm_): per minibatch n = sqrt(sum g^2) over the 13 policy/ tensors (the
+ *     flat grads buffer; its zero padding adds nothing), c = max_grad_norm / (n + 1e-6), and when c < 1 every gradient is
+ *     multiplied by c before ApplyAdam.  The sums have a fixed order: a repeated call is bit-identical.
+ *   target_kl > 0 (Stable-Baselines3's estimator and rule): each minibatch computes, in its own forward pass and before its
+ *     Adam step, approx_kl = mean_b((r_b - 1) - log r_b) with r_b = exp(logp - logp_old).  If approx_kl > 1.5 * target_kl,
+ *     neither that minibatch's Adam step nor any later one of the call is applied: params, Adam m / v and the beta powers
+ *     are left as they are (theta_old <- theta still happens at the start of learn).  Every learn call starts fresh.
+ *
+ *   metrics: float[num_epochs * ceil(rows / batch)][7] (optional): the five columns of the original, approx_kl, and the
+ *     pre-clip gradient norm n.  The row of the minibatch that stopped the update is written; every later row is NaN.
+ *   steps_applied (optional, device int32[1]): set to the number of Adam steps the call applied.
+ *   After a stop, `grads` is unspecified: the later minibatches are still enqueued (the host cannot know of the stop) and
+ *   computed, but they do not touch the model.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    float max_grad_norm;      /* 0 = off */
+    float target_kl;          /* 0 = off */
+} cpb_ppo_learn_options;
+
+int32_t cpb_ppo_learn_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+                           float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                           const float* states, const float* actions, const double* rewards,
+                           const double* values, double bootstrap_value, const double* dones, int32_t T,
+                           double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                           const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                           int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream);
+
+int32_t cpb_ppo_learn_segments_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const double* rewards,
+                                    const double* values, const double* bootstrap_values, const double* dones,
+                                    const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                                    double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                    const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                                    int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* One minibatch step of a bounded update (the reference's Python loop over PPO.train, with the guards above): metrics
+ * float[7]; steps_applied (optional) is set to 1 when the step was applied, else 0.  stop (device uint32[1], optional)
+ * is the update's stop word, owned by the caller: zero it before the update's first step; a step whose approx_kl
+ * exceeds 1.5 * target_kl sets it, and every step is skipped (NaN metrics row) while it is non-zero, so a loop of these
+ * calls stops exactly as cpb_ppo_learn_opts does, with no host sync.  stop == NULL: the stop lasts for this call only. */
+int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const float* params_old,
+                                float* grads, float* adam_m, float* adam_v, float* adam_powers,
+                                const float* lr_dev, const float* states, const float* actions,
+                                const float* returns, const float* advantages, const int32_t* idx,
+                                int32_t batch, float* metrics, const cpb_ppo_learn_options* opts,
+                                uint32_t* stop, int32_t* steps_applied, void* workspace,
+                                int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
