@@ -59,6 +59,29 @@ class PpoConfig(C.Structure):
                 ("epsilon", C.c_float), ("value_scale", C.c_float), ("entropy_scale", C.c_float)]
 
 
+PPO_MAX_LAYERS = 8
+PPO_DEFAULT_HIDDEN = (500, 300)       # the reference's policy and value trunks (ppo.py:17)
+
+
+class PpoSpec(C.Structure):
+    """cpb_ppo_spec: the policy and value trunks' hidden-layer sizes (1..PPO_MAX_LAYERS each, every width >= 1).
+    base.hidden1 / base.hidden2 stay 0."""
+    _fields_ = [("base", PpoConfig), ("num_policy", C.c_int32), ("policy_sizes", C.c_int32 * PPO_MAX_LAYERS),
+                ("num_value", C.c_int32), ("value_sizes", C.c_int32 * PPO_MAX_LAYERS)]
+
+    @classmethod
+    def of(cls, base, policy_sizes, value_sizes):
+        """The spec of the PPO on `base` (a PpoConfig; its hidden1 / hidden2 are dropped) with these trunks.  Lists longer
+        than PPO_MAX_LAYERS raise here; every other bound is checked by the library."""
+        if len(policy_sizes) > PPO_MAX_LAYERS or len(value_sizes) > PPO_MAX_LAYERS:
+            raise ValueError("at most %d hidden layers per trunk, got %d and %d"
+                             % (PPO_MAX_LAYERS, len(policy_sizes), len(value_sizes)))
+        b = PpoConfig.from_buffer_copy(base)
+        b.hidden1 = b.hidden2 = 0
+        return cls(b, len(policy_sizes), (C.c_int32 * PPO_MAX_LAYERS)(*policy_sizes), len(value_sizes),
+                   (C.c_int32 * PPO_MAX_LAYERS)(*value_sizes))
+
+
 class PpoLearnOptions(C.Structure):
     """cpb_ppo_learn_options: 0 turns a guard off."""
     _fields_ = [("max_grad_norm", C.c_float), ("target_kl", C.c_float)]
@@ -72,6 +95,7 @@ _MC = C.POINTER(MlpVaeConfig)
 _MS = C.POINTER(MlpVaeSpec)
 _PC = C.POINTER(PpoConfig)
 _PO = C.POINTER(PpoLearnOptions)
+_PS = C.POINTER(PpoSpec)
 
 # name -> (restype, argtypes); must list every symbol of include/carla_ppo_b200.h
 PROTOTYPES = {
@@ -137,6 +161,27 @@ PROTOTYPES = {
                                            _f64, _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
     "cpb_ppo_train_step_opts": (_i32, [_PC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _PO, _P, _P, _P,
                                        _i64, _P]),
+    "cpb_ppo_spec_num_tensors": (_i32, [_PS]),
+    "cpb_ppo_spec_tensor_name": (C.c_char_p, [_PS, _i32]),
+    "cpb_ppo_spec_layout": (_i32, [_PS, _P, _P, _P, _P]),
+    "cpb_ppo_spec_workspace_bytes": (_i64, [_PS, _i32, _i32]),
+    "cpb_ppo_spec_forward": (_i32, [_PS, _P, _P, _i32, _P, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_loss_grad": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_train_step": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_train_step_opts": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _PO, _P, _P,
+                                            _P, _i64, _P]),
+    "cpb_ppo_spec_learn": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
+                                  _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_learn_opts": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
+                                       _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_learn_segments": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32, _f64,
+                                           _f64, _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_spec_learn_segments_opts": (_i32, [_PS, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32,
+                                                _f64, _f64, _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_vae_spec_ppo_spec_encode_predict": (_i32, [_VS, _P, _P, _P, _i32, _PS, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
+                                                    _i64, _P]),
+    "cpb_mlpvae_ppo_spec_encode_predict": (_i32, [_MS, _P, _P, _P, _i32, _PS, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
+                                                  _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_vae_spec_buffer_offsets": (_i32, [_VS, _i32, _P, _i32]),

@@ -1,5 +1,5 @@
 """Fused per-step inference of the RL loop: camera frames -> VAE mean -> [latent | measurements] -> PPO action / value in
-ONE C call (cpb_encode_predict; cpb_mlpvae_encode_predict for an MlpVAE), one pinned H2D (frames + measurements + noise)
+ONE C call (cpb_vae_spec_ppo_spec_encode_predict; cpb_mlpvae_ppo_spec_encode_predict for an MlpVAE), one pinned H2D (frames + measurements + noise)
 and one D2H (states + actions + values), for one environment or for N environments stepped in lockstep (B = N).
 
 In the reference every environment step costs two TensorFlow session runs with a host round trip in between:
@@ -92,7 +92,7 @@ class FusedActor:
             out = self._out_dev.data_ptr()
             name = vae._API["encode_predict"]
             _lib.check(getattr(vae._libh, name)(
-                C.byref(cfg), _lib.ptr(vae.params), base, base + n * nf, self._m, C.byref(ppo._c), _lib.ptr(ppo.params),
+                C.byref(cfg), _lib.ptr(vae.params), base, base + n * nf, self._m, C.byref(ppo._spec), _lib.ptr(ppo.params),
                 None if self.greedy else base + n * (nf + 4 * self._m), _lib.ptr(self._latent), out, out + 4 * n * sd,
                 out + 4 * n * (sd + a), _lib.ptr(self._flags), _lib.ptr(ws_v), ws_v.numel(), _lib.ptr(ws_p), ws_p.numel(),
                 vae._stream()), name)

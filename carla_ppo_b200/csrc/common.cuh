@@ -89,6 +89,18 @@ struct Arena {
     }
 };
 
+// The cpb_ppo_spec of a cpb_ppo_config: {hidden1, hidden2} in both trunks
+inline int32_t ppo_spec_of(const cpb_ppo_config* c, cpb_ppo_spec* sp) {
+    CPB_REQUIRE(c != nullptr, "ppo cfg is NULL");
+    memset(sp, 0, sizeof(*sp));
+    sp->base = *c;
+    sp->base.hidden1 = sp->base.hidden2 = 0;
+    sp->num_policy = sp->num_value = 2;
+    sp->policy_sizes[0] = sp->value_sizes[0] = c->hidden1;
+    sp->policy_sizes[1] = sp->value_sizes[1] = c->hidden2;
+    return CPB_OK;
+}
+
 // ---- device helpers -------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {

@@ -14,33 +14,83 @@ namespace cpb {
 
 namespace {
 
-enum PpoTensor { P_W1, P_B1, P_W2, P_B2, P_WM, P_BM, P_LOGSTD, P_V1, P_VB1, P_V2, P_VB2, P_WV, P_BV, P_COUNT };
-const char* kPpoNames[P_COUNT] = {"dense/kernel", "dense/bias", "dense_1/kernel", "dense_1/bias",
-                                  "action_mean/kernel", "action_mean/bias", "action_logstd",
-                                  "dense_2/kernel", "dense_2/bias", "dense_3/kernel", "dense_3/bias",
-                                  "value/kernel", "value/bias"};
+constexpr int kMaxPpoDepth = 8;                          // hidden layers per trunk (cpb_ppo_spec)
+constexpr int kMaxPpoTensors = 4 * kMaxPpoDepth + 5;
+constexpr int kLegacyPpoTensors = 13;                     // two layers per trunk (cpb_ppo_config)
 
+// Hidden-layer count and widths of trunk t (0: policy, 1: value) of a checked spec
+__host__ __device__ __forceinline__ int trunk_depth(const cpb_ppo_spec& sp, int t) { return t ? sp.num_value : sp.num_policy; }
+__host__ __device__ __forceinline__ int trunk_width(const cpb_ppo_spec& sp, int t, int l) {
+    return t ? sp.value_sizes[l] : sp.policy_sizes[l];
+}
+// width of layer l's input: the state for layer 0
+__host__ __device__ __forceinline__ int trunk_in(const cpb_ppo_spec& sp, int t, int l) {
+    return l ? trunk_width(sp, t, l - 1) : sp.base.state_dim;
+}
+__host__ __device__ __forceinline__ int trunk_last(const cpb_ppo_spec& sp, int t) { return trunk_width(sp, t, trunk_depth(sp, t) - 1); }
+__host__ __device__ __forceinline__ int max_depth(const cpb_ppo_spec& sp) {
+    return sp.num_policy > sp.num_value ? sp.num_policy : sp.num_value;
+}
+
+// Tensors in TF creation order (ppo.py:38-66): policy layer l {kernel, bias} at 2l, the action head {action_mean/kernel,
+// action_mean/bias, action_logstd} at 2P, value layer l at 2P + 3 + 2l, value/{kernel, bias} last.  Dense layers are
+// named dense, dense_1, ... across both trunks in that order.
 struct PpoLayout {
-    int64_t off[P_COUNT], size[P_COUNT];
-    int32_t shape[P_COUNT][2];
+    int np, nv, n;
+    int64_t off[kMaxPpoTensors], size[kMaxPpoTensors];
+    int32_t shape[kMaxPpoTensors][2];
     int64_t total;
+    __host__ __device__ int w(int t, int l) const { return t ? 2 * np + 3 + 2 * l : 2 * l; }
+    __host__ __device__ int b(int t, int l) const { return w(t, l) + 1; }
+    __host__ __device__ int wm() const { return 2 * np; }
+    __host__ __device__ int bm() const { return 2 * np + 1; }
+    __host__ __device__ int logstd() const { return 2 * np + 2; }
+    __host__ __device__ int wv() const { return 2 * np + 3 + 2 * nv; }
+    __host__ __device__ int bv() const { return wv() + 1; }
 };
 
-PpoLayout make_ppo_layout(const cpb_ppo_config* c) {
+PpoLayout make_ppo_layout(const cpb_ppo_spec* sp) {
     PpoLayout L;
-    const int S = c->state_dim, A = c->num_actions, H1 = c->hidden1, H2 = c->hidden2;
-    const int shp[P_COUNT][2] = {{S, H1}, {H1, 0}, {H1, H2}, {H2, 0}, {H2, A}, {A, 0}, {A, 0},
-                                 {S, H1}, {H1, 0}, {H1, H2}, {H2, 0}, {H2, 1}, {1, 0}};
+    memset(&L, 0, sizeof(L));
+    const int A = sp->base.num_actions;
+    L.np = sp->num_policy; L.nv = sp->num_value; L.n = 2 * (L.np + L.nv) + 5;
+    auto set = [&](int i, int rows, int cols) { L.shape[i][0] = rows; L.shape[i][1] = cols; };
+    for (int t = 0; t < 2; ++t)
+        for (int l = 0; l < trunk_depth(*sp, t); ++l) {
+            set(L.w(t, l), trunk_in(*sp, t, l), trunk_width(*sp, t, l));
+            set(L.b(t, l), trunk_width(*sp, t, l), 0);
+        }
+    set(L.wm(), trunk_last(*sp, 0), A); set(L.bm(), A, 0); set(L.logstd(), A, 0);
+    set(L.wv(), trunk_last(*sp, 1), 1); set(L.bv(), 1, 0);
     int64_t o = 0;
-    for (int i = 0; i < P_COUNT; ++i) {
-        L.shape[i][0] = shp[i][0];
-        L.shape[i][1] = shp[i][1];
-        L.size[i] = (int64_t)shp[i][0] * (shp[i][1] ? shp[i][1] : 1);
+    for (int i = 0; i < L.n; ++i) {
+        L.size[i] = (int64_t)L.shape[i][0] * (L.shape[i][1] ? L.shape[i][1] : 1);
         L.off[i] = o;
         o += align_up(L.size[i], 64);
     }
     L.total = o;
     return L;
+}
+
+const char* ppo_tensor_name(const cpb_ppo_spec* sp, int i) {
+    static char dense[2 * kMaxPpoDepth][2][24];
+    static const bool ready = [] {
+        for (int k = 0; k < 2 * kMaxPpoDepth; ++k)
+            for (int b = 0; b < 2; ++b) {
+                char suffix[8] = "";
+                if (k) snprintf(suffix, sizeof(suffix), "_%d", k);
+                snprintf(dense[k][b], sizeof(dense[k][b]), "dense%s/%s", suffix, b ? "bias" : "kernel");
+            }
+        return true;
+    }();
+    (void)ready;
+    static const char* heads[5] = {"action_mean/kernel", "action_mean/bias", "action_logstd", "value/kernel", "value/bias"};
+    const int P = sp->num_policy, V = sp->num_value;
+    if (i < 0 || i >= 2 * (P + V) + 5) return nullptr;
+    if (i < 2 * P) return dense[i / 2][i % 2];
+    if (i < 2 * P + 3) return heads[i - 2 * P];
+    if (i < 2 * P + 3 + 2 * V) return dense[P + (i - 2 * P - 3) / 2][(i - 2 * P - 3) % 2];
+    return heads[3 + i - (2 * P + 3 + 2 * V)];
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -223,7 +273,7 @@ __host__ __device__ GemmJob bwd_weight_job(const float* x, const int32_t* idx, i
 
 // ---------------------------------------------------------------------------------------------
 // per-sample head: action mean, value, log-prob, ratio, losses and the gradients w.r.t. the two
-// 300-wide trunk outputs.  One warp per sample.
+// trunk outputs (Hp and Hv wide).  One warp per sample.
 // ---------------------------------------------------------------------------------------------
 constexpr float kLogSqrt2Pi = 0.9189385175704956f;
 constexpr float kEntropyConst = 1.4189385175704956f;
@@ -231,15 +281,15 @@ constexpr int kMaxActions = 4;
 constexpr int kMaxPersistentCtas = 1024;   // upper bound of the persistent learn() grid (one CTA per SM)
 
 struct HeadArgs {
-    const float* h2;       // [B,H2] policy trunk output (post-relu)
-    const float* g2;       // [B,H2] value trunk output (post-relu), may be null (old policy)
+    const float* hp;       // [B,Hp] policy trunk output (post-relu)
+    const float* hv;       // [B,Hv] value trunk output (post-relu), may be null (old policy)
     const float* wm; const float* bm; const float* logstd;   // action head
     const float* wv; const float* bv;                        // value head
     const float* actions; const float* returns; const float* adv;   // [T,A], [T], [T] (gathered through idx)
     const int32_t* idx;
     const float* logp_old_in;   // [T] gathered through idx (learn path) or [B] ungathered (train_step path)
     int logp_old_gathered;
-    int B, H2, A;
+    int B, Hp, Hv, A;
     float low[kMaxActions], high[kMaxActions];
     float eps_clip, value_scale, entropy_scale;
     // outputs
@@ -248,8 +298,8 @@ struct HeadArgs {
     float* v_out;          // [B] or null
     float* dpre;           // [B,A] gradient w.r.t. the action head pre-activation
     float* dv;             // [B]   gradient w.r.t. the value output
-    float* dh2;            // [B,H2] masked gradient w.r.t. policy trunk output
-    float* dg2;            // [B,H2] masked gradient w.r.t. value trunk output
+    float* dhp;            // [B,Hp] masked gradient w.r.t. policy trunk output
+    float* dhv;            // [B,Hv] masked gradient w.r.t. value trunk output
     float* partial;        // [nblocks][8]: policy, value, ratio sums, logstd grads (3..3+A), approx-KL sum (7)
     const float* noise;    // predict path: [B,A] or null
     float* action_out;     // predict path
@@ -261,15 +311,20 @@ struct HeadArgs {
 template <int MODE>
 __device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, float* vals) {
     {
-        const float* h = a.h2 + (long long)b * a.H2;
+        const float* h = a.hp + (long long)b * a.Hp;
+        const float* g = MODE != 0 ? a.hv + (long long)b * a.Hv : nullptr;
         float pre[kMaxActions] = {0.f, 0.f, 0.f, 0.f};
         float vsum = 0.f;
-        for (int j = lane; j < a.H2; j += 32) {
-            const float hv = h[j];
+        // one loop over both trunk outputs: with Hp == Hv every lane sums in the order of a fused loop
+        const int hmax = MODE != 0 && a.Hv > a.Hp ? a.Hv : a.Hp;
+        for (int j = lane; j < hmax; j += 32) {
+            if (j < a.Hp) {
+                const float hv = h[j];
 #pragma unroll
-            for (int k = 0; k < kMaxActions; ++k)
-                if (k < a.A) pre[k] = fmaf(hv, a.wm[j * a.A + k], pre[k]);
-            if (MODE != 0) vsum = fmaf(a.g2[(long long)b * a.H2 + j], a.wv[j], vsum);
+                for (int k = 0; k < kMaxActions; ++k)
+                    if (k < a.A) pre[k] = fmaf(hv, a.wm[j * a.A + k], pre[k]);
+            }
+            if (MODE != 0 && j < a.Hv) vsum = fmaf(g[j], a.wv[j], vsum);
         }
 #pragma unroll
         for (int k = 0; k < kMaxActions; ++k) pre[k] = warp_sum(pre[k]);
@@ -333,13 +388,15 @@ __device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, flo
                         if (k < a.A) a.mu_out[(long long)b * a.A + k] = mu[k];
                 if (a.v_out != nullptr) a.v_out[b] = v;
             }
-            for (int j = lane; j < a.H2; j += 32) {
-                float s = 0.f;
+            for (int j = lane; j < hmax; j += 32) {
+                if (j < a.Hp) {
+                    float s = 0.f;
 #pragma unroll
-                for (int k = 0; k < kMaxActions; ++k)
-                    if (k < a.A) s = fmaf(dp[k], a.wm[j * a.A + k], s);
-                a.dh2[(long long)b * a.H2 + j] = h[j] > 0.f ? s : 0.f;
-                a.dg2[(long long)b * a.H2 + j] = a.g2[(long long)b * a.H2 + j] > 0.f ? dvv * a.wv[j] : 0.f;
+                    for (int k = 0; k < kMaxActions; ++k)
+                        if (k < a.A) s = fmaf(dp[k], a.wm[j * a.A + k], s);
+                    a.dhp[(long long)b * a.Hp + j] = h[j] > 0.f ? s : 0.f;
+                }
+                if (j < a.Hv) a.dhv[(long long)b * a.Hv + j] = g[j] > 0.f ? dvv * a.wv[j] : 0.f;
             }
             vals[0] += fminf(unclipped, clipped);
             vals[1] += (v - ret) * (v - ret);
@@ -649,9 +706,9 @@ int32_t launch_gae_segments(const double* rewards, const double* values, const d
 // workspace plan
 // ---------------------------------------------------------------------------------------------
 struct PpoPlan {
-    float *h1, *h2;        // [2][B,H1], [2][B,H2]  (policy trunk, value trunk)
-    float *dh2, *dh1;      // same shapes
-    float *oh1, *oh2;      // old-policy trunk [rows,H1], [rows,H2]
+    float* h[kMaxPpoDepth];    // layer l of both trunks: [B,Wp_l] policy then [B,Wv_l] value (a trunk past its depth: none)
+    float* dh[kMaxPpoDepth];   // same shapes: masked gradients w.r.t. the layer outputs
+    float* oh[kMaxPpoDepth];   // old-policy trunk [rows,Wp_l], l < P
     float *logp_old;       // [rows]
     float *dpre, *dv, *partial;
     float *ret32, *adv32;  // [T]
@@ -662,18 +719,25 @@ struct PpoPlan {
     bool ok;
 };
 
-PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_config* c, int max_batch, int horizon) {
+// width of trunk t's layer l, 0 past its depth
+__host__ __device__ __forceinline__ int width_or_0(const cpb_ppo_spec& sp, int t, int l) {
+    return l < trunk_depth(sp, t) ? trunk_width(sp, t, l) : 0;
+}
+// trunk t's part of a per-layer buffer (pl.h[l] / pl.dh[l]) at batch B
+__host__ __device__ __forceinline__ float* trunk_buf(float* const* bufs, const cpb_ppo_spec& sp, int t, int l, int B) {
+    return bufs[l] + (t ? (long long)B * width_or_0(sp, 0, l) : 0);
+}
+
+PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_spec* sp, int max_batch, int horizon) {
     PpoPlan p;
     memset(&p, 0, sizeof(p));
     Arena a(ws, ws_bytes);
-    const int64_t B = max_batch, H1 = c->hidden1, H2 = c->hidden2;
+    const int64_t B = max_batch;
     const int64_t rows = horizon > max_batch ? horizon : max_batch;
-    p.h1 = a.take<float>(2 * B * H1);
-    p.h2 = a.take<float>(2 * B * H2);
-    p.dh2 = a.take<float>(2 * B * H2);
-    p.dh1 = a.take<float>(2 * B * H1);
-    p.oh1 = a.take<float>(rows * H1);
-    p.oh2 = a.take<float>(rows * H2);
+    const int D = max_depth(*sp);
+    for (int l = 0; l < D; ++l) p.h[l] = a.take<float>(B * (width_or_0(*sp, 0, l) + width_or_0(*sp, 1, l)));
+    for (int l = D - 1; l >= 0; --l) p.dh[l] = a.take<float>(B * (width_or_0(*sp, 0, l) + width_or_0(*sp, 1, l)));
+    for (int l = 0; l < sp->num_policy; ++l) p.oh[l] = a.take<float>(rows * sp->policy_sizes[l]);
     p.logp_old = a.take<float>(rows);
     p.dpre = a.take<float>(B * kMaxActions);
     p.dv = a.take<float>(B);
@@ -688,102 +752,158 @@ PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_config* c, int m
     return p;
 }
 
-int32_t check_ppo_cfg(const cpb_ppo_config* c) {
-    CPB_REQUIRE(c != nullptr, "ppo cfg is NULL");
-    CPB_REQUIRE(c->state_dim >= 1 && c->hidden1 >= 1 && c->hidden2 >= 1, "ppo: bad layer sizes");
+int32_t check_ppo_spec(const cpb_ppo_spec* sp) {
+    CPB_REQUIRE(sp != nullptr, "ppo spec is NULL");
+    const cpb_ppo_config* c = &sp->base;
+    CPB_REQUIRE(c->hidden1 == 0 && c->hidden2 == 0,
+                "ppo spec: base.hidden1 / base.hidden2 must be 0 (the widths are policy_sizes / value_sizes), got %d, %d",
+                c->hidden1, c->hidden2);
+    CPB_REQUIRE(c->state_dim >= 1, "ppo: state_dim must be >= 1, got %d", c->state_dim);
     CPB_REQUIRE(c->num_actions >= 1 && c->num_actions <= kMaxActions, "ppo: num_actions must be in [1,%d]", kMaxActions);
+    CPB_REQUIRE(sp->num_policy >= 1 && sp->num_policy <= kMaxPpoDepth && sp->num_value >= 1 && sp->num_value <= kMaxPpoDepth,
+                "ppo spec: each trunk needs 1 to %d hidden layers, got %d (policy) and %d (value)", kMaxPpoDepth,
+                sp->num_policy, sp->num_value);
+    for (int t = 0; t < 2; ++t)
+        for (int l = 0; l < trunk_depth(*sp, t); ++l)
+            CPB_REQUIRE(trunk_width(*sp, t, l) >= 1, "ppo spec: %s layer %d has width %d (must be >= 1)",
+                        t ? "value" : "policy", l, trunk_width(*sp, t, l));
     return CPB_OK;
 }
 
-HeadArgs head_args(const cpb_ppo_config* c, const PpoLayout& L, const float* params, int B) {
+HeadArgs head_args(const cpb_ppo_spec* sp, const PpoLayout& L, const float* params, int B) {
+    const cpb_ppo_config* c = &sp->base;
     HeadArgs h;
     memset(&h, 0, sizeof(h));
-    h.wm = params + L.off[P_WM]; h.bm = params + L.off[P_BM]; h.logstd = params + L.off[P_LOGSTD];
-    h.wv = params + L.off[P_WV]; h.bv = params + L.off[P_BV];
-    h.B = B; h.H2 = c->hidden2; h.A = c->num_actions;
+    h.wm = params + L.off[L.wm()]; h.bm = params + L.off[L.bm()]; h.logstd = params + L.off[L.logstd()];
+    h.wv = params + L.off[L.wv()]; h.bv = params + L.off[L.bv()];
+    h.B = B; h.Hp = trunk_last(*sp, 0); h.Hv = trunk_last(*sp, 1); h.A = c->num_actions;
     for (int k = 0; k < kMaxActions; ++k) { h.low[k] = c->action_low[k]; h.high[k] = c->action_high[k]; }
     h.eps_clip = c->epsilon; h.value_scale = c->value_scale; h.entropy_scale = c->entropy_scale;
     return h;
 }
 
 // log pi_old(a|s) for `rows` samples (optionally gathered)
-int32_t run_old_logp(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan& pl, const float* params_old,
+int32_t run_old_logp(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, const float* params_old,
                      const float* states, const float* actions, const int32_t* idx, int rows, cudaStream_t s) {
     GemmBatch gb;
-    gb.job[0] = fwd_job(states, idx, rows, c->state_dim, params_old + L.off[P_W1], c->hidden1, params_old + L.off[P_B1], pl.oh1, 1);
-    CPB_TRY(launch_small_gemm(gb, 1, s));
-    gb.job[0] = fwd_job(pl.oh1, nullptr, rows, c->hidden1, params_old + L.off[P_W2], c->hidden2, params_old + L.off[P_B2], pl.oh2, 1);
-    CPB_TRY(launch_small_gemm(gb, 1, s));
-    HeadArgs h = head_args(c, L, params_old, rows);
-    h.h2 = pl.oh2; h.actions = actions; h.idx = idx; h.logp_out = pl.logp_old;
+    for (int l = 0; l < sp->num_policy; ++l) {
+        gb.job[0] = fwd_job(l ? pl.oh[l - 1] : states, l ? nullptr : idx, rows, trunk_in(*sp, 0, l),
+                            params_old + L.off[L.w(0, l)], sp->policy_sizes[l], params_old + L.off[L.b(0, l)], pl.oh[l], 1);
+        CPB_TRY(launch_small_gemm(gb, 1, s));
+    }
+    HeadArgs h = head_args(sp, L, params_old, rows);
+    h.hp = pl.oh[sp->num_policy - 1]; h.actions = actions; h.idx = idx; h.logp_out = pl.logp_old;
     ppo_head_kernel<0><<<cdiv(rows, 8), 256, 0, s>>>(h);
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
-int32_t run_trunks(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan& pl, const float* params,
+// Forward jobs of layer l: one per trunk that has it (layer 0 reads the states through idx)
+__host__ __device__ __forceinline__ int trunk_fwd_jobs(const cpb_ppo_spec& sp, const PpoLayout& L, const PpoPlan& pl,
+                                                       const float* params, const float* states, const int32_t* idx, int B,
+                                                       int l, GemmJob* jobs) {
+    int n = 0;
+    for (int t = 0; t < 2; ++t) {
+        if (l >= trunk_depth(sp, t)) continue;
+        const float* in = l ? trunk_buf(pl.h, sp, t, l - 1, B) : states;
+        jobs[n++] = fwd_job(in, l ? nullptr : idx, B, trunk_in(sp, t, l), params + L.off[L.w(t, l)], trunk_width(sp, t, l),
+                            params + L.off[L.b(t, l)], trunk_buf(pl.h, sp, t, l, B), 1);
+    }
+    return n;
+}
+
+// Backward jobs of layer l: per trunk that has it, the weight and bias gradients and (l > 0) the masked data gradient into
+// layer l - 1.  Layer 0 reads the states through idx, so its jobs gather (GATHER 2 when idx != null) and the rest do not.
+__host__ __device__ __forceinline__ int trunk_bwd_jobs(const cpb_ppo_spec& sp, const PpoLayout& L, const PpoPlan& pl,
+                                                       const float* params, float* grads, const float* states,
+                                                       const int32_t* idx, int B, int l, GemmJob* jobs) {
+    int n = 0;
+    for (int t = 0; t < 2; ++t) {
+        if (l >= trunk_depth(sp, t)) continue;
+        const float* in = l ? trunk_buf(pl.h, sp, t, l - 1, B) : states;
+        jobs[n++] = bwd_weight_job(in, l ? nullptr : idx, B, trunk_in(sp, t, l), trunk_buf(pl.dh, sp, t, l, B),
+                                   trunk_width(sp, t, l), grads + L.off[L.w(t, l)], grads + L.off[L.b(t, l)]);
+    }
+    if (l > 0)
+        for (int t = 0; t < 2; ++t) {
+            if (l >= trunk_depth(sp, t)) continue;
+            jobs[n++] = bwd_data_job(trunk_buf(pl.dh, sp, t, l, B), B, trunk_width(sp, t, l), params + L.off[L.w(t, l)],
+                                     trunk_in(sp, t, l), trunk_buf(pl.h, sp, t, l - 1, B), trunk_buf(pl.dh, sp, t, l - 1, B));
+        }
+    return n;
+}
+
+// Weight and bias gradients of the action and value heads: gWm[Hp,A] = hp^T dpre, gbm = colsum(dpre); gWv[Hv,1] = hv^T dv
+__host__ __device__ __forceinline__ void head_bwd_jobs(const cpb_ppo_spec& sp, const PpoLayout& L, const PpoPlan& pl,
+                                                       float* grads, int B, GemmJob* jobs) {
+    jobs[0] = bwd_weight_job(trunk_buf(pl.h, sp, 0, sp.num_policy - 1, B), nullptr, B, trunk_last(sp, 0), pl.dpre,
+                             sp.base.num_actions, grads + L.off[L.wm()], grads + L.off[L.bm()]);
+    jobs[1] = bwd_weight_job(trunk_buf(pl.h, sp, 1, sp.num_value - 1, B), nullptr, B, trunk_last(sp, 1), pl.dv, 1,
+                             grads + L.off[L.wv()], grads + L.off[L.bv()]);
+}
+
+int32_t run_trunks(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, const float* params,
                    const float* states, const int32_t* idx, int B, cudaStream_t s) {
-    const int S = c->state_dim, H1 = c->hidden1, H2 = c->hidden2;
     GemmBatch gb;
-    gb.job[0] = fwd_job(states, idx, B, S, params + L.off[P_W1], H1, params + L.off[P_B1], pl.h1, 1);
-    gb.job[1] = fwd_job(states, idx, B, S, params + L.off[P_V1], H1, params + L.off[P_VB1], pl.h1 + (long long)B * H1, 1);
-    CPB_TRY(launch_small_gemm(gb, 2, s));
-    gb.job[0] = fwd_job(pl.h1, nullptr, B, H1, params + L.off[P_W2], H2, params + L.off[P_B2], pl.h2, 1);
-    gb.job[1] = fwd_job(pl.h1 + (long long)B * H1, nullptr, B, H1, params + L.off[P_V2], H2, params + L.off[P_VB2],
-                        pl.h2 + (long long)B * H2, 1);
-    return launch_small_gemm(gb, 2, s);
+    for (int l = 0; l < max_depth(*sp); ++l)
+        CPB_TRY(launch_small_gemm(gb, trunk_fwd_jobs(*sp, L, pl, params, states, idx, B, l, gb.job), s));
+    return CPB_OK;
 }
 
 // forward + loss + gradients for one minibatch; logp_old given (gathered or not)
-int32_t run_loss_grad(const cpb_ppo_config* c, const PpoLayout& L, const PpoPlan& pl, const float* params,
+int32_t run_loss_grad(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, const float* params,
                       const float* states, const float* actions, const float* returns, const float* adv,
                       const int32_t* idx, int B, const float* logp_old, int logp_old_gathered, float* grads,
                       float* metrics, const Guards& gd, cudaStream_t s) {
-    const int S = c->state_dim, H1 = c->hidden1, H2 = c->hidden2, A = c->num_actions;
-    CPB_TRY(run_trunks(c, L, pl, params, states, idx, B, s));
-    float* h1p = pl.h1; float* h1v = pl.h1 + (long long)B * H1;
-    float* h2p = pl.h2; float* h2v = pl.h2 + (long long)B * H2;
-    float* dh2p = pl.dh2; float* dh2v = pl.dh2 + (long long)B * H2;
-    float* dh1p = pl.dh1; float* dh1v = pl.dh1 + (long long)B * H1;
-    HeadArgs h = head_args(c, L, params, B);
-    h.h2 = h2p; h.g2 = h2v; h.actions = actions; h.returns = returns; h.adv = adv; h.idx = idx;
+    const cpb_ppo_config* c = &sp->base;
+    const int P = sp->num_policy, V = sp->num_value, D = max_depth(*sp);
+    CPB_TRY(run_trunks(sp, L, pl, params, states, idx, B, s));
+    HeadArgs h = head_args(sp, L, params, B);
+    h.hp = trunk_buf(pl.h, *sp, 0, P - 1, B); h.hv = trunk_buf(pl.h, *sp, 1, V - 1, B);
+    h.actions = actions; h.returns = returns; h.adv = adv; h.idx = idx;
     h.logp_old_in = logp_old; h.logp_old_gathered = logp_old_gathered;
-    h.dpre = pl.dpre; h.dv = pl.dv; h.dh2 = dh2p; h.dg2 = dh2v; h.partial = pl.partial;
+    h.dpre = pl.dpre; h.dv = pl.dv; h.dhp = trunk_buf(pl.dh, *sp, 0, P - 1, B); h.dhv = trunk_buf(pl.dh, *sp, 1, V - 1, B);
+    h.partial = pl.partial;
     h.kl_term = gd.stop != nullptr;
     const int nblocks = cdiv(B, 8);
     ppo_head_kernel<1><<<nblocks, 256, 0, s>>>(h);
     CPB_LAUNCHED();
-    ppo_finalize_kernel<<<1, 32, 0, s>>>(pl.partial, nblocks, B, A, params + L.off[P_LOGSTD], c->value_scale,
-                                         c->entropy_scale, grads + L.off[P_LOGSTD], metrics, gd);
+    ppo_finalize_kernel<<<1, 32, 0, s>>>(pl.partial, nblocks, B, c->num_actions, params + L.off[L.logstd()], c->value_scale,
+                                         c->entropy_scale, grads + L.off[L.logstd()], metrics, gd);
     CPB_LAUNCHED();
+    // one launch per layer, top down, for both trunks: weight gradients and the data gradient into the layer below.  The
+    // head weight gradients only need the head kernel's outputs and join the top layer's launch (at two layers per trunk:
+    // 6 independent GEMMs), unless that launch gathers the states (one layer in both trunks).
     GemmBatch gb;
-    // everything that only needs the head kernel's outputs goes into ONE launch (6 independent GEMMs):
-    // head weights gWm[H2,A] = h2p^T dpre, gbm = colsum(dpre); gWv[H2,1] = h2v^T dv, gbv = sum(dv);
-    // layer-2 weights of both trunks; layer-2 data gradients of both trunks
-    gb.job[0] = bwd_weight_job(h1p, nullptr, B, H1, dh2p, H2, grads + L.off[P_W2], grads + L.off[P_B2]);
-    gb.job[1] = bwd_weight_job(h1v, nullptr, B, H1, dh2v, H2, grads + L.off[P_V2], grads + L.off[P_VB2]);
-    gb.job[2] = bwd_data_job(dh2p, B, H2, params + L.off[P_W2], H1, h1p, dh1p);
-    gb.job[3] = bwd_data_job(dh2v, B, H2, params + L.off[P_V2], H1, h1v, dh1v);
-    gb.job[4] = bwd_weight_job(h2p, nullptr, B, H2, pl.dpre, A, grads + L.off[P_WM], grads + L.off[P_BM]);
-    gb.job[5] = bwd_weight_job(h2v, nullptr, B, H2, pl.dv, 1, grads + L.off[P_WV], grads + L.off[P_BV]);
-    CPB_TRY(launch_small_gemm(gb, 6, s));
-    // layer 1 of both trunks
-    gb.job[0] = bwd_weight_job(states, idx, B, S, dh1p, H1, grads + L.off[P_W1], grads + L.off[P_B1]);
-    gb.job[1] = bwd_weight_job(states, idx, B, S, dh1v, H1, grads + L.off[P_V1], grads + L.off[P_VB1]);
-    return launch_small_gemm(gb, 2, s);
+    for (int l = D - 1; l >= 0; --l) {
+        int n = trunk_bwd_jobs(*sp, L, pl, params, grads, states, idx, B, l, gb.job);
+        if (l == D - 1) {
+            if (l == 0 && idx != nullptr) {
+                GemmBatch hb;
+                head_bwd_jobs(*sp, L, pl, grads, B, hb.job);
+                CPB_TRY(launch_small_gemm(hb, 2, s));
+            } else {
+                head_bwd_jobs(*sp, L, pl, grads, B, gb.job + n);
+                n += 2;
+            }
+        }
+        CPB_TRY(launch_small_gemm(gb, n, s));
+    }
+    return CPB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
 // The driver's whole update block as ONE persistent cooperative kernel (train.py:171-207 after GAE / theta_old):
-// num_epochs x ceil(T / batch) minibatch steps, each = forward (2 trunks x 2 layers) -> head + loss -> backward ->
-// TF-Adam, with grid-wide barriers between the dependent phases instead of ~9 kernel launches per minibatch (~330
-// launches of 5-30 us kernels per learn() otherwise).  One CTA per SM, 2 independent groups of 128 threads per CTA;
+// num_epochs x ceil(T / batch) minibatch steps, each = forward (one phase per layer index, both trunks) -> head + loss ->
+// backward (one phase per layer index, top down) -> TF-Adam, with grid-wide barriers between the dependent phases instead
+// of ~2 D + 5 kernel launches per minibatch (D = the deeper trunk's depth; ~330 launches of 5-30 us kernels per learn()
+// at the default two layers per trunk).  One CTA per SM, 2 independent groups of 128 threads per CTA;
 // a phase's 32x32 output tiles are dealt round-robin to the 4 x gridDim groups; the arithmetic per tile is the
 // stand-alone small_gemm_kernel's (same gemm_tile), so the results are those of the launch-per-kernel path up to the
 // order in which the per-CTA loss partials are summed.
 // ---------------------------------------------------------------------------------------------
 struct LearnArgs {
-    cpb_ppo_config cfg;
+    cpb_ppo_spec spec;
     PpoLayout L;
     PpoPlan pl;
     float* params; float* grads; float* adam_m; float* adam_v; float* adam_powers;
@@ -794,6 +914,8 @@ struct LearnArgs {
     int T, batch_size, num_epochs, nmb;
     Guards gd;             // gd.stop == nullptr: no guards, 5-wide metrics rows
 };
+// a __grid_constant__ kernel parameter: within the 4 KB parameter space at every architecture (8 layers per trunk)
+static_assert(sizeof(LearnArgs) <= 4096, "LearnArgs exceeds the kernel parameter space");
 
 constexpr int kGroupsPerCta = 2;
 constexpr int kLearnThreads = kGroupsPerCta * kTileThreads;
@@ -830,11 +952,12 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
     __shared__ float red[8][8];
     __shared__ float tot[8];
     __shared__ float nred[kLearnThreads / 32];
-    const cpb_ppo_config& c = a.cfg;
+    const cpb_ppo_spec& sp = a.spec;
+    const cpb_ppo_config& c = sp.base;
     const PpoLayout& L = a.L;
     const PpoPlan& pl = a.pl;
     const Guards& gd = a.gd;
-    const int S = c.state_dim, H1 = c.hidden1, H2 = c.hidden2, A = c.num_actions;
+    const int A = c.num_actions, D = max_depth(sp);
     const int ngroups = gridDim.x * kGroupsPerCta;
     const int gid = blockIdx.x * kGroupsPerCta + threadIdx.x / kTileThreads;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -842,41 +965,37 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
     float* params = a.params;
     float* grads = a.grads;
 
-    // Every CTA runs every minibatch and reaches every grid.sync: the guards only predicate the Adam step, on values every
-    // CTA reads after a grid.sync (the stop word ppo_finalize wrote two barriers earlier, the norm partials of all CTAs).
+    // Every CTA runs every minibatch and reaches every grid.sync: the layer loops run to the same D in every CTA, and the
+    // guards only predicate the Adam step, on values every CTA reads after a grid.sync (the stop word ppo_finalize wrote
+    // two barriers earlier, the norm partials of all CTAs).
     for (int e = 0; e < a.num_epochs; ++e)
         for (int i = 0; i < a.nmb; ++i) {
             const int begin = i * a.batch_size;
             const int B = begin + a.batch_size <= a.T ? a.batch_size : a.T - begin;
             const int32_t* idx = a.perms + (long long)e * a.T + begin;
             float* mt = a.metrics ? a.metrics + ((long long)e * a.nmb + i) * mcols : nullptr;
-            float* h1p = pl.h1; float* h1v = pl.h1 + (long long)B * H1;
-            float* h2p = pl.h2; float* h2v = pl.h2 + (long long)B * H2;
-            float* dh2p = pl.dh2; float* dh2v = pl.dh2 + (long long)B * H2;
-            float* dh1p = pl.dh1; float* dh1v = pl.dh1 + (long long)B * H1;
             GemmJob jobs[6];
-            // ---- forward, layer 1 and 2 of both trunks
-            jobs[0] = fwd_job(a.states, idx, B, S, params + L.off[P_W1], H1, params + L.off[P_B1], h1p, 1);
-            jobs[1] = fwd_job(a.states, idx, B, S, params + L.off[P_V1], H1, params + L.off[P_VB1], h1v, 1);
-            run_phase<1>(jobs, 2, learn_smem, gid, ngroups);
-            grid.sync();
-            jobs[0] = fwd_job(h1p, nullptr, B, H1, params + L.off[P_W2], H2, params + L.off[P_B2], h2p, 1);
-            jobs[1] = fwd_job(h1v, nullptr, B, H1, params + L.off[P_V2], H2, params + L.off[P_VB2], h2v, 1);
-            run_phase<0>(jobs, 2, learn_smem, gid, ngroups);
-            grid.sync();
+            // ---- forward: layer l of both trunks per phase
+            for (int l = 0; l < D; ++l) {
+                const int n = trunk_fwd_jobs(sp, L, pl, params, a.states, idx, B, l, jobs);
+                if (l == 0) run_phase<1>(jobs, n, learn_smem, gid, ngroups);
+                else run_phase<0>(jobs, n, learn_smem, gid, ngroups);
+                grid.sync();
+            }
             // ---- head: one warp per sample, per-CTA partial loss sums
             {
                 HeadArgs h;
-                h.h2 = h2p; h.g2 = h2v;
-                h.wm = params + L.off[P_WM]; h.bm = params + L.off[P_BM]; h.logstd = params + L.off[P_LOGSTD];
-                h.wv = params + L.off[P_WV]; h.bv = params + L.off[P_BV];
+                h.hp = trunk_buf(pl.h, sp, 0, sp.num_policy - 1, B); h.hv = trunk_buf(pl.h, sp, 1, sp.num_value - 1, B);
+                h.wm = params + L.off[L.wm()]; h.bm = params + L.off[L.bm()]; h.logstd = params + L.off[L.logstd()];
+                h.wv = params + L.off[L.wv()]; h.bv = params + L.off[L.bv()];
                 h.actions = a.actions; h.returns = pl.ret32; h.adv = pl.adv32; h.idx = idx;
                 h.logp_old_in = pl.logp_old; h.logp_old_gathered = 1;
-                h.B = B; h.H2 = H2; h.A = A;
+                h.B = B; h.Hp = trunk_last(sp, 0); h.Hv = trunk_last(sp, 1); h.A = A;
                 for (int k = 0; k < kMaxActions; ++k) { h.low[k] = c.action_low[k]; h.high[k] = c.action_high[k]; }
                 h.eps_clip = c.epsilon; h.value_scale = c.value_scale; h.entropy_scale = c.entropy_scale;
                 h.logp_out = nullptr; h.mu_out = nullptr; h.v_out = nullptr;
-                h.dpre = pl.dpre; h.dv = pl.dv; h.dh2 = dh2p; h.dg2 = dh2v; h.partial = pl.partial;
+                h.dpre = pl.dpre; h.dv = pl.dv; h.partial = pl.partial;
+                h.dhp = trunk_buf(pl.dh, sp, 0, sp.num_policy - 1, B); h.dhv = trunk_buf(pl.dh, sp, 1, sp.num_value - 1, B);
                 h.noise = nullptr; h.action_out = nullptr;
                 h.kl_term = gd.stop != nullptr;
                 float vals[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -884,21 +1003,25 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
                 head_block_reduce(vals, red, pl.partial + blockIdx.x * 8);
             }
             grid.sync();
-            // ---- loss metrics + logstd gradient (CTA 0), then everything that only needs the head's outputs
+            // ---- loss metrics + logstd gradient (CTA 0), then the backward pass top down: layer l of both trunks per
+            // phase, the head weight gradients with the top layer (their own tile list when that layer gathers the states)
             if (blockIdx.x == 0)
-                ppo_finalize(pl.partial, gridDim.x, B, A, params + L.off[P_LOGSTD], c.value_scale, c.entropy_scale, grads + L.off[P_LOGSTD], mt, tot, gd);
-            jobs[0] = bwd_weight_job(h1p, nullptr, B, H1, dh2p, H2, grads + L.off[P_W2], grads + L.off[P_B2]);
-            jobs[1] = bwd_weight_job(h1v, nullptr, B, H1, dh2v, H2, grads + L.off[P_V2], grads + L.off[P_VB2]);
-            jobs[2] = bwd_data_job(dh2p, B, H2, params + L.off[P_W2], H1, h1p, dh1p);
-            jobs[3] = bwd_data_job(dh2v, B, H2, params + L.off[P_V2], H1, h1v, dh1v);
-            jobs[4] = bwd_weight_job(h2p, nullptr, B, H2, pl.dpre, A, grads + L.off[P_WM], grads + L.off[P_BM]);
-            jobs[5] = bwd_weight_job(h2v, nullptr, B, H2, pl.dv, 1, grads + L.off[P_WV], grads + L.off[P_BV]);
-            run_phase<0>(jobs, 6, learn_smem, gid, ngroups);
-            grid.sync();
-            jobs[0] = bwd_weight_job(a.states, idx, B, S, dh1p, H1, grads + L.off[P_W1], grads + L.off[P_B1]);
-            jobs[1] = bwd_weight_job(a.states, idx, B, S, dh1v, H1, grads + L.off[P_V1], grads + L.off[P_VB1]);
-            run_phase<2>(jobs, 2, learn_smem, gid, ngroups);
-            grid.sync();
+                ppo_finalize(pl.partial, gridDim.x, B, A, params + L.off[L.logstd()], c.value_scale, c.entropy_scale,
+                             grads + L.off[L.logstd()], mt, tot, gd);
+            for (int l = D - 1; l >= 0; --l) {
+                int n = trunk_bwd_jobs(sp, L, pl, params, grads, a.states, idx, B, l, jobs);
+                if (l > 0) {
+                    if (l == D - 1) { head_bwd_jobs(sp, L, pl, grads, B, jobs + n); n += 2; }
+                    run_phase<0>(jobs, n, learn_smem, gid, ngroups);
+                } else {
+                    run_phase<2>(jobs, n, learn_smem, gid, ngroups);
+                    if (D == 1) {
+                        head_bwd_jobs(sp, L, pl, grads, B, jobs);
+                        run_phase<0>(jobs, 2, learn_smem, gid, ngroups);
+                    }
+                }
+                grid.sync();
+            }
             // ---- guards: per-CTA sums of g^2, a barrier, then the same fixed-order sum of all partials in every CTA
             float gscale = 1.f;
             bool apply = true;
@@ -971,7 +1094,7 @@ int32_t learn_persistent_init() {
 
 // Everything of the driver's update block after GAE (train.py:178-207): theta_old <- theta, the old policy's
 // log-probabilities, and num_epochs x ceil(T / batch_size) minibatch Adam steps reading pl.ret32 / pl.adv32.
-int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
+int32_t learn_update(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
                      float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
                      const float* states, const float* actions, int T, int num_epochs, int batch_size,
                      const int32_t* perms, float* metrics, const Guards& gd, cudaStream_t s) {
@@ -979,7 +1102,7 @@ int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPla
     // theta_old <- theta (PPO.update_old_policy, ppo.py:275-276)
     CPB_CUDA(cudaMemcpyAsync(params_old, params, L.total * sizeof(float), cudaMemcpyDeviceToDevice, s));
     // log pi_old(a_t|s_t) is constant during the update: evaluate it once for all T samples
-    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, nullptr, T, s));
+    CPB_TRY(run_old_logp(sp, L, pl, params_old, states, actions, nullptr, T, s));
     CPB_TRY(launch_fill_zero(grads, L.total, s));
     const int nmb = cdiv(T, batch_size);
     CPB_TRY(learn_persistent_init());
@@ -987,7 +1110,7 @@ int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPla
         // all minibatch steps in ONE cooperative launch
         LearnArgs a;
         memset(&a, 0, sizeof(a));
-        a.cfg = *cfg; a.L = L; a.pl = pl;
+        a.spec = *sp; a.L = L; a.pl = pl;
         a.params = params; a.grads = grads; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_powers = adam_powers; a.lr_dev = lr_dev;
         a.states = states; a.actions = actions; a.perms = perms; a.metrics = metrics;
         a.T = T; a.batch_size = batch_size; a.num_epochs = num_epochs; a.nmb = nmb;
@@ -1003,7 +1126,7 @@ int32_t learn_update(const cpb_ppo_config* cfg, const PpoLayout& L, const PpoPla
             const int B = begin + batch_size <= T ? batch_size : T - begin;
             const int32_t* idx = perms + (long long)e * T + begin;
             float* mt = metrics ? metrics + ((long long)e * nmb + i) * mcols : nullptr;
-            CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
+            CPB_TRY(run_loss_grad(sp, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
                                   grads, mt, gd, s));
             if (gd.stop != nullptr) {
                 // the minibatches after a stop are still launched (the host cannot know); Adam skips them on the device
@@ -1046,13 +1169,27 @@ using namespace cpb;
 
 extern "C" {
 
-int32_t cpb_ppo_num_tensors(void) { return P_COUNT; }
-const char* cpb_ppo_tensor_name(int32_t i) { return (i >= 0 && i < P_COUNT) ? kPpoNames[i] : nullptr; }
+int32_t cpb_ppo_num_tensors(void) { return kLegacyPpoTensors; }
+const char* cpb_ppo_tensor_name(int32_t i) {
+    cpb_ppo_spec sp;
+    memset(&sp, 0, sizeof(sp));
+    sp.num_policy = sp.num_value = 2;
+    return ppo_tensor_name(&sp, i);
+}
 
-int32_t cpb_ppo_layout(const cpb_ppo_config* cfg, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
-    CPB_TRY(check_ppo_cfg(cfg));
-    PpoLayout L = make_ppo_layout(cfg);
-    for (int i = 0; i < P_COUNT; ++i) {
+int32_t cpb_ppo_spec_num_tensors(const cpb_ppo_spec* spec) {
+    CPB_TRY(check_ppo_spec(spec));
+    return 2 * (spec->num_policy + spec->num_value) + 5;
+}
+const char* cpb_ppo_spec_tensor_name(const cpb_ppo_spec* spec, int32_t i) {
+    if (check_ppo_spec(spec) != CPB_OK) return nullptr;
+    return ppo_tensor_name(spec, i);
+}
+
+int32_t cpb_ppo_spec_layout(const cpb_ppo_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
+    CPB_TRY(check_ppo_spec(spec));
+    PpoLayout L = make_ppo_layout(spec);
+    for (int i = 0; i < L.n; ++i) {
         if (offsets) offsets[i] = L.off[i];
         if (sizes) sizes[i] = L.size[i];
         if (shapes) { shapes[i * 2] = L.shape[i][0]; shapes[i * 2 + 1] = L.shape[i][1]; }
@@ -1061,68 +1198,69 @@ int32_t cpb_ppo_layout(const cpb_ppo_config* cfg, int64_t* offsets, int64_t* siz
     return CPB_OK;
 }
 
-int64_t cpb_ppo_workspace_bytes(const cpb_ppo_config* cfg, int32_t max_batch, int32_t horizon) {
-    if (check_ppo_cfg(cfg) != CPB_OK || max_batch < 1 || horizon < 0) return CPB_ERR_INVALID_ARGUMENT;
-    return make_ppo_plan(nullptr, 0, cfg, max_batch, horizon).bytes;
+int64_t cpb_ppo_spec_workspace_bytes(const cpb_ppo_spec* spec, int32_t max_batch, int32_t horizon) {
+    if (check_ppo_spec(spec) != CPB_OK || max_batch < 1 || horizon < 0) return CPB_ERR_INVALID_ARGUMENT;
+    return make_ppo_plan(nullptr, 0, spec, max_batch, horizon).bytes;
 }
 
 #define CPB_PPO_PLAN(maxb, horizon)                                                            \
-    CPB_TRY(check_ppo_cfg(cfg));                                                               \
+    CPB_TRY(check_ppo_spec(spec));                                                             \
     CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                    \
-    PpoPlan pl = make_ppo_plan(workspace, workspace_bytes, cfg, maxb, horizon);                \
+    PpoPlan pl = make_ppo_plan(workspace, workspace_bytes, spec, maxb, horizon);               \
     if (!pl.ok) {                                                                              \
         cpb::set_error("ppo workspace too small: need %lld bytes, got %lld", (long long)pl.bytes, \
                        (long long)workspace_bytes);                                            \
         return CPB_ERR_WORKSPACE_TOO_SMALL;                                                    \
     }                                                                                          \
-    PpoLayout L = make_ppo_layout(cfg);                                                        \
+    PpoLayout L = make_ppo_layout(spec);                                                       \
     cudaStream_t s = (cudaStream_t)stream;
 
-int32_t cpb_ppo_forward(const cpb_ppo_config* cfg, const float* params, const float* states, int32_t batch,
-                        const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
-                        void* stream) {
+int32_t cpb_ppo_spec_forward(const cpb_ppo_spec* spec, const float* params, const float* states, int32_t batch,
+                             const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
+                             void* stream) {
     CPB_REQUIRE(batch >= 1, "ppo_forward: batch must be >= 1");
     CPB_PPO_PLAN(batch, 0);
     CPB_REQUIRE(params && states && action && value, "ppo_forward: NULL pointer");
-    CPB_TRY(run_trunks(cfg, L, pl, params, states, nullptr, batch, s));
-    HeadArgs h = head_args(cfg, L, params, batch);
-    h.h2 = pl.h2; h.g2 = pl.h2 + (long long)batch * cfg->hidden2; h.noise = noise; h.action_out = action; h.v_out = value;
+    CPB_TRY(run_trunks(spec, L, pl, params, states, nullptr, batch, s));
+    HeadArgs h = head_args(spec, L, params, batch);
+    h.hp = trunk_buf(pl.h, *spec, 0, spec->num_policy - 1, batch); h.hv = trunk_buf(pl.h, *spec, 1, spec->num_value - 1, batch);
+    h.noise = noise; h.action_out = action; h.v_out = value;
     ppo_head_kernel<2><<<cdiv(batch, 8), 256, 0, s>>>(h);
     CPB_LAUNCHED();
     return CPB_OK;
 }
 
-int32_t cpb_ppo_loss_grad(const cpb_ppo_config* cfg, const float* params, const float* params_old,
-                          const float* states, const float* actions, const float* returns, const float* advantages,
-                          const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
-                          int64_t workspace_bytes, void* stream) {
+int32_t cpb_ppo_spec_loss_grad(const cpb_ppo_spec* spec, const float* params, const float* params_old,
+                               const float* states, const float* actions, const float* returns, const float* advantages,
+                               const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
     CPB_REQUIRE(batch >= 1, "ppo_loss_grad: batch must be >= 1");
     CPB_PPO_PLAN(batch, 0);
     CPB_REQUIRE(params && params_old && states && actions && returns && advantages && grads, "ppo_loss_grad: NULL pointer");
     CPB_TRY(launch_fill_zero(grads, L.total, s));
-    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, idx, batch, s));
-    return run_loss_grad(cfg, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
+    CPB_TRY(run_old_logp(spec, L, pl, params_old, states, actions, idx, batch, s));
+    return run_loss_grad(spec, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
                          metrics, Guards{}, s);
 }
 
-int32_t cpb_ppo_train_step(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
-                           float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
-                           const float* actions, const float* returns, const float* advantages, const int32_t* idx,
-                           int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
+int32_t cpb_ppo_spec_train_step(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
+                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                                const float* actions, const float* returns, const float* advantages, const int32_t* idx,
+                                int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_REQUIRE(lr_dev != nullptr, "ppo_train_step: lr_dev is NULL");
-    CPB_TRY(cpb_ppo_loss_grad(cfg, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
-                              workspace, workspace_bytes, stream));
-    PpoLayout L = make_ppo_layout(cfg);
+    CPB_TRY(cpb_ppo_spec_loss_grad(spec, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
+                                   workspace, workspace_bytes, stream));
+    PpoLayout L = make_ppo_layout(spec);
     return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f,
                        (cudaStream_t)stream);
 }
 
-int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
-                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
-                                const float* states, const float* actions, const float* returns,
-                                const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
-                                const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
-                                void* workspace, int64_t workspace_bytes, void* stream) {
+int32_t cpb_ppo_spec_train_step_opts(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
+                                     float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                     const float* states, const float* actions, const float* returns,
+                                     const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                     const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                     void* workspace, int64_t workspace_bytes, void* stream) {
     CPB_REQUIRE(batch >= 1, "ppo_train_step_opts: batch must be >= 1");
     CPB_PPO_PLAN(batch, 0);
     CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
@@ -1130,8 +1268,8 @@ int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const 
     Guards gd;
     CPB_TRY(make_guards(opts, pl, stop, steps_applied, s, &gd));
     CPB_TRY(launch_fill_zero(grads, L.total, s));
-    CPB_TRY(run_old_logp(cfg, L, pl, params_old, states, actions, idx, batch, s));
-    CPB_TRY(run_loss_grad(cfg, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
+    CPB_TRY(run_old_logp(spec, L, pl, params_old, states, actions, idx, batch, s));
+    CPB_TRY(run_loss_grad(spec, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
                           metrics, gd, s));
     CPB_TRY(launch_grad_norm(grads, L.total, gd, metrics, s));
     return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s, gd.stop,
@@ -1148,8 +1286,8 @@ int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_va
     return CPB_OK;
 }
 
-// cpb_ppo_learn and its options twin (guarded: opts / steps_applied are used and the metrics rows are 7 wide)
-static int32_t ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+// cpb_ppo_spec_learn and its options twin (guarded: opts / steps_applied are used and the metrics rows are 7 wide)
+static int32_t ppo_learn(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
                          float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
                          const float* actions, const double* rewards, const double* values, double bootstrap_value,
                          const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
@@ -1167,29 +1305,29 @@ static int32_t ppo_learn(const cpb_ppo_config* cfg, float* params, float* params
     gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
                                   pl.ret32, pl.adv32, pl.gae_scratch);
     CPB_LAUNCHED();
-    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
+    return learn_update(spec, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
                         num_epochs, batch_size, perms, metrics, gd, s);
 }
 
-int32_t cpb_ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
-                      float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
-                      const float* actions, const double* rewards, const double* values, double bootstrap_value,
-                      const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
-                      int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
-                      int64_t workspace_bytes, void* stream) {
-    return ppo_learn(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
+int32_t cpb_ppo_spec_learn(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
+                           float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                           const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                           const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                           int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+    return ppo_learn(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
                      bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, false, nullptr, nullptr,
                      workspace, workspace_bytes, stream);
 }
 
-int32_t cpb_ppo_learn_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
-                           float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
-                           const float* actions, const double* rewards, const double* values, double bootstrap_value,
-                           const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
-                           int32_t batch_size, const int32_t* perms, float* metrics,
-                           const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
-                           int64_t workspace_bytes, void* stream) {
-    return ppo_learn(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
+int32_t cpb_ppo_spec_learn_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
+                                float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                                const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                                const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                                int32_t batch_size, const int32_t* perms, float* metrics,
+                                const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+    return ppo_learn(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
                      bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, true, opts,
                      steps_applied, workspace, workspace_bytes, stream);
 }
@@ -1204,8 +1342,8 @@ int32_t cpb_gae_segments(const double* rewards, const double* values, const doub
                                advantages, returns, advantages_norm, nullptr, nullptr, (cudaStream_t)stream);
 }
 
-// cpb_ppo_learn_segments and its options twin
-static int32_t ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
+// cpb_ppo_spec_learn_segments and its options twin
+static int32_t ppo_learn_segments(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
                                   float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
                                   const float* states, const float* actions, const double* rewards,
                                   const double* values, const double* bootstrap_values, const double* dones,
@@ -1224,8 +1362,111 @@ static int32_t ppo_learn_segments(const cpb_ppo_config* cfg, float* params, floa
     // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
     CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
                                 pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
-    return learn_update(cfg, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
+    return learn_update(spec, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
                         num_epochs, batch_size, perms, metrics, gd, s);
+}
+
+int32_t cpb_ppo_spec_learn_segments(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const double* rewards,
+                                    const double* values, const double* bootstrap_values, const double* dones,
+                                    const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                    double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                    float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
+    return ppo_learn_segments(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
+                              batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_spec_learn_segments_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
+                                         float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                         const float* states, const float* actions, const double* rewards,
+                                         const double* values, const double* bootstrap_values, const double* dones,
+                                         const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                         double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                         float* metrics, const cpb_ppo_learn_options* opts, int32_t* steps_applied,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+    return ppo_learn_segments(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
+                              batch_size, perms, metrics, true, opts, steps_applied, workspace, workspace_bytes, stream);
+}
+
+// ---- The two-per-side entry points: the spec twins at {hidden1, hidden2} / {hidden1, hidden2}
+#define CPB_PPO_SPEC_OF(cfg) \
+    cpb_ppo_spec spec_;      \
+    CPB_TRY(ppo_spec_of(cfg, &spec_));
+
+int32_t cpb_ppo_layout(const cpb_ppo_config* cfg, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_layout(&spec_, offsets, sizes, shapes, total);
+}
+
+int64_t cpb_ppo_workspace_bytes(const cpb_ppo_config* cfg, int32_t max_batch, int32_t horizon) {
+    cpb_ppo_spec spec_;
+    if (ppo_spec_of(cfg, &spec_) != CPB_OK) return CPB_ERR_INVALID_ARGUMENT;
+    return cpb_ppo_spec_workspace_bytes(&spec_, max_batch, horizon);
+}
+
+int32_t cpb_ppo_forward(const cpb_ppo_config* cfg, const float* params, const float* states, int32_t batch,
+                        const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
+                        void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_forward(&spec_, params, states, batch, noise, action, value, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_loss_grad(const cpb_ppo_config* cfg, const float* params, const float* params_old,
+                          const float* states, const float* actions, const float* returns, const float* advantages,
+                          const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
+                          int64_t workspace_bytes, void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_loss_grad(&spec_, params, params_old, states, actions, returns, advantages, idx, batch, grads,
+                                  metrics, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_train_step(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
+                           float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                           const float* actions, const float* returns, const float* advantages, const int32_t* idx,
+                           int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_train_step(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                                   returns, advantages, idx, batch, metrics, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const float* params_old, float* grads,
+                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                const float* states, const float* actions, const float* returns,
+                                const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_train_step_opts(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states,
+                                        actions, returns, advantages, idx, batch, metrics, opts, stop, steps_applied,
+                                        workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_learn(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+                      float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                      const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                      const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                      int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                      int64_t workspace_bytes, void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_learn(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                              rewards, values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics,
+                              workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_learn_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
+                           float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                           const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                           const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                           int32_t batch_size, const int32_t* perms, float* metrics,
+                           const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_learn_opts(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                                   rewards, values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms,
+                                   metrics, opts, steps_applied, workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads, float* adam_m,
@@ -1235,9 +1476,11 @@ int32_t cpb_ppo_learn_segments(const cpb_ppo_config* cfg, float* params, float* 
                                int32_t num_segments, int32_t rows, double gamma, double lam, int32_t num_epochs,
                                int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
                                int64_t workspace_bytes, void* stream) {
-    return ppo_learn_segments(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
-                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
-                              batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes, stream);
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_learn_segments(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states,
+                                       actions, rewards, values, bootstrap_values, dones, segment_offsets, num_segments,
+                                       rows, gamma, lam, num_epochs, batch_size, perms, metrics, workspace,
+                                       workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_learn_segments_opts(const cpb_ppo_config* cfg, float* params, float* params_old, float* grads,
@@ -1248,9 +1491,11 @@ int32_t cpb_ppo_learn_segments_opts(const cpb_ppo_config* cfg, float* params, fl
                                     double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
                                     float* metrics, const cpb_ppo_learn_options* opts, int32_t* steps_applied,
                                     void* workspace, int64_t workspace_bytes, void* stream) {
-    return ppo_learn_segments(cfg, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
-                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
-                              batch_size, perms, metrics, true, opts, steps_applied, workspace, workspace_bytes, stream);
+    CPB_PPO_SPEC_OF(cfg);
+    return cpb_ppo_spec_learn_segments_opts(&spec_, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states,
+                                            actions, rewards, values, bootstrap_values, dones, segment_offsets,
+                                            num_segments, rows, gamma, lam, num_epochs, batch_size, perms, metrics, opts,
+                                            steps_applied, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -1415,34 +1415,49 @@ __global__ void assemble_state_kernel(const float* __restrict__ latent, const fl
 typedef int32_t (*EncodeMeanFn)(const void* vae, const float* params, const void* frames, float* latent, int32_t* flags,
                                 void* workspace, int64_t workspace_bytes, void* stream);
 
-// cpb_encode_predict and cpb_mlpvae_encode_predict: `encode` on the VAE described by `vae` (whose common part is `base`),
-// then the state assembly and the PPO forward
+// The encode_predict entry points: `encode` on the VAE described by `vae` (whose common part is `base`), then the state
+// assembly and the PPO forward.  The PPO spec is checked before anything is enqueued.
 static int32_t encode_predict(const cpb_vae_config* base, const void* vae, EncodeMeanFn encode, const float* vae_params,
-                              const void* frames, const float* measurements, int32_t num_measurements, const cpb_ppo_config* ppo_cfg,
+                              const void* frames, const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
                               const float* ppo_params, const float* noise, float* latent_tmp, float* state, float* action,
                               float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes, void* ppo_workspace,
                               int64_t ppo_workspace_bytes, void* stream) {
-    CPB_REQUIRE(base && ppo_cfg && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
+    CPB_REQUIRE(base && ppo_spec && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
     CPB_REQUIRE(num_measurements >= 0 && (num_measurements == 0 || measurements != nullptr), "encode_predict: bad measurements");
-    CPB_REQUIRE(ppo_cfg->state_dim == base->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
-                ppo_cfg->state_dim, base->z_dim, num_measurements);
     const int B = base->batch;
+    const int32_t ppo_tensors = cpb_ppo_spec_num_tensors(ppo_spec);   // checks the spec
+    if (ppo_tensors < 0) return ppo_tensors;
+    CPB_REQUIRE(ppo_spec->base.state_dim == base->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
+                ppo_spec->base.state_dim, base->z_dim, num_measurements);
     CPB_TRY(encode(vae, vae_params, frames, latent_tmp, flags, vae_workspace, vae_workspace_bytes, stream));
-    const int total = B * ppo_cfg->state_dim;
+    const int total = B * ppo_spec->base.state_dim;
     assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, base->z_dim, num_measurements, state);
     CPB_LAUNCHED();
-    return cpb_ppo_forward(ppo_cfg, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
+    return cpb_ppo_spec_forward(ppo_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
 }
 
 int32_t cpb_vae_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
                                     int32_t num_measurements, const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
                                     float* latent_tmp, float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
                                     int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
+    cpb_ppo_spec ppo_spec;
+    CPB_TRY(ppo_spec_of(ppo_cfg, &ppo_spec));
+    return cpb_vae_spec_ppo_spec_encode_predict(spec, vae_params, frames, measurements, num_measurements, &ppo_spec, ppo_params,
+                                                noise, latent_tmp, state, action, value, flags, vae_workspace,
+                                                vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_vae_spec_ppo_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                             const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
+                                             const float* ppo_params, const float* noise, float* latent_tmp, float* state,
+                                             float* action, float* value, int32_t* flags, void* vae_workspace,
+                                             int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
+                                             void* stream) {
     EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
                              int64_t ws_bytes, void* stream) {
         return cpb_vae_spec_encode((const cpb_vae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
     };
-    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_cfg,
+    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_spec,
                           ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
                           ppo_workspace, ppo_workspace_bytes, stream);
 }
@@ -1693,11 +1708,24 @@ int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_
                                   int32_t num_measurements, const cpb_ppo_config* ppo_cfg, const float* ppo_params, const float* noise,
                                   float* latent_tmp, float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
                                   int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
+    cpb_ppo_spec ppo_spec;
+    CPB_TRY(ppo_spec_of(ppo_cfg, &ppo_spec));
+    return cpb_mlpvae_ppo_spec_encode_predict(spec, vae_params, frames, measurements, num_measurements, &ppo_spec, ppo_params, noise,
+                                              latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
+                                              ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_ppo_spec_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                           const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
+                                           const float* ppo_params, const float* noise, float* latent_tmp, float* state,
+                                           float* action, float* value, int32_t* flags, void* vae_workspace,
+                                           int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
+                                           void* stream) {
     EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
                              int64_t ws_bytes, void* stream) {
         return cpb_mlpvae_spec_encode((const cpb_mlpvae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
     };
-    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_cfg,
+    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_spec,
                           ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
                           ppo_workspace, ppo_workspace_bytes, stream);
 }

@@ -15,6 +15,11 @@ round trips.
 Additive options of ``learn`` and ``train`` (off by default, which is the reference's update): ``max_grad_norm`` clips the
 global L2 norm of each minibatch gradient and ``target_kl`` stops the update once the approximate KL between the new and
 the old policy exceeds 1.5 x target_kl (include/carla_ppo_b200.h, "Bounded PPO updates").
+
+Additive constructor arguments ``policy_hidden_sizes`` / ``value_hidden_sizes`` (default: the reference's 500, 300 for
+both) size the two trunks independently, 1 to 8 dense + ReLU layers each, like Stable-Baselines3's
+``net_arch=dict(pi=[...], vf=[...])``.  Every call goes through the cpb_ppo_spec_* entry points; checkpoints carry the
+architecture in their variable names and shapes (``checkpoint_architecture``).
 """
 from __future__ import annotations
 
@@ -26,7 +31,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from ._lib import CpbError, PpoConfig
+from ._lib import CpbError, PpoConfig, PpoSpec
 
 ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8
 _METRIC_NAMES = ("train_loss/policy", "train_loss/value", "train_loss/entropy", "train_loss/loss", "train/prob_ratio")
@@ -40,9 +45,96 @@ def learn_options(max_grad_norm=None, target_kl=None):
     return _lib.PpoLearnOptions(float(max_grad_norm or 0.0), float(target_kl or 0.0))
 
 
+ARCH_KEYS = ("ppo_architecture/policy_hidden_sizes", "ppo_architecture/value_hidden_sizes")
+
+
+def _fmt(arch):
+    return "policy %s / value %s" % (list(arch[0]), list(arch[1]))
+
+
+def _inferred_architectures(blob, scope):
+    """Every (policy_sizes, value_sizes) that the dense kernels of a blob can be read as, from their names (dense,
+    dense_1, ... in creation order: the policy trunk, then the value trunk) and shapes."""
+    kernels = []
+    while True:
+        name = "%sdense%s/kernel" % (scope, "_%d" % len(kernels) if kernels else "")
+        if name not in blob:
+            break
+        kernels.append(np.shape(blob[name]))
+    if len(kernels) < 2 or scope + "action_mean/kernel" not in blob or scope + "value/kernel" not in blob:
+        raise ValueError("not a PPO checkpoint: expected %sdense .. dense_N, action_mean and value kernels" % scope)
+    state_dim = kernels[0][0]
+    p_last, v_last = np.shape(blob[scope + "action_mean/kernel"])[0], np.shape(blob[scope + "value/kernel"])[0]
+    chain = lambda ks: all(ks[i][0] == ks[i - 1][1] for i in range(1, len(ks)))
+    out = []
+    for n_pol in range(1, len(kernels)):
+        pol, val = kernels[:n_pol], kernels[n_pol:]
+        if chain(pol) and chain(val) and val[0][0] == state_dim and pol[-1][1] == p_last and val[-1][1] == v_last:
+            out.append((tuple(int(k[1]) for k in pol), tuple(int(k[1]) for k in val)))
+    if not out:
+        raise ValueError("the dense kernels of this checkpoint form no policy / value pair of trunks: %r" % (kernels,))
+    return out
+
+
+def blob_architecture(blob, scope="policy/"):
+    """(policy_sizes, value_sizes) of a checkpoint blob.  ``save`` records it (ARCH_KEYS), and the recorded lists must
+    agree with the variables' names and shapes.  A checkpoint without the record (the reference's) is read from the names
+    and shapes alone; when those fit more than one split between the trunks (a hidden width equal to the state size can
+    make the boundary invisible), it is refused rather than guessed.  Raises ValueError."""
+    found = _inferred_architectures(blob, scope)
+    if ARCH_KEYS[0] in blob and ARCH_KEYS[1] in blob:
+        rec = tuple(tuple(int(v) for v in np.asarray(blob[k]).reshape(-1)) for k in ARCH_KEYS)
+        if rec not in found:
+            raise ValueError("the checkpoint records %s, which its variables do not have (they fit %s)"
+                             % (_fmt(rec), " or ".join(_fmt(a) for a in found)))
+        return rec
+    if len(found) > 1:
+        raise ValueError("the checkpoint's variables fit several architectures (%s) and it does not record which one it is"
+                         % ", ".join(_fmt(a) for a in found))
+    return found[0]
+
+
+def _latest_checkpoint_prefix(checkpoint_dir):
+    """The path prefix that checkpoint_dir's ``checkpoint`` state file names, or None."""
+    state = os.path.join(checkpoint_dir, "checkpoint")
+    if not os.path.isfile(state):
+        return None
+    with open(state) as f:
+        m = re.search(r'^model_checkpoint_path:\s*"(.*)"', f.read(), re.M)
+    if not m:
+        return None
+    prefix = m.group(1)
+    return prefix if os.path.isabs(prefix) else os.path.join(checkpoint_dir, prefix)
+
+
+def _read_blob(prefix):
+    """The variables of the .npz or TF-bundle checkpoint at prefix, or None when neither file exists."""
+    if os.path.isfile(prefix + ".npz"):
+        return dict(np.load(prefix + ".npz"))
+    if os.path.isfile(prefix + ".index"):
+        from .tf_bundle import BundleReader
+        return BundleReader(prefix).all()
+    return None
+
+
+def checkpoint_architecture(checkpoint_dir):
+    """(policy_hidden_sizes, value_hidden_sizes) of the latest checkpoint in checkpoint_dir (a PPO's
+    ``checkpoint_dir``), or None when there is none.  Raises ValueError for a file that is not a PPO checkpoint or whose
+    architecture is ambiguous (blob_architecture)."""
+    prefix = _latest_checkpoint_prefix(checkpoint_dir)
+    blob = _read_blob(prefix) if prefix is not None else None
+    return None if blob is None else blob_architecture(blob)
+
+
 class PPO:
     def __init__(self, input_shape, action_space, learning_rate=3e-4, lr_decay=0.998, epsilon=0.2,
-                 value_scale=0.5, entropy_scale=0.01, initial_std=0.4, model_dir="./", seed=None, device=None):
+                 value_scale=0.5, entropy_scale=0.01, initial_std=0.4, model_dir="./", seed=None, device=None,
+                 policy_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN, value_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN):
+        self.policy_hidden_sizes = tuple(int(v) for v in policy_hidden_sizes)
+        self.value_hidden_sizes = tuple(int(v) for v in value_hidden_sizes)
+        for name, sizes in (("policy_hidden_sizes", self.policy_hidden_sizes), ("value_hidden_sizes", self.value_hidden_sizes)):
+            if not 1 <= len(sizes) <= _lib.PPO_MAX_LAYERS or min(sizes) < 1:
+                raise ValueError("%s: 1 to %d widths, each >= 1, got %r" % (name, _lib.PPO_MAX_LAYERS, sizes))
         input_shape = tuple(int(v) for v in np.atleast_1d(input_shape))
         if len(input_shape) != 1:
             raise ValueError("PPO expects a flat state vector (reference train.py:85 builds [z_dim + measurements])")
@@ -81,9 +173,22 @@ class PPO:
         self.last_steps_applied = None       # device int32[1]: Adam steps applied by the last guarded learn / train call
 
     # ------------------------------------------------------------------ session / state
+    @property
+    def architecture(self):
+        """(policy_hidden_sizes, value_hidden_sizes)"""
+        return self.policy_hidden_sizes, self.value_hidden_sizes
+
+    def _legacy_widths(self):
+        """(hidden1, hidden2) of the cpb_ppo_config that describes this network: its two widths when both trunks are
+        the same two layers, else (0, 0) (only a cpb_ppo_spec describes it)."""
+        two = len(self.policy_hidden_sizes) == 2 and self.policy_hidden_sizes == self.value_hidden_sizes
+        return self.policy_hidden_sizes if two else (0, 0)
+
     def _cfg(self):
+        """The cpb_ppo_config of this agent (hidden1 / hidden2 from _legacy_widths)."""
         cfg = PpoConfig()
-        cfg.state_dim, cfg.num_actions, cfg.hidden1, cfg.hidden2 = self.state_dim, self.num_actions, 500, 300
+        h1, h2 = self._legacy_widths()
+        cfg.state_dim, cfg.num_actions, cfg.hidden1, cfg.hidden2 = self.state_dim, self.num_actions, h1, h2
         for k in range(4):
             cfg.action_low[k] = float(self.action_low[k]) if k < self.num_actions else 0.0
             cfg.action_high[k] = float(self.action_high[k]) if k < self.num_actions else 0.0
@@ -101,11 +206,15 @@ class PPO:
             self._device = torch.device("cuda", torch.cuda.current_device())
         dev = self._device
         self._c = self._cfg()
-        n = lib.cpb_ppo_num_tensors()
+        if (self._c.hidden1, self._c.hidden2) != tuple(self._legacy_widths()):
+            # a subclass that sizes the network through _cfg(), as the two-width interface did: its widths, both trunks
+            self.policy_hidden_sizes = self.value_hidden_sizes = (int(self._c.hidden1), int(self._c.hidden2))
+        self._spec = PpoSpec.of(self._c, self.policy_hidden_sizes, self.value_hidden_sizes)
+        n = _lib.check(lib.cpb_ppo_spec_num_tensors(C.byref(self._spec)), "cpb_ppo_spec_num_tensors")
         offs = (C.c_int64 * n)(); sizes = (C.c_int64 * n)(); shapes = (C.c_int32 * (2 * n))()
         total = C.c_int64()
-        _lib.check(lib.cpb_ppo_layout(C.byref(self._c), offs, sizes, shapes, C.byref(total)), "cpb_ppo_layout")
-        self._names = [lib.cpb_ppo_tensor_name(i).decode() for i in range(n)]
+        _lib.check(lib.cpb_ppo_spec_layout(C.byref(self._spec), offs, sizes, shapes, C.byref(total)), "cpb_ppo_spec_layout")
+        self._names = [lib.cpb_ppo_spec_tensor_name(C.byref(self._spec), i).decode() for i in range(n)]
         self._offsets = {self._names[i]: int(offs[i]) for i in range(n)}
         self._shapes = {self._names[i]: tuple(int(s) for s in shapes[2 * i:2 * i + 2] if s > 0) for i in range(n)}
         self._total = int(total.value)
@@ -204,8 +313,8 @@ class PPO:
             return _lib.check(getattr(self._libh, name)(*args), name)
 
     def _workspace(self, max_batch, horizon=0):
-        need = self._libh.cpb_ppo_workspace_bytes(C.byref(self._c), int(max_batch), int(horizon))
-        _lib.check(need, "cpb_ppo_workspace_bytes")
+        need = self._libh.cpb_ppo_spec_workspace_bytes(C.byref(self._spec), int(max_batch), int(horizon))
+        _lib.check(need, "cpb_ppo_spec_workspace_bytes")
         if self._ws is None or self._ws.numel() < need:
             self._ws = None
             self._ws = self._torch.empty(int(need), dtype=self._torch.uint8, device=self._device)
@@ -239,6 +348,8 @@ class PPO:
         blob["episode_counter"] = np.int32(self.episode_counter)
         blob["train_step_counter"] = np.int32(self.train_step_counter)
         blob["predict_step_counter"] = np.int32(self.predict_step_counter)
+        for key, sizes in zip(ARCH_KEYS, self.architecture):
+            blob[key] = np.asarray(sizes, np.int32)
         if tf_format:
             from .tf_bundle import write_bundle
             write_bundle(prefix, {k: np.asarray(v) for k, v in blob.items()})
@@ -266,23 +377,12 @@ class PPO:
     def load_latest_checkpoint(self):
         """True / False (restore raised) / None (no checkpoint), like ppo.py:207-216."""
         self._require_session()
-        from .tf_bundle import BundleReader
-        state = os.path.join(self.checkpoint_dir, "checkpoint")
-        if not os.path.isfile(state):
+        prefix = _latest_checkpoint_prefix(self.checkpoint_dir)
+        if prefix is None:
             return None
-        with open(state) as f:
-            m = re.search(r'^model_checkpoint_path:\s*"(.*)"', f.read(), re.M)
-        if not m:
-            return None
-        prefix = m.group(1)
-        if not os.path.isabs(prefix):
-            prefix = os.path.join(self.checkpoint_dir, prefix)
         try:
-            if os.path.isfile(prefix + ".npz"):
-                blob = dict(np.load(prefix + ".npz"))
-            elif os.path.isfile(prefix + ".index"):
-                blob = BundleReader(prefix).all()
-            else:
+            blob = _read_blob(prefix)
+            if blob is None:
                 return None
             self.load_blob(blob)
             print("Model checkpoint restored from {}".format(prefix))
@@ -292,6 +392,10 @@ class PPO:
             return False
 
     def load_blob(self, blob):
+        """Restore from a checkpoint's variables; a checkpoint of another architecture is refused (ValueError)."""
+        found = blob_architecture(blob)
+        if found != self.architecture:
+            raise ValueError("checkpoint architecture %s does not match this PPO's %s" % (_fmt(found), _fmt(self.architecture)))
         pol = {n: blob["policy/" + n] for n in self._names}
         old = {n: blob["policy_old/" + n] for n in self._names}
         m_ = v_ = pw = None
@@ -329,15 +433,15 @@ class PPO:
         metrics = torch.empty(5 if opts is None else 7, dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
         if opts is None:
-            self._call("cpb_ppo_train_step", 
-                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+            self._call("cpb_ppo_spec_train_step", 
+                C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), _lib.ptr(ws),
                 ws.numel(), self._stream())
         else:
             applied = torch.empty(1, dtype=torch.int32, device=self._device)
-            self._call("cpb_ppo_train_step_opts",
-                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+            self._call("cpb_ppo_spec_train_step_opts",
+                C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), C.byref(opts),
                 _lib.ptr(stop), _lib.ptr(applied), _lib.ptr(ws), ws.numel(), self._stream())
@@ -363,8 +467,8 @@ class PPO:
         b = s.shape[0]
         metrics = torch.empty(5, dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
-        self._call("cpb_ppo_loss_grad", 
-            C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(s), _lib.ptr(a), _lib.ptr(r),
+        self._call("cpb_ppo_spec_loss_grad", 
+            C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(s), _lib.ptr(a), _lib.ptr(r),
             _lib.ptr(adv), None, b, _lib.ptr(self.grads), _lib.ptr(metrics), _lib.ptr(ws), ws.numel(),
             self._stream())
         return metrics.cpu().numpy(), self.get_grads()
@@ -388,7 +492,7 @@ class PPO:
         nz = None if greedy else dev[b * self.state_dim:]
         out = torch.empty(b * (a_dim + 1), dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
-        self._call("cpb_ppo_forward", C.byref(self._c), _lib.ptr(self.params), _lib.ptr(s), b, _lib.ptr(nz),
+        self._call("cpb_ppo_spec_forward", C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(s), b, _lib.ptr(nz),
                                               _lib.ptr(out), _lib.ptr(out[b * a_dim:]), _lib.ptr(ws), ws.numel(),
                                               self._stream())
         host = out.cpu().numpy()
@@ -453,23 +557,23 @@ class PPO:
         ws = self._workspace(min(batch_size, t_len), t_len)
         if opts is not None:
             applied = torch.empty(1, dtype=torch.int32, device=self._device)
-            common = (C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+            common = (C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                       _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                       _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v))
             tail = (float(gamma), float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics),
                     C.byref(opts), _lib.ptr(applied), _lib.ptr(ws), ws.numel(), self._stream())
             if segment_lengths is None:
-                self._call("cpb_ppo_learn_opts", *common, float(last_value), _lib.ptr(d), t_len, *tail)
+                self._call("cpb_ppo_spec_learn_opts", *common, float(last_value), _lib.ptr(d), t_len, *tail)
             else:
                 b = self._dev(boot, torch.float64)
                 offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
-                self._call("cpb_ppo_learn_segments_opts", *common, _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
+                self._call("cpb_ppo_spec_learn_segments_opts", *common, _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
                            len(lengths), t_len, *tail)
             self._pending_applied.append(applied)
             self.last_steps_applied = applied
         elif segment_lengths is None:
-            self._call("cpb_ppo_learn",
-                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+            self._call("cpb_ppo_spec_learn",
+                C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), float(last_value), _lib.ptr(d), t_len, float(gamma),
                 float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics), _lib.ptr(ws), ws.numel(),
@@ -477,8 +581,8 @@ class PPO:
         else:
             b = self._dev(boot, torch.float64)
             offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
-            self._call("cpb_ppo_learn_segments",
-                C.byref(self._c), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
+            self._call("cpb_ppo_spec_learn_segments",
+                C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
                 len(lengths), t_len, float(gamma), float(lam), int(num_epochs), int(batch_size), _lib.ptr(p),

@@ -8,6 +8,19 @@ import os
 import numpy as np
 
 
+def load_model(input_shape, action_space, model_dir):
+    """The PPO of model_dir, built at its latest checkpoint's architecture (the reference's 500, 300 when there is none)
+    and restored from it (``load_latest_checkpoint``'s result is printed, as in the reference)."""
+    from ._lib import PPO_DEFAULT_HIDDEN
+    from .ppo import PPO, checkpoint_architecture
+    arch = checkpoint_architecture("{}/checkpoints/".format(model_dir)) or (PPO_DEFAULT_HIDDEN, PPO_DEFAULT_HIDDEN)
+    model = PPO(input_shape, action_space, model_dir=model_dir, seed=0, policy_hidden_sizes=arch[0],
+                value_hidden_sizes=arch[1])
+    model.init_session(init_logging=False)
+    model.load_latest_checkpoint()
+    return model
+
+
 def run_eval(env, model, video_filename=None, actor=None):
     """One greedy episode (std = 0, run_eval.py:51); returns the total reward.  ``actor`` (FusedActor, optional) serves
     the per-step encode + predict in one C call."""
@@ -48,7 +61,6 @@ def run_eval(env, model, video_filename=None, actor=None):
 def main(argv=None):
     import argparse
     from .actor import FusedActor
-    from .ppo import PPO
     from .replay_env import ReplayEnv, reward_functions
     from .train import load_replay_frames
     from .vae_common import create_encode_state_fn, load_vae
@@ -77,9 +89,7 @@ def main(argv=None):
     np.random.seed(0)
     env.seed(0)
     input_shape = np.array([vae.z_dim + len(measurements_to_include)])
-    model = PPO(input_shape, env.action_space, model_dir=os.path.join(args.models_root, args.model_name), seed=0)
-    model.init_session(init_logging=False)
-    model.load_latest_checkpoint()
+    model = load_model(input_shape, env.action_space, os.path.join(args.models_root, args.model_name))
     actor = None
     if not args.unfused:
         actor = FusedActor(vae, model, measurements_to_include)

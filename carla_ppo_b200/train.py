@@ -22,7 +22,8 @@ import shutil
 
 import numpy as np
 
-from .ppo import PPO
+from ._lib import PPO_DEFAULT_HIDDEN
+from .ppo import PPO, checkpoint_architecture
 from .replay_env import ReplayEnv, reward_functions
 from .run_eval import run_eval
 from .utils import compute_gae
@@ -43,6 +44,20 @@ def load_replay_frames(path, limit=None):
     if not names:
         raise FileNotFoundError("no PNG frames under %s" % d)
     return np.stack([np.asarray(Image.open(os.path.join(d, f)))[:, :, :3] for f in names])
+
+
+def resolve_architecture(policy_sizes, value_sizes, checkpoint_arch):
+    """(policy_hidden_sizes, value_hidden_sizes) of a run: the checkpoint's when resuming one (a given size list must
+    equal it), else the given lists, else the reference's 500, 300.  Raises ValueError on a disagreement."""
+    given = (None if policy_sizes is None else tuple(int(v) for v in policy_sizes),
+             None if value_sizes is None else tuple(int(v) for v in value_sizes))
+    if checkpoint_arch is None:
+        return tuple(g if g is not None else PPO_DEFAULT_HIDDEN for g in given)
+    for flag, g, c in zip(("--policy_hidden_sizes", "--value_hidden_sizes"), given, checkpoint_arch):
+        if g is not None and g != tuple(c):
+            raise ValueError("%s %s disagrees with the checkpoint being resumed, which has %s (pass -restart to start over)"
+                             % (flag, " ".join(map(str, g)), " ".join(map(str, c))))
+    return tuple(tuple(c) for c in checkpoint_arch)
 
 
 def train(params, start_carla=False, restart=False, env=None, vae=None, models_root="models", interactive=True):
@@ -96,17 +111,24 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     best_eval_reward = -float("inf")
 
     input_shape = np.array([vae.z_dim + len(measurements_to_include)])
-    print("Creating model")
-    model = PPO(input_shape, envs[0].action_space, learning_rate=learning_rate, lr_decay=lr_decay, epsilon=ppo_epsilon,
-                initial_std=initial_std, value_scale=value_scale, entropy_scale=entropy_scale,
-                model_dir=os.path.join(models_root, model_name), seed=seed if isinstance(seed, int) else None)
+    model_dir = os.path.join(models_root, model_name)
+    log_dir = "{}/logs/".format(model_dir)
     if not restart and interactive:
-        if os.path.isdir(model.log_dir) and len(os.listdir(model.log_dir)) > 0:
+        if os.path.isdir(log_dir) and len(os.listdir(log_dir)) > 0:
             answer = input("Model \"{}\" already exists. Do you wish to continue (C) or restart training (R)? ".format(model_name))
             if answer.upper() == "R":
                 restart = True
             elif answer.upper() != "C":
                 raise Exception("There are already log files for model \"{}\". Please delete it or change model_name and try again".format(model_name))
+    # a resumed run takes its checkpoint's architecture; a size flag that disagrees with it is an error
+    policy_sizes, value_sizes = resolve_architecture(params.get("policy_hidden_sizes"), params.get("value_hidden_sizes"),
+                                                     None if restart else checkpoint_architecture("{}/checkpoints/".format(model_dir)))
+    params["policy_hidden_sizes"], params["value_hidden_sizes"] = list(policy_sizes), list(value_sizes)
+    print("Creating model")
+    model = PPO(input_shape, envs[0].action_space, learning_rate=learning_rate, lr_decay=lr_decay, epsilon=ppo_epsilon,
+                initial_std=initial_std, value_scale=value_scale, entropy_scale=entropy_scale,
+                model_dir=model_dir, seed=seed if isinstance(seed, int) else None,
+                policy_hidden_sizes=policy_sizes, value_hidden_sizes=value_sizes)
     if restart:
         shutil.rmtree(model.model_dir)
         for d in model.dirs:
@@ -286,6 +308,12 @@ def main(argv=None):
                         "gradient to this value (default: off, like the reference)")
     parser.add_argument("--target_kl", type=float, default=None, help="stop an update once the approximate KL between the "
                         "new and the old policy exceeds 1.5 x this value (default: off, like the reference)")
+    parser.add_argument("--policy_hidden_sizes", type=int, nargs="+", default=None, metavar="WIDTH",
+                        help="hidden-layer widths of the policy network, 1 to 8 of them (default: 500 300, or the "
+                        "checkpoint's when resuming)")
+    parser.add_argument("--value_hidden_sizes", type=int, nargs="+", default=None, metavar="WIDTH",
+                        help="hidden-layer widths of the value network, 1 to 8 of them (default: 500 300, or the "
+                        "checkpoint's when resuming)")
     params = vars(parser.parse_args(argv))
     start_carla = params.pop("start_carla")
     restart = params.pop("restart")

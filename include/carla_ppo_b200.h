@@ -260,13 +260,32 @@ int32_t cpb_mlpvae_loss_grad(const cpb_mlpvae_config* cfg, const float* params, 
 typedef struct {
     int32_t state_dim;        /* 67 = 64-d latent + steer, throttle, speed (train.py:68,85) */
     int32_t num_actions;      /* 2 */
-    int32_t hidden1, hidden2; /* 500, 300 for both trunks (ppo.py:17) */
+    int32_t hidden1, hidden2; /* 500, 300 for both trunks (ppo.py:17); 0 in a cpb_ppo_spec */
     float   action_low[4];    /* action_space.low / .high (ppo.py:38) */
     float   action_high[4];
     float   epsilon;          /* clip range (ppo.py:124) */
     float   value_scale;      /* ppo.py:127 */
     float   entropy_scale;    /* ppo.py:130 */
 } cpb_ppo_config;
+
+/* The policy and value networks with their own lists of hidden-layer sizes (Stable-Baselines3's
+ * net_arch=dict(pi=[...], vf=[...])): num_policy / num_value dense + ReLU layers (1..8 each, every width >= 1) from the
+ * state to the action head and to the value head.  base.hidden1 / base.hidden2 must be 0 (refused otherwise: the widths
+ * are the lists).  Variables, in TF creation order and naming (ppo.py:38-66), 2P + 2V + 5 of them:
+ *   dense, dense_1 .. dense_{P-1} (kernel, bias), action_mean/kernel, action_mean/bias, action_logstd,
+ *   dense_P .. dense_{P+V-1} (kernel, bias), value/kernel, value/bias.
+ * Every cpb_ppo_* entry point below on a cpb_ppo_config is its cpb_ppo_spec_* twin at {hidden1, hidden2} /
+ * {hidden1, hidden2}: same layout, workspace, launches and results.  A bad spec (NULL, a depth outside [1, 8], a width
+ * < 1, nonzero base.hidden*, num_actions outside [1, 4]) is refused with CPB_ERR_INVALID_ARGUMENT before anything is
+ * enqueued.  Under CPB_PPO_PERSISTENT=1 the learn twins run every architecture in the persistent kernel. */
+#define CPB_PPO_MAX_LAYERS 8
+typedef struct {
+    cpb_ppo_config base;      /* hidden1 = hidden2 = 0 */
+    int32_t num_policy;
+    int32_t policy_sizes[CPB_PPO_MAX_LAYERS];
+    int32_t num_value;
+    int32_t value_sizes[CPB_PPO_MAX_LAYERS];
+} cpb_ppo_spec;
 
 int32_t     cpb_ppo_num_tensors(void);             /* 13 */
 const char* cpb_ppo_tensor_name(int32_t index);    /* "dense/kernel", ... (scope-relative) */
@@ -491,6 +510,78 @@ int32_t cpb_ppo_train_step_opts(const cpb_ppo_config* cfg, float* params, const 
                                 int32_t batch, float* metrics, const cpb_ppo_learn_options* opts,
                                 uint32_t* stop, int32_t* steps_applied, void* workspace,
                                 int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Spec twins: the entry points above for a cpb_ppo_spec (arguments after the first are those of the original).
+ * Layout arrays hold cpb_ppo_spec_num_tensors(spec) entries (shapes: 2 per tensor).
+ * ---------------------------------------------------------------------------------------- */
+int32_t     cpb_ppo_spec_num_tensors(const cpb_ppo_spec* spec);                 /* 2P + 2V + 5 */
+const char* cpb_ppo_spec_tensor_name(const cpb_ppo_spec* spec, int32_t index);  /* NULL for a bad spec or index */
+int32_t cpb_ppo_spec_layout(const cpb_ppo_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes,
+                            int64_t* total_floats);
+int64_t cpb_ppo_spec_workspace_bytes(const cpb_ppo_spec* spec, int32_t max_batch, int32_t horizon);
+int32_t cpb_ppo_spec_forward(const cpb_ppo_spec* spec, const float* params, const float* states, int32_t batch,
+                             const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+int32_t cpb_ppo_spec_loss_grad(const cpb_ppo_spec* spec, const float* params, const float* params_old,
+                               const float* states, const float* actions, const float* returns,
+                               const float* advantages, const int32_t* idx, int32_t batch, float* grads,
+                               float* metrics, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_train_step(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
+                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                const float* states, const float* actions, const float* returns,
+                                const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_train_step_opts(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
+                                     float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                     const float* states, const float* actions, const float* returns,
+                                     const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                     const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                     void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_learn(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
+                           float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                           const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                           const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                           int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                           int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_learn_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
+                                float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                const float* states, const float* actions, const double* rewards,
+                                const double* values, double bootstrap_value, const double* dones, int32_t T,
+                                double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                                int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_learn_segments(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const double* rewards,
+                                    const double* values, const double* bootstrap_values, const double* dones,
+                                    const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                                    double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                    const int32_t* perms, float* metrics, void* workspace,
+                                    int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_spec_learn_segments_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
+                                         float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                         const float* states, const float* actions, const double* rewards,
+                                         const double* values, const double* bootstrap_values, const double* dones,
+                                         const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                                         double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                         const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                                         int32_t* steps_applied, void* workspace, int64_t workspace_bytes,
+                                         void* stream);
+/* cpb_vae_spec_encode_predict / cpb_mlpvae_encode_predict with the PPO described by a cpb_ppo_spec (checked
+ * before the VAE is enqueued). */
+int32_t cpb_vae_spec_ppo_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                             const float* measurements, int32_t num_measurements,
+                                             const cpb_ppo_spec* ppo_spec, const float* ppo_params, const float* noise,
+                                             float* latent_tmp, float* state, float* action, float* value,
+                                             int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+                                             void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
+int32_t cpb_mlpvae_ppo_spec_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                           const float* measurements, int32_t num_measurements,
+                                           const cpb_ppo_spec* ppo_spec, const float* ppo_params, const float* noise,
+                                           float* latent_tmp, float* state, float* action, float* value,
+                                           int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+                                           void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
