@@ -82,6 +82,26 @@ class PpoSpec(C.Structure):
                    (C.c_int32 * PPO_MAX_LAYERS)(*value_sizes))
 
 
+PPO_MAX_LOGITS = 64
+
+
+class PpoCatSpec(C.Structure):
+    """cpb_ppo_cat_spec: a cpb_ppo_spec with a categorical policy head.  spec.base.num_actions = K components (1..4),
+    num_categories[k] = n_k (2..64 each, 64 in all); spec.base.action_low / action_high stay 0."""
+    _fields_ = [("spec", PpoSpec), ("num_categories", C.c_int32 * 4)]
+
+    @classmethod
+    def of(cls, base, policy_sizes, value_sizes, categories):
+        """The spec of the categorical PPO on `base` (its num_actions and action bounds are replaced) with these trunks
+        and components.  Every bound is checked by the library."""
+        b = PpoConfig.from_buffer_copy(base)
+        b.num_actions = len(categories)
+        for k in range(4):
+            b.action_low[k] = b.action_high[k] = 0.0
+        cats = list(categories)[:4] + [0] * max(0, 4 - len(categories))
+        return cls(PpoSpec.of(b, policy_sizes, value_sizes), (C.c_int32 * 4)(*cats))
+
+
 class PpoLearnOptions(C.Structure):
     """cpb_ppo_learn_options: 0 turns a guard off."""
     _fields_ = [("max_grad_norm", C.c_float), ("target_kl", C.c_float)]
@@ -96,6 +116,7 @@ _MS = C.POINTER(MlpVaeSpec)
 _PC = C.POINTER(PpoConfig)
 _PO = C.POINTER(PpoLearnOptions)
 _PS = C.POINTER(PpoSpec)
+_PK = C.POINTER(PpoCatSpec)
 
 # name -> (restype, argtypes); must list every symbol of include/carla_ppo_b200.h
 PROTOTYPES = {
@@ -182,6 +203,27 @@ PROTOTYPES = {
                                                     _i64, _P]),
     "cpb_mlpvae_ppo_spec_encode_predict": (_i32, [_MS, _P, _P, _P, _i32, _PS, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
                                                   _i64, _P]),
+    "cpb_ppo_cat_num_tensors": (_i32, [_PK]),
+    "cpb_ppo_cat_tensor_name": (C.c_char_p, [_PK, _i32]),
+    "cpb_ppo_cat_layout": (_i32, [_PK, _P, _P, _P, _P]),
+    "cpb_ppo_cat_workspace_bytes": (_i64, [_PK, _i32, _i32]),
+    "cpb_ppo_cat_forward": (_i32, [_PK, _P, _P, _i32, _P, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_loss_grad": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_train_step": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_train_step_opts": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _P, _PO, _P, _P,
+                                           _P, _i64, _P]),
+    "cpb_ppo_cat_learn": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
+                                 _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_learn_opts": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _f64, _P, _i32, _f64, _f64,
+                                      _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_learn_segments": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32, _f64,
+                                          _f64, _i32, _i32, _P, _P, _P, _i64, _P]),
+    "cpb_ppo_cat_learn_segments_opts": (_i32, [_PK, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _i32, _i32,
+                                               _f64, _f64, _i32, _i32, _P, _P, _PO, _P, _P, _i64, _P]),
+    "cpb_vae_spec_ppo_cat_encode_predict": (_i32, [_VS, _P, _P, _P, _i32, _PK, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
+                                                   _i64, _P]),
+    "cpb_mlpvae_ppo_cat_encode_predict": (_i32, [_MS, _P, _P, _P, _i32, _PK, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
+                                                 _i64, _P]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_vae_spec_buffer_offsets": (_i32, [_VS, _i32, _P, _i32]),

@@ -8,7 +8,8 @@ In the reference every environment step costs two TensorFlow session runs with a
 the loop a ``predict`` -- but computes both at ``encode_state_fn`` time and serves ``predict(state)`` from the cached result
 when it is asked about the very state it just produced.  ``encode_predict(envs)`` does the same for several environments
 at once.  Noise is drawn from the PPO object's generator exactly once per sampled action, in call order, so the fused and
-the unfused loop (``UnfusedActor`` for several environments) produce identical trajectories.
+the unfused loop (``UnfusedActor`` for several environments) produce identical trajectories.  A categorical PPO
+(discrete action space) runs through the cpb_*_ppo_cat_encode_predict twins with uniform noise.
 """
 from __future__ import annotations
 
@@ -65,7 +66,7 @@ class FusedActor:
         """The current frames of `envs` -> (states, actions [n, A], values [n]) in ONE cpb_encode_predict call at B = n:
         one H2D copy of the packed frames, measurements and noise, one D2H copy of the results.  states[i] is what
         encode_state_fn(envs[i]) returns.  The noise is ppo._rng.randn(n, A), rows in environment order (none when
-        greedy)."""
+        greedy); for a categorical PPO it is ppo._rng.rand(n, K) and the actions are int64 indices."""
         vae, ppo, torch = self.vae, self.ppo, self._torch
         n, a, sd, nf = len(envs), ppo.num_actions, ppo.state_dim, self._frame_bytes
         self._buffers(n)
@@ -81,7 +82,8 @@ class FusedActor:
         if self._m:
             fview[:n * self._m] = np.asarray(meas, np.float32).reshape(-1)
         if not self.greedy:
-            fview[n * self._m:] = ppo._rng.randn(n, a).astype(np.float32).reshape(-1)   # the draw PPO.predict would make
+            draw = ppo._rng.randn if ppo.action_categories is None else ppo._rng.rand
+            fview[n * self._m:] = draw(n, a).astype(np.float32).reshape(-1)   # the draw PPO.predict would make
         with torch.cuda.device(vae._device):
             n_in = n * (nf + 4 * (self._m + a))
             self._in_dev[:n_in].copy_(self._in_host[:n_in], non_blocking=True)
@@ -90,7 +92,7 @@ class FusedActor:
             ws_v = vae._workspace(n, _lib.WS_ENCODE)
             ws_p = ppo._workspace(n)
             out = self._out_dev.data_ptr()
-            name = vae._API["encode_predict"]
+            name = vae._API["encode_predict" if ppo.action_categories is None else "encode_predict_cat"]
             _lib.check(getattr(vae._libh, name)(
                 C.byref(cfg), _lib.ptr(vae.params), base, base + n * nf, self._m, C.byref(ppo._spec), _lib.ptr(ppo.params),
                 None if self.greedy else base + n * (nf + 4 * self._m), _lib.ptr(self._latent), out, out + 4 * n * sd,
@@ -104,7 +106,10 @@ class FusedActor:
         # vae_common.py:61: np.append(float32 latent, python floats) -> float64 state vector
         states = [np.append(st[i, :vae.z_dim].copy(), meas[i]) for i in range(n)]
         self.calls += 1
-        return states, res[n * sd:n * (sd + a)].reshape(n, a).copy(), res[n * (sd + a):n_out].copy()
+        actions = res[n * sd:n * (sd + a)].reshape(n, a).copy()
+        if ppo.action_categories is not None:
+            actions = actions.astype(np.int64)
+        return states, actions, res[n * (sd + a):n_out].copy()
 
     # -- the callback CarlaEnv / ReplayEnv invokes from reset() / step()
     def encode_state_fn(self, env):
@@ -128,8 +133,8 @@ class FusedActor:
 
 class UnfusedActor:
     """FusedActor.encode_predict as the reference's two separate steps: one ``vae.encode`` on all frames (through
-    vae_common.create_encode_states_fn), then one ``ppo.predict`` on all states, which draws ppo._rng.randn(n, A) --
-    the noise FusedActor draws, so both produce the same trajectories."""
+    vae_common.create_encode_states_fn), then one ``ppo.predict`` on all states, which draws ppo._rng.randn(n, A)
+    (rand(n, K) for a categorical PPO) -- the noise FusedActor draws, so both produce the same trajectories."""
 
     def __init__(self, vae, ppo, measurements_to_include=("steer", "throttle", "speed")):
         from .vae_common import create_encode_states_fn

@@ -49,7 +49,23 @@ struct PpoLayout {
     __host__ __device__ int bv() const { return wv() + 1; }
 };
 
-PpoLayout make_ppo_layout(const cpb_ppo_spec* sp) {
+// The policy head of a plan.  Gaussian (cat == 0): N = K = num_actions columns of action_mean and an action_logstd.
+// Categorical (cpb_ppo_cat_spec, cat == 1): N = sum n_k logits in action_logits, component k's at columns
+// [off[k], off[k+1]); its layout keeps the logstd slot at size 0, so both kinds share PpoLayout's indexing.
+constexpr int kMaxLogits = 64;
+struct HeadShape {
+    int cat, K, N;
+    int off[5];
+};
+
+HeadShape gauss_head(const cpb_ppo_spec* sp) {
+    HeadShape hs;
+    memset(&hs, 0, sizeof(hs));
+    hs.K = hs.N = sp->base.num_actions;
+    return hs;
+}
+
+PpoLayout make_ppo_layout(const cpb_ppo_spec* sp, const HeadShape& hs) {
     PpoLayout L;
     memset(&L, 0, sizeof(L));
     const int A = sp->base.num_actions;
@@ -60,7 +76,8 @@ PpoLayout make_ppo_layout(const cpb_ppo_spec* sp) {
             set(L.w(t, l), trunk_in(*sp, t, l), trunk_width(*sp, t, l));
             set(L.b(t, l), trunk_width(*sp, t, l), 0);
         }
-    set(L.wm(), trunk_last(*sp, 0), A); set(L.bm(), A, 0); set(L.logstd(), A, 0);
+    if (hs.cat) { set(L.wm(), trunk_last(*sp, 0), hs.N); set(L.bm(), hs.N, 0); }
+    else { set(L.wm(), trunk_last(*sp, 0), A); set(L.bm(), A, 0); set(L.logstd(), A, 0); }
     set(L.wv(), trunk_last(*sp, 1), 1); set(L.bv(), 1, 0);
     int64_t o = 0;
     for (int i = 0; i < L.n; ++i) {
@@ -71,6 +88,9 @@ PpoLayout make_ppo_layout(const cpb_ppo_spec* sp) {
     L.total = o;
     return L;
 }
+
+// A categorical layout has no action_logstd: its public index i is PpoLayout's index i, or i + 1 past the head
+__host__ __device__ __forceinline__ int cat_internal_index(const cpb_ppo_spec& sp, int i) { return i < 2 * sp.num_policy + 2 ? i : i + 1; }
 
 const char* ppo_tensor_name(const cpb_ppo_spec* sp, int i) {
     static char dense[2 * kMaxPpoDepth][2][24];
@@ -304,12 +324,15 @@ struct HeadArgs {
     const float* noise;    // predict path: [B,A] or null
     float* action_out;     // predict path
     int kl_term;           // training head: add (r - 1) - log r to slot 7 (options entry points only)
+    // categorical head only (A = K components): N logits, component k at [coff[k], coff[k+1]); dpre / mu_out are [B,N]
+    int N;
+    int coff[kMaxActions + 1];
 };
 
 // mode 0: log-prob only (old policy); mode 1: full training head; mode 2: predict (mu / sampled action, value)
 // one sample (row b) by one warp; MODE 1 adds its loss terms to vals[8]
 template <int MODE>
-__device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, float* vals) {
+__device__ __forceinline__ void gauss_head_row(const HeadArgs& a, int b, int lane, float* vals) {
     {
         const float* h = a.hp + (long long)b * a.Hp;
         const float* g = MODE != 0 ? a.hv + (long long)b * a.Hv : nullptr;
@@ -409,6 +432,171 @@ __device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, flo
     }
 }
 
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+// logit i (< 64) of a row whose lane l holds logits l in v0 and l + 32 in v1; i is the same in every lane
+__device__ __forceinline__ float logit_at(float v0, float v1, int i) { return __shfl_sync(0xffffffffu, i < 32 ? v0 : v1, i & 31); }
+
+// The categorical head of row b (one warp): logits z = h_P W + b with lane l owning logits l and l + 32, one softmax per
+// component (segmented warp reductions over a.coff), log-prob of the taken indices, entropy, and in MODE 1 the gradient
+//   dz_ki = dlogp (1[i = a_k] - p_ki) + (entropy_scale / B) p_ki (log p_ki + H_k)
+// into dpre [B,N] and the masked dh_P.  Every sum has a fixed order, so a repeated call is bit-identical.
+template <int MODE>
+__device__ __forceinline__ void cat_head_row(const HeadArgs& a, int b, int lane, float* vals) {
+    const float* h = a.hp + (long long)b * a.Hp;
+    const int N = a.N, K = a.A;
+    const bool has0 = lane < N, has1 = lane + 32 < N;
+    // logits: the rows of W are read coalesced, h 32 values at a time and broadcast lane to lane
+    float z0 = 0.f, z1 = 0.f;
+    for (int j0 = 0; j0 < a.Hp; j0 += 32) {
+        const float hl = j0 + lane < a.Hp ? h[j0 + lane] : 0.f;
+        const int n = a.Hp - j0 < 32 ? a.Hp - j0 : 32;
+        for (int t = 0; t < n; ++t) {
+            const float hj = __shfl_sync(0xffffffffu, hl, t);
+            const float* w = a.wm + (long long)(j0 + t) * N;
+            if (has0) z0 = fmaf(hj, w[lane], z0);
+            if (has1) z1 = fmaf(hj, w[lane + 32], z1);
+        }
+    }
+    if (has0) z0 += a.bm[lane];
+    if (has1) z1 += a.bm[lane + 32];
+    // component of each owned logit, and the per-component softmax: max, sum of exp, entropy (warp-uniform values)
+    int c0 = 0, c1 = 0;
+#pragma unroll
+    for (int k = 1; k < kMaxActions; ++k)
+        if (k < K) { c0 += lane >= a.coff[k]; c1 += lane + 32 >= a.coff[k]; }
+    float mx[kMaxActions], lse[kMaxActions], ent[kMaxActions];
+    float m0 = 0.f, m1 = 0.f, l0 = 0.f, l1 = 0.f, s0 = 1.f, s1 = 1.f, H0 = 0.f, H1 = 0.f;
+#pragma unroll
+    for (int k = 0; k < kMaxActions; ++k) {
+        if (k >= K) continue;
+        float v = -INFINITY;
+        if (has0 && c0 == k) v = z0;
+        if (has1 && c1 == k) v = fmaxf(v, z1);
+        mx[k] = warp_max(v);
+        if (c0 == k) m0 = mx[k];
+        if (c1 == k) m1 = mx[k];
+    }
+    const float e0 = has0 ? expf(z0 - m0) : 0.f, e1 = has1 ? expf(z1 - m1) : 0.f;
+#pragma unroll
+    for (int k = 0; k < kMaxActions; ++k) {
+        if (k >= K) continue;
+        const float s = warp_sum((c0 == k ? e0 : 0.f) + (c1 == k ? e1 : 0.f));
+        lse[k] = logf(s);
+        if (c0 == k) { l0 = lse[k]; s0 = s; }
+        if (c1 == k) { l1 = lse[k]; s1 = s; }
+    }
+    const float lp0 = has0 ? z0 - m0 - l0 : 0.f, lp1 = has1 ? z1 - m1 - l1 : 0.f;   // log p
+    const float p0 = e0 / s0, p1 = e1 / s1;
+    float entropy = 0.f;
+#pragma unroll
+    for (int k = 0; k < kMaxActions; ++k) {
+        if (k >= K) continue;
+        ent[k] = -warp_sum((c0 == k ? p0 * lp0 : 0.f) + (c1 == k ? p1 * lp1 : 0.f));
+        entropy += ent[k];
+        if (c0 == k) H0 = ent[k];
+        if (c1 == k) H1 = ent[k];
+    }
+    (void)mx; (void)lse;
+    if (MODE == 2) {
+        float vsum = 0.f;
+        const float* g = a.hv + (long long)b * a.Hv;
+        for (int j = lane; j < a.Hv; j += 32) vsum = fmaf(g[j], a.wv[j], vsum);
+        vsum = warp_sum(vsum);
+        // greedy: the first largest logit; sampled: the first i with u < cumsum_i p (fp32, index order), else the last
+        // index with p > 0.  Every lane runs the same scan on broadcast values; lane 0 writes.
+        for (int k = 0; k < K; ++k) {
+            const int lo = a.coff[k], hi = a.coff[k + 1];
+            int pick = -1, last_pos = 0;
+            if (a.noise == nullptr) {
+                float best = -INFINITY;
+                pick = 0;
+                for (int i = lo; i < hi; ++i) {
+                    const float zi = logit_at(z0, z1, i);
+                    if (zi > best) { best = zi; pick = i - lo; }
+                }
+            } else {
+                const float u = a.noise[(long long)b * K + k];
+                float c = 0.f;
+                for (int i = lo; i < hi; ++i) {
+                    const float pi = logit_at(p0, p1, i);
+                    c += pi;
+                    if (pick < 0 && u < c) pick = i - lo;
+                    if (pi > 0.f) last_pos = i - lo;
+                }
+                if (pick < 0) pick = last_pos;
+            }
+            if (lane == 0) a.action_out[(long long)b * K + k] = (float)pick;
+        }
+        if (lane == 0) a.v_out[b] = vsum + a.bv[0];
+        return;
+    }
+    // log-prob of the taken indices (clamped into each component's range)
+    const int row = a.idx != nullptr ? a.idx[b] : b;
+    float logp = 0.f;
+    int t0 = -1, t1 = -1;   // the taken index of the component of logit lane / lane + 32
+#pragma unroll
+    for (int k = 0; k < kMaxActions; ++k) {
+        if (k >= K) continue;
+        const float av = a.actions[(long long)row * K + k];
+        const int t = a.coff[k] + (int)fminf(fmaxf(av, 0.f), (float)(a.coff[k + 1] - a.coff[k] - 1));
+        logp += logit_at(lp0, lp1, t);
+        if (c0 == k) t0 = t;
+        if (c1 == k) t1 = t;
+    }
+    if (MODE == 0) {
+        if (lane == 0) a.logp_out[b] = logp;
+        return;
+    }
+    const float* g = a.hv + (long long)b * a.Hv;
+    float vsum = 0.f;
+    for (int j = lane; j < a.Hv; j += 32) vsum = fmaf(g[j], a.wv[j], vsum);
+    vsum = warp_sum(vsum);
+    const float v = vsum + a.bv[0];
+    const float logp_old = a.logp_old_in[a.logp_old_gathered ? row : b];
+    const float ratio = expf(logp - logp_old);
+    const float adv = a.adv[row], ret = a.returns[row];
+    const float unclipped = ratio * adv;
+    const float clipped = fminf(fmaxf(ratio, 1.f - a.eps_clip), 1.f + a.eps_clip) * adv;
+    const float inv_b = 1.f / (float)a.B;
+    const float dratio = unclipped <= clipped ? -adv * inv_b : 0.f;   // the Gaussian head's tf.minimum rule
+    const float dlogp = dratio * ratio;
+    const float dvv = a.value_scale * 2.f * inv_b * (v - ret);
+    const float es = a.entropy_scale * inv_b;
+    const float dz0 = has0 ? dlogp * ((lane == t0 ? 1.f : 0.f) - p0) + es * p0 * (lp0 + H0) : 0.f;
+    const float dz1 = has1 ? dlogp * ((lane + 32 == t1 ? 1.f : 0.f) - p1) + es * p1 * (lp1 + H1) : 0.f;
+    if (has0) a.dpre[(long long)b * N + lane] = dz0;
+    if (has1) a.dpre[(long long)b * N + lane + 32] = dz1;
+    if (lane == 0) {
+        a.dv[b] = dvv;
+        if (a.v_out != nullptr) a.v_out[b] = v;
+    }
+    // dh_P[j] = sum_i dz_i W[j, i] (i in index order), masked by h_P > 0; lane l owns j = j0 + l
+    for (int j0 = 0; j0 < a.Hp; j0 += 32) {
+        const int j = j0 + lane;
+        const float* w = a.wm + (long long)(j < a.Hp ? j : 0) * N;
+        float s = 0.f;
+        for (int i = 0; i < N; ++i) s = fmaf(logit_at(dz0, dz1, i), w[i], s);
+        if (j < a.Hp) a.dhp[(long long)b * a.Hp + j] = h[j] > 0.f ? s : 0.f;
+    }
+    for (int j = lane; j < a.Hv; j += 32) a.dhv[(long long)b * a.Hv + j] = g[j] > 0.f ? dvv * a.wv[j] : 0.f;
+    vals[0] += fminf(unclipped, clipped);
+    vals[1] += (v - ret) * (v - ret);
+    vals[2] += ratio;
+    vals[3] += entropy;
+    if (a.kl_term) vals[7] += (ratio - 1.f) - (logp - logp_old);
+}
+
+// CAT: 0 = the Gaussian head, 1 = the categorical head
+template <int MODE, int CAT>
+__device__ __forceinline__ void head_row(const HeadArgs& a, int b, int lane, float* vals) {
+    if constexpr (CAT != 0) cat_head_row<MODE>(a, b, lane, vals);
+    else gauss_head_row<MODE>(a, b, lane, vals);
+}
+
 // CTA-level sum of the 8 warps' loss terms -> partial[block][8] (fixed order: deterministic)
 __device__ __forceinline__ void head_block_reduce(const float* vals, float (*red)[8], float* partial_out) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -425,15 +613,21 @@ __device__ __forceinline__ void head_block_reduce(const float* vals, float (*red
     __syncthreads();
 }
 
-template <int MODE>
+template <int MODE, int CAT>
 __global__ void __launch_bounds__(256)
 ppo_head_kernel(const __grid_constant__ HeadArgs a) {
     __shared__ float red[8][8];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * 8 + warp;
     float vals[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (b < a.B) head_row<MODE>(a, b, lane, vals);
+    if (b < a.B) head_row<MODE, CAT>(a, b, lane, vals);
     if (MODE == 1) head_block_reduce(vals, red, a.partial + blockIdx.x * 8);
+}
+
+template <int MODE>
+void launch_head(const HeadShape& hs, int B, const HeadArgs& h, cudaStream_t s) {
+    if (hs.cat) ppo_head_kernel<MODE, 1><<<cdiv(B, 8), 256, 0, s>>>(h);
+    else ppo_head_kernel<MODE, 0><<<cdiv(B, 8), 256, 0, s>>>(h);
 }
 
 // The per-call guards of the cpb_ppo_*_opts entry points (cpb_ppo_learn_options).  stop == nullptr on every other entry
@@ -454,6 +648,8 @@ struct Guards {
 // metrics[5] = policy_loss, value_loss, entropy_loss, loss, mean ratio; grads[logstd], value-bias etc.
 // With guards, metrics rows are 7 wide: [5] = approx_kl (written here), [6] = the pre-clip gradient norm (written by the
 // norm reduction); a minibatch evaluated after the stop gets a NaN row.
+// CAT: the categorical head's entropy is the batch mean of slot 3 (sum_b H_b), and there is no logstd gradient.
+template <int CAT>
 __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, int B, int A, const float* logstd, float value_scale,
                                              float entropy_scale, float* glogstd, float* metrics, float* tot /* shared [8] */,
                                              const Guards& g) {
@@ -466,10 +662,12 @@ __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, 
     if (threadIdx.x == 0) {
         const float inv_b = 1.f / (float)B;
         float ent = 0.f;
-        for (int k = 0; k < A; ++k) {
-            ent += kEntropyConst + logstd[k];
-            glogstd[k] = tot[3 + k] - entropy_scale;
-        }
+        if constexpr (CAT != 0) ent = tot[3] * inv_b;
+        else
+            for (int k = 0; k < A; ++k) {
+                ent += kEntropyConst + logstd[k];
+                glogstd[k] = tot[3 + k] - entropy_scale;
+            }
         const float pl = tot[0] * inv_b;
         const float vl = tot[1] * inv_b * value_scale;
         const float el = ent * entropy_scale;
@@ -491,11 +689,12 @@ __device__ __forceinline__ void ppo_finalize(const float* partial, int nblocks, 
     __syncthreads();
 }
 
+template <int CAT>
 __global__ void ppo_finalize_kernel(const float* __restrict__ partial, int nblocks, int B, int A,
                                     const float* __restrict__ logstd, float value_scale, float entropy_scale,
                                     float* __restrict__ glogstd, float* __restrict__ metrics, const Guards g) {
     __shared__ float tot[8];
-    ppo_finalize(partial, nblocks, B, A, logstd, value_scale, entropy_scale, glogstd, metrics, tot, g);
+    ppo_finalize<CAT>(partial, nblocks, B, A, logstd, value_scale, entropy_scale, glogstd, metrics, tot, g);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -728,7 +927,7 @@ __host__ __device__ __forceinline__ float* trunk_buf(float* const* bufs, const c
     return bufs[l] + (t ? (long long)B * width_or_0(sp, 0, l) : 0);
 }
 
-PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_spec* sp, int max_batch, int horizon) {
+PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_spec* sp, const HeadShape& hs, int max_batch, int horizon) {
     PpoPlan p;
     memset(&p, 0, sizeof(p));
     Arena a(ws, ws_bytes);
@@ -739,7 +938,7 @@ PpoPlan make_ppo_plan(void* ws, int64_t ws_bytes, const cpb_ppo_spec* sp, int ma
     for (int l = D - 1; l >= 0; --l) p.dh[l] = a.take<float>(B * (width_or_0(*sp, 0, l) + width_or_0(*sp, 1, l)));
     for (int l = 0; l < sp->num_policy; ++l) p.oh[l] = a.take<float>(rows * sp->policy_sizes[l]);
     p.logp_old = a.take<float>(rows);
-    p.dpre = a.take<float>(B * kMaxActions);
+    p.dpre = a.take<float>(B * (hs.cat ? hs.N : kMaxActions));
     p.dv = a.take<float>(B);
     p.partial = a.take<float>((int64_t)(cdiv(B, 8) > kMaxPersistentCtas ? cdiv(B, 8) : kMaxPersistentCtas) * 8);
     p.ret32 = a.take<float>(rows);
@@ -770,7 +969,30 @@ int32_t check_ppo_spec(const cpb_ppo_spec* sp) {
     return CPB_OK;
 }
 
-HeadArgs head_args(const cpb_ppo_spec* sp, const PpoLayout& L, const float* params, int B) {
+// A cpb_ppo_cat_spec -> its HeadShape, refusing a bad one (the Gaussian spec's checks first)
+int32_t cat_head(const cpb_ppo_cat_spec* cs, HeadShape* hs) {
+    CPB_REQUIRE(cs != nullptr, "ppo categorical spec is NULL");
+    CPB_TRY(check_ppo_spec(&cs->spec));
+    const cpb_ppo_config& c = cs->spec.base;
+    for (int k = 0; k < kMaxActions; ++k)
+        CPB_REQUIRE(c.action_low[k] == 0.f && c.action_high[k] == 0.f,
+                    "ppo categorical spec: spec.base.action_low / action_high must be 0 (component %d)", k);
+    memset(hs, 0, sizeof(*hs));
+    hs->cat = 1;
+    hs->K = c.num_actions;
+    for (int k = 0; k < hs->K; ++k) {
+        const int n = cs->num_categories[k];
+        CPB_REQUIRE(n >= 2 && n <= kMaxLogits, "ppo categorical spec: component %d has %d categories (must be 2..%d)", k, n,
+                    kMaxLogits);
+        hs->off[k + 1] = hs->off[k] + n;
+    }
+    hs->N = hs->off[hs->K];
+    for (int k = hs->K + 1; k < 5; ++k) hs->off[k] = hs->N;
+    CPB_REQUIRE(hs->N <= kMaxLogits, "ppo categorical spec: %d logits in all (at most %d)", hs->N, kMaxLogits);
+    return CPB_OK;
+}
+
+HeadArgs head_args(const cpb_ppo_spec* sp, const HeadShape& hs, const PpoLayout& L, const float* params, int B) {
     const cpb_ppo_config* c = &sp->base;
     HeadArgs h;
     memset(&h, 0, sizeof(h));
@@ -779,11 +1001,13 @@ HeadArgs head_args(const cpb_ppo_spec* sp, const PpoLayout& L, const float* para
     h.B = B; h.Hp = trunk_last(*sp, 0); h.Hv = trunk_last(*sp, 1); h.A = c->num_actions;
     for (int k = 0; k < kMaxActions; ++k) { h.low[k] = c->action_low[k]; h.high[k] = c->action_high[k]; }
     h.eps_clip = c->epsilon; h.value_scale = c->value_scale; h.entropy_scale = c->entropy_scale;
+    h.N = hs.N;
+    for (int k = 0; k < 5; ++k) h.coff[k] = hs.off[k];
     return h;
 }
 
 // log pi_old(a|s) for `rows` samples (optionally gathered)
-int32_t run_old_logp(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, const float* params_old,
+int32_t run_old_logp(const cpb_ppo_spec* sp, const HeadShape& hs, const PpoLayout& L, const PpoPlan& pl, const float* params_old,
                      const float* states, const float* actions, const int32_t* idx, int rows, cudaStream_t s) {
     GemmBatch gb;
     for (int l = 0; l < sp->num_policy; ++l) {
@@ -791,9 +1015,9 @@ int32_t run_old_logp(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& 
                             params_old + L.off[L.w(0, l)], sp->policy_sizes[l], params_old + L.off[L.b(0, l)], pl.oh[l], 1);
         CPB_TRY(launch_small_gemm(gb, 1, s));
     }
-    HeadArgs h = head_args(sp, L, params_old, rows);
+    HeadArgs h = head_args(sp, hs, L, params_old, rows);
     h.hp = pl.oh[sp->num_policy - 1]; h.actions = actions; h.idx = idx; h.logp_out = pl.logp_old;
-    ppo_head_kernel<0><<<cdiv(rows, 8), 256, 0, s>>>(h);
+    launch_head<0>(hs, rows, h, s);
     CPB_LAUNCHED();
     return CPB_OK;
 }
@@ -833,11 +1057,12 @@ __host__ __device__ __forceinline__ int trunk_bwd_jobs(const cpb_ppo_spec& sp, c
     return n;
 }
 
-// Weight and bias gradients of the action and value heads: gWm[Hp,A] = hp^T dpre, gbm = colsum(dpre); gWv[Hv,1] = hv^T dv
+// Weight and bias gradients of the action and value heads: gWm[Hp,N] = hp^T dpre, gbm = colsum(dpre); gWv[Hv,1] = hv^T dv
+// (N: the head's columns, num_actions for the Gaussian head, the logits for the categorical one)
 __host__ __device__ __forceinline__ void head_bwd_jobs(const cpb_ppo_spec& sp, const PpoLayout& L, const PpoPlan& pl,
-                                                       float* grads, int B, GemmJob* jobs) {
+                                                       float* grads, int B, int N, GemmJob* jobs) {
     jobs[0] = bwd_weight_job(trunk_buf(pl.h, sp, 0, sp.num_policy - 1, B), nullptr, B, trunk_last(sp, 0), pl.dpre,
-                             sp.base.num_actions, grads + L.off[L.wm()], grads + L.off[L.bm()]);
+                             N, grads + L.off[L.wm()], grads + L.off[L.bm()]);
     jobs[1] = bwd_weight_job(trunk_buf(pl.h, sp, 1, sp.num_value - 1, B), nullptr, B, trunk_last(sp, 1), pl.dv, 1,
                              grads + L.off[L.wv()], grads + L.off[L.bv()]);
 }
@@ -851,14 +1076,14 @@ int32_t run_trunks(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl
 }
 
 // forward + loss + gradients for one minibatch; logp_old given (gathered or not)
-int32_t run_loss_grad(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, const float* params,
+int32_t run_loss_grad(const cpb_ppo_spec* sp, const HeadShape& hs, const PpoLayout& L, const PpoPlan& pl, const float* params,
                       const float* states, const float* actions, const float* returns, const float* adv,
                       const int32_t* idx, int B, const float* logp_old, int logp_old_gathered, float* grads,
                       float* metrics, const Guards& gd, cudaStream_t s) {
     const cpb_ppo_config* c = &sp->base;
     const int P = sp->num_policy, V = sp->num_value, D = max_depth(*sp);
     CPB_TRY(run_trunks(sp, L, pl, params, states, idx, B, s));
-    HeadArgs h = head_args(sp, L, params, B);
+    HeadArgs h = head_args(sp, hs, L, params, B);
     h.hp = trunk_buf(pl.h, *sp, 0, P - 1, B); h.hv = trunk_buf(pl.h, *sp, 1, V - 1, B);
     h.actions = actions; h.returns = returns; h.adv = adv; h.idx = idx;
     h.logp_old_in = logp_old; h.logp_old_gathered = logp_old_gathered;
@@ -866,10 +1091,14 @@ int32_t run_loss_grad(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan&
     h.partial = pl.partial;
     h.kl_term = gd.stop != nullptr;
     const int nblocks = cdiv(B, 8);
-    ppo_head_kernel<1><<<nblocks, 256, 0, s>>>(h);
+    launch_head<1>(hs, B, h, s);
     CPB_LAUNCHED();
-    ppo_finalize_kernel<<<1, 32, 0, s>>>(pl.partial, nblocks, B, c->num_actions, params + L.off[L.logstd()], c->value_scale,
-                                         c->entropy_scale, grads + L.off[L.logstd()], metrics, gd);
+    if (hs.cat)
+        ppo_finalize_kernel<1><<<1, 32, 0, s>>>(pl.partial, nblocks, B, c->num_actions, nullptr, c->value_scale,
+                                                c->entropy_scale, nullptr, metrics, gd);
+    else
+        ppo_finalize_kernel<0><<<1, 32, 0, s>>>(pl.partial, nblocks, B, c->num_actions, params + L.off[L.logstd()],
+                                                c->value_scale, c->entropy_scale, grads + L.off[L.logstd()], metrics, gd);
     CPB_LAUNCHED();
     // one launch per layer, top down, for both trunks: weight gradients and the data gradient into the layer below.  The
     // head weight gradients only need the head kernel's outputs and join the top layer's launch (at two layers per trunk:
@@ -880,10 +1109,10 @@ int32_t run_loss_grad(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan&
         if (l == D - 1) {
             if (l == 0 && idx != nullptr) {
                 GemmBatch hb;
-                head_bwd_jobs(*sp, L, pl, grads, B, hb.job);
+                head_bwd_jobs(*sp, L, pl, grads, B, hs.N, hb.job);
                 CPB_TRY(launch_small_gemm(hb, 2, s));
             } else {
-                head_bwd_jobs(*sp, L, pl, grads, B, gb.job + n);
+                head_bwd_jobs(*sp, L, pl, grads, B, hs.N, gb.job + n);
                 n += 2;
             }
         }
@@ -913,6 +1142,7 @@ struct LearnArgs {
     float* metrics;
     int T, batch_size, num_epochs, nmb;
     Guards gd;             // gd.stop == nullptr: no guards, 5-wide metrics rows
+    HeadShape hs;          // read by the categorical instantiation only
 };
 // a __grid_constant__ kernel parameter: within the 4 KB parameter space at every architecture (8 layers per trunk)
 static_assert(sizeof(LearnArgs) <= 4096, "LearnArgs exceeds the kernel parameter space");
@@ -944,6 +1174,7 @@ __device__ __forceinline__ void run_phase(const GemmJob* jobs, int njobs, float*
     }
 }
 
+template <int CAT>
 __global__ void __launch_bounds__(kLearnThreads, 1)
 ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
     namespace cg = cooperative_groups;
@@ -998,25 +1229,29 @@ ppo_learn_persistent_kernel(const __grid_constant__ LearnArgs a) {
                 h.dhp = trunk_buf(pl.dh, sp, 0, sp.num_policy - 1, B); h.dhv = trunk_buf(pl.dh, sp, 1, sp.num_value - 1, B);
                 h.noise = nullptr; h.action_out = nullptr;
                 h.kl_term = gd.stop != nullptr;
+                if constexpr (CAT != 0) {
+                    h.N = a.hs.N;
+                    for (int k = 0; k < 5; ++k) h.coff[k] = a.hs.off[k];
+                }
                 float vals[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                for (int b = blockIdx.x * 8 + warp; b < B; b += gridDim.x * 8) head_row<1>(h, b, lane, vals);
+                for (int b = blockIdx.x * 8 + warp; b < B; b += gridDim.x * 8) head_row<1, CAT>(h, b, lane, vals);
                 head_block_reduce(vals, red, pl.partial + blockIdx.x * 8);
             }
             grid.sync();
             // ---- loss metrics + logstd gradient (CTA 0), then the backward pass top down: layer l of both trunks per
             // phase, the head weight gradients with the top layer (their own tile list when that layer gathers the states)
             if (blockIdx.x == 0)
-                ppo_finalize(pl.partial, gridDim.x, B, A, params + L.off[L.logstd()], c.value_scale, c.entropy_scale,
-                             grads + L.off[L.logstd()], mt, tot, gd);
+                ppo_finalize<CAT>(pl.partial, gridDim.x, B, A, params + L.off[L.logstd()], c.value_scale, c.entropy_scale,
+                                  grads + L.off[L.logstd()], mt, tot, gd);
             for (int l = D - 1; l >= 0; --l) {
                 int n = trunk_bwd_jobs(sp, L, pl, params, grads, a.states, idx, B, l, jobs);
                 if (l > 0) {
-                    if (l == D - 1) { head_bwd_jobs(sp, L, pl, grads, B, jobs + n); n += 2; }
+                    if (l == D - 1) { head_bwd_jobs(sp, L, pl, grads, B, CAT ? a.hs.N : sp.base.num_actions, jobs + n); n += 2; }
                     run_phase<0>(jobs, n, learn_smem, gid, ngroups);
                 } else {
                     run_phase<2>(jobs, n, learn_smem, gid, ngroups);
                     if (D == 1) {
-                        head_bwd_jobs(sp, L, pl, grads, B, jobs);
+                        head_bwd_jobs(sp, L, pl, grads, B, CAT ? a.hs.N : sp.base.num_actions, jobs);
                         run_phase<0>(jobs, 2, learn_smem, gid, ngroups);
                     }
                 }
@@ -1080,8 +1315,12 @@ int32_t learn_persistent_init() {
     CPB_CUDA(cudaGetDevice(&dev));
     CPB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     CPB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    CPB_CUDA(cudaFuncSetAttribute(ppo_learn_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLearnSmem));
-    CPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ppo_learn_persistent_kernel, kLearnThreads, kLearnSmem));
+    int per_sm_cat = 0;     // the categorical instantiation shares the grid
+    CPB_CUDA(cudaFuncSetAttribute(ppo_learn_persistent_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLearnSmem));
+    CPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ppo_learn_persistent_kernel<0>, kLearnThreads, kLearnSmem));
+    CPB_CUDA(cudaFuncSetAttribute(ppo_learn_persistent_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLearnSmem));
+    CPB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_cat, ppo_learn_persistent_kernel<1>, kLearnThreads, kLearnSmem));
+    if (per_sm_cat < per_sm) per_sm = per_sm_cat;
     // Opt-in (CPB_PPO_PERSISTENT=1): slower than the launch-per-kernel path -- the 32x32 / 64-thread gemm_tile is latency-bound
     // (8 dependent global round trips per K = 500 tile) and one CTA per SM leaves 8 warps to hide them, where the stand-alone
     // kernels run ~16 CTAs per SM; the barriers are not the cost.  Kept because it is parity-green (tests run both paths) and is the skeleton for a tile routine that
@@ -1094,7 +1333,7 @@ int32_t learn_persistent_init() {
 
 // Everything of the driver's update block after GAE (train.py:178-207): theta_old <- theta, the old policy's
 // log-probabilities, and num_epochs x ceil(T / batch_size) minibatch Adam steps reading pl.ret32 / pl.adv32.
-int32_t learn_update(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
+int32_t learn_update(const cpb_ppo_spec* sp, const HeadShape& hs, const PpoLayout& L, const PpoPlan& pl, float* params, float* params_old,
                      float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
                      const float* states, const float* actions, int T, int num_epochs, int batch_size,
                      const int32_t* perms, float* metrics, const Guards& gd, cudaStream_t s) {
@@ -1102,7 +1341,7 @@ int32_t learn_update(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& 
     // theta_old <- theta (PPO.update_old_policy, ppo.py:275-276)
     CPB_CUDA(cudaMemcpyAsync(params_old, params, L.total * sizeof(float), cudaMemcpyDeviceToDevice, s));
     // log pi_old(a_t|s_t) is constant during the update: evaluate it once for all T samples
-    CPB_TRY(run_old_logp(sp, L, pl, params_old, states, actions, nullptr, T, s));
+    CPB_TRY(run_old_logp(sp, hs, L, pl, params_old, states, actions, nullptr, T, s));
     CPB_TRY(launch_fill_zero(grads, L.total, s));
     const int nmb = cdiv(T, batch_size);
     CPB_TRY(learn_persistent_init());
@@ -1115,8 +1354,10 @@ int32_t learn_update(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& 
         a.states = states; a.actions = actions; a.perms = perms; a.metrics = metrics;
         a.T = T; a.batch_size = batch_size; a.num_epochs = num_epochs; a.nmb = nmb;
         a.gd = gd;
+        a.hs = hs;
         void* args[] = {&a};
-        CPB_CUDA(cudaLaunchCooperativeKernel((void*)ppo_learn_persistent_kernel, dim3((unsigned)g_learn_grid), dim3(kLearnThreads), args, kLearnSmem, s));
+        void* kernel = hs.cat ? (void*)ppo_learn_persistent_kernel<1> : (void*)ppo_learn_persistent_kernel<0>;
+        CPB_CUDA(cudaLaunchCooperativeKernel(kernel, dim3((unsigned)g_learn_grid), dim3(kLearnThreads), args, kLearnSmem, s));
         CPB_LAUNCHED();
         return CPB_OK;
     }
@@ -1126,7 +1367,7 @@ int32_t learn_update(const cpb_ppo_spec* sp, const PpoLayout& L, const PpoPlan& 
             const int B = begin + batch_size <= T ? batch_size : T - begin;
             const int32_t* idx = perms + (long long)e * T + begin;
             float* mt = metrics ? metrics + ((long long)e * nmb + i) * mcols : nullptr;
-            CPB_TRY(run_loss_grad(sp, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
+            CPB_TRY(run_loss_grad(sp, hs, L, pl, params, states, actions, pl.ret32, pl.adv32, idx, B, pl.logp_old, 1,
                                   grads, mt, gd, s));
             if (gd.stop != nullptr) {
                 // the minibatches after a stop are still launched (the host cannot know); Adam skips them on the device
@@ -1167,6 +1408,141 @@ int32_t make_guards(const cpb_ppo_learn_options* opts, const PpoPlan& pl, uint32
 
 using namespace cpb;
 
+// The cpb_ppo_spec and cpb_ppo_cat_spec entry points share one implementation each, on (spec, head shape) of a checked spec
+#define CPB_PPO_PLAN(maxb, horizon)                                                            \
+    CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                    \
+    PpoPlan pl = make_ppo_plan(workspace, workspace_bytes, spec, hs, maxb, horizon);           \
+    if (!pl.ok) {                                                                              \
+        cpb::set_error("ppo workspace too small: need %lld bytes, got %lld", (long long)pl.bytes, \
+                       (long long)workspace_bytes);                                            \
+        return CPB_ERR_WORKSPACE_TOO_SMALL;                                                    \
+    }                                                                                          \
+    PpoLayout L = make_ppo_layout(spec, hs);                                                   \
+    cudaStream_t s = (cudaStream_t)stream;
+
+static int32_t ppo_layout(const cpb_ppo_spec* spec, const HeadShape& hs, int64_t* offsets, int64_t* sizes, int32_t* shapes,
+                          int64_t* total) {
+    PpoLayout L = make_ppo_layout(spec, hs);
+    const int n = hs.cat ? L.n - 1 : L.n;
+    for (int e = 0; e < n; ++e) {
+        const int i = hs.cat ? cat_internal_index(*spec, e) : e;
+        if (offsets) offsets[e] = L.off[i];
+        if (sizes) sizes[e] = L.size[i];
+        if (shapes) { shapes[e * 2] = L.shape[i][0]; shapes[e * 2 + 1] = L.shape[i][1]; }
+    }
+    if (total) *total = L.total;
+    return CPB_OK;
+}
+
+static int32_t ppo_forward(const cpb_ppo_spec* spec, const HeadShape& hs, const float* params, const float* states,
+                           int32_t batch, const float* noise, float* action, float* value, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(batch >= 1, "ppo_forward: batch must be >= 1");
+    CPB_PPO_PLAN(batch, 0);
+    CPB_REQUIRE(params && states && action && value, "ppo_forward: NULL pointer");
+    CPB_TRY(run_trunks(spec, L, pl, params, states, nullptr, batch, s));
+    HeadArgs h = head_args(spec, hs, L, params, batch);
+    h.hp = trunk_buf(pl.h, *spec, 0, spec->num_policy - 1, batch); h.hv = trunk_buf(pl.h, *spec, 1, spec->num_value - 1, batch);
+    h.noise = noise; h.action_out = action; h.v_out = value;
+    launch_head<2>(hs, batch, h, s);
+    CPB_LAUNCHED();
+    return CPB_OK;
+}
+
+static int32_t ppo_loss_grad(const cpb_ppo_spec* spec, const HeadShape& hs, const float* params, const float* params_old,
+                             const float* states, const float* actions, const float* returns, const float* advantages,
+                             const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
+                             int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(batch >= 1, "ppo_loss_grad: batch must be >= 1");
+    CPB_PPO_PLAN(batch, 0);
+    CPB_REQUIRE(params && params_old && states && actions && returns && advantages && grads, "ppo_loss_grad: NULL pointer");
+    CPB_TRY(launch_fill_zero(grads, L.total, s));
+    CPB_TRY(run_old_logp(spec, hs, L, pl, params_old, states, actions, idx, batch, s));
+    return run_loss_grad(spec, hs, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
+                         metrics, Guards{}, s);
+}
+
+static int32_t ppo_train_step(const cpb_ppo_spec* spec, const HeadShape& hs, float* params, const float* params_old,
+                              float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                              const float* states, const float* actions, const float* returns, const float* advantages,
+                              const int32_t* idx, int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes,
+                              void* stream) {
+    CPB_REQUIRE(lr_dev != nullptr, "ppo_train_step: lr_dev is NULL");
+    CPB_TRY(ppo_loss_grad(spec, hs, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
+                          workspace, workspace_bytes, stream));
+    PpoLayout L = make_ppo_layout(spec, hs);
+    return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f,
+                       (cudaStream_t)stream);
+}
+
+static int32_t ppo_train_step_opts(const cpb_ppo_spec* spec, const HeadShape& hs, float* params, const float* params_old,
+                                   float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                   const float* states, const float* actions, const float* returns,
+                                   const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                   const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                   void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(batch >= 1, "ppo_train_step_opts: batch must be >= 1");
+    CPB_PPO_PLAN(batch, 0);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                returns && advantages, "ppo_train_step_opts: NULL pointer");
+    Guards gd;
+    CPB_TRY(make_guards(opts, pl, stop, steps_applied, s, &gd));
+    CPB_TRY(launch_fill_zero(grads, L.total, s));
+    CPB_TRY(run_old_logp(spec, hs, L, pl, params_old, states, actions, idx, batch, s));
+    CPB_TRY(run_loss_grad(spec, hs, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
+                          metrics, gd, s));
+    CPB_TRY(launch_grad_norm(grads, L.total, gd, metrics, s));
+    return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s, gd.stop,
+                       gd.clip, gd.steps);
+}
+
+// learn and its options twin (guarded: opts / steps_applied are used and the metrics rows are 7 wide)
+static int32_t ppo_learn(const cpb_ppo_spec* spec, const HeadShape& hs, float* params, float* params_old, float* grads,
+                         float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                         const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                         const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                         int32_t batch_size, const int32_t* perms, float* metrics, bool guarded,
+                         const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                         int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(T >= 1 && batch_size >= 1 && num_epochs >= 0, "ppo_learn: bad sizes");
+    CPB_PPO_PLAN(batch_size < T ? batch_size : T, T);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                rewards && values && dones, "ppo_learn: NULL pointer");
+    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn: perms is NULL");
+    Guards gd{};
+    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
+    // GAE, returns, normalised advantages (float64), rounded to float32 like the reference's feed
+    gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
+                                  pl.ret32, pl.adv32, pl.gae_scratch);
+    CPB_LAUNCHED();
+    return learn_update(spec, hs, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
+                        num_epochs, batch_size, perms, metrics, gd, s);
+}
+
+// learn_segments and its options twin
+static int32_t ppo_learn_segments(const cpb_ppo_spec* spec, const HeadShape& hs, float* params, float* params_old,
+                                  float* grads, float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                  const float* states, const float* actions, const double* rewards,
+                                  const double* values, const double* bootstrap_values, const double* dones,
+                                  const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                  double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                  float* metrics, bool guarded, const cpb_ppo_learn_options* opts,
+                                  int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments && batch_size >= 1 && num_epochs >= 0,
+                "ppo_learn_segments: bad sizes");
+    CPB_PPO_PLAN(batch_size < rows ? batch_size : rows, rows);
+    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
+                rewards && values && bootstrap_values && dones && segment_offsets, "ppo_learn_segments: NULL pointer");
+    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn_segments: perms is NULL");
+    Guards gd{};
+    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
+    // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
+    CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                                pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
+    return learn_update(spec, hs, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
+                        num_epochs, batch_size, perms, metrics, gd, s);
+}
+
 extern "C" {
 
 int32_t cpb_ppo_num_tensors(void) { return kLegacyPpoTensors; }
@@ -1188,71 +1564,42 @@ const char* cpb_ppo_spec_tensor_name(const cpb_ppo_spec* spec, int32_t i) {
 
 int32_t cpb_ppo_spec_layout(const cpb_ppo_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
     CPB_TRY(check_ppo_spec(spec));
-    PpoLayout L = make_ppo_layout(spec);
-    for (int i = 0; i < L.n; ++i) {
-        if (offsets) offsets[i] = L.off[i];
-        if (sizes) sizes[i] = L.size[i];
-        if (shapes) { shapes[i * 2] = L.shape[i][0]; shapes[i * 2 + 1] = L.shape[i][1]; }
-    }
-    if (total) *total = L.total;
-    return CPB_OK;
+    return ppo_layout(spec, gauss_head(spec), offsets, sizes, shapes, total);
 }
 
 int64_t cpb_ppo_spec_workspace_bytes(const cpb_ppo_spec* spec, int32_t max_batch, int32_t horizon) {
     if (check_ppo_spec(spec) != CPB_OK || max_batch < 1 || horizon < 0) return CPB_ERR_INVALID_ARGUMENT;
-    return make_ppo_plan(nullptr, 0, spec, max_batch, horizon).bytes;
+    return make_ppo_plan(nullptr, 0, spec, gauss_head(spec), max_batch, horizon).bytes;
 }
 
-#define CPB_PPO_PLAN(maxb, horizon)                                                            \
-    CPB_TRY(check_ppo_spec(spec));                                                             \
-    CPB_REQUIRE(workspace != nullptr, "workspace is NULL");                                    \
-    PpoPlan pl = make_ppo_plan(workspace, workspace_bytes, spec, maxb, horizon);               \
-    if (!pl.ok) {                                                                              \
-        cpb::set_error("ppo workspace too small: need %lld bytes, got %lld", (long long)pl.bytes, \
-                       (long long)workspace_bytes);                                            \
-        return CPB_ERR_WORKSPACE_TOO_SMALL;                                                    \
-    }                                                                                          \
-    PpoLayout L = make_ppo_layout(spec);                                                       \
-    cudaStream_t s = (cudaStream_t)stream;
+// the cpb_ppo_spec_* entry points: check the spec, then the shared implementation with the Gaussian head
+#define CPB_PPO_GAUSS()              \
+    CPB_TRY(check_ppo_spec(spec));   \
+    const HeadShape hs = gauss_head(spec);
 
 int32_t cpb_ppo_spec_forward(const cpb_ppo_spec* spec, const float* params, const float* states, int32_t batch,
                              const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
                              void* stream) {
-    CPB_REQUIRE(batch >= 1, "ppo_forward: batch must be >= 1");
-    CPB_PPO_PLAN(batch, 0);
-    CPB_REQUIRE(params && states && action && value, "ppo_forward: NULL pointer");
-    CPB_TRY(run_trunks(spec, L, pl, params, states, nullptr, batch, s));
-    HeadArgs h = head_args(spec, L, params, batch);
-    h.hp = trunk_buf(pl.h, *spec, 0, spec->num_policy - 1, batch); h.hv = trunk_buf(pl.h, *spec, 1, spec->num_value - 1, batch);
-    h.noise = noise; h.action_out = action; h.v_out = value;
-    ppo_head_kernel<2><<<cdiv(batch, 8), 256, 0, s>>>(h);
-    CPB_LAUNCHED();
-    return CPB_OK;
+    CPB_PPO_GAUSS();
+    return ppo_forward(spec, hs, params, states, batch, noise, action, value, workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_spec_loss_grad(const cpb_ppo_spec* spec, const float* params, const float* params_old,
                                const float* states, const float* actions, const float* returns, const float* advantages,
                                const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
                                int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(batch >= 1, "ppo_loss_grad: batch must be >= 1");
-    CPB_PPO_PLAN(batch, 0);
-    CPB_REQUIRE(params && params_old && states && actions && returns && advantages && grads, "ppo_loss_grad: NULL pointer");
-    CPB_TRY(launch_fill_zero(grads, L.total, s));
-    CPB_TRY(run_old_logp(spec, L, pl, params_old, states, actions, idx, batch, s));
-    return run_loss_grad(spec, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
-                         metrics, Guards{}, s);
+    CPB_PPO_GAUSS();
+    return ppo_loss_grad(spec, hs, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
+                         workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_spec_train_step(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
                                 float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
                                 const float* actions, const float* returns, const float* advantages, const int32_t* idx,
                                 int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(lr_dev != nullptr, "ppo_train_step: lr_dev is NULL");
-    CPB_TRY(cpb_ppo_spec_loss_grad(spec, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
-                                   workspace, workspace_bytes, stream));
-    PpoLayout L = make_ppo_layout(spec);
-    return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f,
-                       (cudaStream_t)stream);
+    CPB_PPO_GAUSS();
+    return ppo_train_step(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, returns,
+                          advantages, idx, batch, metrics, workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_spec_train_step_opts(const cpb_ppo_spec* spec, float* params, const float* params_old, float* grads,
@@ -1261,19 +1608,10 @@ int32_t cpb_ppo_spec_train_step_opts(const cpb_ppo_spec* spec, float* params, co
                                      const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
                                      const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
                                      void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(batch >= 1, "ppo_train_step_opts: batch must be >= 1");
-    CPB_PPO_PLAN(batch, 0);
-    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
-                returns && advantages, "ppo_train_step_opts: NULL pointer");
-    Guards gd;
-    CPB_TRY(make_guards(opts, pl, stop, steps_applied, s, &gd));
-    CPB_TRY(launch_fill_zero(grads, L.total, s));
-    CPB_TRY(run_old_logp(spec, L, pl, params_old, states, actions, idx, batch, s));
-    CPB_TRY(run_loss_grad(spec, L, pl, params, states, actions, returns, advantages, idx, batch, pl.logp_old, 0, grads,
-                          metrics, gd, s));
-    CPB_TRY(launch_grad_norm(grads, L.total, gd, metrics, s));
-    return launch_adam(params, grads, adam_m, adam_v, L.total, adam_powers, 0.f, lr_dev, 0.9f, 0.999f, 1e-8f, s, gd.stop,
-                       gd.clip, gd.steps);
+    CPB_PPO_GAUSS();
+    return ppo_train_step_opts(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                               returns, advantages, idx, batch, metrics, opts, stop, steps_applied, workspace,
+                               workspace_bytes, stream);
 }
 
 int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_value, const double* dones, int32_t T,
@@ -1286,38 +1624,16 @@ int32_t cpb_gae(const double* rewards, const double* values, double bootstrap_va
     return CPB_OK;
 }
 
-// cpb_ppo_spec_learn and its options twin (guarded: opts / steps_applied are used and the metrics rows are 7 wide)
-static int32_t ppo_learn(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
-                         float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
-                         const float* actions, const double* rewards, const double* values, double bootstrap_value,
-                         const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
-                         int32_t batch_size, const int32_t* perms, float* metrics, bool guarded,
-                         const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
-                         int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(T >= 1 && batch_size >= 1 && num_epochs >= 0, "ppo_learn: bad sizes");
-    CPB_PPO_PLAN(batch_size < T ? batch_size : T, T);
-    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
-                rewards && values && dones, "ppo_learn: NULL pointer");
-    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn: perms is NULL");
-    Guards gd{};
-    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
-    // GAE, returns, normalised advantages (float64), rounded to float32 like the reference's feed
-    gae_kernel<<<1, 1024, 0, s>>>(rewards, values, bootstrap_value, dones, T, gamma, lam, nullptr, nullptr, nullptr,
-                                  pl.ret32, pl.adv32, pl.gae_scratch);
-    CPB_LAUNCHED();
-    return learn_update(spec, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, T,
-                        num_epochs, batch_size, perms, metrics, gd, s);
-}
-
 int32_t cpb_ppo_spec_learn(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
                            float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
                            const float* actions, const double* rewards, const double* values, double bootstrap_value,
                            const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
                            int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
                            int64_t workspace_bytes, void* stream) {
-    return ppo_learn(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
-                     bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, false, nullptr, nullptr,
-                     workspace, workspace_bytes, stream);
+    CPB_PPO_GAUSS();
+    return ppo_learn(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                     values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, false, nullptr,
+                     nullptr, workspace, workspace_bytes, stream);
 }
 
 int32_t cpb_ppo_spec_learn_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
@@ -1327,8 +1643,9 @@ int32_t cpb_ppo_spec_learn_opts(const cpb_ppo_spec* spec, float* params, float* 
                                 int32_t batch_size, const int32_t* perms, float* metrics,
                                 const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
                                 int64_t workspace_bytes, void* stream) {
-    return ppo_learn(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards, values,
-                     bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, true, opts,
+    CPB_PPO_GAUSS();
+    return ppo_learn(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                     values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, true, opts,
                      steps_applied, workspace, workspace_bytes, stream);
 }
 
@@ -1342,30 +1659,6 @@ int32_t cpb_gae_segments(const double* rewards, const double* values, const doub
                                advantages, returns, advantages_norm, nullptr, nullptr, (cudaStream_t)stream);
 }
 
-// cpb_ppo_spec_learn_segments and its options twin
-static int32_t ppo_learn_segments(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
-                                  float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
-                                  const float* states, const float* actions, const double* rewards,
-                                  const double* values, const double* bootstrap_values, const double* dones,
-                                  const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
-                                  double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
-                                  float* metrics, bool guarded, const cpb_ppo_learn_options* opts,
-                                  int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream) {
-    CPB_REQUIRE(num_segments >= 1 && rows >= num_segments && batch_size >= 1 && num_epochs >= 0,
-                "ppo_learn_segments: bad sizes");
-    CPB_PPO_PLAN(batch_size < rows ? batch_size : rows, rows);
-    CPB_REQUIRE(params && params_old && grads && adam_m && adam_v && adam_powers && lr_dev && states && actions &&
-                rewards && values && bootstrap_values && dones && segment_offsets, "ppo_learn_segments: NULL pointer");
-    CPB_REQUIRE(perms != nullptr || num_epochs == 0, "ppo_learn_segments: perms is NULL");
-    Guards gd{};
-    if (guarded) CPB_TRY(make_guards(opts, pl, nullptr, steps_applied, s, &gd));
-    // GAE per segment, then returns and advantages normalised over all rows (float64), rounded to float32
-    CPB_TRY(launch_gae_segments(rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
-                                pl.gae_scratch, nullptr, nullptr, pl.ret32, pl.adv32, s));
-    return learn_update(spec, L, pl, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rows,
-                        num_epochs, batch_size, perms, metrics, gd, s);
-}
-
 int32_t cpb_ppo_spec_learn_segments(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
                                     float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
                                     const float* states, const float* actions, const double* rewards,
@@ -1373,9 +1666,11 @@ int32_t cpb_ppo_spec_learn_segments(const cpb_ppo_spec* spec, float* params, flo
                                     const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
                                     double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
                                     float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
-    return ppo_learn_segments(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
-                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
-                              batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes, stream);
+    CPB_PPO_GAUSS();
+    return ppo_learn_segments(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                              rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                              num_epochs, batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes,
+                              stream);
 }
 
 int32_t cpb_ppo_spec_learn_segments_opts(const cpb_ppo_spec* spec, float* params, float* params_old, float* grads,
@@ -1386,9 +1681,132 @@ int32_t cpb_ppo_spec_learn_segments_opts(const cpb_ppo_spec* spec, float* params
                                          double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
                                          float* metrics, const cpb_ppo_learn_options* opts, int32_t* steps_applied,
                                          void* workspace, int64_t workspace_bytes, void* stream) {
-    return ppo_learn_segments(spec, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
-                              values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam, num_epochs,
-                              batch_size, perms, metrics, true, opts, steps_applied, workspace, workspace_bytes, stream);
+    CPB_PPO_GAUSS();
+    return ppo_learn_segments(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                              rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                              num_epochs, batch_size, perms, metrics, true, opts, steps_applied, workspace,
+                              workspace_bytes, stream);
+}
+
+// ---- The categorical twins: check the cpb_ppo_cat_spec, then the shared implementation with its head
+#define CPB_PPO_CAT()                 \
+    HeadShape hs;                     \
+    CPB_TRY(cat_head(cspec, &hs));    \
+    const cpb_ppo_spec* spec = &cspec->spec;
+
+int32_t cpb_ppo_cat_num_tensors(const cpb_ppo_cat_spec* cspec) {
+    CPB_PPO_CAT();
+    return 2 * (spec->num_policy + spec->num_value) + 4;
+}
+const char* cpb_ppo_cat_tensor_name(const cpb_ppo_cat_spec* cspec, int32_t i) {
+    HeadShape hs;
+    if (cat_head(cspec, &hs) != CPB_OK) return nullptr;
+    const cpb_ppo_spec* spec = &cspec->spec;
+    if (i < 0 || i >= 2 * (spec->num_policy + spec->num_value) + 4) return nullptr;
+    const int k = cat_internal_index(*spec, i);
+    if (k == 2 * spec->num_policy) return "action_logits/kernel";
+    if (k == 2 * spec->num_policy + 1) return "action_logits/bias";
+    return ppo_tensor_name(spec, k);
+}
+int32_t cpb_ppo_cat_layout(const cpb_ppo_cat_spec* cspec, int64_t* offsets, int64_t* sizes, int32_t* shapes, int64_t* total) {
+    CPB_PPO_CAT();
+    return ppo_layout(spec, hs, offsets, sizes, shapes, total);
+}
+int64_t cpb_ppo_cat_workspace_bytes(const cpb_ppo_cat_spec* cspec, int32_t max_batch, int32_t horizon) {
+    HeadShape hs;
+    if (cat_head(cspec, &hs) != CPB_OK || max_batch < 1 || horizon < 0) return CPB_ERR_INVALID_ARGUMENT;
+    return make_ppo_plan(nullptr, 0, &cspec->spec, hs, max_batch, horizon).bytes;
+}
+
+int32_t cpb_ppo_cat_forward(const cpb_ppo_cat_spec* cspec, const float* params, const float* states, int32_t batch,
+                            const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
+                            void* stream) {
+    CPB_PPO_CAT();
+    return ppo_forward(spec, hs, params, states, batch, noise, action, value, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_loss_grad(const cpb_ppo_cat_spec* cspec, const float* params, const float* params_old,
+                              const float* states, const float* actions, const float* returns, const float* advantages,
+                              const int32_t* idx, int32_t batch, float* grads, float* metrics, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_loss_grad(spec, hs, params, params_old, states, actions, returns, advantages, idx, batch, grads, metrics,
+                         workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_train_step(const cpb_ppo_cat_spec* cspec, float* params, const float* params_old, float* grads,
+                               float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                               const float* actions, const float* returns, const float* advantages, const int32_t* idx,
+                               int32_t batch, float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_train_step(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, returns,
+                          advantages, idx, batch, metrics, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_train_step_opts(const cpb_ppo_cat_spec* cspec, float* params, const float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const float* returns,
+                                    const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                    const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                    void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_train_step_opts(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                               returns, advantages, idx, batch, metrics, opts, stop, steps_applied, workspace,
+                               workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_learn(const cpb_ppo_cat_spec* cspec, float* params, float* params_old, float* grads, float* adam_m,
+                          float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                          const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                          const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                          int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                          int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_learn(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                     values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, false, nullptr,
+                     nullptr, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_learn_opts(const cpb_ppo_cat_spec* cspec, float* params, float* params_old, float* grads,
+                               float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                               const float* actions, const double* rewards, const double* values,
+                               double bootstrap_value, const double* dones, int32_t T, double gamma, double lam,
+                               int32_t num_epochs, int32_t batch_size, const int32_t* perms, float* metrics,
+                               const cpb_ppo_learn_options* opts, int32_t* steps_applied, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_learn(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions, rewards,
+                     values, bootstrap_value, dones, T, gamma, lam, num_epochs, batch_size, perms, metrics, true, opts,
+                     steps_applied, workspace, workspace_bytes, stream);
+}
+
+int32_t cpb_ppo_cat_learn_segments(const cpb_ppo_cat_spec* cspec, float* params, float* params_old, float* grads,
+                                   float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                   const float* states, const float* actions, const double* rewards,
+                                   const double* values, const double* bootstrap_values, const double* dones,
+                                   const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                   double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                   float* metrics, void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_learn_segments(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                              rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                              num_epochs, batch_size, perms, metrics, false, nullptr, nullptr, workspace, workspace_bytes,
+                              stream);
+}
+
+int32_t cpb_ppo_cat_learn_segments_opts(const cpb_ppo_cat_spec* cspec, float* params, float* params_old, float* grads,
+                                        float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                        const float* states, const float* actions, const double* rewards,
+                                        const double* values, const double* bootstrap_values, const double* dones,
+                                        const int32_t* segment_offsets, int32_t num_segments, int32_t rows, double gamma,
+                                        double lam, int32_t num_epochs, int32_t batch_size, const int32_t* perms,
+                                        float* metrics, const cpb_ppo_learn_options* opts, int32_t* steps_applied,
+                                        void* workspace, int64_t workspace_bytes, void* stream) {
+    CPB_PPO_CAT();
+    return ppo_learn_segments(spec, hs, params, params_old, grads, adam_m, adam_v, adam_powers, lr_dev, states, actions,
+                              rewards, values, bootstrap_values, dones, segment_offsets, num_segments, rows, gamma, lam,
+                              num_epochs, batch_size, perms, metrics, true, opts, steps_applied, workspace,
+                              workspace_bytes, stream);
 }
 
 // ---- The two-per-side entry points: the spec twins at {hidden1, hidden2} / {hidden1, hidden2}

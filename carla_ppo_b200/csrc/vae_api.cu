@@ -1416,16 +1416,18 @@ typedef int32_t (*EncodeMeanFn)(const void* vae, const float* params, const void
                                 void* workspace, int64_t workspace_bytes, void* stream);
 
 // The encode_predict entry points: `encode` on the VAE described by `vae` (whose common part is `base`), then the state
-// assembly and the PPO forward.  The PPO spec is checked before anything is enqueued.
+// assembly and the PPO forward, with the Gaussian head of ppo_spec or (cat_spec != NULL) the categorical head of
+// cat_spec.  The PPO spec is checked before anything is enqueued.
 static int32_t encode_predict(const cpb_vae_config* base, const void* vae, EncodeMeanFn encode, const float* vae_params,
                               const void* frames, const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
-                              const float* ppo_params, const float* noise, float* latent_tmp, float* state, float* action,
-                              float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes, void* ppo_workspace,
-                              int64_t ppo_workspace_bytes, void* stream) {
+                              const cpb_ppo_cat_spec* cat_spec, const float* ppo_params, const float* noise, float* latent_tmp,
+                              float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
+                              int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
+    if (cat_spec != nullptr) ppo_spec = &cat_spec->spec;
     CPB_REQUIRE(base && ppo_spec && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
     CPB_REQUIRE(num_measurements >= 0 && (num_measurements == 0 || measurements != nullptr), "encode_predict: bad measurements");
     const int B = base->batch;
-    const int32_t ppo_tensors = cpb_ppo_spec_num_tensors(ppo_spec);   // checks the spec
+    const int32_t ppo_tensors = cat_spec ? cpb_ppo_cat_num_tensors(cat_spec) : cpb_ppo_spec_num_tensors(ppo_spec);   // checks the spec
     if (ppo_tensors < 0) return ppo_tensors;
     CPB_REQUIRE(ppo_spec->base.state_dim == base->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
                 ppo_spec->base.state_dim, base->z_dim, num_measurements);
@@ -1433,6 +1435,8 @@ static int32_t encode_predict(const cpb_vae_config* base, const void* vae, Encod
     const int total = B * ppo_spec->base.state_dim;
     assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, base->z_dim, num_measurements, state);
     CPB_LAUNCHED();
+    if (cat_spec != nullptr)
+        return cpb_ppo_cat_forward(cat_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
     return cpb_ppo_spec_forward(ppo_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
 }
 
@@ -1447,19 +1451,31 @@ int32_t cpb_vae_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_p
                                                 vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
 }
 
+static int32_t conv_encode_mean(const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
+                                int64_t ws_bytes, void* stream) {
+    return cpb_vae_spec_encode((const cpb_vae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
+}
+
 int32_t cpb_vae_spec_ppo_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
                                              const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
                                              const float* ppo_params, const float* noise, float* latent_tmp, float* state,
                                              float* action, float* value, int32_t* flags, void* vae_workspace,
                                              int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
                                              void* stream) {
-    EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
-                             int64_t ws_bytes, void* stream) {
-        return cpb_vae_spec_encode((const cpb_vae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
-    };
-    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_spec,
-                          ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
-                          ppo_workspace, ppo_workspace_bytes, stream);
+    return encode_predict(spec ? &spec->base : nullptr, spec, conv_encode_mean, vae_params, frames, measurements, num_measurements,
+                          ppo_spec, nullptr, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_vae_spec_ppo_cat_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                            const float* measurements, int32_t num_measurements, const cpb_ppo_cat_spec* ppo_spec,
+                                            const float* ppo_params, const float* noise, float* latent_tmp, float* state,
+                                            float* action, float* value, int32_t* flags, void* vae_workspace,
+                                            int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
+                                            void* stream) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, conv_encode_mean, vae_params, frames, measurements, num_measurements,
+                          nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
 }
 
 static int64_t frame_bytes(const cpb_vae_spec* spec, int dtype, int channels) {
@@ -1715,19 +1731,31 @@ int32_t cpb_mlpvae_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_
                                               ppo_workspace, ppo_workspace_bytes, stream);
 }
 
+static int32_t mlp_encode_mean(const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
+                               int64_t ws_bytes, void* stream) {
+    return cpb_mlpvae_spec_encode((const cpb_mlpvae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
+}
+
 int32_t cpb_mlpvae_ppo_spec_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
                                            const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
                                            const float* ppo_params, const float* noise, float* latent_tmp, float* state,
                                            float* action, float* value, int32_t* flags, void* vae_workspace,
                                            int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
                                            void* stream) {
-    EncodeMeanFn encode = [](const void* vae, const float* params, const void* frames, float* latent, int32_t* flags, void* ws,
-                             int64_t ws_bytes, void* stream) {
-        return cpb_mlpvae_spec_encode((const cpb_mlpvae_spec*)vae, params, frames, latent, nullptr, flags, ws, ws_bytes, stream);
-    };
-    return encode_predict(spec ? &spec->base : nullptr, spec, encode, vae_params, frames, measurements, num_measurements, ppo_spec,
-                          ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace, vae_workspace_bytes,
-                          ppo_workspace, ppo_workspace_bytes, stream);
+    return encode_predict(spec ? &spec->base : nullptr, spec, mlp_encode_mean, vae_params, frames, measurements, num_measurements,
+                          ppo_spec, nullptr, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_ppo_cat_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                          const float* measurements, int32_t num_measurements, const cpb_ppo_cat_spec* ppo_spec,
+                                          const float* ppo_params, const float* noise, float* latent_tmp, float* state,
+                                          float* action, float* value, int32_t* flags, void* vae_workspace,
+                                          int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes,
+                                          void* stream) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, mlp_encode_mean, vae_params, frames, measurements, num_measurements,
+                          nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
 }
 
 /* The two-per-side entry points: the spec entry points on {enc1, enc2} / {dec1, dec2} */

@@ -20,6 +20,12 @@ Additive constructor arguments ``policy_hidden_sizes`` / ``value_hidden_sizes`` 
 both) size the two trunks independently, 1 to 8 dense + ReLU layers each, like Stable-Baselines3's
 ``net_arch=dict(pi=[...], vf=[...])``.  Every call goes through the cpb_ppo_spec_* entry points; checkpoints carry the
 architecture in their variable names and shapes (``checkpoint_architecture``).
+
+Discrete action spaces (an addition: the reference's policy is always the tanh-squashed Gaussian over a Box):
+``action_space`` may be a Discrete(n) (anything with ``.n``) or a MultiDiscrete(nvec) (anything with ``.nvec``): 1 to 4
+components of 2 to 64 categories, 64 in all.  The policy head is then a categorical distribution per component
+(cpb_ppo_cat_* entry points, include/carla_ppo_b200.h "Categorical policies"); actions are int64 indices, ``predict``
+samples with [B, K] uniforms, and checkpoints record the categories (``checkpoint_action_categories``).
 """
 from __future__ import annotations
 
@@ -31,7 +37,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from . import _lib
-from ._lib import CpbError, PpoConfig, PpoSpec
+from ._lib import CpbError, PpoCatSpec, PpoConfig, PpoSpec
 
 ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8
 _METRIC_NAMES = ("train_loss/policy", "train_loss/value", "train_loss/entropy", "train_loss/loss", "train/prob_ratio")
@@ -46,6 +52,36 @@ def learn_options(max_grad_norm=None, target_kl=None):
 
 
 ARCH_KEYS = ("ppo_architecture/policy_hidden_sizes", "ppo_architecture/value_hidden_sizes")
+CATEGORIES_KEY = "ppo_architecture/action_categories"
+
+
+def action_categories(action_space):
+    """The categories (n_1 .. n_K) of a discrete action space -- ``.nvec`` (MultiDiscrete) or ``.n`` (Discrete) -- or None
+    for a Box (``.shape`` / ``.low`` / ``.high``).  Raises ValueError outside 1..4 components of 2..64 categories, 64 in
+    all."""
+    if hasattr(action_space, "nvec"):
+        cats = tuple(int(v) for v in np.asarray(action_space.nvec).reshape(-1))
+    elif hasattr(action_space, "n"):
+        cats = (int(action_space.n),)
+    else:
+        return None
+    if not 1 <= len(cats) <= 4 or min(cats) < 2 or max(cats) > _lib.PPO_MAX_LOGITS or sum(cats) > _lib.PPO_MAX_LOGITS:
+        raise ValueError("discrete action spaces take 1 to 4 components of 2 to %d categories, %d in all; got %r"
+                         % (_lib.PPO_MAX_LOGITS, _lib.PPO_MAX_LOGITS, cats))
+    return cats
+
+
+def blob_action_categories(blob, scope="policy/"):
+    """The categories a checkpoint blob records, or () for a Gaussian one (no record: the reference's).  Raises ValueError
+    when the record and the action_logits kernel disagree."""
+    if CATEGORIES_KEY not in blob:
+        if scope + "action_logits/kernel" in blob:
+            raise ValueError("the checkpoint has a categorical head but does not record its categories")
+        return ()
+    cats = tuple(int(v) for v in np.asarray(blob[CATEGORIES_KEY]).reshape(-1))
+    if scope + "action_logits/kernel" not in blob or np.shape(blob[scope + "action_logits/kernel"])[1] != sum(cats):
+        raise ValueError("the checkpoint records categories %r, which its action_logits kernel does not have" % (cats,))
+    return cats
 
 
 def _fmt(arch):
@@ -61,10 +97,12 @@ def _inferred_architectures(blob, scope):
         if name not in blob:
             break
         kernels.append(np.shape(blob[name]))
-    if len(kernels) < 2 or scope + "action_mean/kernel" not in blob or scope + "value/kernel" not in blob:
-        raise ValueError("not a PPO checkpoint: expected %sdense .. dense_N, action_mean and value kernels" % scope)
+    head = scope + ("action_mean/kernel" if scope + "action_mean/kernel" in blob else "action_logits/kernel")
+    if len(kernels) < 2 or head not in blob or scope + "value/kernel" not in blob:
+        raise ValueError("not a PPO checkpoint: expected %sdense .. dense_N, action_mean (or action_logits) and value kernels"
+                         % scope)
     state_dim = kernels[0][0]
-    p_last, v_last = np.shape(blob[scope + "action_mean/kernel"])[0], np.shape(blob[scope + "value/kernel"])[0]
+    p_last, v_last = np.shape(blob[head])[0], np.shape(blob[scope + "value/kernel"])[0]
     chain = lambda ks: all(ks[i][0] == ks[i - 1][1] for i in range(1, len(ks)))
     out = []
     for n_pol in range(1, len(kernels)):
@@ -126,6 +164,14 @@ def checkpoint_architecture(checkpoint_dir):
     return None if blob is None else blob_architecture(blob)
 
 
+def checkpoint_action_categories(checkpoint_dir):
+    """The action categories of the latest checkpoint in checkpoint_dir: a tuple for a categorical agent, () for a
+    Gaussian one, None when there is no checkpoint.  Raises ValueError like blob_action_categories."""
+    prefix = _latest_checkpoint_prefix(checkpoint_dir)
+    blob = _read_blob(prefix) if prefix is not None else None
+    return None if blob is None else blob_action_categories(blob)
+
+
 class PPO:
     def __init__(self, input_shape, action_space, learning_rate=3e-4, lr_decay=0.998, epsilon=0.2,
                  value_scale=0.5, entropy_scale=0.01, initial_std=0.4, model_dir="./", seed=None, device=None,
@@ -140,11 +186,16 @@ class PPO:
             raise ValueError("PPO expects a flat state vector (reference train.py:85 builds [z_dim + measurements])")
         self.input_shape = input_shape
         self.state_dim = input_shape[0]
-        self.num_actions = int(action_space.shape[0])
-        if self.num_actions > 4:
-            raise ValueError("at most 4 action dimensions are supported")
-        self.action_low = np.broadcast_to(np.asarray(action_space.low, np.float32), (self.num_actions,)).copy()
-        self.action_high = np.broadcast_to(np.asarray(action_space.high, np.float32), (self.num_actions,)).copy()
+        self.action_categories = action_categories(action_space)     # None: the reference's Gaussian over a Box
+        if self.action_categories is not None:
+            self.num_actions = len(self.action_categories)
+            self.action_low = self.action_high = np.zeros(self.num_actions, np.float32)
+        else:
+            self.num_actions = int(action_space.shape[0])
+            if self.num_actions > 4:
+                raise ValueError("at most 4 action dimensions are supported")
+            self.action_low = np.broadcast_to(np.asarray(action_space.low, np.float32), (self.num_actions,)).copy()
+            self.action_high = np.broadcast_to(np.asarray(action_space.high, np.float32), (self.num_actions,)).copy()
         self.base_learning_rate = float(learning_rate)
         self.lr_decay = float(lr_decay)
         self.epsilon = float(epsilon)
@@ -209,12 +260,18 @@ class PPO:
         if (self._c.hidden1, self._c.hidden2) != tuple(self._legacy_widths()):
             # a subclass that sizes the network through _cfg(), as the two-width interface did: its widths, both trunks
             self.policy_hidden_sizes = self.value_hidden_sizes = (int(self._c.hidden1), int(self._c.hidden2))
-        self._spec = PpoSpec.of(self._c, self.policy_hidden_sizes, self.value_hidden_sizes)
-        n = _lib.check(lib.cpb_ppo_spec_num_tensors(C.byref(self._spec)), "cpb_ppo_spec_num_tensors")
+        if self.action_categories is None:
+            self._spec = PpoSpec.of(self._c, self.policy_hidden_sizes, self.value_hidden_sizes)
+            self._api = "cpb_ppo_spec_"
+        else:
+            self._spec = PpoCatSpec.of(self._c, self.policy_hidden_sizes, self.value_hidden_sizes, self.action_categories)
+            self._api = "cpb_ppo_cat_"
+        api = lambda name: getattr(lib, self._api + name)
+        n = _lib.check(api("num_tensors")(C.byref(self._spec)), self._api + "num_tensors")
         offs = (C.c_int64 * n)(); sizes = (C.c_int64 * n)(); shapes = (C.c_int32 * (2 * n))()
         total = C.c_int64()
-        _lib.check(lib.cpb_ppo_spec_layout(C.byref(self._spec), offs, sizes, shapes, C.byref(total)), "cpb_ppo_spec_layout")
-        self._names = [lib.cpb_ppo_spec_tensor_name(C.byref(self._spec), i).decode() for i in range(n)]
+        _lib.check(api("layout")(C.byref(self._spec), offs, sizes, shapes, C.byref(total)), self._api + "layout")
+        self._names = [api("tensor_name")(C.byref(self._spec), i).decode() for i in range(n)]
         self._offsets = {self._names[i]: int(offs[i]) for i in range(n)}
         self._shapes = {self._names[i]: tuple(int(s) for s in shapes[2 * i:2 * i + 2] if s > 0) for i in range(n)}
         self._total = int(total.value)
@@ -236,7 +293,8 @@ class PPO:
 
     def _initial_weights(self) -> Dict[str, np.ndarray]:
         """tf.layers.dense defaults (glorot uniform / zeros); action_mean kernel = variance_scaling(0.1)
-        truncated normal (ppo.py:44-47); action_logstd = log(initial_std) (ppo.py:49)."""
+        truncated normal (ppo.py:44-47); action_logstd = log(initial_std) (ppo.py:49).  A categorical head's
+        action_logits kernel is drawn like action_mean's (a near-uniform initial policy)."""
         rng = np.random.RandomState(self._seed if self._seed is not None else np.random.randint(0, 2 ** 31 - 1))
         out = {}
         for name in self._names:
@@ -245,7 +303,7 @@ class PPO:
                 out[name] = np.full(shape, np.log(self.initial_std), np.float32)
             elif name.endswith("bias"):
                 out[name] = np.zeros(shape, np.float32)
-            elif name == "action_mean/kernel":
+            elif name in ("action_mean/kernel", "action_logits/kernel"):
                 std = np.sqrt(0.1 / shape[0]) / 0.87962566103423978
                 t = rng.randn(*shape)
                 bad = np.abs(t) > 2
@@ -313,12 +371,25 @@ class PPO:
             return _lib.check(getattr(self._libh, name)(*args), name)
 
     def _workspace(self, max_batch, horizon=0):
-        need = self._libh.cpb_ppo_spec_workspace_bytes(C.byref(self._spec), int(max_batch), int(horizon))
-        _lib.check(need, "cpb_ppo_spec_workspace_bytes")
+        need = getattr(self._libh, self._api + "workspace_bytes")(C.byref(self._spec), int(max_batch), int(horizon))
+        _lib.check(need, self._api + "workspace_bytes")
         if self._ws is None or self._ws.numel() < need:
             self._ws = None
             self._ws = self._torch.empty(int(need), dtype=self._torch.uint8, device=self._device)
         return self._ws
+
+    def _actions(self, a, rows=-1):
+        """Taken actions as a device float32 [rows, K] tensor.  A categorical agent takes integer indices; host arrays are
+        checked (ValueError for a non-integer or out-of-range index), device tensors are passed as they are (the kernels
+        clamp every index into its component's range)."""
+        torch = self._torch
+        if self.action_categories is not None and not isinstance(a, torch.Tensor):
+            host = np.asarray(a, np.float64).reshape(rows, self.num_actions)
+            if not np.all(np.isfinite(host)) or np.any(host != np.round(host)):
+                raise ValueError("discrete actions must be integer indices")
+            if np.any(host < 0) or np.any(host >= np.asarray(self.action_categories)):
+                raise ValueError("discrete actions must lie in [0, n_k) for categories %r" % (self.action_categories,))
+        return self._dev(a, torch.float32).reshape(rows, self.num_actions)
 
     def _dev(self, a, dtype):
         torch = self._torch
@@ -350,6 +421,8 @@ class PPO:
         blob["predict_step_counter"] = np.int32(self.predict_step_counter)
         for key, sizes in zip(ARCH_KEYS, self.architecture):
             blob[key] = np.asarray(sizes, np.int32)
+        if self.action_categories is not None:
+            blob[CATEGORIES_KEY] = np.asarray(self.action_categories, np.int32)
         if tf_format:
             from .tf_bundle import write_bundle
             write_bundle(prefix, {k: np.asarray(v) for k, v in blob.items()})
@@ -396,6 +469,10 @@ class PPO:
         found = blob_architecture(blob)
         if found != self.architecture:
             raise ValueError("checkpoint architecture %s does not match this PPO's %s" % (_fmt(found), _fmt(self.architecture)))
+        cats = blob_action_categories(blob)
+        if cats != (self.action_categories or ()):
+            kind = lambda c: "categories %r" % (c,) if c else "a Gaussian policy"
+            raise ValueError("the checkpoint has %s, this PPO %s" % (kind(cats), kind(self.action_categories)))
         pol = {n: blob["policy/" + n] for n in self._names}
         old = {n: blob["policy_old/" + n] for n in self._names}
         m_ = v_ = pw = None
@@ -421,7 +498,7 @@ class PPO:
         self._require_session()
         torch = self._torch
         s = self._dev(input_states, torch.float32).reshape(-1, self.state_dim)
-        a = self._dev(taken_actions, torch.float32).reshape(-1, self.num_actions)
+        a = self._actions(taken_actions)
         r = self._dev(returns, torch.float32).reshape(-1)
         adv = self._dev(advantage, torch.float32).reshape(-1)
         b = s.shape[0]
@@ -433,14 +510,14 @@ class PPO:
         metrics = torch.empty(5 if opts is None else 7, dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
         if opts is None:
-            self._call("cpb_ppo_spec_train_step", 
+            self._call(self._api + "train_step",
                 C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), _lib.ptr(ws),
                 ws.numel(), self._stream())
         else:
             applied = torch.empty(1, dtype=torch.int32, device=self._device)
-            self._call("cpb_ppo_spec_train_step_opts",
+            self._call(self._api + "train_step_opts",
                 C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(adv), None, b, _lib.ptr(metrics), C.byref(opts),
@@ -461,13 +538,13 @@ class PPO:
         self._require_session()
         torch = self._torch
         s = self._dev(input_states, torch.float32).reshape(-1, self.state_dim)
-        a = self._dev(taken_actions, torch.float32).reshape(-1, self.num_actions)
+        a = self._actions(taken_actions)
         r = self._dev(returns, torch.float32).reshape(-1)
         adv = self._dev(advantage, torch.float32).reshape(-1)
         b = s.shape[0]
         metrics = torch.empty(5, dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
-        self._call("cpb_ppo_spec_loss_grad", 
+        self._call(self._api + "loss_grad",
             C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(s), _lib.ptr(a), _lib.ptr(r),
             _lib.ptr(adv), None, b, _lib.ptr(self.grads), _lib.ptr(metrics), _lib.ptr(ws), ws.numel(),
             self._stream())
@@ -475,7 +552,9 @@ class PPO:
 
     def predict(self, input_states, greedy=False, write_to_summary=False, noise=None):
         """-> (action, value); squeezed when a single state is given (ppo.py:231-251).  ``noise`` (optional
-        [B,A] standard-normal draws) makes the sampled action reproducible."""
+        [B,A] standard-normal draws) makes the sampled action reproducible.  A categorical agent returns int64 indices
+        [B,K]: the most likely category of each component when greedy, else the inverse-CDF draw of ``noise`` ([B,K]
+        uniforms in [0, 1), default self._rng.rand)."""
         self._require_session()
         torch = self._torch
         x = np.asarray(input_states, dtype=np.float32)
@@ -485,18 +564,21 @@ class PPO:
         if greedy:
             packed = x
         else:
-            eps = self._rng.randn(b, a_dim).astype(np.float32) if noise is None else np.asarray(noise, np.float32).reshape(b, a_dim)
+            draw = self._rng.randn if self.action_categories is None else self._rng.rand
+            eps = draw(b, a_dim).astype(np.float32) if noise is None else np.asarray(noise, np.float32).reshape(b, a_dim)
             packed = np.concatenate([x.reshape(-1), eps.reshape(-1)])
         dev = torch.from_numpy(np.ascontiguousarray(packed).reshape(-1)).to(self._device)
         s = dev[:b * self.state_dim]
         nz = None if greedy else dev[b * self.state_dim:]
         out = torch.empty(b * (a_dim + 1), dtype=torch.float32, device=self._device)
         ws = self._workspace(b)
-        self._call("cpb_ppo_spec_forward", C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(s), b, _lib.ptr(nz),
+        self._call(self._api + "forward", C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(s), b, _lib.ptr(nz),
                                               _lib.ptr(out), _lib.ptr(out[b * a_dim:]), _lib.ptr(ws), ws.numel(),
                                               self._stream())
         host = out.cpu().numpy()
         action, value = host[:b * a_dim].reshape(b, a_dim), host[b * a_dim:]
+        if self.action_categories is not None:
+            action = action.astype(np.int64)
         if write_to_summary:
             if self.train_writer is not None:
                 for i in range(a_dim):
@@ -538,7 +620,7 @@ class PPO:
         torch = self._torch
         s = self._dev(states, torch.float32).reshape(-1, self.state_dim)
         t_len = s.shape[0]
-        a = self._dev(actions, torch.float32).reshape(t_len, self.num_actions)
+        a = self._actions(actions, t_len)
         r = self._dev(rewards, torch.float64).reshape(t_len)
         v = self._dev(values, torch.float64).reshape(t_len)
         d = self._dev(np.asarray(dones, dtype=np.float64) if not isinstance(dones, torch.Tensor) else dones, torch.float64).reshape(t_len)
@@ -563,16 +645,16 @@ class PPO:
             tail = (float(gamma), float(lam), int(num_epochs), int(batch_size), _lib.ptr(p), _lib.ptr(metrics),
                     C.byref(opts), _lib.ptr(applied), _lib.ptr(ws), ws.numel(), self._stream())
             if segment_lengths is None:
-                self._call("cpb_ppo_spec_learn_opts", *common, float(last_value), _lib.ptr(d), t_len, *tail)
+                self._call(self._api + "learn_opts", *common, float(last_value), _lib.ptr(d), t_len, *tail)
             else:
                 b = self._dev(boot, torch.float64)
                 offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
-                self._call("cpb_ppo_spec_learn_segments_opts", *common, _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
+                self._call(self._api + "learn_segments_opts", *common, _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),
                            len(lengths), t_len, *tail)
             self._pending_applied.append(applied)
             self.last_steps_applied = applied
         elif segment_lengths is None:
-            self._call("cpb_ppo_spec_learn",
+            self._call(self._api + "learn",
                 C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), float(last_value), _lib.ptr(d), t_len, float(gamma),
@@ -581,7 +663,7 @@ class PPO:
         else:
             b = self._dev(boot, torch.float64)
             offsets = self._dev(np.concatenate([[0], np.cumsum(lengths)]), torch.int32)
-            self._call("cpb_ppo_spec_learn_segments",
+            self._call(self._api + "learn_segments",
                 C.byref(self._spec), _lib.ptr(self.params), _lib.ptr(self.params_old), _lib.ptr(self.grads),
                 _lib.ptr(self.adam_m), _lib.ptr(self.adam_v), _lib.ptr(self.adam_powers), _lib.ptr(self._lr_dev),
                 _lib.ptr(s), _lib.ptr(a), _lib.ptr(r), _lib.ptr(v), _lib.ptr(b), _lib.ptr(d), _lib.ptr(offsets),

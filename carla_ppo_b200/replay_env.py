@@ -4,7 +4,8 @@
 Only the surface the training / evaluation loops and ``vae_common.create_encode_state_fn`` touch is provided
 (SURVEY.md section 8f-3); the simulator itself (sensors, HUD, planner, reward shaping on real waypoints) is out of scope:
 
-  * ``action_space`` with ``.shape / .low / .high``          (steer in [-1, 1], throttle in [0, 1], carla_lap_env.py)
+  * ``action_space`` with ``.shape / .low / .high``          (steer in [-1, 1], throttle in [0, 1], carla_lap_env.py), or
+    with ``discrete_actions=(n_steer, n_throttle)`` a MultiDiscrete whose index i of a control is linspace(low, high, n)[i]
   * ``observation``                                           uint8 [80, 160, 3] camera frame (served from a recorded dataset)
   * ``vehicle.control.steer / .throttle``, ``vehicle.get_speed()``, ``vehicle.get_forward_vector()``
   * ``reset(is_training=True) -> state``, ``step(action) -> (state, reward, terminal, info)`` with ``info["closed"]``
@@ -35,6 +36,33 @@ class Box:
         return rng.uniform(self.low, self.high).astype(np.float32)
 
 
+class Discrete:
+    """gym.spaces.Discrete(n): the ``.n`` the PPO class reads."""
+
+    def __init__(self, n):
+        self.n = int(n)
+        self.shape = ()
+
+    def sample(self, rng=np.random):
+        return int(rng.randint(self.n))
+
+
+class MultiDiscrete:
+    """gym.spaces.MultiDiscrete(nvec): the ``.nvec`` the PPO class reads."""
+
+    def __init__(self, nvec):
+        self.nvec = np.asarray(nvec, np.int64).reshape(-1)
+        self.shape = self.nvec.shape
+
+    def sample(self, rng=np.random):
+        return np.array([rng.randint(n) for n in self.nvec], np.int64)
+
+
+def discrete_controls(nvec, low=(-1.0, 0.0), high=(1.0, 1.0)):
+    """Index -> control tables of a discretised (steer, throttle): component k's index i is linspace(low_k, high_k, n_k)[i]."""
+    return [np.linspace(lo, hi, int(n)) for n, lo, hi in zip(nvec, low, high)]
+
+
 class _Vehicle:
     def __init__(self):
         self.control = types.SimpleNamespace(steer=0.0, throttle=0.0)
@@ -62,13 +90,19 @@ reward_functions = {"reward_speed_centering_angle_multiply": reward_speed_center
 
 
 class ReplayEnv:
+    action_space_box_low, action_space_box_high = (-1.0, 0.0), (1.0, 1.0)     # steer, throttle
     def __init__(self, frames, obs_res=(160, 80), action_smoothing=0.0, encode_state_fn=None, reward_fn=None,
-                 synchronous=True, fps=30, start_carla=False, episode_length=256, seed=0):
+                 synchronous=True, fps=30, start_carla=False, episode_length=256, seed=0, discrete_actions=None):
         frames = np.asarray(frames)
         if frames.dtype != np.uint8 or frames.ndim != 4 or tuple(frames.shape[1:]) != (obs_res[1], obs_res[0], 3):
             raise ValueError("frames must be uint8 [N, %d, %d, 3]" % (obs_res[1], obs_res[0]))
         self.frames = frames
-        self.action_space = Box([-1.0, 0.0], [1.0, 1.0])
+        self.action_space = Box(self.action_space_box_low, self.action_space_box_high)
+        # discrete_actions = (n_steer, n_throttle): the agent picks one of n_k evenly spaced values of each control
+        self._controls = None
+        if discrete_actions is not None:
+            self.action_space = MultiDiscrete(discrete_actions)
+            self._controls = discrete_controls(self.action_space.nvec, self.action_space_box_low, self.action_space_box_high)
         self.action_smoothing = float(action_smoothing)
         self.encode_state_fn = encode_state_fn if encode_state_fn is not None else (lambda env: env.observation)
         self.reward_fn = reward_fn if reward_fn is not None else reward_speed_centering
@@ -109,7 +143,10 @@ class ReplayEnv:
 
     def step(self, action):
         if action is not None:
-            steer, throttle = [float(a) for a in np.asarray(action, np.float64).reshape(-1)[:2]]
+            if self._controls is not None:
+                steer, throttle = [float(t[int(i)]) for t, i in zip(self._controls, np.asarray(action).reshape(-1)[:2])]
+            else:
+                steer, throttle = [float(a) for a in np.asarray(action, np.float64).reshape(-1)[:2]]
             c = self.vehicle.control
             c.steer = c.steer * self.action_smoothing + steer * (1.0 - self.action_smoothing)
             c.throttle = c.throttle * self.action_smoothing + throttle * (1.0 - self.action_smoothing)

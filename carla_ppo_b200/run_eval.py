@@ -10,10 +10,15 @@ import numpy as np
 
 def load_model(input_shape, action_space, model_dir):
     """The PPO of model_dir, built at its latest checkpoint's architecture (the reference's 500, 300 when there is none)
-    and restored from it (``load_latest_checkpoint``'s result is printed, as in the reference)."""
+    and action space (a MultiDiscrete of its recorded categories for a categorical agent, else ``action_space``), and
+    restored from it (``load_latest_checkpoint``'s result is printed, as in the reference)."""
     from ._lib import PPO_DEFAULT_HIDDEN
-    from .ppo import PPO, checkpoint_architecture
+    from .ppo import PPO, checkpoint_action_categories, checkpoint_architecture
+    from .replay_env import MultiDiscrete
     arch = checkpoint_architecture("{}/checkpoints/".format(model_dir)) or (PPO_DEFAULT_HIDDEN, PPO_DEFAULT_HIDDEN)
+    cats = checkpoint_action_categories("{}/checkpoints/".format(model_dir))
+    if cats:
+        action_space = MultiDiscrete(cats)
     model = PPO(input_shape, action_space, model_dir=model_dir, seed=0, policy_hidden_sizes=arch[0],
                 value_hidden_sizes=arch[1])
     model.init_session(init_logging=False)
@@ -90,6 +95,11 @@ def main(argv=None):
     env.seed(0)
     input_shape = np.array([vae.z_dim + len(measurements_to_include)])
     model = load_model(input_shape, env.action_space, os.path.join(args.models_root, args.model_name))
+    if model.action_categories is not None:          # drive the environment with the checkpoint's discrete controls
+        env = ReplayEnv(env.frames, obs_res=obs_res, action_smoothing=args.action_smoothing,
+                        encode_state_fn=env.encode_state_fn, reward_fn=env.reward_fn, synchronous=args.synchronous,
+                        fps=args.fps, start_carla=False, discrete_actions=model.action_categories)
+        env.seed(0)
     actor = None
     if not args.unfused:
         actor = FusedActor(vae, model, measurements_to_include)

@@ -13,6 +13,8 @@ hyper-parameter flags and TensorBoard tags, with the neural work on the H100 lib
                              per environment (PPO.learn(segment_lengths=...)); N = 1 is the reference's loop
   * ``--max_grad_norm`` / ``--target_kl``: bound each update (global gradient-norm clipping, approximate-KL early
                              stopping) on the device, in both the learn and the --reference_loop path; off by default
+  * ``--discrete_actions N_STEER N_THROTTLE``: a categorical policy over N_STEER x N_THROTTLE evenly spaced controls
+                             (a MultiDiscrete action space) instead of the reference's Gaussian over the Box; off by default
 """
 from __future__ import annotations
 
@@ -23,7 +25,7 @@ import shutil
 import numpy as np
 
 from ._lib import PPO_DEFAULT_HIDDEN
-from .ppo import PPO, checkpoint_architecture
+from .ppo import PPO, action_categories, checkpoint_action_categories, checkpoint_architecture
 from .replay_env import ReplayEnv, reward_functions
 from .run_eval import run_eval
 from .utils import compute_gae
@@ -60,6 +62,21 @@ def resolve_architecture(policy_sizes, value_sizes, checkpoint_arch):
     return tuple(tuple(c) for c in checkpoint_arch)
 
 
+def resolve_action_categories(flag, checkpoint_cats):
+    """The discrete action categories of a run (None: the reference's Box): the checkpoint's when resuming one (a given
+    --discrete_actions must equal it, and a Gaussian checkpoint takes none), else the flag.  Raises ValueError on a
+    disagreement."""
+    given = None if flag is None else tuple(int(v) for v in flag)
+    if checkpoint_cats is None:
+        return given
+    ckpt = tuple(checkpoint_cats) or None
+    if given is not None and given != ckpt:
+        raise ValueError("--discrete_actions %s disagrees with the checkpoint being resumed, which has %s (pass -restart to "
+                         "start over)" % (" ".join(map(str, given)),
+                                          "categories " + " ".join(map(str, ckpt)) if ckpt else "a Gaussian policy"))
+    return ckpt
+
+
 def train(params, start_carla=False, restart=False, env=None, vae=None, models_root="models", interactive=True):
     """reference train.py:23-216.  ``env`` / ``vae`` may be passed in (tests); otherwise a ReplayEnv over
     ``params["replay_data"]`` and ``load_vae(params["vae_model"], ...)`` are created.  Returns the PPO model."""
@@ -91,26 +108,6 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     print("")
 
     measurements_to_include = set(["steer", "throttle", "speed"])
-    num_envs = int(params.get("num_envs", 1))
-    if num_envs < 1:
-        raise ValueError("num_envs must be >= 1")
-    if env is None:
-        print("Creating environment")
-        frames = load_replay_frames(params.get("replay_data", "vae/data"))
-        obs_res = (vae.source_shape[1], vae.source_shape[0])          # (width, height) of the frames the VAE takes
-        envs = [ReplayEnv(frames, obs_res=obs_res, action_smoothing=params["action_smoothing"], encode_state_fn=None,
-                          reward_fn=reward_functions[params["reward_fn"]], synchronous=params["synchronous"], fps=params["fps"],
-                          start_carla=False, episode_length=params.get("episode_length", 256)) for _ in range(num_envs)]
-    else:
-        envs = list(env) if isinstance(env, (list, tuple)) else [env]
-        if len(envs) != num_envs:
-            raise ValueError("num_envs = %d but %d environments were given" % (num_envs, len(envs)))
-    if isinstance(seed, int):
-        for i, e in enumerate(envs):
-            e.seed(seed + i)
-    best_eval_reward = -float("inf")
-
-    input_shape = np.array([vae.z_dim + len(measurements_to_include)])
     model_dir = os.path.join(models_root, model_name)
     log_dir = "{}/logs/".format(model_dir)
     if not restart and interactive:
@@ -120,6 +117,34 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
                 restart = True
             elif answer.upper() != "C":
                 raise Exception("There are already log files for model \"{}\". Please delete it or change model_name and try again".format(model_name))
+    # a resumed run takes its checkpoint's action space; a --discrete_actions that disagrees with it is an error
+    categories = resolve_action_categories(params.get("discrete_actions"),
+                                           None if restart else checkpoint_action_categories("{}/checkpoints/".format(model_dir)))
+    params["discrete_actions"] = list(categories) if categories else None
+    num_envs = int(params.get("num_envs", 1))
+    if num_envs < 1:
+        raise ValueError("num_envs must be >= 1")
+    if env is None:
+        print("Creating environment")
+        frames = load_replay_frames(params.get("replay_data", "vae/data"))
+        obs_res = (vae.source_shape[1], vae.source_shape[0])          # (width, height) of the frames the VAE takes
+        envs = [ReplayEnv(frames, obs_res=obs_res, action_smoothing=params["action_smoothing"], encode_state_fn=None,
+                          reward_fn=reward_functions[params["reward_fn"]], synchronous=params["synchronous"], fps=params["fps"],
+                          start_carla=False, episode_length=params.get("episode_length", 256), discrete_actions=categories)
+                for _ in range(num_envs)]
+    else:
+        envs = list(env) if isinstance(env, (list, tuple)) else [env]
+        if len(envs) != num_envs:
+            raise ValueError("num_envs = %d but %d environments were given" % (num_envs, len(envs)))
+    if action_categories(envs[0].action_space) != categories:
+        raise ValueError("the environments' action space %r is not the run's (%s)"
+                         % (action_categories(envs[0].action_space), "categories %r" % (categories,) if categories else "a Box"))
+    if isinstance(seed, int):
+        for i, e in enumerate(envs):
+            e.seed(seed + i)
+    best_eval_reward = -float("inf")
+
+    input_shape = np.array([vae.z_dim + len(measurements_to_include)])
     # a resumed run takes its checkpoint's architecture; a size flag that disagrees with it is an error
     policy_sizes, value_sizes = resolve_architecture(params.get("policy_hidden_sizes"), params.get("value_hidden_sizes"),
                                                      None if restart else checkpoint_architecture("{}/checkpoints/".format(model_dir)))
@@ -308,6 +333,10 @@ def main(argv=None):
                         "gradient to this value (default: off, like the reference)")
     parser.add_argument("--target_kl", type=float, default=None, help="stop an update once the approximate KL between the "
                         "new and the old policy exceeds 1.5 x this value (default: off, like the reference)")
+    parser.add_argument("--discrete_actions", type=int, nargs=2, default=None, metavar=("N_STEER", "N_THROTTLE"),
+                        help="a categorical policy over N_STEER evenly spaced steering values in [-1, 1] times N_THROTTLE "
+                        "throttle values in [0, 1] (default: the reference's continuous Box, or the checkpoint's when "
+                        "resuming)")
     parser.add_argument("--policy_hidden_sizes", type=int, nargs="+", default=None, metavar="WIDTH",
                         help="hidden-layer widths of the policy network, 1 to 8 of them (default: 500 300, or the "
                         "checkpoint's when resuming)")

@@ -131,7 +131,8 @@ class VAE:
     # C entry points of the architecture (ConvVAE: cpb_vae_spec_*, MlpVAE: cpb_mlpvae_spec_*; identical argument lists)
     _API = {"num_tensors": "cpb_vae_num_tensors", "tensor_name": "cpb_vae_tensor_name", "encode": "cpb_vae_spec_encode",
             "decode": "cpb_vae_spec_decode", "forward": "cpb_vae_spec_forward", "loss_grad": "cpb_vae_spec_loss_grad",
-            "encode_predict": "cpb_vae_spec_ppo_spec_encode_predict"}
+            "encode_predict": "cpb_vae_spec_ppo_spec_encode_predict",
+            "encode_predict_cat": "cpb_vae_spec_ppo_cat_encode_predict"}
     _HOST_STEP = True        # cpb_vae_train_step_host exists for this architecture
 
     def __init__(self, source_shape, target_shape, build_encoder_fn=None, build_decoder_fn=None,
@@ -847,7 +848,8 @@ class MlpVAE(VAE):
     workspace is re-sized on every call, so switching the mode between calls is safe."""
 
     _API = {"encode": "cpb_mlpvae_spec_encode", "decode": "cpb_mlpvae_spec_decode", "forward": "cpb_mlpvae_spec_forward",
-            "loss_grad": "cpb_mlpvae_spec_loss_grad", "encode_predict": "cpb_mlpvae_ppo_spec_encode_predict"}
+            "loss_grad": "cpb_mlpvae_spec_loss_grad", "encode_predict": "cpb_mlpvae_ppo_spec_encode_predict",
+            "encode_predict_cat": "cpb_mlpvae_ppo_cat_encode_predict"}
     _HOST_STEP = False
 
     def __init__(self, source_shape, target_shape=None, encoder_sizes=(512, 256), decoder_sizes=(256, 512), **kwargs):

@@ -583,6 +583,106 @@ int32_t cpb_mlpvae_ppo_spec_encode_predict(const cpb_mlpvae_spec* spec, const fl
                                            int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
                                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Categorical policies: discrete action spaces (Stable-Baselines3's Discrete(n) / MultiDiscrete(nvec)), an addition
+ * over the reference, whose policy is always the tanh-squashed Gaussian (ppo.py:38-66).
+ *
+ * K = spec.base.num_actions components (1..4); component k has n_k = num_categories[k] categories (2..64), and
+ * N = sum n_k <= 64.  spec.base.action_low / action_high must be all 0.  The head computes logits
+ * z = h_P W + b (W = action_logits/kernel [H_P, N], b = action_logits/bias [N], columns grouped by component in order),
+ * p_k = softmax(z_k) with the max subtracted, log p = z - m - log sum exp(z - m), and per row
+ *   logp(a) = sum_k log p_k[a_k],   H = sum_k -sum_i p_ki log p_ki.
+ * loss = -policy_loss + value_loss - entropy_scale * mean_b H (policy and value terms, clip and tie rule as above);
+ * metrics keep their columns, entropy_loss = entropy_scale * mean H, and the guarded rows add approx_kl and the pre-clip
+ * norm as above.
+ * Variables, in TF creation order, 2P + 2V + 4 of them (no action_logstd):
+ *   dense .. dense_{P-1}, action_logits/kernel, action_logits/bias, dense_P .. dense_{P+V-1}, value/kernel, value/bias.
+ * Actions: the `actions` [T, K] buffers hold the taken indices as integer-valued floats; an index outside [0, n_k) is
+ * clamped into it.  forward writes action [B, K] the same way: greedy (noise == NULL) the first largest logit of each
+ * component; sampled, noise [B, K] uniforms in [0, 1) and the smallest i with u < cumsum_i p_k (fp32, index order), or the
+ * last index with p > 0 when rounding leaves u above the last partial sum.
+ * Each cpb_ppo_cat_* entry point is the cpb_ppo_spec_* entry point of the same name with the categorical head: the same
+ * arguments after the spec, the same launches.  A bad spec (NULL, anything cpb_ppo_spec refuses, an n_k outside [2, 64],
+ * N > 64, a nonzero action_low / action_high) is refused with CPB_ERR_INVALID_ARGUMENT before anything is enqueued.
+ * ---------------------------------------------------------------------------------------- */
+#define CPB_PPO_MAX_LOGITS 64
+typedef struct {
+    cpb_ppo_spec spec;            /* the trunks and hyper-parameters; spec.base.num_actions = K */
+    int32_t num_categories[4];    /* n_k, the first K are used */
+} cpb_ppo_cat_spec;
+
+int32_t     cpb_ppo_cat_num_tensors(const cpb_ppo_cat_spec* spec);                 /* 2P + 2V + 4 */
+const char* cpb_ppo_cat_tensor_name(const cpb_ppo_cat_spec* spec, int32_t index);  /* NULL for a bad spec or index */
+int32_t cpb_ppo_cat_layout(const cpb_ppo_cat_spec* spec, int64_t* offsets, int64_t* sizes, int32_t* shapes,
+                           int64_t* total_floats);
+int64_t cpb_ppo_cat_workspace_bytes(const cpb_ppo_cat_spec* spec, int32_t max_batch, int32_t horizon);
+/* PPO.predict over a discrete space: action [B,K] (indices as floats), value [B]; noise [B,K] uniforms or NULL (greedy) */
+int32_t cpb_ppo_cat_forward(const cpb_ppo_cat_spec* spec, const float* params, const float* states, int32_t batch,
+                            const float* noise, float* action, float* value, void* workspace, int64_t workspace_bytes,
+                            void* stream);
+/* cpb_ppo_spec_loss_grad / train_step / train_step_opts with the categorical head */
+int32_t cpb_ppo_cat_loss_grad(const cpb_ppo_cat_spec* spec, const float* params, const float* params_old,
+                              const float* states, const float* actions, const float* returns,
+                              const float* advantages, const int32_t* idx, int32_t batch, float* grads,
+                              float* metrics, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_cat_train_step(const cpb_ppo_cat_spec* spec, float* params, const float* params_old, float* grads,
+                               float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                               const float* states, const float* actions, const float* returns,
+                               const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                               void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_cat_train_step_opts(const cpb_ppo_cat_spec* spec, float* params, const float* params_old, float* grads,
+                                    float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                    const float* states, const float* actions, const float* returns,
+                                    const float* advantages, const int32_t* idx, int32_t batch, float* metrics,
+                                    const cpb_ppo_learn_options* opts, uint32_t* stop, int32_t* steps_applied,
+                                    void* workspace, int64_t workspace_bytes, void* stream);
+/* cpb_ppo_spec_learn / learn_opts / learn_segments / learn_segments_opts with the categorical head (launch-per-kernel,
+ * or the persistent kernel under CPB_PPO_PERSISTENT=1) */
+int32_t cpb_ppo_cat_learn(const cpb_ppo_cat_spec* spec, float* params, float* params_old, float* grads, float* adam_m,
+                          float* adam_v, float* adam_powers, const float* lr_dev, const float* states,
+                          const float* actions, const double* rewards, const double* values, double bootstrap_value,
+                          const double* dones, int32_t T, double gamma, double lam, int32_t num_epochs,
+                          int32_t batch_size, const int32_t* perms, float* metrics, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_cat_learn_opts(const cpb_ppo_cat_spec* spec, float* params, float* params_old, float* grads,
+                               float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                               const float* states, const float* actions, const double* rewards,
+                               const double* values, double bootstrap_value, const double* dones, int32_t T,
+                               double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                               const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                               int32_t* steps_applied, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_cat_learn_segments(const cpb_ppo_cat_spec* spec, float* params, float* params_old, float* grads,
+                                   float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                   const float* states, const float* actions, const double* rewards,
+                                   const double* values, const double* bootstrap_values, const double* dones,
+                                   const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                                   double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                   const int32_t* perms, float* metrics, void* workspace,
+                                   int64_t workspace_bytes, void* stream);
+int32_t cpb_ppo_cat_learn_segments_opts(const cpb_ppo_cat_spec* spec, float* params, float* params_old, float* grads,
+                                        float* adam_m, float* adam_v, float* adam_powers, const float* lr_dev,
+                                        const float* states, const float* actions, const double* rewards,
+                                        const double* values, const double* bootstrap_values, const double* dones,
+                                        const int32_t* segment_offsets, int32_t num_segments, int32_t rows,
+                                        double gamma, double lam, int32_t num_epochs, int32_t batch_size,
+                                        const int32_t* perms, float* metrics, const cpb_ppo_learn_options* opts,
+                                        int32_t* steps_applied, void* workspace, int64_t workspace_bytes,
+                                        void* stream);
+/* cpb_vae_spec_ppo_spec_encode_predict / cpb_mlpvae_ppo_spec_encode_predict with a categorical PPO: action [B,K] holds
+ * the indices as floats, noise [B,K] uniforms (NULL: greedy). */
+int32_t cpb_vae_spec_ppo_cat_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                            const float* measurements, int32_t num_measurements,
+                                            const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params, const float* noise,
+                                            float* latent_tmp, float* state, float* action, float* value,
+                                            int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+                                            void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
+int32_t cpb_mlpvae_ppo_cat_encode_predict(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                          const float* measurements, int32_t num_measurements,
+                                          const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params, const float* noise,
+                                          float* latent_tmp, float* state, float* action, float* value,
+                                          int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+                                          void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
