@@ -39,7 +39,7 @@ def learn_times(calls):
     from helpers import Box
     from carla_ppo_b200.ppo import PPO
     from bench import ppo_config3_inputs, shipped_agent
-    from ppo_depth_oracle import init_params
+    from ppo_restatement import init_params
     pol, old, am, av, pw = shipped_agent()
     s, a, r, v, d, perms = ppo_config3_inputs()
     models = {}
@@ -50,7 +50,7 @@ def learn_times(calls):
         if ps == (500, 300) and vs == (500, 300):
             m.set_weights(pol, old, am, av, pw)
         else:
-            w = init_params(67, 2, ps, vs, seed=1)
+            w = init_params(67, (np.array([-1.0, 0.0]), np.array([1.0, 1.0])), ps, vs, seed=1)
             m.set_weights(w, w)
         if "legacy" in name:
             _legacy(m)

@@ -25,14 +25,13 @@ def child(reps):
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import numpy as np
     import torch
-    import ppo_options_cases as oc
-    from ppo_cases import baseline_config3
+    import ppo_cases as oc
     dev = torch.device("cuda")
     tmp = Path(tempfile.mkdtemp())
     out = {}
     for wname, lengths in WORKLOADS.items():
         if lengths is None:
-            s, a, r, v, d, perms = baseline_config3(oc.T, oc.E)
+            s, a, r, v, d, perms = oc.baseline_config3(oc.T3, oc.E3)
             last = 0.3
         else:
             s, a, r, v, d, last, perms = oc.segment_rollout(lengths)
@@ -40,21 +39,21 @@ def child(reps):
         args = (on(s, torch.float32), on(a, torch.float32), on(v, torch.float64), on(r, torch.float64),
                 on(np.asarray(d, np.float64), torch.float64), last)
         p = on(perms, torch.int32)
-        models = {k: oc.model(tmp / wname / k) for k in VARIANTS}
+        models = {k: oc.shipped_model(tmp / wname / k) for k in VARIANTS}
         for k, m in models.items():          # warm-up: workspace, modules, the first launches
-            m.learn(*args, num_epochs=oc.E, batch_size=oc.B, perms=p, segment_lengths=lengths, **VARIANTS[k])
+            m.learn(*args, num_epochs=oc.E3, batch_size=oc.B3, perms=p, segment_lengths=lengths, **VARIANTS[k])
         times = {k: [] for k in VARIANTS}
         for _ in range(reps):
             for k, m in models.items():
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 torch.cuda.synchronize()
                 e0.record()
-                m.learn(*args, num_epochs=oc.E, batch_size=oc.B, perms=p, segment_lengths=lengths, **VARIANTS[k])
+                m.learn(*args, num_epochs=oc.E3, batch_size=oc.B3, perms=p, segment_lengths=lengths, **VARIANTS[k])
                 e1.record()
                 torch.cuda.synchronize()
                 times[k].append(e0.elapsed_time(e1))
         for k in VARIANTS:
-            applied = int(models[k].last_steps_applied.item()) if VARIANTS[k] else oc.E * (oc.T // oc.B)
+            applied = int(models[k].last_steps_applied.item()) if VARIANTS[k] else oc.E3 * (oc.T3 // oc.B3)
             t = np.asarray(times[k])
             out["%s/%s" % (wname, k)] = dict(median_ms=float(np.median(t)), min_ms=float(t.min()), max_ms=float(t.max()),
                                              steps_applied=applied)

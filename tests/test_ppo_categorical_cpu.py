@@ -1,4 +1,4 @@
-"""Categorical PPO heads without a GPU: the float64 restatement tests/ppo_categorical_oracle.py against torch autograd,
+"""Categorical PPO heads without a GPU: the float64 restatement tests/ppo_restatement.py against torch autograd,
 the cpb_ppo_cat_* layout and names, the refusal of every bad cpb_ppo_cat_spec by every twin before any launch, the
 action-space duck typing, the replay environment's index -> control mapping and the checkpoint record."""
 import ctypes as C
@@ -6,50 +6,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import ppo_categorical_oracle as pco
+import ppo_restatement as pr
 from harness import lib  # noqa: F401
+from ppo_checks import SPEC_ENTRIES, ppo_call, torch_loss_and_grads
 
 S = 67
-
-
-def _torch_loss(p, old, s, a, ret, adv, cats, epsilon=0.2, value_scale=1.0, entropy_scale=0.01):
-    """The loss of the spec in torch float64 (autograd for the gradients)."""
-    import torch
-    t = {k: torch.tensor(np.asarray(v, np.float64), requires_grad=True) for k, v in p.items()}
-    o = {k: torch.tensor(np.asarray(v, np.float64)) for k, v in old.items()}
-    st = torch.tensor(np.asarray(s, np.float64))
-    pol, val = pco.trunk_names(p)
-
-    def logits(q):
-        h = st
-        for w, b in pol:
-            h = torch.relu(h @ q[w] + q[b])
-        return h @ q["action_logits/kernel"] + q["action_logits/bias"]
-    off = pco.offsets(cats)
-    ai = torch.tensor(np.asarray(a).astype(np.int64))
-
-    def logp_and_h(z):
-        lp, H = 0.0, 0.0
-        for k in range(len(cats)):
-            l = torch.log_softmax(z[:, off[k]:off[k + 1]], dim=1)
-            lp = lp + l.gather(1, ai[:, k:k + 1])[:, 0]
-            H = H - (l.exp() * l).sum(dim=1)
-        return lp, H
-    lp, H = logp_and_h(logits(t))
-    lp_old, _ = logp_and_h(logits(o))
-    g = st
-    for w, b in val:
-        g = torch.relu(g @ t[w] + t[b])
-    v = (g @ t["value/kernel"] + t["value/bias"])[:, 0]
-    ratio = torch.exp(lp - lp_old)
-    advt = torch.tensor(np.asarray(adv, np.float64))
-    lo, hi = float(np.float32(1 - epsilon)), float(np.float32(1 + epsilon))
-    pl = torch.minimum(ratio * advt, torch.clamp(ratio, lo, hi) * advt).mean()
-    vl = ((v - torch.tensor(np.asarray(ret, np.float64))) ** 2).mean() * float(np.float32(value_scale))
-    el = H.mean() * float(np.float32(entropy_scale))
-    loss = -pl + vl - el
-    loss.backward()
-    return float(loss.detach()), {k: x.grad.numpy() for k, x in t.items()}
 
 
 @pytest.mark.parametrize("arch", [((1,), (1,)), ((3, 2), (1,))])
@@ -58,7 +19,7 @@ def _torch_loss(p, old, s, a, ret, adv, cats, epsilon=0.2, value_scale=1.0, entr
 def test_restatement_matches_autograd(arch, nvec, case):
     rs = np.random.RandomState(len(nvec) + 7 * sum(nvec))
     B = 12
-    p = {k: v.astype(np.float64) for k, v in pco.init_params(5, nvec, arch[0], arch[1], seed=3).items()}
+    p = {k: v.astype(np.float64) for k, v in pr.init_params(5, nvec, arch[0], arch[1], seed=3).items()}
     for k in p:
         p[k] = p[k] + 0.3 * rs.randn(*p[k].shape)          # nonzero biases, logits far from uniform
     old = {k: v + 0.2 * rs.randn(*v.shape) for k, v in p.items()}
@@ -70,8 +31,8 @@ def test_restatement_matches_autograd(arch, nvec, case):
         adv = np.zeros(B)
     elif case == "policy_only":
         es = 0.0
-    r = pco.loss_and_grads(p, old, s, a, ret, adv, nvec, 0.2, 1.0, es)
-    loss, grads = _torch_loss(p, old, s, a, ret, adv, nvec, 0.2, 1.0, es)
+    r = pr.loss_and_grads(p, old, s, a, ret, adv, nvec, 0.2, 1.0, es)
+    loss, grads = torch_loss_and_grads(p, old, s, a, ret, adv, nvec, 0.2, 1.0, es)
     assert abs(r["loss"] - loss) <= 1e-10 * max(1.0, abs(loss))
     for k, g in grads.items():
         assert np.abs(r["grads"][k] - g).max() <= 1e-10 * max(1.0, np.abs(g).max()), k
@@ -89,7 +50,7 @@ def _spec(cats, pol=(500, 300), val=(500, 300), state_dim=S):
 def test_layout_and_names_equal_the_restatement(lib, cats, arch):
     sp = _spec(cats, *arch)
     n = lib.cpb_ppo_cat_num_tensors(C.byref(sp))
-    shapes_ref = pco.param_shapes(S, cats, *arch)
+    shapes_ref = pr.param_shapes(S, cats, *arch)
     assert n == len(shapes_ref) == 2 * (len(arch[0]) + len(arch[1])) + 4
     offs = (C.c_int64 * n)(); sizes = (C.c_int64 * n)(); shapes = (C.c_int32 * (2 * n))(); total = C.c_int64()
     assert lib.cpb_ppo_cat_layout(C.byref(sp), offs, sizes, shapes, C.byref(total)) == 0
@@ -125,40 +86,11 @@ def _bad_specs():
 
 @pytest.mark.parametrize("bad", list(_bad_specs()))
 def test_every_twin_refuses_a_bad_spec_before_any_launch(lib, bad):
-    from carla_ppo_b200 import _lib
     sp = _bad_specs()[bad]
     ref = None if sp is None else C.byref(sp)
-    F = C.c_void_p(16)         # never dereferenced: the spec is refused first
-    ws, n = C.c_void_p(16), 1 << 30
-    vs = _lib.VaeSpec(_lib.VaeConfig(4, 3, 64, 1, 1, 0, 1.0, 1.0, 0.0, 1.0), 80, 160)
-    ms = _lib.MlpVaeSpec.of(_lib.VaeConfig(4, 3, 64, 1, 1, 0, 1.0, 1.0, 0.0, 1.0), (512, 256), (256, 512))
-    opts = _lib.PpoLearnOptions(0.0, 0.0)
-    calls = {
-        "num_tensors": lambda: lib.cpb_ppo_cat_num_tensors(ref),
-        "layout": lambda: lib.cpb_ppo_cat_layout(ref, None, None, None, None),
-        "workspace_bytes": lambda: lib.cpb_ppo_cat_workspace_bytes(ref, 4, 0),
-        "forward": lambda: lib.cpb_ppo_cat_forward(ref, F, F, 4, None, F, F, ws, n, None),
-        "loss_grad": lambda: lib.cpb_ppo_cat_loss_grad(ref, F, F, F, F, F, F, None, 4, F, F, ws, n, None),
-        "train_step": lambda: lib.cpb_ppo_cat_train_step(ref, F, F, F, F, F, F, F, F, F, F, F, None, 4, F, ws, n, None),
-        "train_step_opts": lambda: lib.cpb_ppo_cat_train_step_opts(ref, F, F, F, F, F, F, F, F, F, F, F, None, 4, F,
-                                                                   C.byref(opts), None, None, ws, n, None),
-        "learn": lambda: lib.cpb_ppo_cat_learn(ref, F, F, F, F, F, F, F, F, F, F, F, 0.0, F, 8, 0.99, 0.95, 1, 4, F, F,
-                                               ws, n, None),
-        "learn_opts": lambda: lib.cpb_ppo_cat_learn_opts(ref, F, F, F, F, F, F, F, F, F, F, F, 0.0, F, 8, 0.99, 0.95, 1,
-                                                         4, F, F, C.byref(opts), None, ws, n, None),
-        "learn_segments": lambda: lib.cpb_ppo_cat_learn_segments(ref, F, F, F, F, F, F, F, F, F, F, F, F, F, F, 1, 8,
-                                                                 0.99, 0.95, 1, 4, F, F, ws, n, None),
-        "learn_segments_opts": lambda: lib.cpb_ppo_cat_learn_segments_opts(ref, F, F, F, F, F, F, F, F, F, F, F, F, F, F,
-                                                                           1, 8, 0.99, 0.95, 1, 4, F, F, C.byref(opts),
-                                                                           None, ws, n, None),
-        "vae_actor": lambda: lib.cpb_vae_spec_ppo_cat_encode_predict(C.byref(vs), F, F, F, 3, ref, F, None, F, F, F, F,
-                                                                     None, ws, n, ws, n, None),
-        "mlp_actor": lambda: lib.cpb_mlpvae_ppo_cat_encode_predict(C.byref(ms), F, F, F, 3, ref, F, None, F, F, F, F,
-                                                                   None, ws, n, ws, n, None),
-    }
     lib.cpb_reset_launch_count()
-    for name, call in calls.items():
-        assert call() == -1, name
+    for entry in SPEC_ENTRIES:
+        assert ppo_call(lib, "cpb_ppo_cat_", entry, ref) == -1, entry
     assert lib.cpb_ppo_cat_tensor_name(ref, 0) is None
     assert lib.cpb_launch_count() == 0
 
@@ -196,7 +128,7 @@ def test_checkpoint_record(tmp_path):
     from carla_ppo_b200.ppo import (CATEGORIES_KEY, blob_action_categories, blob_architecture,
                                     checkpoint_action_categories)
     from carla_ppo_b200.train import resolve_action_categories
-    p = pco.init_params(S, (7, 3), (64,), (32,), seed=0)
+    p = pr.init_params(S, (7, 3), (64,), (32,), seed=0)
     blob = {"policy/" + k: v for k, v in p.items()}
     blob[CATEGORIES_KEY] = np.array([7, 3], np.int32)
     assert blob_action_categories(blob) == (7, 3)

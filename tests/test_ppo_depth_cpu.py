@@ -1,4 +1,4 @@
-"""PPO policy / value trunks of any depth without a GPU: the float64 restatement (tests/ppo_depth_oracle.py) against
+"""PPO policy / value trunks of any depth without a GPU: the float64 restatement (tests/ppo_restatement.py) against
 oracle/ppo_oracle.py bit for bit at two layers per trunk and against torch autograd elsewhere; cpb_ppo_spec layouts,
 names and workspace sizes; the refusals of a bad spec; the checkpoint architecture reader and the train.py flags."""
 import ctypes as C
@@ -6,10 +6,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import ppo_depth_oracle as pdo
+import ppo_restatement as pr
 from harness import lib, library_state  # noqa: F401
 from oracle import ppo_oracle as po
 from ppo_cases import bounds
+from ppo_checks import ppo_call, SPEC_ENTRIES, torch_loss_and_grads
 
 ARCHS = [((1,), (1,)), ((3, 2), (1,)), ((7,), (4, 4, 4)), ((64,), (64,)), ((256, 256), (256, 256, 256)),
          ((33, 7, 65), (31,)), ((64,) * 8, (32,) * 8), ((2048,), (1024, 1024)), ((500, 300), (500, 300))]
@@ -30,18 +31,18 @@ def _perturbed(p, seed, scale=0.05):
 
 def test_oracle_equals_ppo_oracle_bit_for_bit_at_two_layers():
     S, A, H = 20, 2, (12, 9)
-    p = {k: v.astype(np.float64) for k, v in pdo.init_params(S, A, H, H, seed=1).items()}
+    p = {k: v.astype(np.float64) for k, v in pr.init_params(S, bounds(A), H, H, seed=1).items()}
     p = _perturbed(p, 2)
     old = _perturbed(p, 3, 0.02)
     s, a, ret, adv, low, high = _batch(S, A, 37, 4)
-    mine = pdo.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
+    mine = pr.loss_and_grads(p, old, s, a, ret, adv, (low, high), 0.2, 1.0, 0.01)
     ref = po.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
     for k in ("policy_loss", "value_loss", "entropy_loss", "loss", "mean_ratio"):
         assert mine[k] == ref[k], k
     assert set(mine["grads"]) == set(ref["grads"]) == set(po.PPO_TENSORS)
     for k in po.PPO_TENSORS:
         assert np.array_equal(mine["grads"][k], ref["grads"][k]), k
-    assert all(np.array_equal(x, y) for x, y in zip(pdo.forward(p, s, low, high), po.forward(p, s, low, high)))
+    assert all(np.array_equal(x, y) for x, y in zip(pr.forward(p, s, (low, high)), po.forward(p, s, low, high)))
     # learn: Adam over 2 epochs x 3 minibatches, records and parameters
     from oracle.vae_oracle import adam_init_state
     T = 40
@@ -52,8 +53,8 @@ def test_oracle_equals_ppo_oracle_bit_for_bit_at_two_layers():
     pa, pb = {k: v.copy() for k, v in p.items()}, {k: v.copy() for k, v in p.items()}
     sa, sb = adam_init_state(pa), adam_init_state(pb)
     rec_ref = po.learn(pa, sa, states, actions, vals, rews, dones, 0.3, low, high, num_epochs=2, batch_size=16, perms=perms)
-    rec, applied = pdo.learn(pb, sb, states, actions, vals, rews, dones, 0.3, low, high, num_epochs=2, batch_size=16,
-                             perms=perms)
+    rec, applied = pr.learn(pb, sb, states, actions, vals, rews, dones, 0.3, (low, high), num_epochs=2, batch_size=16,
+                            perms=perms)
     assert applied == len(rec_ref)
     assert np.array_equal(np.asarray(rec_ref, np.float64), rec[:, :5])
     for k in pa:
@@ -62,50 +63,23 @@ def test_oracle_equals_ppo_oracle_bit_for_bit_at_two_layers():
 
 @pytest.mark.parametrize("arch", [((1,), (1,)), ((3, 2), (1,)), ((7,), (4, 4, 4))])
 def test_oracle_matches_torch_autograd(arch):
-    torch = pytest.importorskip("torch")
+    pytest.importorskip("torch")
     pol, val = arch
     S, A = 5, 3
-    p = _perturbed({k: v.astype(np.float64) for k, v in pdo.init_params(S, A, pol, val, seed=7).items()}, 8, 0.3)
+    p = _perturbed({k: v.astype(np.float64) for k, v in pr.init_params(S, bounds(A), pol, val, seed=7).items()}, 8, 0.3)
     old = _perturbed(p, 9, 0.05)
     s, a, ret, adv, low, high = _batch(S, A, 23, 10)
-    ref = pdo.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
-
-    tp = {k: torch.tensor(v, dtype=torch.float64, requires_grad=True) for k, v in p.items()}
-
-    def net(q, x):
-        h = x
-        for w, b in pdo.trunk_names(p)[0]:
-            h = torch.relu(h @ q[w] + q[b])
-        t = torch.tanh(h @ q["action_mean/kernel"] + q["action_mean/bias"])
-        lo, hi = torch.tensor(low), torch.tensor(high)
-        mu = lo + (t + 1) / 2 * (hi - lo)
-        g = x
-        for w, b in pdo.trunk_names(p)[1]:
-            g = torch.relu(g @ q[w] + q[b])
-        return mu, (g @ q["value/kernel"] + q["value/bias"])[:, 0]
-
-    x = torch.tensor(s)
-    act = torch.tensor(a)
-    mu, v = net(tp, x)
-    with torch.no_grad():
-        mu_old, _ = net({k: torch.tensor(vv) for k, vv in old.items()}, x)
-    lp = lambda m, ls: (-0.5 * ((act - m) / torch.exp(ls)) ** 2 - (po.LOG_SQRT_2PI + ls)).sum(-1, keepdim=True)
-    ratio = torch.exp(lp(mu, tp["action_logstd"]) - lp(mu_old, torch.tensor(old["action_logstd"])))
-    advc = torch.tensor(adv)[:, None]
-    clo, chi = float(np.float32(0.8)), float(np.float32(1.2))
-    pl_ = torch.mean(torch.minimum(ratio * advc, torch.clamp(ratio, clo, chi) * advc))
-    vl_ = torch.mean((v - torch.tensor(ret)) ** 2) * float(np.float32(1.0))
-    el_ = torch.sum(po.ENTROPY_CONST + tp["action_logstd"]) * float(np.float32(0.01))
-    (-pl_ + vl_ - el_).backward()
-    assert abs(float(-pl_ + vl_ - el_) - ref["loss"]) <= 1e-10
-    for k, t in tp.items():
-        assert np.max(np.abs(t.grad.numpy() - ref["grads"][k])) <= 1e-10, k
+    ref = pr.loss_and_grads(p, old, s, a, ret, adv, (low, high), 0.2, 1.0, 0.01)
+    loss, grads = torch_loss_and_grads(p, old, s, a, ret, adv, (low, high), 0.2, 1.0, 0.01)
+    assert abs(loss - ref["loss"]) <= 1e-10
+    for k, g in grads.items():
+        assert np.max(np.abs(g - ref["grads"][k])) <= 1e-10, k
 
 
 def test_options_rule_runs_on_top_of_the_oracle():
-    """The clipping / KL rule of tests/ppo_options_oracle.py on a non-default network: a clip that binds and a stop."""
+    """The clipping / KL rule of the restatement on a non-default network: a clip that binds and a stop."""
     S, A, pol, val = 6, 2, (9, 5, 3), (4,)
-    p = _perturbed({k: v.astype(np.float64) for k, v in pdo.init_params(S, A, pol, val, seed=11).items()}, 12, 0.2)
+    p = _perturbed({k: v.astype(np.float64) for k, v in pr.init_params(S, bounds(A), pol, val, seed=11).items()}, 12, 0.2)
     rs = np.random.RandomState(13)
     T = 64
     low, high = bounds(A)
@@ -113,8 +87,8 @@ def test_options_rule_runs_on_top_of_the_oracle():
     vals, rews, dones = rs.randn(T), rs.randn(T), np.zeros(T)
     perms = [rs.permutation(T) for _ in range(3)]
     from oracle.vae_oracle import adam_init_state
-    rec, applied = pdo.learn({k: v.copy() for k, v in p.items()}, adam_init_state(p), states, actions, vals, rews, dones, 0.3, low, high,
-                             lr=3e-2, num_epochs=3, batch_size=16, perms=perms, max_grad_norm=1e-3, target_kl=1e-4)
+    rec, applied = pr.learn({k: v.copy() for k, v in p.items()}, adam_init_state(p), states, actions, vals, rews, dones, 0.3,
+                            (low, high), lr=3e-2, num_epochs=3, batch_size=16, perms=perms, max_grad_norm=1e-3, target_kl=1e-4)
     assert 1 <= applied < len(rec)
     assert np.isnan(rec[applied + 1:]).all() and np.isfinite(rec[:applied + 1]).all()
     assert (rec[:applied + 1, 6] > 1e-3).all()          # every evaluated gradient was clipped
@@ -135,7 +109,7 @@ def test_spec_layout_and_names_match_the_oracle(lib, arch):
     S, A = 67, 2
     sp = _spec(_lib, S, A, pol, val)
     n = lib.cpb_ppo_spec_num_tensors(C.byref(sp))
-    ref = pdo.param_shapes(S, A, pol, val)
+    ref = pr.param_shapes(S, bounds(A), pol, val)
     assert n == len(ref) == 2 * (len(pol) + len(val)) + 5
     names = [lib.cpb_ppo_spec_tensor_name(C.byref(sp), i).decode() for i in range(n)]
     assert names == list(ref)
@@ -150,7 +124,7 @@ def test_spec_layout_and_names_match_the_oracle(lib, arch):
         assert offs[i] % 64 == 0 and offs[i] >= end, name
         end = offs[i] + sizes[i]
     assert total.value >= end and total.value % 64 == 0
-    assert pdo.architecture(pdo.init_params(S, A, pol, val)) == (tuple(pol), tuple(val))
+    assert pr.architecture(pr.init_params(S, bounds(A), pol, val)) == (tuple(pol), tuple(val))
 
 
 @pytest.mark.parametrize("hidden", [(500, 300), (17, 5)])
@@ -172,9 +146,6 @@ def test_legacy_equals_twin_at_two_layers(lib, hidden):
         assert lib.cpb_ppo_workspace_bytes(C.byref(cfg), mb, hz) == lib.cpb_ppo_spec_workspace_bytes(C.byref(sp), mb, hz) > 0
 
 
-FAKE = 1 << 44       # never dereferenced: every call below is refused first
-
-
 def _bad_specs():
     from carla_ppo_b200 import _lib
     good = ((64, 64), (32,))
@@ -188,56 +159,19 @@ def _bad_specs():
     return out
 
 
-def _spec_calls(lib, sp):
-    s, F, ws = sp, FAKE, 1 << 40
-    return {
-        "forward": lambda: lib.cpb_ppo_spec_forward(s, F, F, 4, None, F, F, F, ws, None),
-        "loss_grad": lambda: lib.cpb_ppo_spec_loss_grad(s, F, F, F, F, F, F, None, 4, F, F, F, ws, None),
-        "train_step": lambda: lib.cpb_ppo_spec_train_step(s, F, F, F, F, F, F, F, F, F, F, F, None, 4, F, F, ws, None),
-        "train_step_opts": lambda: lib.cpb_ppo_spec_train_step_opts(s, F, F, F, F, F, F, F, F, F, F, F, None, 4, F, None,
-                                                                    None, None, F, ws, None),
-        "learn": lambda: lib.cpb_ppo_spec_learn(s, F, F, F, F, F, F, F, F, F, F, F, 0.0, F, 64, 0.99, 0.95, 1, 16, F, None,
-                                                F, ws, None),
-        "learn_opts": lambda: lib.cpb_ppo_spec_learn_opts(s, F, F, F, F, F, F, F, F, F, F, F, 0.0, F, 64, 0.99, 0.95, 1,
-                                                          16, F, None, None, None, F, ws, None),
-        "learn_segments": lambda: lib.cpb_ppo_spec_learn_segments(s, F, F, F, F, F, F, F, F, F, F, F, F, F, F, 2, 64, 0.99,
-                                                                  0.95, 1, 16, F, None, F, ws, None),
-        "learn_segments_opts": lambda: lib.cpb_ppo_spec_learn_segments_opts(s, F, F, F, F, F, F, F, F, F, F, F, F, F, F, 2,
-                                                                            64, 0.99, 0.95, 1, 16, F, None, None, None,
-                                                                            F, ws, None),
-        "layout": lambda: lib.cpb_ppo_spec_layout(s, None, None, None, None),
-        "num_tensors": lambda: lib.cpb_ppo_spec_num_tensors(s),
-        "workspace_bytes": lambda: lib.cpb_ppo_spec_workspace_bytes(s, 4, 0),
-    }
-
-
-def _actor_calls(lib, ppo_spec):
-    from carla_ppo_b200 import _lib
-    vs = _lib.VaeSpec()
-    vs.base.batch, vs.base.target_channels, vs.base.z_dim, vs.height, vs.width = 2, 3, 64, 80, 160
-    ms = _lib.MlpVaeSpec.of(vs.base, (256, 128), (128, 256))
-    F, ws = FAKE, 1 << 40
-    return {
-        "vae_actor": lambda: lib.cpb_vae_spec_ppo_spec_encode_predict(C.byref(vs), F, F, F, 3, ppo_spec, F, None, F, F, F,
-                                                                      F, None, F, ws, F, ws, None),
-        "mlp_actor": lambda: lib.cpb_mlpvae_ppo_spec_encode_predict(C.byref(ms), F, F, F, 3, ppo_spec, F, None, F, F, F, F,
-                                                                    None, F, ws, F, ws, None),
-    }
-
-
 @pytest.mark.parametrize("bad", list(_bad_specs()) + ["null"])
 def test_bad_specs_are_refused_before_any_launch(lib, bad):
     sp = None if bad == "null" else C.byref(_bad_specs()[bad])
     before = lib.cpb_launch_count()
-    for name, call in list(_spec_calls(lib, sp).items()) + list(_actor_calls(lib, sp).items()):
-        assert call() == -1, name          # CPB_ERR_INVALID_ARGUMENT
+    for entry in SPEC_ENTRIES:
+        assert ppo_call(lib, "cpb_ppo_spec_", entry, sp) == -1, entry          # CPB_ERR_INVALID_ARGUMENT
     assert lib.cpb_ppo_spec_tensor_name(sp, 0) is None
     assert lib.cpb_launch_count() == before
 
 
 def _blob(S, pol, val, record=True):
     from carla_ppo_b200.ppo import ARCH_KEYS
-    blob = {"policy/" + k: v for k, v in pdo.init_params(S, 2, pol, val).items()}
+    blob = {"policy/" + k: v for k, v in pr.init_params(S, bounds(2), pol, val).items()}
     if record:
         blob[ARCH_KEYS[0]], blob[ARCH_KEYS[1]] = np.asarray(pol, np.int32), np.asarray(val, np.int32)
     return blob

@@ -1,51 +1,38 @@
 """PPO policy / value trunks of any depth on the device (cpb_ppo_spec_*): every entry point against the float64
-restatement tests/ppo_depth_oracle.py at architectures from one unit per trunk to eight layers and 2048 wide, with the
+restatement tests/ppo_restatement.py at architectures from one unit per trunk to eight layers and 2048 wide, with the
 workspace filled with NaN before each call; the default architecture through the spec bit for bit the legacy entry
 points; the fused actor; checkpoints of a non-default architecture."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-import ppo_depth_oracle as pdo
-from harness import lib, library_state, make_conv_vae, make_mlp  # noqa: F401
-from helpers import rel_l2, shipped_vae_weights
-from ppo_depth_cases import A, ARCHS, KINK_MARGIN, LR, S, learn_refs, learn_setup, make_batch, make_ppo
-from ppo_cases import bounds
-from vae_checks import mlp_weights
+import ppo_restatement as pr
+from harness import lib, library_state  # noqa: F401
+from helpers import rel_l2
+from ppo_cases import ARCHS, KINK_MARGIN, gauss_net, learn_refs, learn_setup, make_batch, make_ppo
+from ppo_checks import (TOL, actor_vae, check_fused_actor, check_learn, check_learn_opts_clip_and_kl_stop,
+                        check_learn_segments, check_loss, check_two_train_steps, five, fresh_process, nan_workspace)
 
 pytestmark = pytest.mark.gpu
 
-TOL = 1e-5
-
-
-def _nan_workspace(m, *shape):
-    ws = m._workspace(*shape)
-    ws.fill_(0xFF)                  # every float of the workspace reads as NaN until written
-    return ws
-
-
-def _gate(got, r64, r32):
-    """max(TOL, 2 x the float32 restatement's distance from float64)"""
-    return rel_l2(got, r64) < max(TOL, 2 * rel_l2(r32, r64))
+A, S = 2, 67
 
 
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_predict_greedy_and_sampled(tmp_path, arch):
-    net = ARCHS[arch]
-    p, _, s, _, _, _ = make_batch(net, 37, seed=1)
-    assert pdo.relu_margin(p, s) > KINK_MARGIN
+    net = gauss_net(ARCHS[arch])
+    low, high = net[1]
+    p, _, s, _, _, _ = make_batch(net, 37, 1)
+    assert pr.relu_margin(p, s) > KINK_MARGIN
     m = make_ppo(tmp_path, net, p)
-    low, high = bounds(A)
     p64 = {k: v.astype(np.float64) for k, v in p.items()}
     noise = np.random.RandomState(2).randn(37, A).astype(np.float32) * 4.0        # clips at both bounds
     for nz in (None, noise):
-        _nan_workspace(m, 37)
+        nan_workspace(m, 37)
         act, val = m.predict(s, greedy=nz is None, noise=nz)
         assert np.isfinite(act).all() and np.isfinite(val).all()
-        ract, rval = pdo.predict(p64, s.astype(np.float64), low, high, noise=nz)
+        ract, rval = pr.predict(p64, s.astype(np.float64), net[1], noise=nz)
         assert rel_l2(act, ract) < TOL and rel_l2(val, rval) < TOL, (rel_l2(act, ract), rel_l2(val, rval))
     assert (act == low).any() and (act == high).any()
 
@@ -53,216 +40,67 @@ def test_predict_greedy_and_sampled(tmp_path, arch):
 @pytest.mark.parametrize("B", [1, 9, 256, 8200])
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_loss_and_gradients(tmp_path, arch, B):
-    net = ARCHS[arch]
-    low, high = bounds(A)
-    p, old, s, a, ret, adv = make_batch(net, B, seed=3 + B)
-    assert pdo.relu_margin(p, s) > KINK_MARGIN
+    net = gauss_net(ARCHS[arch])
+    p, old, s, a, ret, adv = make_batch(net, B, 3 + B)
+    assert pr.relu_margin(p, s) > KINK_MARGIN
     m = make_ppo(tmp_path, net, p, old)
-    _nan_workspace(m, B)
-    metrics, grads = m.loss_and_grads(s, a, ret, adv)
-    r64 = pdo.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
-    r32 = pdo.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01, dtype=np.float32)
-    assert np.isfinite(metrics).all()
-    for i, k in enumerate(("policy_loss", "value_loss", "entropy_loss", "loss", "mean_ratio")):
-        assert _gate(np.atleast_1d(metrics[i]), np.atleast_1d(r64[k]), np.atleast_1d(r32[k])), k
-    assert set(grads) == set(r64["grads"])
-    for k, g in grads.items():
-        assert np.isfinite(g).all(), k
-        assert _gate(g, r64["grads"][k], r32["grads"][k]), (k, rel_l2(g, r64["grads"][k]))
+    nan_workspace(m, B)
+    check_loss(m, p, old, s, a, ret, adv, net[1])
 
 
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_two_train_steps(tmp_path, arch):
-    from oracle import vae_oracle as vo
-    from ppo_cases import warm_adam
-    net = ARCHS[arch]
-    low, high = bounds(A)
-    p, old, s, a, ret, adv = make_batch(net, 64, seed=17)
-    m_, v_, powers = warm_adam(p, pdo.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)["grads"], 19)
-    m = make_ppo(tmp_path, net, p, old)
-    m.set_weights(p, old, m_, v_, powers)
-    for _ in range(2):
-        _nan_workspace(m, 64)
-        m.train(s, a, ret, adv)
-
-    def steps(dtype):
-        q = {k: x.astype(dtype) for k, x in p.items()}
-        st = dict(m={k: m_[k].astype(dtype) for k in p}, v={k: v_[k].astype(dtype) for k in p}, beta1_power=powers[0],
-                  beta2_power=powers[1])
-        for _ in range(2):
-            vo.adam_apply(q, pdo.loss_and_grads(q, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01, dtype=dtype)["grads"],
-                          st, LR)
-        return q
-    p64, p32 = steps(np.float64), steps(np.float32)
-    got = m.get_weights()
-    for k in p64:
-        assert _gate(got[k], p64[k], p32[k]), k
-
-
-def _check_learn(got, metrics, refs, applied=None):
-    (p64, rec64, n64), (p32, rec32, _) = refs
-    for k in p64:
-        assert np.isfinite(got[k]).all(), k
-        assert _gate(got[k], p64[k], p32[k]), (k, rel_l2(got[k], p64[k]))
-    ncol = metrics.shape[1]
-    ok = ~np.isnan(rec64[:, 0])
-    assert np.array_equal(np.isnan(metrics[:, 0]), ~ok)
-    for col in range(ncol):
-        # approx_kl (column 5) is 0 at the first minibatch and ~1e-8 soon after: gated absolutely as well
-        assert (_gate(metrics[ok, col], rec64[ok, col], rec32[ok, col])
-                or (col == 5 and np.abs(metrics[ok, col] - rec64[ok, col]).max() < 1e-6)), col
-    if applied is not None:
-        assert applied == n64
+    net = gauss_net(ARCHS[arch])
+    check_two_train_steps(tmp_path, net, make_batch(net, 64, 17))
 
 
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_learn(tmp_path, arch):
     """T = 2048 in 4 epochs of 8 minibatches of 256, launch per kernel."""
-    net = ARCHS[arch]
-    p, data, perms, adam = learn_setup(net, 2048, 256, 4, seed=40)
-    assert pdo.relu_margin(p, data[0]) > KINK_MARGIN
+    net = gauss_net(ARCHS[arch])
+    p, data, perms, adam = learn_setup(net, 2048, 4, 40)
+    assert pr.relu_margin(p, data[0]) > KINK_MARGIN
     m = make_ppo(tmp_path, net, p)
-    m.set_weights(p, p, adam[0], adam[1], adam[2])
+    m.set_weights(p, p, *adam)
     s, a, r, v, d = data
-    _nan_workspace(m, 256, 2048)
+    nan_workspace(m, 256, 2048)
     metrics = m.learn(s, a, v, r, d, 0.3, num_epochs=4, batch_size=256, perms=perms, return_metrics=True)
-    refs = learn_refs(p, data, perms, 256, adam)
-    _check_learn(m.get_weights(), metrics, ((refs[0][0], refs[0][1][:, :5], refs[0][2]), (refs[1][0], refs[1][1][:, :5], 0)))
+    check_learn(m.get_weights(), metrics, five(learn_refs(net, p, data, perms, 256, adam)))
 
 
 def test_persistent_learn_equals_launch_per_kernel(tmp_path):
     """The persistent kernel (CPB_PPO_PERSISTENT=1, read once per process) at every architecture: within 1e-6 of the
     launch-per-kernel path, and within the float32 gate of float64."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    snippet = r"""
-import sys, numpy as np
-sys.path[:0] = [%r, %r]
-from pathlib import Path
-import ppo_depth_cases as t
-out = {}
-for name in t.ARCHS:
-    w, metrics = t.persistent_learn(Path(%r) / name, name, 2048, 256, 4)
-    out.update({name + ":" + k: x for k, x in w.items()})
-    out[name + ":metrics"] = metrics
-np.savez(%r, **out)
-"""
-    outs = []
-    for flag in ("0", "1"):
-        path = str(tmp_path / ("w%s.npz" % flag))
-        code = snippet % (root, os.path.join(root, "tests"), str(tmp_path / ("m" + flag)), path)
-        res = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CPB_PPO_PERSISTENT=flag),
-                             capture_output=True, text=True, timeout=1200)
-        assert res.returncode == 0, res.stderr[-3000:]
-        outs.append(dict(np.load(path)))
-    for name, net in ARCHS.items():
-        p, data, perms, adam = learn_setup(net, 2048, 256, 4, seed=40)
-        refs = learn_refs(p, data, perms, 256, adam)
-        w1 = {k: outs[1][name + ":" + k] for k in p}
-        _check_learn(w1, outs[1][name + ":metrics"],
-                     ((refs[0][0], refs[0][1][:, :5], refs[0][2]), (refs[1][0], refs[1][1][:, :5], 0)))
+    cases = [(name, gauss_net(arch), ("rollout", 2048, 4, 256, 40), {}) for name, arch in ARCHS.items()]
+    outs = fresh_process(tmp_path, cases)
+    for name, arch in ARCHS.items():
+        net = gauss_net(arch)
+        p, data, perms, adam = learn_setup(net, 2048, 4, 40)
+        w1 = {k: outs[1][name + ":w:" + k] for k in p}
+        check_learn(w1, outs[1][name + ":metrics"], five(learn_refs(net, p, data, perms, 256, adam)))
         for k in p:
-            assert rel_l2(w1[k], outs[0][name + ":" + k]) < 1e-6, (name, k)
+            assert rel_l2(w1[k], outs[0][name + ":w:" + k]) < 1e-6, (name, k)
 
 
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_learn_segments(tmp_path, arch):
     """16 segments x 128 rows."""
-    net = ARCHS[arch]
-    p, data, perms, adam = learn_setup(net, 2048, 256, 2, seed=50)
-    s, a, r, v, d = data
-    lengths = [128] * 16
-    boot = np.random.RandomState(51).randn(16)
-    m = make_ppo(tmp_path, net, p)
-    m.set_weights(p, p, adam[0], adam[1], adam[2])
-    _nan_workspace(m, 256, 2048)
-    metrics = m.learn(s, a, v, r, d, boot, num_epochs=2, batch_size=256, perms=perms, return_metrics=True,
-                      segment_lengths=lengths)
-    refs = learn_refs(p, data, perms, 256, adam, segment_lengths=lengths, bootstrap_values=boot)
-    _check_learn(m.get_weights(), metrics, ((refs[0][0], refs[0][1][:, :5], refs[0][2]), (refs[1][0], refs[1][1][:, :5], 0)))
+    check_learn_segments(tmp_path, gauss_net(ARCHS[arch]))
 
 
 @pytest.mark.parametrize("arch", list(ARCHS))
 def test_learn_opts_clip_and_kl_stop(tmp_path, arch):
     """Clipping binding on 25-75 % of the minibatches, then a KL stop at a minibatch k > 1 (steps_applied = k).  The
     learning rate is 3e-3 so that the approximate KL of the later minibatches stands well above float32 rounding."""
-    net = ARCHS[arch]
-    lr = 3e-3
-    p, data, perms, adam = learn_setup(net, 2048, 256, 4, seed=60)
-    s, a, r, v, d = data
-    # the pre-clip norms of the unguarded update set the clip; its KL values set the stop
-    (_, rec0, _), _ = learn_refs(p, data, perms, 256, adam, lr=lr)
-    for q in (0.375, 0.5, 0.625):          # the first quantile of the unclipped norms that clips 25-75 % of the steps
-        max_norm = float(np.quantile(rec0[:, 6], q))
-        (_, rec, _), _ = learn_refs(p, data, perms, 256, adam, lr=lr, max_grad_norm=max_norm)
-        clipped = (rec[:, 6] > max_norm).mean()
-        if 0.25 <= clipped <= 0.75:
-            break
-    assert 0.25 <= clipped <= 0.75, clipped
-    kl = rec[:, 5]
-    # the first minibatch from the third on whose KL exceeds every earlier one by 20 %, and is above float32 noise
-    k = next(i for i in range(2, len(kl)) if kl[i] > 1.2 * kl[:i].max() and kl[i] > 1e-5)
-    target_kl = float((kl[:k].max() + kl[k]) / 2 / 1.5)
-    refs = learn_refs(p, data, perms, 256, adam, lr=lr, max_grad_norm=max_norm, target_kl=target_kl)
-    stop = refs[0][2]
-    assert stop == k > 1, (stop, k)
-    m = make_ppo(tmp_path, net, p, learning_rate=lr)
-    m.set_weights(p, p, adam[0], adam[1], adam[2])
-    _nan_workspace(m, 256, 2048)
-    metrics = m.learn(s, a, v, r, d, 0.3, num_epochs=4, batch_size=256, perms=perms, return_metrics=True,
-                      max_grad_norm=max_norm, target_kl=target_kl)
-    _check_learn(m.get_weights(), metrics, refs, applied=int(m.last_steps_applied.item()))
+    check_learn_opts_clip_and_kl_stop(tmp_path, gauss_net(ARCHS[arch]))
 
 
 # ------------------------------------------------------------------------------ the default architecture: spec == legacy
-_DEFAULT_SNIPPET = r"""
-import sys, ctypes as C, numpy as np
-sys.path[:0] = [%r, %r]
-from pathlib import Path
-import ppo_depth_cases as t
-from carla_ppo_b200 import _lib
-lib = _lib.load()
-p, data, perms, adam = t.learn_setup(t.ARCHS["default"], 2048, 256, 2, seed=70)
-s, a, r, v, d = data
-out = {}
-for use_spec in (0, 1):
-    m = t.make_ppo(Path(%r) / str(use_spec), t.ARCHS["default"], p)
-    if not use_spec:                  # the legacy entry points: the spec names mapped back
-        real = m._call
-        m._call = lambda name, *args, _r=real, _m=m: _r(name.replace("cpb_ppo_spec_", "cpb_ppo_"),
-                                                        *((C.byref(_m._c),) + args[1:]))
-    for opts in ({}, {"max_grad_norm": 0.05, "target_kl": 0.004}):
-        for seg in (None, [1024, 1024]):
-            m.set_weights(p, p, adam[0], adam[1], adam[2])
-            lib.cpb_reset_launch_count()
-            boot = 0.3 if seg is None else np.array([0.3, -0.1])
-            met = m.learn(s, a, v, r, d, boot, num_epochs=2, batch_size=256, perms=perms, return_metrics=True,
-                          segment_lengths=seg, **opts)
-            tag = "%%d:%%d:%%d" %% (use_spec, bool(opts), seg is not None)
-            out[tag + ":launches"] = np.int64(lib.cpb_launch_count())
-            out[tag + ":metrics"] = met
-            for k, w in m.get_weights().items():
-                out[tag + ":" + k] = w
-            out[tag + ":old"] = m.params_old.cpu().numpy()
-            out[tag + ":m"] = m.adam_m.cpu().numpy(); out[tag + ":v"] = m.adam_v.cpu().numpy()
-            out[tag + ":pw"] = m.adam_powers.cpu().numpy()
-            if opts:
-                out[tag + ":applied"] = m.last_steps_applied.cpu().numpy()
-np.savez(%r, **out)
-"""
-
-
 def test_default_architecture_spec_equals_legacy(tmp_path):
     """learn, learn_opts, learn_segments and learn_segments_opts through the spec twins and through the legacy entry
     points: parameters, theta_old, Adam m / v, beta powers, metrics, steps_applied and launch counts identical, on the
     launch-per-kernel path and in the persistent kernel."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for flag in ("0", "1"):
-        path = str(tmp_path / ("d%s.npz" % flag))
-        code = _DEFAULT_SNIPPET % (root, os.path.join(root, "tests"), str(tmp_path / ("m" + flag)), path)
-        res = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CPB_PPO_PERSISTENT=flag),
-                             capture_output=True, text=True, timeout=600)
-        assert res.returncode == 0, res.stderr[-3000:]
-        o = dict(np.load(path))
+    for flag, o in zip("01", fresh_process(tmp_path, 70, body="spec_vs_legacy", timeout=600)):
         legacy = {k[2:]: x for k, x in o.items() if k.startswith("0:")}
         spec = {k[2:]: x for k, x in o.items() if k.startswith("1:")}
         assert legacy.keys() == spec.keys() and len(legacy) > 0
@@ -274,8 +112,8 @@ def test_default_architecture_predict_train_loss_equal_legacy(tmp_path, lib):
     import ctypes as C
     import torch
     from carla_ppo_b200 import _lib
-    p, old, s, a, ret, adv = make_batch(ARCHS["default"], 256, seed=80)
-    m = make_ppo(tmp_path, ARCHS["default"], p, old)
+    p, old, s, a, ret, adv = make_batch(gauss_net(ARCHS["default"]), 256, 80)
+    m = make_ppo(tmp_path, gauss_net(ARCHS["default"]), p, old)
     ptr = _lib.ptr
     st, at = torch.from_numpy(s).cuda(), torch.from_numpy(a).cuda()
     rt, vt = torch.from_numpy(ret).cuda(), torch.from_numpy(adv).cuda()
@@ -324,8 +162,9 @@ def test_default_architecture_actor_twins_equal_legacy(tmp_path, lib, kind):
     from carla_ppo_b200 import _lib
     from helpers import committed_frames
     legacy = {"conv": "cpb_vae_spec_encode_predict", "mlp": "cpb_mlpvae_encode_predict"}[kind]
-    vae = _vae(tmp_path, kind)
-    m = make_ppo(tmp_path / "ppo", ARCHS["default"], pdo.init_params(S, A, *ARCHS["default"], seed=5))
+    vae = actor_vae(tmp_path, kind)
+    net = gauss_net(ARCHS["default"])
+    m = make_ppo(tmp_path / "ppo", net, pr.init_params(*net, seed=5))
     n = 4
     rgb, _ = committed_frames()
     frames = torch.from_numpy(np.ascontiguousarray(rgb[:n])).cuda()
@@ -352,39 +191,10 @@ def test_default_architecture_actor_twins_equal_legacy(tmp_path, lib, kind):
 
 
 # ----------------------------------------------------------------------------------------------------- fused actor
-def _vae(tmp_path, kind):
-    if kind == "conv":
-        return make_conv_vae(tmp_path, shipped_vae_weights()[0], loss="bce", tag="vae", training=False)
-    enc, dec = (96, 256, 64), (160, 64)
-    return make_mlp(tmp_path, mlp_weights(2, encoder_sizes=enc, decoder_sizes=dec), enc, dec, tag="vec", training=False)
-
-
-def _fake_envs(n):
-    import types
-    from helpers import committed_frames
-    rgb, _ = committed_frames()
-    envs = []
-    for i in range(n):
-        v = types.SimpleNamespace(control=types.SimpleNamespace(steer=0.1 * (i % 7) - 0.3, throttle=0.05 * (i % 11)),
-                                  get_speed=(lambda s=0.37 * i: s))
-        envs.append(types.SimpleNamespace(observation=rgb[(5 * i) % len(rgb)], vehicle=v))
-    return envs
-
-
 @pytest.mark.parametrize("kind", ["conv", "mlp"])
 @pytest.mark.parametrize("n", [1, 4])
 def test_fused_actor_equals_unfused(tmp_path, lib, kind, n):
-    from carla_ppo_b200.actor import FusedActor, UnfusedActor
-    net = ARCHS["odd"]
-    vae = _vae(tmp_path, kind)
-    meas = ("steer", "throttle", "speed")
-    p = pdo.init_params(S, A, net[0], net[1], seed=90)
-    models = [make_ppo(tmp_path / tag, net, p, initial_std=0.4) for tag in ("fused", "unfused")]
-    envs = _fake_envs(n)
-    fs, fa, fv = FusedActor(vae, models[0], meas).encode_predict(envs)
-    us, ua, uv = UnfusedActor(vae, models[1], meas).encode_predict(envs)
-    assert all(np.array_equal(x, y) for x, y in zip(fs, us))
-    assert np.array_equal(fa, ua) and np.array_equal(fv, uv) and np.isfinite(fa).all()
+    check_fused_actor(tmp_path, gauss_net(ARCHS["odd"]), kind, n, greedy=(False,))
 
 
 # ------------------------------------------------------------------------------------------------------ checkpoints
@@ -392,22 +202,22 @@ def test_fused_actor_equals_unfused(tmp_path, lib, kind, n):
 def test_checkpoint_round_trip_and_architecture_refusal(tmp_path, tf_format):
     from carla_ppo_b200.ppo import checkpoint_architecture
     net = ARCHS["odd"]
-    p, data, perms, adam = learn_setup(net, 512, 128, 1, seed=100)
-    a = make_ppo(tmp_path / "a", net, p)
-    a.set_weights(p, p, adam[0], adam[1], adam[2])
+    p, data, perms, adam = learn_setup(gauss_net(net), 512, 1, 100)
+    a = make_ppo(tmp_path / "a", gauss_net(net), p)
+    a.set_weights(p, p, *adam)
     s, act, r, v, d = data
     a.learn(s, act, v, r, d, 0.3, num_epochs=1, batch_size=128, perms=perms)
     a.episode_counter = 3
     a.save(tf_format=tf_format)
     assert checkpoint_architecture(a.checkpoint_dir) == net
-    b = make_ppo(tmp_path / "a", net)
+    b = make_ppo(tmp_path / "a", gauss_net(net))
     assert b.load_latest_checkpoint() is True
     for x, y in ((a.params, b.params), (a.params_old, b.params_old), (a.adam_m, b.adam_m), (a.adam_v, b.adam_v),
                  (a.adam_powers, b.adam_powers)):
         assert np.array_equal(x.cpu().numpy(), y.cpu().numpy())
     assert b.get_episode_idx() == 3
     for other in (ARCHS["default"], ((33, 7, 65), (32,))):
-        c = make_ppo(tmp_path / "a", other)
+        c = make_ppo(tmp_path / "a", gauss_net(other))
         before = c.params.cpu().numpy().copy()
         assert c.load_latest_checkpoint() is False
         assert np.array_equal(before, c.params.cpu().numpy())

@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 from helpers import rel_l2, shipped_ppo
-from ppo_cases import HIGH, LOW, baseline_config3, make_ppo
+from ppo_cases import HIGH, LOW, REFERENCE, baseline_config3, make_ppo
+from ppo_checks import fresh_process
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +26,7 @@ def rollout(T, seed=0):
 def test_predict_matches_oracle(tmp_path):
     from oracle import ppo_oracle as po
     pol, _ = shipped_ppo("policy")
-    m = make_ppo(tmp_path, pol)
+    m = make_ppo(tmp_path, REFERENCE, pol)
     states = rollout(33)[0]
     p64 = {k: v.astype(np.float64) for k, v in pol.items()}
     act, val = m.predict(states, greedy=True)
@@ -48,7 +49,7 @@ def test_loss_and_gradients_match_oracle(tmp_path, batch):
     from oracle import ppo_oracle as po, torch_ref
     pol, _ = shipped_ppo("policy")
     old, _ = shipped_ppo("policy_old")
-    m = make_ppo(tmp_path, pol, old)
+    m = make_ppo(tmp_path, REFERENCE, pol, old)
     rs = np.random.RandomState(1)
     s, a = rollout(batch, 2)[:2]
     ret = rs.randn(batch).astype(np.float32); adv = rs.randn(batch).astype(np.float32)
@@ -67,7 +68,7 @@ def test_train_step_matches_oracle(tmp_path):
     from oracle import ppo_oracle as po, vae_oracle as vo
     pol, z = shipped_ppo("policy")
     old, _ = shipped_ppo("policy_old")
-    m = make_ppo(tmp_path, pol, old)
+    m = make_ppo(tmp_path, REFERENCE, pol, old)
     s, a = rollout(64, 3)[:2]
     rs = np.random.RandomState(4)
     ret = rs.randn(64).astype(np.float32); adv = rs.randn(64).astype(np.float32)
@@ -100,7 +101,7 @@ def test_learn_matches_oracle_driver_block(tmp_path):
     shipped ckpt-705 weights; parameters after learn() vs the float64 restatement of train.py:171-207."""
     from oracle import ppo_oracle as po, vae_oracle as vo
     pol, _ = shipped_ppo("policy")
-    m = make_ppo(tmp_path, pol)
+    m = make_ppo(tmp_path, REFERENCE, pol)
     T, E, B = 512, 2, 96
     s, a, r, v, d = rollout(T, 7)
     perms = np.stack([np.random.RandomState(10 + e).permutation(T) for e in range(E)])
@@ -121,7 +122,7 @@ def test_learn_matches_oracle_driver_block(tmp_path):
 
 def test_checkpoint_round_trip_and_lr_decay(tmp_path):
     pol, _ = shipped_ppo("policy")
-    m = make_ppo(tmp_path, pol, lr_decay=0.5)
+    m = make_ppo(tmp_path, REFERENCE, pol, lr_decay=0.5)
     assert abs(float(m.learning_rate) - 1e-4) < 1e-11          # float32(1e-4), like the TF tensor
     m.write_episodic_summaries()
     assert m.get_episode_idx() == 1 and abs(float(m._lr_dev.item()) - 5e-5) < 1e-10
@@ -143,7 +144,7 @@ def test_learn_at_baseline_config3_matches_oracle(tmp_path):
     adam_m = {k: z["adam_m/" + k] for k in pol}
     adam_v = {k: z["adam_v/" + k] for k in pol}
     powers = (float(z["beta1_power"]), float(z["beta2_power"]))
-    m = make_ppo(tmp_path, pol, old)
+    m = make_ppo(tmp_path, REFERENCE, pol, old)
     m.set_weights(pol, old, adam_m, adam_v, powers)
     T, E, B = 2048, 4, 256
     s, a, r, v, d, perms = baseline_config3(T, E)
@@ -174,7 +175,7 @@ def test_update_old_policy_and_zero_epoch_learn(tmp_path):
     """PPO.update_old_policy (ppo.py:275-276) called directly; learn(num_epochs=0) still does theta_old <- theta."""
     pol, _ = shipped_ppo("policy")
     old, _ = shipped_ppo("policy_old")
-    m = make_ppo(tmp_path, pol, old)
+    m = make_ppo(tmp_path, REFERENCE, pol, old)
     assert not all(np.array_equal(m.get_old_weights()[k], pol[k]) for k in pol)
     m.update_old_policy()
     assert all(np.array_equal(m.get_old_weights()[k], pol[k]) for k in pol)
@@ -189,29 +190,8 @@ def test_update_old_policy_and_zero_epoch_learn(tmp_path):
 def test_persistent_learn_kernel_matches_launch_per_kernel_path(tmp_path):
     """CPB_PPO_PERSISTENT=1 (one cooperative kernel for all minibatch steps) vs the default launch-per-kernel learn():
     same parameters to fp32 round-off (the per-CTA loss partials are summed in a different order)."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    snippet = r"""
-import sys, numpy as np
-sys.path.insert(0, %r); sys.path.insert(0, %r)
-import ppo_cases as t
-from helpers import shipped_ppo
-from pathlib import Path
-pol, z = shipped_ppo("policy")
-m = t.make_ppo(Path(%r), pol, pol)
-m.set_weights(pol, pol, {k: z["adam_m/" + k] for k in pol}, {k: z["adam_v/" + k] for k in pol}, (float(z["beta1_power"]), float(z["beta2_power"])))
-s, a, r, v, d, perms = t.baseline_config3(2048, 2)
-m.learn(s, a, v, r, d, 0.3, num_epochs=2, batch_size=200, perms=perms)       # ragged last minibatch (2048 = 10 x 200 + 48)
-np.savez(%r, **m.get_weights())
-"""
-    outs = []
-    for flag in ("0", "1"):
-        out = str(tmp_path / ("w%s.npz" % flag))
-        code = snippet % (root, os.path.join(root, "tests"), str(tmp_path / ("m" + flag)), out)
-        res = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CPB_PPO_PERSISTENT=flag), capture_output=True, text=True, timeout=300)
-        assert res.returncode == 0, res.stderr[-2000:]
-        outs.append(dict(np.load(out)))
-    for k in outs[0]:
-        assert rel_l2(outs[1][k], outs[0][k]) < 1e-6, (k, rel_l2(outs[1][k], outs[0][k]))
+    # ragged last minibatch (2048 = 10 x 200 + 48)
+    outs = fresh_process(tmp_path, [("ckpt", REFERENCE, ("ckpt705", 2048, 2, 200, "policy", 1e-4, False), {})])
+    for k in shipped_ppo("policy")[0]:
+        w0, w1 = outs[0]["ckpt:w:" + k], outs[1]["ckpt:w:" + k]
+        assert rel_l2(w1, w0) < 1e-6, (k, rel_l2(w1, w0))

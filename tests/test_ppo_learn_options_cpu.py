@@ -6,9 +6,10 @@ import math
 import numpy as np
 import pytest
 
-import ppo_options_oracle as oo
+import ppo_restatement as pr
 from harness import lib, library_state  # noqa: F401
-from ppo_cases import CASES, bounds, learn_setup, ppo_config
+from ppo_cases import CASES, bounds, learn_setup, ppo_config, shape_net
+from ppo_checks import LEGACY_OPTS_ENTRIES, ppo_args
 
 
 # ------------------------------------------------------------------------------------------------ float64 restatement
@@ -17,7 +18,7 @@ def test_clipping_is_torch_clip_grad_norm(max_norm):
     import torch
     rs = np.random.RandomState(1)
     grads = {"a": rs.randn(7, 5), "b": rs.randn(5) * 0.1, "c": rs.randn(3, 2) * 0.01}
-    norm, clipped = oo.clip_grad_norm(grads, max_norm)
+    norm, clipped = pr.clip_grad_norm(grads, max_norm)
     ts = [torch.tensor(g, dtype=torch.float64, requires_grad=True) for g in grads.values()]
     for t, g in zip(ts, grads.values()):
         t.grad = torch.tensor(g, dtype=torch.float64)
@@ -30,24 +31,23 @@ def test_clipping_is_torch_clip_grad_norm(max_norm):
 
 def test_clipping_off_and_the_input_untouched():
     g = {"a": np.full(4, 3.0)}
-    norm, out = oo.clip_grad_norm(g, 0.0)
+    norm, out = pr.clip_grad_norm(g, 0.0)
     assert norm == 6.0 and np.array_equal(out["a"], g["a"])
-    norm, out = oo.clip_grad_norm(g, 1.0)
+    norm, out = pr.clip_grad_norm(g, 1.0)
     assert np.allclose(out["a"], 3.0 / (6.0 + 1e-6)) and np.array_equal(g["a"], np.full(4, 3.0))
 
 
 def test_approx_kl_estimator():
     e = math.e
-    assert oo.approx_kl([1.0, 1.0]) == 0.0
-    assert oo.approx_kl([e, 1 / e]) == pytest.approx(((e - 2) + (1 / e)) / 2, rel=1e-15)
+    assert pr.approx_kl([1.0, 1.0]) == 0.0
+    assert pr.approx_kl([e, 1 / e]) == pytest.approx(((e - 2) + (1 / e)) / 2, rel=1e-15)
     r = np.exp(np.random.RandomState(0).randn(1000) * 0.3)
-    kl = oo.approx_kl(r)
+    kl = pr.approx_kl(r)
     assert kl > 0 and kl == pytest.approx(np.mean(r - 1 - np.log(r)), rel=1e-15)
 
 
 def _scripted_learn(monkeypatch, kls, target_kl, epochs=2, nmb=3):
-    """oo.learn over scripted minibatches: minibatch j has approx_kl kls[j] (ratios {x, x} with (x - 1) - log x = kl)."""
-    from oracle import ppo_oracle as po, vae_oracle as vo
+    """pr.learn over scripted minibatches: minibatch j has approx_kl kls[j] (ratios {x, x} with (x - 1) - log x = kl)."""
     from scipy.optimize import brentq
     calls, steps = [], []
 
@@ -58,11 +58,11 @@ def _scripted_learn(monkeypatch, kls, target_kl, epochs=2, nmb=3):
         return dict(ratio=np.array([[x], [x]]), policy_loss=float(j), value_loss=0.0, entropy_loss=0.0, loss=0.0,
                     mean_ratio=x, grads={"w": np.array([3.0, 4.0])})
 
-    monkeypatch.setattr(po, "loss_and_grads", fake_loss)
-    monkeypatch.setattr(vo, "adam_apply", lambda p, g, st, lr: steps.append(g["w"].copy()))
+    monkeypatch.setattr(pr, "loss_and_grads", fake_loss)
+    monkeypatch.setattr(pr, "adam_apply", lambda p, g, st, lr: steps.append(g["w"].copy()))
     n = nmb * 2
-    rec, applied = oo.learn({"w": np.zeros(2)}, {}, np.zeros((n, 1)), np.zeros((n, 1)), np.zeros(n), np.zeros(n),
-                            np.zeros(n), 0.0, 0, 1, num_epochs=epochs, batch_size=2,
+    rec, applied = pr.learn({"w": np.zeros(2)}, {}, np.zeros((n, 1)), np.zeros((n, 1)), np.zeros(n), np.zeros(n),
+                            np.zeros(n), 0.0, (np.zeros(1), np.ones(1)), num_epochs=epochs, batch_size=2,
                             perms=[np.arange(n)] * epochs, max_grad_norm=2.5, target_kl=target_kl)
     return rec, applied, calls, steps
 
@@ -90,20 +90,20 @@ def test_kl_stop_at_the_first_minibatch_and_a_target_that_never_triggers(monkeyp
 
 
 def test_guards_off_are_the_oracle_update_bit_for_bit():
-    """oo.learn with both guards 0 is oracle.ppo_oracle.learn: the same parameters, Adam state and loss records."""
+    """pr.learn with both guards 0 is oracle.ppo_oracle.learn: the same parameters, Adam state and loss records."""
     from oracle import ppo_oracle as po
     shape, T, batch, epochs = CASES["odd"], 40, 16, 2
-    p, (s, a, r, v, d), perms, (m, vv, powers) = learn_setup(shape, T, batch, epochs, seed=3)
+    p, (s, a, r, v, d), perms, (m, vv, powers) = learn_setup(shape_net(*shape), T, epochs, seed=3)
     low, high = bounds(shape[1])
 
-    def run(fn, **kw):
+    def run(fn, *head, **kw):
         prm = {k: x.astype(np.float64) for k, x in p.items()}
         st = dict(m={k: m[k].astype(np.float64) for k in p}, v={k: vv[k].astype(np.float64) for k in p},
                   beta1_power=powers[0], beta2_power=powers[1])
-        out = fn(prm, st, s, a, v, r, d, 0.3, low, high, 0.99, 0.95, 1e-3, 0.2, 1.0, 0.01, epochs, batch, perms, **kw)
+        out = fn(prm, st, s, a, v, r, d, 0.3, *head, 0.99, 0.95, 1e-3, 0.2, 1.0, 0.01, epochs, batch, perms, **kw)
         return prm, st, out
-    p0, st0, rec0 = run(po.learn)
-    p1, st1, (rec1, applied) = run(oo.learn, max_grad_norm=0.0, target_kl=0.0)
+    p0, st0, rec0 = run(po.learn, low, high)
+    p1, st1, (rec1, applied) = run(pr.learn, (low, high), max_grad_norm=0.0, target_kl=0.0)
     assert applied == epochs * 3
     for k in p0:
         assert np.array_equal(p0[k], p1[k]) and np.array_equal(st0["m"][k], st1["m"][k]), k
@@ -113,7 +113,6 @@ def test_guards_off_are_the_oracle_update_bit_for_bit():
 
 
 # ------------------------------------------------------------------------------------------------ C ABI refusals
-FAKE = 0x1000          # never dereferenced: every call below must be refused before it touches memory
 BAD_OPTIONS = [(-1.0, 0.0), (0.0, -0.01), (float("nan"), 0.0), (0.0, float("nan")), (float("inf"), 0.0),
                (0.0, float("inf")), (-float("inf"), 0.5)]
 
@@ -123,42 +122,7 @@ def _opts(m, t):
     return C.byref(_lib.PpoLearnOptions(m, t))
 
 
-LEARN_POINTERS = ("params", "params_old", "grads", "adam_m", "adam_v", "adam_powers", "lr_dev", "states", "actions",
-                  "rewards", "values", "dones", "perms")
-
-
-def _learn_args(cfg, opts, **over):
-    a = {k: FAKE for k in LEARN_POINTERS}
-    a.update(over)
-    return (C.byref(cfg), a["params"], a["params_old"], a["grads"], a["adam_m"], a["adam_v"], a["adam_powers"], a["lr_dev"],
-            a["states"], a["actions"], a["rewards"], a["values"], 0.3, a["dones"], 40, 0.99, 0.95, 2, 16, a["perms"], FAKE,
-            opts, FAKE, FAKE, 1 << 40, None)
-
-
-SEG_POINTERS = LEARN_POINTERS + ("bootstrap", "offsets")
-
-
-def _segments_args(cfg, opts, **over):
-    a = {k: FAKE for k in SEG_POINTERS}
-    a.update(over)
-    return (C.byref(cfg), a["params"], a["params_old"], a["grads"], a["adam_m"], a["adam_v"], a["adam_powers"], a["lr_dev"],
-            a["states"], a["actions"], a["rewards"], a["values"], a["bootstrap"], a["dones"], a["offsets"], 3, 40, 0.99,
-            0.95, 2, 16, a["perms"], FAKE, opts, FAKE, FAKE, 1 << 40, None)
-
-
-STEP_POINTERS = ("params", "params_old", "grads", "adam_m", "adam_v", "adam_powers", "lr_dev", "states", "actions",
-                 "returns", "advantages")
-
-
-def _step_args(cfg, opts, **over):
-    a = {k: FAKE for k in STEP_POINTERS}
-    a.update(over)
-    return (C.byref(cfg), a["params"], a["params_old"], a["grads"], a["adam_m"], a["adam_v"], a["adam_powers"], a["lr_dev"],
-            a["states"], a["actions"], a["returns"], a["advantages"], None, 16, FAKE, opts, FAKE, FAKE, FAKE, 1 << 40, None)
-
-
-ENTRIES = [("cpb_ppo_learn_opts", _learn_args, LEARN_POINTERS), ("cpb_ppo_learn_segments_opts", _segments_args, SEG_POINTERS),
-           ("cpb_ppo_train_step_opts", _step_args, STEP_POINTERS)]
+ENTRIES = [("cpb_ppo_" + e, e, names) for e, names in LEGACY_OPTS_ENTRIES.items()]
 
 
 @pytest.mark.parametrize("entry, args, _", ENTRIES, ids=[e[0] for e in ENTRIES])
@@ -166,7 +130,7 @@ ENTRIES = [("cpb_ppo_learn_opts", _learn_args, LEARN_POINTERS), ("cpb_ppo_learn_
 def test_bad_options_are_refused_without_a_launch(lib, entry, args, _, bad):
     cfg = ppo_config(67, 2, 500, 300)
     before = lib.cpb_launch_count()
-    assert getattr(lib, entry)(*args(cfg, _opts(*bad))) == -1
+    assert getattr(lib, entry)(*ppo_args(args, C.byref(cfg), _opts(*bad))) == -1
     assert lib.cpb_launch_count() == before
     assert b"ppo options" in lib.cpb_last_error()
 
@@ -177,7 +141,7 @@ def test_null_pointers_are_refused_without_a_launch(lib, entry, args, names):
     for name in names:
         for opts in (None, _opts(0.5, 0.01)):
             before = lib.cpb_launch_count()
-            assert getattr(lib, entry)(*args(cfg, opts, **{name: None})) == -1, name
+            assert getattr(lib, entry)(*ppo_args(args, C.byref(cfg), opts, **{name: None})) == -1, name
             assert lib.cpb_launch_count() == before, name
 
 

@@ -11,7 +11,9 @@ import pytest
 import single_env_train
 from harness import lib, library_state  # noqa: F401
 from helpers import Box
-from ppo_cases import ppo_config, segment_inputs, segmented_gae
+from ppo_cases import ppo_config, segment_inputs
+from ppo_checks import SEGMENTS_POINTERS, ppo_args
+from ppo_restatement import segmented_gae
 
 
 # ------------------------------------------------------------------------------------------------ float64 restatement
@@ -60,35 +62,20 @@ def test_gae_segments_refuses_bad_arguments_without_a_launch(lib, over):
     assert b"gae_segments" in lib.cpb_last_error()
 
 
-LEARN_POINTERS = ("params", "params_old", "grads", "adam_m", "adam_v", "adam_powers", "lr_dev", "states", "actions",
-                  "rewards", "values", "bootstrap", "dones", "offsets", "perms")
-
-
-def _learn_args(cfg, **over):
-    a = {k: FAKE for k in LEARN_POINTERS}
-    a.update(S=3, rows=40, epochs=2, batch=16)
-    a.update(over)
-    ws_bytes = 1 << 40                  # large enough for any plan; the pointer is never used
-    return (C.byref(cfg), a["params"], a["params_old"], a["grads"], a["adam_m"], a["adam_v"], a["adam_powers"], a["lr_dev"],
-            a["states"], a["actions"], a["rewards"], a["values"], a["bootstrap"], a["dones"], a["offsets"], a["S"],
-            a["rows"], 0.99, 0.95, a["epochs"], a["batch"], a["perms"], None, FAKE, ws_bytes, None)
-
-
 @pytest.mark.parametrize("over", [dict(S=0), dict(S=-2), dict(S=41), dict(rows=2), dict(batch=0), dict(epochs=-1)]
-                         + [{k: None} for k in LEARN_POINTERS],
+                         + [{k: None} for k in SEGMENTS_POINTERS],
                          ids=lambda d: "_".join("%s%s" % kv for kv in d.items()))
 def test_learn_segments_refuses_bad_arguments_without_a_launch(lib, over):
     cfg = ppo_config(67, 2, 500, 300)
     before = lib.cpb_launch_count()
-    assert lib.cpb_ppo_learn_segments(*_learn_args(cfg, **over)) == -1
+    assert lib.cpb_ppo_learn_segments(*ppo_args("learn_segments", C.byref(cfg), **over)) == -1
     assert lib.cpb_launch_count() == before
 
 
 def test_learn_segments_refuses_a_small_workspace(lib):
     cfg = ppo_config(67, 2, 500, 300)
     need = lib.cpb_ppo_workspace_bytes(C.byref(cfg), 16, 40)
-    args = list(_learn_args(cfg))
-    args[-2] = need - 1
+    args = ppo_args("learn_segments", C.byref(cfg), ws_bytes=need - 1)
     assert lib.cpb_ppo_learn_segments(*args) == -3          # CPB_ERR_WORKSPACE_TOO_SMALL
 
 

@@ -1,23 +1,17 @@
 """N environments on the device: the segmented GAE and PPO update against the float64 restatement
 (tests/test_ppo_segments_cpu.py), bit-identity with the single-rollout entry points at one segment, the batched fused
 encode + predict, and train.train with --num_envs."""
-import os
-import subprocess
-import sys
-import types
-
 import numpy as np
 import pytest
 
-from harness import lib, library_state, make_conv_vae, make_mlp, math_mode  # noqa: F401
+from harness import lib, library_state, math_mode  # noqa: F401
 from helpers import committed_frames, rel_l2, shipped_ppo, shipped_vae_weights
-from ppo_cases import (HIGH, LOW, baseline_config3, make_ppo, segment_inputs, segmented_gae, shipped_vae,
-                       train_params)
-from vae_checks import mlp_weights
+from ppo_cases import (HIGH, LOW, REFERENCE, baseline_config3, make_ppo, model_state, restate, segment_inputs,
+                       shipped_adam, shipped_vae, train_params)
+from ppo_checks import TOL, actor_vae, fake_envs, fresh_process
+from ppo_restatement import segmented_gae
 
 pytestmark = pytest.mark.gpu
-
-TOL = 1e-5             # tests/test_ppo_gpu.py's
 
 LENGTHS = (1, 31, 32, 33, 1023, 1024, 1025, 4097)
 
@@ -65,67 +59,16 @@ def test_one_segment_is_cpb_gae_bit_for_bit():
 
 
 # ------------------------------------------------------------------------------------------------ learn over segments
-def _state(m):
-    return dict(params=m.params.cpu().numpy(), old=m.params_old.cpu().numpy(), m=m.adam_m.cpu().numpy(),
-                v=m.adam_v.cpu().numpy(), powers=m.adam_powers.cpu().numpy())
-
-
-_SNIPPET = r"""
-import sys, numpy as np
-sys.path.insert(0, %r); sys.path.insert(0, %r)
-import ppo_cases as t
-from helpers import shipped_ppo
-from pathlib import Path
-pol, z = shipped_ppo("policy")
-old, _ = shipped_ppo("policy_old")
-out = {}
-for tag, seg in (("one", None), ("seg", [2048])):
-    m = t.make_ppo(Path(%r) / tag, pol, old)
-    m.set_weights(pol, old, {k: z["adam_m/" + k] for k in pol}, {k: z["adam_v/" + k] for k in pol}, (float(z["beta1_power"]), float(z["beta2_power"])))
-    s, a, r, v, d, perms = t.baseline_config3(2048, 2)
-    last = 0.3 if seg is None else [0.3]
-    met = m.learn(s, a, v, r, d, last, num_epochs=2, batch_size=200, perms=perms, return_metrics=True, segment_lengths=seg)
-    for k, x in dict(params=m.params, old=m.params_old, m=m.adam_m, v=m.adam_v, powers=m.adam_powers).items():
-        out[tag + "_" + k] = x.cpu().numpy()
-    out[tag + "_metrics"] = met
-np.savez(%r, **out)
-"""
-
-
 @pytest.mark.parametrize("persistent", ["0", "1"])
 def test_one_segment_learn_is_cpb_ppo_learn_bit_for_bit(tmp_path, persistent):
     """cpb_ppo_learn_segments at S = 1 vs cpb_ppo_learn from ckpt-705 with warm Adam slots (2 epochs x 200, a short last
     minibatch): parameters, theta_old, Adam m / v, beta powers and every minibatch metric, launch-per-kernel and under
     CPB_PPO_PERSISTENT=1 (read once per process, hence the subprocess)."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = str(tmp_path / "out.npz")
-    code = _SNIPPET % (root, os.path.join(root, "tests"), str(tmp_path), out)
-    res = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, CPB_PPO_PERSISTENT=persistent),
-                         capture_output=True, text=True, timeout=300)
-    assert res.returncode == 0, res.stderr[-2000:]
-    z = np.load(out)
+    ckpt = ("ckpt705", 2048, 2, 200, "policy_old", 1e-4, False)
+    z, = fresh_process(tmp_path, [("one", REFERENCE, ckpt, {}), ("seg", REFERENCE, ckpt, dict(segment_lengths=[2048]))],
+                       flags=(persistent,), timeout=300)
     for k in ("params", "old", "m", "v", "powers", "metrics"):
-        assert np.array_equal(z["one_" + k], z["seg_" + k]), k
-
-
-def _oracle_learn_segments(pol, adam, s, a, v, r, d, boot, lengths, E, B, perms, dtype):
-    """ppo_oracle.learn with the segmented GAE in place of the single-rollout one."""
-    from oracle import ppo_oracle as po, vae_oracle as vo
-    p = {k: x.astype(dtype) for k, x in pol.items()}
-    st = dict(m={k: adam[0][k].astype(dtype) for k in pol}, v={k: adam[1][k].astype(dtype) for k in pol},
-              beta1_power=adam[2][0], beta2_power=adam[2][1])
-    returns, adv_n, _ = segmented_gae(r, v, boot, d, lengths, 0.99, 0.95)
-    ret32, adv32 = returns.astype(np.float32).astype(dtype), adv_n.astype(np.float32).astype(dtype)
-    old = {k: x.copy() for k, x in p.items()}
-    s, a = np.asarray(s, dtype), np.asarray(a, dtype)
-    n, rec = s.shape[0], []
-    for e in range(E):
-        for i in range(int(np.ceil(n / B))):
-            mb = np.asarray(perms[e])[i * B:(i + 1) * B]
-            out = po.loss_and_grads(p, old, s[mb], a[mb], ret32[mb], adv32[mb], LOW, HIGH, 0.2, 1.0, 0.01, True, dtype)
-            vo.adam_apply(p, out["grads"], st, 1e-4)
-            rec.append((out["policy_loss"], out["value_loss"], out["entropy_loss"], out["loss"], out["mean_ratio"]))
-    return p, np.asarray(rec, np.float64)
+        assert np.array_equal(z["one:" + k], z["seg:" + k]), k
 
 
 @pytest.mark.parametrize("lengths, E, B", [([128] * 16, 4, 256), ([1, 7, 128, 60, 3], 3, 64)], ids=["16x128", "ragged"])
@@ -133,10 +76,10 @@ def test_learn_segments_match_the_oracle(tmp_path, lengths, E, B):
     """configs[2]'s shapes (ckpt-705 with warm Adam slots, RandomState(0) permutations) over 16 segments of 128 rows, and
     ragged segments with a short last minibatch; gates as test_ppo_gpu's configs[2] test: max(1e-5, 2 x the float32
     restatement's error)."""
-    pol, z = shipped_ppo("policy")
+    pol, _ = shipped_ppo("policy")
     old, _ = shipped_ppo("policy_old")
-    adam = ({k: z["adam_m/" + k] for k in pol}, {k: z["adam_v/" + k] for k in pol}, (float(z["beta1_power"]), float(z["beta2_power"])))
-    m = make_ppo(tmp_path, pol, old)
+    adam = shipped_adam()
+    m = make_ppo(tmp_path, REFERENCE, pol, old)
     m.set_weights(pol, old, *adam)
     T = int(np.sum(lengths))
     s, a, r, v, _, perms = baseline_config3(T, E)
@@ -147,8 +90,11 @@ def test_learn_segments_match_the_oracle(tmp_path, lengths, E, B):
     boot = np.random.RandomState(6).randn(len(lengths)).astype(np.float32)
     metrics = m.learn(s, a, v, r, d, boot, num_epochs=E, batch_size=B, perms=perms, return_metrics=True,
                       segment_lengths=lengths)
-    p64, rec64 = _oracle_learn_segments(pol, adam, s, a, v, r, d, boot, lengths, E, B, perms, np.float64)
-    p32, rec32 = _oracle_learn_segments(pol, adam, s, a, v, r, d, boot, lengths, E, B, perms, np.float32)
+    p64, _, rec64, _ = restate((LOW, HIGH), pol, adam, (s, a, r, v, d), perms, B, np.float64, segment_lengths=lengths,
+                               bootstrap_values=boot)
+    p32, _, rec32, _ = restate((LOW, HIGH), pol, adam, (s, a, r, v, d), perms, B, np.float32, segment_lengths=lengths,
+                               bootstrap_values=boot)
+    rec64, rec32 = rec64[:, :5], rec32[:, :5]
     got = m.get_weights()
     for name in p64:
         gate = max(TOL, 2 * rel_l2(p32[name], p64[name]))
@@ -162,23 +108,6 @@ def test_learn_segments_match_the_oracle(tmp_path, lengths, E, B):
 
 
 # ------------------------------------------------------------------------------------------------ batched encode + predict
-def _fake_envs(n):
-    rgb, _ = committed_frames()
-    envs = []
-    for i in range(n):
-        v = types.SimpleNamespace(control=types.SimpleNamespace(steer=0.1 * (i % 7) - 0.3, throttle=0.05 * (i % 11)),
-                                  get_speed=(lambda s=0.37 * i: s))
-        envs.append(types.SimpleNamespace(observation=rgb[(5 * i) % len(rgb)], vehicle=v))
-    return envs
-
-
-def _vae(tmp_path, kind):
-    if kind == "conv":
-        return make_conv_vae(tmp_path, shipped_vae_weights()[0], loss="bce", tag="vae", training=False)
-    enc, dec = (96, 256, 64), (160, 64)
-    return make_mlp(tmp_path, mlp_weights(2, encoder_sizes=enc, decoder_sizes=dec), enc, dec, tag="vec", training=False)
-
-
 def _oracle_mean(vae, kind, frames):
     x = frames.astype(np.float64) / 255.0
     if kind == "conv":
@@ -200,7 +129,7 @@ def test_batched_encode_predict(tmp_path, lib, n, kind, mode):
     from oracle import ppo_oracle as po
     from helpers import Box
     with math_mode(lib, mode):
-        vae = _vae(tmp_path, kind)
+        vae = actor_vae(tmp_path, kind)
         meas = ("steer", "throttle", "speed")
         models = []
         for tag in ("fused", "unfused"):
@@ -208,7 +137,7 @@ def test_batched_encode_predict(tmp_path, lib, n, kind, mode):
             m.init_session(init_logging=False)
             m.set_weights(shipped_ppo("policy")[0])
             models.append(m)
-        envs = _fake_envs(n)
+        envs = fake_envs(n)
         fs, fa, fv = FusedActor(vae, models[0], meas).encode_predict(envs)
         us, ua, uv = UnfusedActor(vae, models[1], meas).encode_predict(envs)
         assert len(fs) == n and fa.shape == (n, 2) and fv.shape == (n,)
@@ -247,12 +176,12 @@ def test_one_environment_reproduces_the_loop_before_num_envs(tmp_path):
     import single_env_train
     a, env_a = _train(tmp_path, "vec1", 1)
     b, env_b = _train(tmp_path, "old1", 1, fn=single_env_train.train_one_env)
-    sa, sb = _state(a), _state(b)
+    sa, sb = model_state(a), model_state(b)
     assert all(np.array_equal(sa[k], sb[k]) for k in sa)
     assert a.reward_history == b.reward_history and a.get_train_step_idx() == b.get_train_step_idx() > 0
     assert a.predict_step_counter == b.predict_step_counter and env_a[0].step_count == env_b[0].step_count
     c, _ = _train(tmp_path, "vec1_again", 1)
-    assert all(np.array_equal(sa[k], x) for k, x in _state(c).items()) and c.reward_history == a.reward_history
+    assert all(np.array_equal(sa[k], x) for k, x in model_state(c).items()) and c.reward_history == a.reward_history
 
 
 def test_four_environments(tmp_path):

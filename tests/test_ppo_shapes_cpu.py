@@ -8,8 +8,8 @@ import pytest
 
 from harness import lib, library_state  # noqa: F401
 from helpers import Box, rel_l2
-from ppo_cases import (CASES, CLIPPED, KINK_MARGIN, bounds, clip_groups, init_params, make_batch, ppo_config,
-                       pre_activations, relu_margin)
+from ppo_cases import CASES, CLIPPED, KINK_MARGIN, bounds, clip_groups, make_batch, ppo_config, shape_net
+from ppo_restatement import init_params, pre_activations, relu_margin
 
 # ------------------------------------------------------------------------------------------------------------ tests
 @pytest.mark.parametrize("case", list(CASES))
@@ -19,7 +19,7 @@ def test_oracle_backward_matches_autograd_with_clipped_rows(case):
     from oracle import ppo_oracle as po, torch_ref as tr
     S, A, H1, H2 = CASES[case]
     low, high = bounds(A)
-    p, old, s, a, ret, adv = make_batch(init_params(S, A, H1, H2, seed=3), 128, seed=4, **CLIPPED)
+    p, old, s, a, ret, adv = make_batch(shape_net(S, A, H1, H2), 128, 4, init_seed=3, **CLIPPED)
     ref = po.loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
     auto = tr.ppo_loss_and_grads(p, old, s, a, ret, adv, low, high, 0.2, 1.0, 0.01)
     groups = clip_groups(ref["ratio"], adv)
@@ -42,7 +42,7 @@ def test_initialiser_follows_the_ppo_class(tmp_path, case):
     m = PPO((S,), Box(*bounds(A)), model_dir=str(tmp_path / "ppo"), seed=7)
     shapes = param_shapes(S, A, (H1, H2), (H1, H2))
     m._names, m._shapes = list(shapes), dict(shapes)
-    got, ref = m._initial_weights(), init_params(S, A, H1, H2, seed=7)
+    got, ref = m._initial_weights(), init_params(*shape_net(S, A, H1, H2), seed=7)
     assert list(got) == list(ref)
     for k in ref:
         assert got[k].dtype == ref[k].dtype and np.array_equal(got[k], ref[k]), k
@@ -50,9 +50,8 @@ def test_initialiser_follows_the_ppo_class(tmp_path, case):
 
 @pytest.mark.parametrize("case", list(CASES))
 def test_biases_keep_pre_activations_off_the_relu_kink(case):
-    S, A, H1, H2 = CASES[case]
     for batch in (1, 9, 256):
-        p, _, s = make_batch(init_params(S, A, H1, H2), batch, seed=batch)[:3]
+        p, _, s = make_batch(shape_net(*CASES[case]), batch, batch, init_seed=0)[:3]
         assert relu_margin(p, s) > KINK_MARGIN, batch
         if batch >= 4:                                          # every unit active on some rows and off on others
             for z in pre_activations(p, s):
