@@ -107,8 +107,22 @@ class PpoLearnOptions(C.Structure):
     _fields_ = [("max_grad_norm", C.c_float), ("target_kl", C.c_float)]
 
 
+class RunningNorm(C.Structure):
+    """cpb_running_norm: the statistics' width, the clip and the epsilon under the square root."""
+    _fields_ = [("dim", C.c_int32), ("clip", C.c_float), ("epsilon", C.c_double)]
+
+
+class ActorNorm(C.Structure):
+    """cpb_actor_norm: the normalisation of one actor call (rewards = None: no rewards this step)."""
+    _fields_ = [("obs", RunningNorm), ("obs_stats", C.c_void_p), ("update", C.c_int32), ("reward", RunningNorm),
+                ("ret_stats", C.c_void_p), ("returns", C.c_void_p), ("env_ids", C.c_void_p), ("rewards", C.c_void_p),
+                ("dones", C.c_void_p), ("num_envs", C.c_int32), ("gamma", C.c_double), ("rewards_out", C.c_void_p)]
+
+
 _P = C.c_void_p
 _i32, _i64, _f32, _f64 = C.c_int32, C.c_int64, C.c_float, C.c_double
+_RN = C.POINTER(RunningNorm)
+_AN = C.POINTER(ActorNorm)
 _VC = C.POINTER(VaeConfig)
 _VS = C.POINTER(VaeSpec)
 _MC = C.POINTER(MlpVaeConfig)
@@ -224,6 +238,17 @@ PROTOTYPES = {
                                                    _i64, _P]),
     "cpb_mlpvae_ppo_cat_encode_predict": (_i32, [_MS, _P, _P, _P, _i32, _PK, _P, _P, _P, _P, _P, _P, _P, _P, _i64, _P,
                                                  _i64, _P]),
+    "cpb_running_norm_init": (_i32, [_RN, _P, _P]),
+    "cpb_obs_normalize": (_i32, [_RN, _P, _P, _i32, _i32, _P, _P]),
+    "cpb_reward_normalize": (_i32, [_RN, _P, _P, _P, _P, _P, _i32, _i32, _f64, _P, _P]),
+    "cpb_vae_spec_ppo_spec_encode_predict_norm": (_i32, [_VS, _P, _P, _P, _i32, _PS, _P, _P, _P, _P, _P, _P, _P, _P, _i64,
+                                                         _P, _i64, _P, _AN]),
+    "cpb_mlpvae_ppo_spec_encode_predict_norm": (_i32, [_MS, _P, _P, _P, _i32, _PS, _P, _P, _P, _P, _P, _P, _P, _P, _i64,
+                                                       _P, _i64, _P, _AN]),
+    "cpb_vae_spec_ppo_cat_encode_predict_norm": (_i32, [_VS, _P, _P, _P, _i32, _PK, _P, _P, _P, _P, _P, _P, _P, _P, _i64,
+                                                        _P, _i64, _P, _AN]),
+    "cpb_mlpvae_ppo_cat_encode_predict_norm": (_i32, [_MS, _P, _P, _P, _i32, _PK, _P, _P, _P, _P, _P, _P, _P, _P, _i64,
+                                                      _P, _i64, _P, _AN]),
     "cpb_set_math_mode": (_i32, [_i32]),
     "cpb_debug_vae_buffer_offsets": (_i32, [_i32, _i32, _i32, _i32, _P, _i32]),
     "cpb_debug_vae_spec_buffer_offsets": (_i32, [_VS, _i32, _P, _i32]),

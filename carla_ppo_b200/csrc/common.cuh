@@ -101,6 +101,13 @@ inline int32_t ppo_spec_of(const cpb_ppo_config* c, cpb_ppo_spec* sp) {
     return CPB_OK;
 }
 
+// ---- the normalisation half of an actor call (vecnorm.cu) -----------------------------------
+int32_t check_actor_norm(const cpb_actor_norm* n, int32_t state_dim, int32_t batch);   // before anything is enqueued
+// the state [B, z + m] of latent [B, z] | meas [B, m], normalised, in place of assemble_state_kernel
+int32_t launch_actor_obs_norm(const cpb_actor_norm* n, const float* latent, int z, const float* meas, int m, int batch,
+                              float* state, cudaStream_t stream);
+int32_t launch_actor_reward_norm(const cpb_actor_norm* n, int batch, cudaStream_t stream);   // nothing when n->rewards == NULL
+
 // ---- device helpers -------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {

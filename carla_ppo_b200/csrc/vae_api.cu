@@ -1417,12 +1417,14 @@ typedef int32_t (*EncodeMeanFn)(const void* vae, const float* params, const void
 
 // The encode_predict entry points: `encode` on the VAE described by `vae` (whose common part is `base`), then the state
 // assembly and the PPO forward, with the Gaussian head of ppo_spec or (cat_spec != NULL) the categorical head of
-// cat_spec.  The PPO spec is checked before anything is enqueued.
+// cat_spec.  The PPO spec is checked before anything is enqueued.  with_norm (the *_norm twins): `norm` is checked too,
+// the state is assembled normalised (vecnorm.cu) and, when it carries rewards, the reward path runs after the forward.
 static int32_t encode_predict(const cpb_vae_config* base, const void* vae, EncodeMeanFn encode, const float* vae_params,
                               const void* frames, const float* measurements, int32_t num_measurements, const cpb_ppo_spec* ppo_spec,
                               const cpb_ppo_cat_spec* cat_spec, const float* ppo_params, const float* noise, float* latent_tmp,
                               float* state, float* action, float* value, int32_t* flags, void* vae_workspace,
-                              int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream) {
+                              int64_t vae_workspace_bytes, void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream,
+                              bool with_norm = false, const cpb_actor_norm* norm = nullptr) {
     if (cat_spec != nullptr) ppo_spec = &cat_spec->spec;
     CPB_REQUIRE(base && ppo_spec && frames && latent_tmp && state && action && value, "encode_predict: NULL pointer");
     CPB_REQUIRE(num_measurements >= 0 && (num_measurements == 0 || measurements != nullptr), "encode_predict: bad measurements");
@@ -1431,13 +1433,20 @@ static int32_t encode_predict(const cpb_vae_config* base, const void* vae, Encod
     if (ppo_tensors < 0) return ppo_tensors;
     CPB_REQUIRE(ppo_spec->base.state_dim == base->z_dim + num_measurements, "encode_predict: state_dim %d != z_dim %d + %d measurements",
                 ppo_spec->base.state_dim, base->z_dim, num_measurements);
+    if (with_norm) CPB_TRY(check_actor_norm(norm, ppo_spec->base.state_dim, B));
     CPB_TRY(encode(vae, vae_params, frames, latent_tmp, flags, vae_workspace, vae_workspace_bytes, stream));
-    const int total = B * ppo_spec->base.state_dim;
-    assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, base->z_dim, num_measurements, state);
-    CPB_LAUNCHED();
+    if (with_norm) {
+        CPB_TRY(launch_actor_obs_norm(norm, latent_tmp, base->z_dim, measurements, num_measurements, B, state, (cudaStream_t)stream));
+    } else {
+        const int total = B * ppo_spec->base.state_dim;
+        assemble_state_kernel<<<cdiv(total, 128), 128, 0, (cudaStream_t)stream>>>(latent_tmp, measurements, B, base->z_dim, num_measurements, state);
+        CPB_LAUNCHED();
+    }
     if (cat_spec != nullptr)
-        return cpb_ppo_cat_forward(cat_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
-    return cpb_ppo_spec_forward(ppo_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream);
+        CPB_TRY(cpb_ppo_cat_forward(cat_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream));
+    else
+        CPB_TRY(cpb_ppo_spec_forward(ppo_spec, ppo_params, state, B, noise, action, value, ppo_workspace, ppo_workspace_bytes, stream));
+    return with_norm ? launch_actor_reward_norm(norm, B, (cudaStream_t)stream) : CPB_OK;
 }
 
 int32_t cpb_vae_spec_encode_predict(const cpb_vae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
@@ -1476,6 +1485,24 @@ int32_t cpb_vae_spec_ppo_cat_encode_predict(const cpb_vae_spec* spec, const floa
     return encode_predict(spec ? &spec->base : nullptr, spec, conv_encode_mean, vae_params, frames, measurements, num_measurements,
                           nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
                           vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_vae_spec_ppo_spec_encode_predict_norm(const cpb_vae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
+        int32_t num_measurements, const cpb_ppo_spec* ppo_spec, const float* ppo_params, const float* noise, float* latent_tmp,
+        float* state, float* action, float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+        void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, conv_encode_mean, vae_params, frames, measurements, num_measurements,
+                          ppo_spec, nullptr, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream, true, norm);
+}
+
+int32_t cpb_vae_spec_ppo_cat_encode_predict_norm(const cpb_vae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
+        int32_t num_measurements, const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params, const float* noise, float* latent_tmp,
+        float* state, float* action, float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+        void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, conv_encode_mean, vae_params, frames, measurements, num_measurements,
+                          nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream, true, norm);
 }
 
 static int64_t frame_bytes(const cpb_vae_spec* spec, int dtype, int channels) {
@@ -1756,6 +1783,24 @@ int32_t cpb_mlpvae_ppo_cat_encode_predict(const cpb_mlpvae_spec* spec, const flo
     return encode_predict(spec ? &spec->base : nullptr, spec, mlp_encode_mean, vae_params, frames, measurements, num_measurements,
                           nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
                           vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream);
+}
+
+int32_t cpb_mlpvae_ppo_spec_encode_predict_norm(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
+        int32_t num_measurements, const cpb_ppo_spec* ppo_spec, const float* ppo_params, const float* noise, float* latent_tmp,
+        float* state, float* action, float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+        void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, mlp_encode_mean, vae_params, frames, measurements, num_measurements,
+                          ppo_spec, nullptr, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream, true, norm);
+}
+
+int32_t cpb_mlpvae_ppo_cat_encode_predict_norm(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames, const float* measurements,
+        int32_t num_measurements, const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params, const float* noise, float* latent_tmp,
+        float* state, float* action, float* value, int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
+        void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm) {
+    return encode_predict(spec ? &spec->base : nullptr, spec, mlp_encode_mean, vae_params, frames, measurements, num_measurements,
+                          nullptr, ppo_spec, ppo_params, noise, latent_tmp, state, action, value, flags, vae_workspace,
+                          vae_workspace_bytes, ppo_workspace, ppo_workspace_bytes, stream, true, norm);
 }
 
 /* The two-per-side entry points: the spec entry points on {enc1, enc2} / {dec1, dec2} */

@@ -26,6 +26,11 @@ Discrete action spaces (an addition: the reference's policy is always the tanh-s
 components of 2 to 64 categories, 64 in all.  The policy head is then a categorical distribution per component
 (cpb_ppo_cat_* entry points, include/carla_ppo_b200.h "Categorical policies"); actions are int64 indices, ``predict``
 samples with [B, K] uniforms, and checkpoints record the categories (``checkpoint_action_categories``).
+
+Running normalisation (an addition, Stable-Baselines3's VecNormalize): ``normalize_observations`` /
+``normalize_rewards`` (with ``clip_obs``, ``clip_reward`` and ``reward_gamma``) give the agent a ``vec_normalize``
+(vec_normalize.py) that the actors use to normalise the states and rewards the agent sees.  The checkpoint carries its
+statistics (``vec_normalize/*``), and one whose settings differ from the agent's is refused.
 """
 from __future__ import annotations
 
@@ -38,6 +43,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import CpbError, PpoCatSpec, PpoConfig, PpoSpec
+from .vec_normalize import VecNormalize, blob_normalization
 
 ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8
 _METRIC_NAMES = ("train_loss/policy", "train_loss/value", "train_loss/entropy", "train_loss/loss", "train/prob_ratio")
@@ -164,6 +170,16 @@ def checkpoint_architecture(checkpoint_dir):
     return None if blob is None else blob_architecture(blob)
 
 
+def checkpoint_normalization(checkpoint_dir):
+    """(normalize_observations, normalize_rewards, clip_obs, clip_reward) of the latest checkpoint in checkpoint_dir,
+    (False, False, None, None) for one without normalisation, None when there is no checkpoint."""
+    prefix = _latest_checkpoint_prefix(checkpoint_dir)
+    blob = _read_blob(prefix) if prefix is not None else None
+    if blob is None:
+        return None
+    return blob_normalization(blob) or (False, False, None, None)
+
+
 def checkpoint_action_categories(checkpoint_dir):
     """The action categories of the latest checkpoint in checkpoint_dir: a tuple for a categorical agent, () for a
     Gaussian one, None when there is no checkpoint.  Raises ValueError like blob_action_categories."""
@@ -175,7 +191,8 @@ def checkpoint_action_categories(checkpoint_dir):
 class PPO:
     def __init__(self, input_shape, action_space, learning_rate=3e-4, lr_decay=0.998, epsilon=0.2,
                  value_scale=0.5, entropy_scale=0.01, initial_std=0.4, model_dir="./", seed=None, device=None,
-                 policy_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN, value_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN):
+                 policy_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN, value_hidden_sizes=_lib.PPO_DEFAULT_HIDDEN,
+                 normalize_observations=False, normalize_rewards=False, clip_obs=10.0, clip_reward=10.0, reward_gamma=0.99):
         self.policy_hidden_sizes = tuple(int(v) for v in policy_hidden_sizes)
         self.value_hidden_sizes = tuple(int(v) for v in value_hidden_sizes)
         for name, sizes in (("policy_hidden_sizes", self.policy_hidden_sizes), ("value_hidden_sizes", self.value_hidden_sizes)):
@@ -186,6 +203,9 @@ class PPO:
             raise ValueError("PPO expects a flat state vector (reference train.py:85 builds [z_dim + measurements])")
         self.input_shape = input_shape
         self.state_dim = input_shape[0]
+        # the running normalisation of the states and rewards the agent sees (None: off, the reference's)
+        self.vec_normalize = (VecNormalize(self.state_dim, normalize_observations, normalize_rewards, clip_obs, clip_reward,
+                                           reward_gamma) if normalize_observations or normalize_rewards else None)
         self.action_categories = action_categories(action_space)     # None: the reference's Gaussian over a Box
         if self.action_categories is not None:
             self.num_actions = len(self.action_categories)
@@ -283,6 +303,8 @@ class PPO:
         w = self._initial_weights()
         self.set_weights(w, w)
         self._sync_lr()
+        if self.vec_normalize is not None:
+            self.vec_normalize.init_session(torch, lib, dev, self._stream)
         self.sess = self
         if init_logging:
             try:
@@ -423,6 +445,8 @@ class PPO:
             blob[key] = np.asarray(sizes, np.int32)
         if self.action_categories is not None:
             blob[CATEGORIES_KEY] = np.asarray(self.action_categories, np.int32)
+        if self.vec_normalize is not None:
+            blob.update(self.vec_normalize.state_dict())
         if tf_format:
             from .tf_bundle import write_bundle
             write_bundle(prefix, {k: np.asarray(v) for k, v in blob.items()})
@@ -465,7 +489,8 @@ class PPO:
             return False
 
     def load_blob(self, blob):
-        """Restore from a checkpoint's variables; a checkpoint of another architecture is refused (ValueError)."""
+        """Restore from a checkpoint's variables; a checkpoint of another architecture, action space or normalisation
+        setting is refused (ValueError)."""
         found = blob_architecture(blob)
         if found != self.architecture:
             raise ValueError("checkpoint architecture %s does not match this PPO's %s" % (_fmt(found), _fmt(self.architecture)))
@@ -473,6 +498,12 @@ class PPO:
         if cats != (self.action_categories or ()):
             kind = lambda c: "categories %r" % (c,) if c else "a Gaussian policy"
             raise ValueError("the checkpoint has %s, this PPO %s" % (kind(cats), kind(self.action_categories)))
+        found_norm = blob_normalization(blob)
+        mine = None if self.vec_normalize is None else self.vec_normalize.settings
+        if found_norm != mine:
+            kind = lambda n: ("no normalisation" if n is None else "normalize_observations=%s, normalize_rewards=%s, "
+                              "clip_obs=%g, clip_reward=%g" % n)
+            raise ValueError("the checkpoint has %s, this PPO %s" % (kind(found_norm), kind(mine)))
         pol = {n: blob["policy/" + n] for n in self._names}
         old = {n: blob["policy_old/" + n] for n in self._names}
         m_ = v_ = pw = None
@@ -481,6 +512,8 @@ class PPO:
             v_ = {n: blob["policy/%s/Adam_1" % n] for n in self._names}
             pw = (float(blob["beta1_power"]), float(blob["beta2_power"]))
         self.set_weights(pol, old, m_, v_, pw)
+        if self.vec_normalize is not None:
+            self.vec_normalize.load_state_dict(blob)
         for attr in ("episode_counter", "train_step_counter", "predict_step_counter"):
             if attr in blob:
                 setattr(self, attr, int(blob[attr]))

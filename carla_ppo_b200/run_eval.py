@@ -9,28 +9,39 @@ import numpy as np
 
 
 def load_model(input_shape, action_space, model_dir):
-    """The PPO of model_dir, built at its latest checkpoint's architecture (the reference's 500, 300 when there is none)
-    and action space (a MultiDiscrete of its recorded categories for a categorical agent, else ``action_space``), and
-    restored from it (``load_latest_checkpoint``'s result is printed, as in the reference)."""
+    """The PPO of model_dir, built at its latest checkpoint's architecture (the reference's 500, 300 when there is none),
+    action space (a MultiDiscrete of its recorded categories for a categorical agent, else ``action_space``) and running
+    normalisation, and restored from it (``load_latest_checkpoint``'s result is printed, as in the reference).  Its
+    normalisation statistics are frozen (``training`` off)."""
     from ._lib import PPO_DEFAULT_HIDDEN
-    from .ppo import PPO, checkpoint_action_categories, checkpoint_architecture
+    from .ppo import PPO, checkpoint_action_categories, checkpoint_architecture, checkpoint_normalization
     from .replay_env import MultiDiscrete
     arch = checkpoint_architecture("{}/checkpoints/".format(model_dir)) or (PPO_DEFAULT_HIDDEN, PPO_DEFAULT_HIDDEN)
     cats = checkpoint_action_categories("{}/checkpoints/".format(model_dir))
     if cats:
         action_space = MultiDiscrete(cats)
+    norm = checkpoint_normalization("{}/checkpoints/".format(model_dir))
+    norm_kw = {} if not norm or norm[2] is None else dict(normalize_observations=norm[0], normalize_rewards=norm[1],
+                                                          clip_obs=norm[2], clip_reward=norm[3])
     model = PPO(input_shape, action_space, model_dir=model_dir, seed=0, policy_hidden_sizes=arch[0],
-                value_hidden_sizes=arch[1])
+                value_hidden_sizes=arch[1], **norm_kw)
     model.init_session(init_logging=False)
     model.load_latest_checkpoint()
+    if model.vec_normalize is not None:
+        model.vec_normalize.training = False
     return model
 
 
 def run_eval(env, model, video_filename=None, actor=None):
     """One greedy episode (std = 0, run_eval.py:51); returns the total reward.  ``actor`` (FusedActor, optional) serves
-    the per-step encode + predict in one C call."""
+    the per-step encode + predict in one C call.  The model's normalisation statistics (if any) are frozen for the
+    episode, and the reward it returns is raw."""
+    norm = getattr(model, "vec_normalize", None)
+    training = norm is not None and norm.training
     if actor is not None:
         actor.greedy = True
+    if norm is not None:
+        norm.training = False
     try:
         state, terminal, total_reward = env.reset(is_training=False), False, 0
         rendered_frame = env.render(mode="rgb_array")
@@ -61,6 +72,8 @@ def run_eval(env, model, video_filename=None, actor=None):
     finally:
         if actor is not None:
             actor.greedy = False
+        if norm is not None:
+            norm.training = training
 
 
 def main(argv=None):
@@ -88,18 +101,18 @@ def main(argv=None):
     vae = load_vae(args.vae_model, args.vae_z_dim, args.vae_model_type)
     measurements_to_include = set(["steer", "throttle", "speed"])
     obs_res = (vae.source_shape[1], vae.source_shape[0])                  # (width, height) of the frames the VAE takes
-    env = ReplayEnv(load_replay_frames(args.replay_data), obs_res=obs_res, action_smoothing=args.action_smoothing,
-                    encode_state_fn=create_encode_state_fn(vae, measurements_to_include), reward_fn=reward_functions[args.reward_fn],
-                    synchronous=args.synchronous, fps=args.fps, start_carla=False)
-    np.random.seed(0)
-    env.seed(0)
+    frames = load_replay_frames(args.replay_data)
     input_shape = np.array([vae.z_dim + len(measurements_to_include)])
-    model = load_model(input_shape, env.action_space, os.path.join(args.models_root, args.model_name))
-    if model.action_categories is not None:          # drive the environment with the checkpoint's discrete controls
-        env = ReplayEnv(env.frames, obs_res=obs_res, action_smoothing=args.action_smoothing,
-                        encode_state_fn=env.encode_state_fn, reward_fn=env.reward_fn, synchronous=args.synchronous,
-                        fps=args.fps, start_carla=False, discrete_actions=model.action_categories)
-        env.seed(0)
+    # the model first: its action space picks the environment's controls, its normaliser the states' encoding
+    from .replay_env import Box
+    model = load_model(input_shape, Box(ReplayEnv.action_space_box_low, ReplayEnv.action_space_box_high),
+                       os.path.join(args.models_root, args.model_name))
+    np.random.seed(0)
+    env = ReplayEnv(frames, obs_res=obs_res, action_smoothing=args.action_smoothing,
+                    encode_state_fn=create_encode_state_fn(vae, measurements_to_include, model.vec_normalize),
+                    reward_fn=reward_functions[args.reward_fn], synchronous=args.synchronous, fps=args.fps,
+                    start_carla=False, discrete_actions=model.action_categories)
+    env.seed(0)
     actor = None
     if not args.unfused:
         actor = FusedActor(vae, model, measurements_to_include)

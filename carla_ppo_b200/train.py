@@ -15,6 +15,9 @@ hyper-parameter flags and TensorBoard tags, with the neural work on the H100 lib
                              stopping) on the device, in both the learn and the --reference_loop path; off by default
   * ``--discrete_actions N_STEER N_THROTTLE``: a categorical policy over N_STEER x N_THROTTLE evenly spaced controls
                              (a MultiDiscrete action space) instead of the reference's Gaussian over the Box; off by default
+  * ``--normalize_observations`` / ``--normalize_rewards``: Stable-Baselines3's VecNormalize on the device (running
+                             statistics of the states and of the discounted return); the rollout stores the normalised
+                             states and rewards, the logged rewards stay raw; off by default
 """
 from __future__ import annotations
 
@@ -25,7 +28,7 @@ import shutil
 import numpy as np
 
 from ._lib import PPO_DEFAULT_HIDDEN
-from .ppo import PPO, action_categories, checkpoint_action_categories, checkpoint_architecture
+from .ppo import PPO, action_categories, checkpoint_action_categories, checkpoint_architecture, checkpoint_normalization
 from .replay_env import ReplayEnv, reward_functions
 from .run_eval import run_eval
 from .utils import compute_gae
@@ -75,6 +78,20 @@ def resolve_action_categories(flag, checkpoint_cats):
                          "start over)" % (" ".join(map(str, given)),
                                           "categories " + " ".join(map(str, ckpt)) if ckpt else "a Gaussian policy"))
     return ckpt
+
+
+def resolve_normalization(normalize_observations, normalize_rewards, checkpoint_norm):
+    """(normalize_observations, normalize_rewards) of a run: the checkpoint's when resuming one (a flag the checkpoint
+    does not have is an error), else the flags.  checkpoint_norm: checkpoint_normalization's result.  Raises ValueError
+    on a disagreement."""
+    if checkpoint_norm is None:
+        return bool(normalize_observations), bool(normalize_rewards)
+    for flag, given, ckpt in (("--normalize_observations", normalize_observations, checkpoint_norm[0]),
+                              ("--normalize_rewards", normalize_rewards, checkpoint_norm[1])):
+        if given and not ckpt:
+            raise ValueError("%s disagrees with the checkpoint being resumed, which was trained without it (pass -restart "
+                             "to start over)" % flag)
+    return bool(checkpoint_norm[0]), bool(checkpoint_norm[1])
 
 
 def train(params, start_carla=False, restart=False, env=None, vae=None, models_root="models", interactive=True):
@@ -149,11 +166,18 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     policy_sizes, value_sizes = resolve_architecture(params.get("policy_hidden_sizes"), params.get("value_hidden_sizes"),
                                                      None if restart else checkpoint_architecture("{}/checkpoints/".format(model_dir)))
     params["policy_hidden_sizes"], params["value_hidden_sizes"] = list(policy_sizes), list(value_sizes)
+    # a resumed run takes its checkpoint's normalisation; a flag the checkpoint does not have is an error
+    ckpt_norm = None if restart else checkpoint_normalization("{}/checkpoints/".format(model_dir))
+    norm_obs, norm_reward = resolve_normalization(params.get("normalize_observations"), params.get("normalize_rewards"),
+                                                  ckpt_norm)
+    params["normalize_observations"], params["normalize_rewards"] = norm_obs, norm_reward
+    clips = {} if not ckpt_norm or ckpt_norm[2] is None else dict(clip_obs=ckpt_norm[2], clip_reward=ckpt_norm[3])
     print("Creating model")
     model = PPO(input_shape, envs[0].action_space, learning_rate=learning_rate, lr_decay=lr_decay, epsilon=ppo_epsilon,
                 initial_std=initial_std, value_scale=value_scale, entropy_scale=entropy_scale,
                 model_dir=model_dir, seed=seed if isinstance(seed, int) else None,
-                policy_hidden_sizes=policy_sizes, value_hidden_sizes=value_sizes)
+                policy_hidden_sizes=policy_sizes, value_hidden_sizes=value_sizes, normalize_observations=norm_obs,
+                normalize_rewards=norm_reward, reward_gamma=discount_factor, **clips)
     if restart:
         shutil.rmtree(model.model_dir)
         for d in model.dirs:
@@ -166,6 +190,7 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
     # Training steps every environment, then encodes all of their new frames and predicts their actions in one batched
     # call (actor.encode_predict); the environments' own encode_state_fn does nothing meanwhile.  Evaluation runs the
     # single-environment callback on envs[0].
+    normalizer = getattr(model, "vec_normalize", None)
     actor = None
     if fused:
         from .actor import FusedActor
@@ -173,7 +198,8 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
         vec_actor, eval_encode_state_fn = actor, actor.encode_state_fn
     else:
         from .actor import UnfusedActor
-        vec_actor, eval_encode_state_fn = UnfusedActor(vae, model, measurements_to_include), create_encode_state_fn(vae, measurements_to_include)
+        vec_actor = UnfusedActor(vae, model, measurements_to_include)
+        eval_encode_state_fn = create_encode_state_fn(vae, measurements_to_include, normalizer)
     for e in envs:
         e.encode_state_fn = _deferred_encode
 
@@ -229,18 +255,26 @@ def train(params, start_carla=False, restart=False, env=None, vae=None, models_r
             rollout = {i: ([], [], [], [], []) for i in active}      # states, taken_actions, values, rewards, dones
             for _ in range(horizon):
                 log_sampled_actions([action[i] for i in active])
-                stepped, terminal = list(active), {}
+                stepped, terminal, raw = list(active), {}, {}
                 for i in stepped:
-                    _, reward, terminal[i], info = envs[i].step(action[i])
+                    _, raw[i], terminal[i], info = envs[i].step(action[i])
                     if info["closed"]:
                         return model
                     envs[i].extra_info.extend(["Episode {}".format(episode_idx), "Training...", "", "Value:  % 20.2f" % value[i]])
                     envs[i].render()
-                    total_reward[i] += reward
-                    for buf, x in zip(rollout[i], (state[i], action[i], value[i], reward, terminal[i])):
+                    total_reward[i] += raw[i]
+                    for buf, x in zip(rollout[i], (state[i], action[i], value[i])):
                         buf.append(x)
-                new_state, new_action, new_value = vec_actor.encode_predict([envs[i] for i in stepped])
+                if normalizer is None:
+                    new_state, new_action, new_value = vec_actor.encode_predict([envs[i] for i in stepped])
+                    reward = [raw[i] for i in stepped]
+                else:                                  # the rewards the agent sees: normalised in the same call
+                    new_state, new_action, new_value, reward = vec_actor.encode_predict(
+                        [envs[i] for i in stepped], [raw[i] for i in stepped], [terminal[i] for i in stepped], stepped)
+                    reward = [float(r) for r in reward]
                 for j, i in enumerate(stepped):
+                    rollout[i][3].append(reward[j])
+                    rollout[i][4].append(terminal[i])
                     state[i], action[i], value[i] = new_state[j], new_action[j], new_value[j]
                 active = [i for i in stepped if not terminal[i]]
                 if not active:
@@ -343,6 +377,12 @@ def main(argv=None):
     parser.add_argument("--value_hidden_sizes", type=int, nargs="+", default=None, metavar="WIDTH",
                         help="hidden-layer widths of the value network, 1 to 8 of them (default: 500 300, or the "
                         "checkpoint's when resuming)")
+    parser.add_argument("--normalize_observations", action="store_true", help="normalise the states the agent sees with "
+                        "running statistics, like Stable-Baselines3's VecNormalize (default: off, or the checkpoint's "
+                        "setting when resuming)")
+    parser.add_argument("--normalize_rewards", action="store_true", help="scale the rewards the agent learns from by the "
+                        "running standard deviation of the discounted return, like VecNormalize (default: off, or the "
+                        "checkpoint's setting when resuming)")
     params = vars(parser.parse_args(argv))
     start_carla = params.pop("start_carla")
     restart = params.pop("restart")

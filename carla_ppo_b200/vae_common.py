@@ -46,17 +46,18 @@ def _vector(v):
     return np.asarray(v)
 
 
-def create_encode_state_fn(vae, measurements_to_include):
+def create_encode_state_fn(vae, measurements_to_include, normalizer=None):
     """Returns fn(env) -> np.float64[z_dim + M]: VAE mean of the current camera frame with the selected
     measurements appended (vae_common.py:33-62).  A uint8 observation is uploaded as uint8 and scaled by
-    1/255 inside the conv1 loader -- numerically the same as preprocess_frame followed by a float feed."""
-    encode_states = create_encode_states_fn(vae, measurements_to_include)
+    1/255 inside the conv1 loader -- numerically the same as preprocess_frame followed by a float feed.
+    ``normalizer`` (a VecNormalize with observation normalisation on): the state is normalised by it, as float32."""
+    encode_states = create_encode_states_fn(vae, measurements_to_include, normalizer)
     return lambda env: encode_states([env])[0]
 
 
-def create_encode_states_fn(vae, measurements_to_include):
+def create_encode_states_fn(vae, measurements_to_include, normalizer=None):
     """create_encode_state_fn for several environments: fn(envs) -> [state of envs[i]], with ONE vae.encode on all their
-    frames."""
+    frames (and one normalizer.normalize_obs on all their states)."""
     measure_flags = ["steer" in measurements_to_include, "throttle" in measurements_to_include,
                      "speed" in measurements_to_include, "orientation" in measurements_to_include]
 
@@ -73,6 +74,8 @@ def create_encode_states_fn(vae, measurements_to_include):
             if measure_flags[2]: measurements.append(env.vehicle.get_speed())
             if measure_flags[3]: measurements.extend(_vector(env.vehicle.get_forward_vector()))
             states.append(np.append(encoded_state, measurements))
+        if normalizer is not None and normalizer.norm_obs:
+            states = list(normalizer.normalize_obs(np.stack(states)))
         return states
 
     return encode_states

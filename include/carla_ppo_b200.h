@@ -683,6 +683,93 @@ int32_t cpb_mlpvae_ppo_cat_encode_predict(const cpb_mlpvae_spec* spec, const flo
                                           int32_t* flags, void* vae_workspace, int64_t vae_workspace_bytes,
                                           void* ppo_workspace, int64_t ppo_workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Running normalisation: Stable-Baselines3's VecNormalize (an addition; the reference feeds raw states and rewards).
+ *
+ * Statistics are RunningMeanStd(epsilon=1e-4): a device double[2*dim + 1] = [mean | var | count], initially 0, 1, 1e-4.
+ * Updating them with a batch of n rows computes the batch mean and variance (ddof 0, two-pass) in float64 and merges
+ * them with Chan's formula: delta = mu_b - mu, t = c + n, mu' = mu + delta*n/t,
+ * var' = (var*c + var_b*n + delta^2*c*n/t)/t, c' = t.  Every sum has a fixed order that depends only on the shape, so
+ * equal inputs give bit-identical statistics and outputs.
+ *
+ * cpb_obs_normalize: x [batch, dim] -> out [batch, dim].  With update != 0 the statistics are first updated with the
+ * batch; every row is then normalised with the (updated) statistics, clip((x - mu) / sqrt(var + epsilon), +-clip), in
+ * float64 rounded once to fp32.  With update == 0 the statistics are only read.
+ *
+ * cpb_reward_normalize: the reward path of VecNormalize for the environments env_ids [batch] (distinct, in any order) of
+ * num_envs, with the return statistics ret_stats (dim 1) and the discounted returns `returns` [num_envs] (float64,
+ * caller-owned, start at 0).  For each stepped environment, in this order: returns[e] = returns[e]*gamma + rewards[i];
+ * the statistics are updated with the batch returns[env_ids]; out[i] = clip(rewards[i] / sqrt(var + epsilon), +-clip);
+ * returns[e] = 0 where dones[i] != 0.  env_ids live on the device and are not checked: an id outside [0, num_envs) is
+ * clamped into it.
+ *
+ * Refused with CPB_ERR_INVALID_ARGUMENT before anything is enqueued: a NULL pointer, dim < 1 (a reward config's dim must
+ * be 1), a clip that is <= 0, NaN or infinite, an epsilon that is <= 0 or not finite, gamma outside [0, 1], batch < 1,
+ * num_envs < 1.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t dim;        /* columns of the statistics (1 for the returns) */
+    float clip;         /* clip_obs / clip_reward (SB3's default: 10) */
+    double epsilon;     /* added to var under the square root (SB3's default: 1e-8) */
+} cpb_running_norm;
+
+/* stats [2*dim + 1] <- mean 0, var 1, count 1e-4 (one kernel on `stream`) */
+int32_t cpb_running_norm_init(const cpb_running_norm* cfg, double* stats, void* stream);
+int32_t cpb_obs_normalize(const cpb_running_norm* cfg, double* stats, const float* x, int32_t batch, int32_t update,
+                          float* out, void* stream);
+int32_t cpb_reward_normalize(const cpb_running_norm* cfg, double* ret_stats, double* returns, const int32_t* env_ids,
+                             const float* rewards, const int32_t* dones, int32_t batch, int32_t num_envs, double gamma,
+                             float* out, void* stream);
+
+/* The normalisation of an actor call (the *_encode_predict_norm twins).  `state` then holds the normalised state, made
+ * in the launch that assembles it (no extra launch); with rewards != NULL the reward path of cpb_reward_normalize runs
+ * on the call's batch B (env_ids, rewards, dones and rewards_out are [B]), one launch more.  rewards == NULL: no
+ * rewards this step, and the reward fields are not read. */
+typedef struct {
+    cpb_running_norm obs;       /* obs.dim must be the PPO's state_dim */
+    double* obs_stats;          /* [2*state_dim + 1] */
+    int32_t update;             /* 0: the observation statistics are only read (evaluation) */
+    cpb_running_norm reward;    /* dim 1 */
+    double* ret_stats;          /* [3] */
+    double* returns;            /* [num_envs] */
+    const int32_t* env_ids;     /* [B] */
+    const float* rewards;       /* [B], or NULL */
+    const int32_t* dones;       /* [B] */
+    int32_t num_envs;
+    double gamma;
+    float* rewards_out;         /* [B] */
+} cpb_actor_norm;
+
+/* The four actor entry points above with running normalisation: the same arguments, then `norm`. */
+int32_t cpb_vae_spec_ppo_spec_encode_predict_norm(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                                  const float* measurements, int32_t num_measurements,
+                                                  const cpb_ppo_spec* ppo_spec, const float* ppo_params,
+                                                  const float* noise, float* latent_tmp, float* state, float* action,
+                                                  float* value, int32_t* flags, void* vae_workspace,
+                                                  int64_t vae_workspace_bytes, void* ppo_workspace,
+                                                  int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm);
+int32_t cpb_mlpvae_ppo_spec_encode_predict_norm(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                                const float* measurements, int32_t num_measurements,
+                                                const cpb_ppo_spec* ppo_spec, const float* ppo_params,
+                                                const float* noise, float* latent_tmp, float* state, float* action,
+                                                float* value, int32_t* flags, void* vae_workspace,
+                                                int64_t vae_workspace_bytes, void* ppo_workspace,
+                                                int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm);
+int32_t cpb_vae_spec_ppo_cat_encode_predict_norm(const cpb_vae_spec* spec, const float* vae_params, const void* frames,
+                                                 const float* measurements, int32_t num_measurements,
+                                                 const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params,
+                                                 const float* noise, float* latent_tmp, float* state, float* action,
+                                                 float* value, int32_t* flags, void* vae_workspace,
+                                                 int64_t vae_workspace_bytes, void* ppo_workspace,
+                                                 int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm);
+int32_t cpb_mlpvae_ppo_cat_encode_predict_norm(const cpb_mlpvae_spec* spec, const float* vae_params, const void* frames,
+                                               const float* measurements, int32_t num_measurements,
+                                               const cpb_ppo_cat_spec* ppo_spec, const float* ppo_params,
+                                               const float* noise, float* latent_tmp, float* state, float* action,
+                                               float* value, int32_t* flags, void* vae_workspace,
+                                               int64_t vae_workspace_bytes, void* ppo_workspace,
+                                               int64_t ppo_workspace_bytes, void* stream, const cpb_actor_norm* norm);
+
 #ifdef __cplusplus
 }
 #endif
