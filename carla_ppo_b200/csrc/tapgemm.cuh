@@ -94,10 +94,14 @@ struct TcWeightJob {
     int N, C;                   // logical rows / reduction length per tap
     long long count;
     int round_nearest;          // 0: hi = x truncated to TF32 (3xTF32 split); 1: hi = x rounded to nearest (single pass)
+    int ksplit;                 // nonzero: the image feeds a k-split problem (TapGemmParams::ksplit > 1), see tc_bn
 };
-// rows of the N axis handled per CTA tile (also fixes the block size of the stored operand); at most 64, because each
-// consumer thread holds 1.5 x BN fp32 accumulators plus a k-block's 32 hi / lo A-fragment registers
-__host__ __device__ constexpr int tc_bn(int N) { return N % 64 == 0 ? 64 : 32; }
+// rows of the N axis handled per CTA tile (also fixes the block size of the stored operand).  At BN 32 / 64 a consumer
+// thread holds the tile's running sums in registers next to its two 128-k chunk accumulators; at BN 128 those would
+// not fit beside the chunk accumulators and the 32 hi / lo A-fragment registers, so the running sums live in shared
+// memory (tc_tapgemm_kernel).  K-split problems stay at BN <= 64: their work items are (tile, split) pairs, and the
+// MlpVAE's 512-column layers at B = 512 make 128 of them at BN 64 (132 SMs) but only 64 at BN 128.
+__host__ __device__ constexpr int tc_bn(int N, bool ksplit) { return N % 128 == 0 && !ksplit ? 128 : (N % 64 == 0 ? 64 : 32); }
 constexpr int kMaxTcWeightJobs = 12;
 struct TcWeightTable {
     int njobs;

@@ -24,13 +24,14 @@
 //   * the cross terms (2^-11 of the main term) accumulate in their OWN registers, so they do not re-truncate the
 //     large accumulator;
 //   * wgmma accumulation only runs over chunks of 128 k (4 k-blocks); each finished chunk is added to per-thread fp32
-//     register accumulators (round-to-nearest).
-// The register accumulators are what the bias / ReLU / ReLU-mask epilogue receives.
+//     accumulators (round-to-nearest): registers at BN 32 / 64; at BN 128, where they would not fit beside the chunk
+//     accumulators, the thread's positions of the tile's output buffer in shared memory.
+// These running sums are what the bias / ReLU / ReLU-mask epilogue receives.
 //
 // Single-pass variant (PASSES = 1, math mode 2): a*b ~= rna(a) * rna(b), both operands rounded to the nearest TF32
 // value (the A fragment in registers, the weights by tc_weights_kernel), ONE wgmma per 8-wide k-step into the chunk
 // accumulator, no cross terms; a stage holds A + the hi weight image only.  Relative error ~3e-4 per product, unbiased;
-// the chunked accumulation into fp32 registers is the same as above.
+// the chunked accumulation into fp32 running sums is the same as above.
 #include "tapgemm.cuh"
 #include "tc_common.cuh"
 
@@ -45,11 +46,17 @@ struct TcCfg {
     static constexpr int B_TILE_BYTES = BN * TBK * 4;
     static constexpr int B_IMAGES = PASSES == 3 ? 2 : 1;                    // weight images per k-block: [hi | lo] or [hi]
     static constexpr int STAGE_BYTES = A_TILE_BYTES + B_IMAGES * B_TILE_BYTES;   // raw A rows | weight image(s)
-    static constexpr int OUT_BYTES = TBM * BN * 4;                          // the finished tile's raw sums, for the epilogue warps
-    static constexpr int STAGES = (224 * 1024 - OUT_BYTES) / STAGE_BYTES;   // 3 passes: BN 64: 6, BN 32: 8; 1 pass: 8, 10
+    static constexpr int OUT_BYTES = TBM * BN * 4;                          // the tile's raw sums, for the epilogue warps
+    static constexpr int STAGES = (224 * 1024 - OUT_BYTES) / STAGE_BYTES;   // 3 passes: BN 128 / 64 / 32: 3 / 6 / 8; 1 pass: 5 / 8 / 10
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_BYTES + 1024;   // +1024: manual 1 KB alignment
+    // registers per thread of each warpgroup role.  A 3-pass BN 128 consumer thread holds 128 chunk-accumulator and 32
+    // A-fragment registers; below 192 ptxas serialises its wgmma (C7512).  Its loader and epilogue warpgroups fit in 56
+    // and 72.  Every other instantiation: 168 / 80 / 80.  (The k-split variant runs at BN <= 64 only, see tc_bn.)
+    static constexpr bool WIDE = BN == 128 && PASSES == 3;
+    static constexpr int CONSUMER_REGS = WIDE ? 192 : 168, LOADER_REGS = WIDE ? 56 : 80, EPILOGUE_REGS = WIDE ? 72 : 80;
+    static_assert(256 * CONSUMER_REGS + 128 * (LOADER_REGS + EPILOGUE_REGS) <= 512 * 128, "register file of one CTA");
 };
-constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 register accumulators
+constexpr int CHUNK_KB = 4;   // k-blocks accumulated by the tensor core before adding into the fp32 running sums
 
 constexpr int kConsumerWarps = 8;                     // warps 0-7: two wgmma warpgroups
 constexpr int kLoaderWarp0 = 8;                       // warps 8-11: A loaders (cp.async)
@@ -59,14 +66,14 @@ constexpr int kEpilogueWarp0 = 12;                    // warps 12-15: tile epilo
 constexpr int kEpilogueWarps = 4;
 constexpr int kEpilogueThreads = kEpilogueWarps * 32;
 constexpr int kTcThreads = 512;                       // four warpgroups: setmaxnreg moves registers between whole warpgroups
-// 512 threads start with 128 registers each; the loader and epilogue warpgroups give theirs back down to kSideRegs and
-// the two consumer warpgroups grow to kConsumerRegs: 256 * 168 + 256 * 80 <= 65 536
-constexpr int kLaunchRegs = 128, kConsumerRegs = 168, kSideRegs = 80;
+// 512 threads start with kLaunchRegs registers each; setmaxnreg then shrinks the loader and the epilogue warpgroup and
+// grows the two consumer warpgroups (TcCfg::*_REGS)
+constexpr int kLaunchRegs = 128;
 template <int R> __device__ __forceinline__ void reg_grow() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void reg_shrink() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 int g_tc_cluster = 1;         // CTAs per cluster = multicast width of the weight tiles (CPB_TC_CLUSTER, 1/2/4/8)
-int g_tc_clusters[2][2] = {{0, 0}, {0, 0}};   // co-resident clusters of the persistent grid, per instantiation [passes 3/1][BN 32/64]
+int g_tc_clusters[2][3] = {};   // co-resident clusters of the persistent grid, per instantiation [passes 3/1][BN 32/64/128]
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
@@ -128,9 +135,10 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     // the same offset everywhere -- which the multicast copies rely on
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     // Output buffer (behind the stage ring): the tile's 128 x BN raw fp32 sums, rows of BN * 4 bytes, the 16-byte chunk
-    // index of row r XORed with 2 * (r % 4).  A consumer warp's float2 fragment store covers rows g .. g+3 (per half
+    // index of row r XORed with 2 * (r % 4).  A consumer warp's float2 fragment access covers rows g .. g+3 (per half
     // warp) x 32 bytes at the same columns, which the XOR spreads over all 32 banks; an epilogue thread's float4 read
-    // stays inside one row, whose chunks the XOR only permutes.  Neither access has a bank conflict.
+    // stays inside one row, whose chunks the XOR only permutes.  Neither access has a bank conflict.  At BN 128 the
+    // buffer is also where the consumers keep the running sums while the tile is accumulated.
     const uint32_t out_base = smem_base + STAGES * STAGE_BYTES;
 
     if (tid == 0) {
@@ -153,7 +161,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
     auto split_kb = [&](int nkb, int ks) { return (int)((long long)nkb * ks / ksplit); };
 
     if (warp >= kEpilogueWarp0) {
-        reg_shrink<kSideRegs>();
+        reg_shrink<Cfg::EPILOGUE_REGS>();
         // ================================ tile epilogue ================================
         // The epilogue warps walk the same work items as the consumers.  Thread et owns 16-byte column chunk et % CPR of
         // tile rows et / CPR + RPP * i: a row's BN columns are contiguous in the destination (quad form: each parity
@@ -161,8 +169,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         // destination offsets and the mask's sign bits of item w are computed / fetched while the consumers are still
         // accumulating w; once the sums arrive only shared loads, the arithmetic and the stores remain.
         constexpr int CPR = BN / 4;                        // 16-byte chunks per tile row
-        constexpr int RPP = kEpilogueThreads / CPR;        // tile rows per pass of the four warps: 8 (BN 64) / 16 (BN 32)
-        constexpr int NR = TBM / RPP;                      // rows per thread: 16 / 8
+        constexpr int RPP = kEpilogueThreads / CPR;        // tile rows per pass of the four warps: 4 / 8 / 16 (BN 128 / 64 / 32)
+        constexpr int NR = TBM / RPP;                      // rows per thread: 32 / 16 / 8
         constexpr uint32_t SKIP = 0xffffffffu;             // no destination: row beyond M or quad position outside the image
         const int et = tid - kEpilogueWarp0 * 32;
         const int ec = et % CPR, er = et / CPR;
@@ -266,7 +274,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
             if (lane == 0) mbar_arrive(&out_empty);         // this warp has read its part of the buffer
         }
     } else if (warp >= kLoaderWarp0) {
-        reg_shrink<kSideRegs>();
+        reg_shrink<Cfg::LOADER_REGS>();
         // ================================ A loaders ================================
         // The raw fp32 activation rows are copied global -> swizzled shared memory with cp.async (16 B per thread and
         // row, zero-filled outside the image); the consumers split them into TF32 hi / lo in registers.  Completion is
@@ -400,14 +408,19 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         }
     } else {
         // ================================ wgmma consumers ================================
-        reg_grow<kConsumerRegs>();
+        reg_grow<Cfg::CONSUMER_REGS>();
         // warpgroup wg owns tile rows [64*wg, 64*wg + 64); thread layout of the accumulators: see wgmma_tf32
         constexpr int HALF = BN / 2;                 // accumulator registers per thread for a 64 x BN product
+        constexpr bool SACC = BN == 128;             // the running sums live in the output buffer, not in registers
         const int wg = warp >> 2;
-        float acc[HALF];                             // fp32 register accumulators of the tile (main + cross)
+        float acc[SACC ? 1 : HALF];                  // BN 32 / 64: fp32 register running sums of the tile (main + cross)
         float dm[HALF], dc[HALF];                    // chunk accumulators of the main and the cross terms (3 passes)
 #pragma unroll
-        for (int i = 0; i < HALF; ++i) { acc[i] = 0.f; dm[i] = 0.f; dc[i] = 0.f; }
+        for (int i = 0; i < HALF; ++i) { dm[i] = 0.f; dc[i] = 0.f; }
+        if constexpr (!SACC) {
+#pragma unroll
+            for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
+        }
 
         // stage s is free in this CTA's consumers: lane r < CS arrives on the stage's empty barrier of cluster CTA r
         auto release = [&](int s) {
@@ -420,13 +433,14 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
         // A fragment of this thread (wgmma_tf32_rs): tile rows r0 = 64*wg + 16*(warp%4) + lane/4 and r0 + 8 (the next
         // 1 KB row group), k = lane%4 (+4) of each 8-wide k-step, i.e. 16-byte chunk 2*ks (+1) XOR r0%8 of the row.  The
         // 8 rows a warp reads at once sit in 8 different chunks, so the 32-bit shared loads are bank-conflict free.
+        // a_row addresses chunk 0 XOR r0%8; a stage is 1 KB aligned, so chunk c is (stage + a_row) ^ (c << 4).
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        const uint32_t a_row = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + (lane & 3) * 4);
-        const uint32_t a_swz = (uint32_t)((r0 & 7) << 4);
+        const uint32_t a_row = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128 + ((r0 & 7) << 4) + (lane & 3) * 4);
 
         // The finished tile goes to the epilogue warps through the output buffer: acc[4*j + 2*h + c] is row r0 + 8*h,
         // columns 8*j + 2*(lane%4) + c, i.e. bytes 8*(lane%4) of the 32-byte pair of chunks j XOR r0%4 (layout: see
-        // out_base).  The consumers then go straight on to the next item's first k-block.
+        // out_base).  The consumers then go straight on to the next item's first k-block.  At BN 128 the sums are
+        // already there (same positions) and only the arrival on out_full remains.
         const uint32_t o_dst = (uint32_t)(r0 * (BN * 4) + ((r0 & 3) << 5) + (lane & 3) * 8);
         uint32_t phE = 1;                            // parity out_empty shows once free (fresh barrier: 1 counts as complete)
         auto hand_off = [&]() {
@@ -454,6 +468,8 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                 // the k-block's A fragment, split into TF32 hi / lo: ahi[ks][2*h + v], alo[ks][2*h + v]
                 // (single pass: ahi = the fragment rounded to nearest TF32, no alo)
                 uint32_t ahi[TBK / 8][4], alo[TBK / 8][4];
+                uint32_t a_at = stage + a_row;       // opaque: one XOR per load rather than 8 chunk offsets held in registers
+                asm volatile("" : "+r"(a_at));
 #pragma unroll
                 for (int ks = 0; ks < TBK / 8; ++ks)
 #pragma unroll
@@ -462,7 +478,7 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                         for (int v = 0; v < 2; ++v) {
                             float x;
                             asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
-                                         : "r"(stage + a_row + v * 1024 + ((uint32_t)((2 * ks + h) << 4) ^ a_swz)));
+                                         : "r"((a_at ^ (uint32_t)((2 * ks + h) << 4)) + (uint32_t)(v * 1024)));
                             if constexpr (PASSES == 3) {
                                 float hi, lo;
                                 split_tf32(x, hi, lo);
@@ -505,23 +521,73 @@ tc_tapgemm_kernel(const __grid_constant__ TapGemmParams p, const int mgroups, co
                 if constexpr (PASSES == 3) fence_regs<HALF>(dc);
                 release(s);
                 if (kb % CHUNK_KB == CHUNK_KB - 1 || kb == nkb - 1) {
+                    if constexpr (SACC) {
+                        // read-modify-write of the thread's running sums in the output buffer, eight float2 loads in
+                        // flight at a time.  The item's first chunk writes 0 + chunk (the register sums' first add,
+                        // signed zeros included) once the epilogue warps have read the previous item's sums: a whole
+                        // chunk after the previous item's out_full, which gives them that long to drain the buffer.
+                        const bool first = kb < CHUNK_KB;
+                        if (first && !(p.debug & 16)) {
+                            mbar_wait(&out_empty, phE);
+                            phE ^= 1u;
+                        }
+                        // out_base is 1 KB aligned, so pair j of the thread's row is (out_base + o_dst) ^ (j << 5): one
+                        // XOR per access on a base made opaque here, instead of 16 pair addresses held in registers
+                        // across the k-loop
+                        uint32_t ob = out_base + o_dst;
+                        asm volatile("" : "+r"(ob));
 #pragma unroll
-                    for (int i = 0; i < HALF; ++i) {
-                        acc[i] += dm[i];
-                        if constexpr (PASSES == 3) acc[i] += dc[i];
+                        for (int j0 = 0; j0 < BN / 8; j0 += 4) {
+                            float sum[4][2][2];
+#pragma unroll
+                            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                                for (int h = 0; h < 2; ++h) {
+                                    sum[j][h][0] = 0.f; sum[j][h][1] = 0.f;
+                                    if (!first)
+                                        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(sum[j][h][0]), "=f"(sum[j][h][1])
+                                                     : "r"((ob ^ (uint32_t)((j0 + j) << 5)) + (uint32_t)(h * 8 * BN * 4)) : "memory");
+                                }
+#pragma unroll
+                            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                                    for (int c = 0; c < 2; ++c) {
+                                        sum[j][h][c] += dm[4 * (j0 + j) + 2 * h + c];
+                                        if constexpr (PASSES == 3) sum[j][h][c] += dc[4 * (j0 + j) + 2 * h + c];
+                                    }
+                                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};"
+                                                 ::"r"((ob ^ (uint32_t)((j0 + j) << 5)) + (uint32_t)(h * 8 * BN * 4)),
+                                                 "f"(sum[j][h][0]), "f"(sum[j][h][1]) : "memory");
+                                }
+                        }
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < HALF; ++i) {
+                            acc[i] += dm[i];
+                            if constexpr (PASSES == 3) acc[i] += dc[i];
+                        }
                     }
                 }
             }
-            if (!(p.debug & 16)) hand_off();         // timing decomposition: no epilogue
+            if constexpr (SACC) {
+                if (!(p.debug & 16)) {               // timing decomposition: no epilogue
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&out_full);
+                }
+            } else {
+                if (!(p.debug & 16)) hand_off();     // timing decomposition: no epilogue
 #pragma unroll
-            for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
+                for (int i = 0; i < HALF; ++i) acc[i] = 0.f;
+            }
         }
     }
     __syncthreads();
     if (CS > 1) cluster_sync_all();             // nobody leaves while a peer may still multicast to / arrive on it
 }
 
-constexpr int tc_bn_slot(int BN) { return BN == 64 ? 1 : 0; }
+constexpr int tc_bn_slot(int BN) { return BN == 128 ? 2 : (BN == 64 ? 1 : 0); }
 constexpr int tc_passes_slot(int PASSES) { return PASSES == 1 ? 1 : 0; }
 
 template <int BN, int PASSES, bool KSPLIT>
@@ -571,14 +637,14 @@ int32_t tc_launch(const TapGemmParams& p0, cudaStream_t stream) {
     }
     const unsigned grid = (unsigned)((total_w < resident ? total_w : resident) * p.cluster);
     if (p.ksplit == 1) return tc_launch_t<BN, PASSES, false>(p, (int)mgroups, (int)total_w, grid, stream);
-    if constexpr (PASSES == 1) {
+    if constexpr (PASSES == 1 && BN <= 64) {
         // raw split sums into kpartial; the reduction adds them in split order and applies p's epilogue
         TapGemmParams q = p;
         q.dst = p.kpartial; q.bias = nullptr; q.mask = nullptr; q.relu = 0;
         CPB_TRY((tc_launch_t<BN, PASSES, true>(q, (int)mgroups, (int)total_w, grid, stream)));
         return launch_ksplit_reduce(p, stream);
     } else {
-        CPB_REQUIRE(false, "tc_tapgemm: the k-split is built for the single TF32 pass only");
+        CPB_REQUIRE(false, "tc_tapgemm: the k-split is built for the single TF32 pass at BN <= 64 only");
         return CPB_ERR_UNSUPPORTED;
     }
 }
@@ -588,7 +654,7 @@ int32_t tc_init_one() {
     using Cfg = TcCfg<BN, PASSES>;
     CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    if constexpr (PASSES == 1) {   // the k-split variant: same threads and shared memory, so the same resident count
+    if constexpr (PASSES == 1 && BN <= 64) {   // the k-split variant: same threads and shared memory, so the same resident count
         CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         if (g_tc_cluster > 1) CPB_CUDA(cudaFuncSetAttribute(tc_tapgemm_kernel<BN, PASSES, true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     }
@@ -654,7 +720,7 @@ __global__ void tc_weights_kernel(const float* __restrict__ params, float* __res
         x = params[job.src_off + (((long long)kh * job.k + kw) * job.cb + cb) * job.cs + cs];
         tap = kh; n = cs; c = cc;
     }
-    const int BN = tc_bn(job.N);
+    const int BN = tc_bn(job.N, job.ksplit != 0);
     const int nn = n % BN, cc = c % TBK;
     const long long block = ((long long)tap * (job.N / BN) + n / BN) * (job.C / TBK) + c / TBK;
     const long long at = job.dst_hi + block * (2 * BN * TBK) + (nn >> 3) * 256 + (nn & 7) * 32 + ((((cc >> 2) ^ (nn & 7))) << 2) + (cc & 3);
@@ -673,14 +739,17 @@ int32_t tc_tapgemm_init() {
     CPB_REQUIRE(g_tc_cluster == 1 || g_tc_cluster == 2 || g_tc_cluster == 4 || g_tc_cluster == 8, "CPB_TC_CLUSTER must be 1, 2, 4 or 8");
     CPB_TRY((tc_init_one<32, 3>()));
     CPB_TRY((tc_init_one<64, 3>()));
+    CPB_TRY((tc_init_one<128, 3>()));
     CPB_TRY((tc_init_one<32, 1>()));
     CPB_TRY((tc_init_one<64, 1>()));
+    CPB_TRY((tc_init_one<128, 1>()));
     return CPB_OK;
 }
 
 int tc_tapgemm_pick_ksplit(int K) {
     // splits of at most 320 k-blocks, at most 4 of them: the MlpVAE's 38 400-long reductions into 512 columns run as
-    // 4 splits of 300 k-blocks, which at B = 512 (32 output tiles) fills the 132 SMs of an H100 SXM in one wave
+    // 4 splits of 300 k-blocks, which at B = 512 (32 output tiles of 128 x 64: k-split problems stay at BN 64, see
+    // tc_bn) fills the 132 SMs of an H100 SXM in one wave
     const int s = (int)cdiv(K / TBK, 320);
     return s < 1 ? 1 : (s > 4 ? 4 : s);
 }
@@ -698,8 +767,9 @@ bool tc_tapgemm_supported(const TapGemmParams& p) {
 int32_t launch_tc_tapgemm(const TapGemmParams& p, cudaStream_t stream) {
     CPB_REQUIRE(tc_tapgemm_supported(p), "tc_tapgemm: unsupported problem (C=%d, N=%d)", p.C, p.N);
     CPB_REQUIRE(p.passes == 3 || p.passes == 1, "tc_tapgemm: passes must be 3 or 1, got %d", p.passes);
-    if (p.passes == 1) return tc_bn(p.N) == 64 ? tc_launch<64, 1>(p, stream) : tc_launch<32, 1>(p, stream);
-    return tc_bn(p.N) == 64 ? tc_launch<64, 3>(p, stream) : tc_launch<32, 3>(p, stream);
+    const int bn = tc_bn(p.N, p.ksplit > 1);
+    if (p.passes == 1) return bn == 128 ? tc_launch<128, 1>(p, stream) : bn == 64 ? tc_launch<64, 1>(p, stream) : tc_launch<32, 1>(p, stream);
+    return bn == 128 ? tc_launch<128, 3>(p, stream) : bn == 64 ? tc_launch<64, 3>(p, stream) : tc_launch<32, 3>(p, stream);
 }
 
 int32_t launch_tc_weights(const float* params, float* dst, const TcWeightTable& table, cudaStream_t stream) {

@@ -314,7 +314,7 @@ int32_t tc_wg_init_one() {
     return CPB_OK;
 }
 
-int tc_wg_bn(int J) { return J % 64 == 0 ? 64 : 32; }   // at most 64: see tc_bn
+int tc_wg_bn(int J) { return J % 64 == 0 ? 64 : 32; }   // at most 64: 1.5 x BN fp32 accumulator registers per MMA thread
 
 }  // namespace
 

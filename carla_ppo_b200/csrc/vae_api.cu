@@ -1000,6 +1000,7 @@ static int32_t mlp_relayout_weights(const MlpPlan& pl, const MlpLayout& L, const
     auto add = [&](int tensor, int64_t dst, int mode, int N, int C) {
         TcWeightJob& j = w.jobs[w.njobs++];
         j.src_off = L.off[tensor]; j.dst_hi = j.dst_lo = dst; j.mode = mode; j.N = N; j.C = C; j.round_nearest = 1;
+        j.ksplit = tc_tapgemm_pick_ksplit(C) > 1;     // the split mlp_dense picks for this layer (one tap: K = C)
         j.count = (long long)N * C; w.total += j.count;
     };
     const int out = L.dec(pl.ndec);
