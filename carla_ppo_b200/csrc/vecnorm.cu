@@ -209,7 +209,7 @@ static RewardNormArgs reward_args(const cpb_running_norm* cfg, double* ret_stats
                           cfg->epsilon, out};
 }
 
-// The normalisation half of an actor call (vae_api.cu's encode_predict): checked before anything is enqueued, then the
+// The normalisation half of an actor call (actor.cu's encode_predict): checked before anything is enqueued, then the
 // normalised state assembly in place of the plain one, and the reward kernel when rewards are given.
 int32_t check_actor_norm(const cpb_actor_norm* n, int32_t state_dim, int32_t batch) {
     CPB_REQUIRE(n != nullptr, "actor normalisation: NULL cpb_actor_norm");
