@@ -4,7 +4,7 @@
 set -e
 cd "$(dirname "$0")"
 OUT=../libcarla_ppo_b200.so
-SRCS="runtime.cu vae_shared.cu conv_vae.cu mlp_vae.cu actor.cu tapgemm.cu tc_tapgemm.cu tc_wgrad.cu wgrad.cu elementwise.cu edge.cu ppo.cu vecnorm.cu"
+SRCS="runtime.cu vae_shared.cu conv_vae.cu mlp_vae.cu actor.cu tapgemm.cu tc_tapgemm.cu tc_wgrad.cu wgrad.cu elementwise.cu edge.cu ppo.cu ppo_persistent.cu gae.cu ppo_api.cu vecnorm.cu"
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC"
 mkdir -p ../build
 OBJS=""

@@ -407,11 +407,7 @@ __global__ void adam_kernel(float4* __restrict__ p, const float4* __restrict__ g
         gv.x *= c; gv.y *= c; gv.z *= c; gv.w *= c;
     }
     float4 mv = m[i], vv = v[i], pv = p[i];
-    mv.x += (gv.x - mv.x) * omb1; mv.y += (gv.y - mv.y) * omb1; mv.z += (gv.z - mv.z) * omb1; mv.w += (gv.w - mv.w) * omb1;
-    vv.x += (gv.x * gv.x - vv.x) * omb2; vv.y += (gv.y * gv.y - vv.y) * omb2;
-    vv.z += (gv.z * gv.z - vv.z) * omb2; vv.w += (gv.w * gv.w - vv.w) * omb2;
-    pv.x -= (mv.x * alpha) / (sqrtf(vv.x) + epsilon); pv.y -= (mv.y * alpha) / (sqrtf(vv.y) + epsilon);
-    pv.z -= (mv.z * alpha) / (sqrtf(vv.z) + epsilon); pv.w -= (mv.w * alpha) / (sqrtf(vv.w) + epsilon);
+    adam_update(gv, mv, vv, pv, alpha, omb1, omb2, epsilon);
     m[i] = mv; v[i] = vv; p[i] = pv;
 }
 

@@ -105,6 +105,18 @@ int32_t launch_adam(float* params, const float* grads, float* m, float* v, long 
                     float lr, const float* lr_dev, float beta1, float beta2, float epsilon, cudaStream_t stream,
                     const void* guard = nullptr, const float* gscale = nullptr, int32_t* steps = nullptr);
 
+// TF ApplyAdam on four parameters p with slots m, v and (already scaled) gradient g; alpha = lr sqrt(1 - beta2^t) /
+// (1 - beta1^t), omb1 = 1 - beta1, omb2 = 1 - beta2.  adam_kernel and the persistent PPO learn() kernel both run it; each
+// loads and stores the float4s itself.
+__device__ __forceinline__ void adam_update(const float4& g, float4& m, float4& v, float4& p, float alpha, float omb1,
+                                            float omb2, float epsilon) {
+    m.x += (g.x - m.x) * omb1; m.y += (g.y - m.y) * omb1; m.z += (g.z - m.z) * omb1; m.w += (g.w - m.w) * omb1;
+    v.x += (g.x * g.x - v.x) * omb2; v.y += (g.y * g.y - v.y) * omb2;
+    v.z += (g.z * g.z - v.z) * omb2; v.w += (g.w * g.w - v.w) * omb2;
+    p.x -= (m.x * alpha) / (sqrtf(v.x) + epsilon); p.y -= (m.y * alpha) / (sqrtf(v.y) + epsilon);
+    p.z -= (m.z * alpha) / (sqrtf(v.z) + epsilon); p.w -= (m.w * alpha) / (sqrtf(v.w) + epsilon);
+}
+
 int32_t launch_fill_zero(float* p, long long n, cudaStream_t stream);
 
 }  // namespace cpb

@@ -182,7 +182,7 @@ def test_constants_pinned_to_the_shipped_graphs():
     assert po.LOG_SQRT_2PI == p["log_prob_const"] and po.ENTROPY_CONST == p["entropy_const"] and p["log_prob_half"] == -0.5
     # clip bounds: Python 1 -/+ 0.2 rounded to float32 (what the oracle uses) ...
     assert float(np.float32(1.0 - 0.2)) == p["clip_low"] and float(np.float32(1.0 + 0.2)) == p["clip_high"]
-    # ... and what the CUDA head kernel computes in float32 from eps_clip = 0.2f (ppo.cu: 1.f -/+ a.eps_clip)
+    # ... and what the CUDA head kernel computes in float32 from eps_clip = 0.2f (ppo_device.cuh: 1.f -/+ a.eps_clip)
     assert float(np.float32(1) - np.float32(0.2)) == p["clip_low"] and float(np.float32(1) + np.float32(0.2)) == p["clip_high"]
     assert float(np.float32(0.01)) == p["entropy_scale"] and p["value_scale"] == 1.0
     assert p["mean_affine_add"] == 1.0 and p["mean_affine_div"] == 2.0        # mu = low + (tanh + 1)/2 * (high - low)
@@ -212,10 +212,11 @@ def test_constants_pinned_to_the_shipped_graphs():
         assert tuple(mc["ppo"]["variables"]["policy/" + name]) == shape == tuple(mc["ppo"]["variables"]["policy_old/" + name])
 
 
-def test_cuda_sources_use_the_pinned_constants():
-    """The kernels spell the same literals (grep-level check; the GPU tests check the numerics)."""
+def test_cuda_device_code_uses_the_pinned_constants():
+    """The PPO device code (ppo_device.cuh, which both learn paths compile) spells the same literals (grep-level check; the
+    GPU tests check the numerics)."""
     mc = _meta_constants()["ppo"]["constants"]
-    src = open(os.path.join(ROOT, "carla_ppo_b200", "csrc", "ppo.cu")).read()
+    src = open(os.path.join(ROOT, "carla_ppo_b200", "csrc", "ppo_device.cuh")).read()
     assert ("kLogSqrt2Pi = %sf" % repr(mc["log_prob_const"])) in src
     assert ("kEntropyConst = %sf" % repr(mc["entropy_const"])) in src
     assert "unclipped <= clipped" in src
